@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — the driver's measurement contract for the seekstorm_b200 hot path.
+"""bench.py — measures the seekstorm_b200 hot paths on the GPU and prints one JSON result line.
 
 Metric (BASELINE.json): queries/sec at top-10.  N=1 workload = configs[1]: brute-force cosine kNN over
 1M x 768 f32 (C2).  A "step" = one call of the hot path over one batch of synthetic queries (batch = --batch
@@ -59,7 +59,10 @@ def parse():
     p.add_argument("--parity-queries", type=int, default=64, help="queries per path of the post-run oracle check")
     p.add_argument("--cpu-seconds", type=float, default=12.0, help="budget of each cpu_baseline sample")
     p.add_argument("--vector-kernel", default="both", choices=["both", "all", "ffma", "tc", "tc64", "tcb", "tcb64", "tcb256", "filt", "filt256", "filt256p"],
-                   help="FP32 FFMA2 scan, tcgen05 scans, or both = ffma + tcb + tcb256 (headline = the fastest: what AUTO picks)")
+                   help="FP32 FFMA scan, tensor-core scans, or both = ffma + tcb + tcb256 (headline = the fastest: what AUTO picks)")
+    p.add_argument("--dump-outputs", metavar="DIR", default=None,
+                   help="after the timed steps, write what each timed vector scan computed in its last step (top-10 doc ids and scores "
+                        "per query) as DIR/<name>.npy, for comparing two builds output for output")
     return p.parse_args()
 
 
@@ -68,20 +71,20 @@ def peaks():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured"
     except Exception:
-        return 6650.0, "fallback"
+        return 3350.0, "H100 SXM data sheet"
 
 
 def tensor_peak():
-    """dense bf16 TFLOP/s: the burst figure (kernel timed alone) of MEASURED_PEAKS.json, else the nominal 2250."""
+    """dense bf16 TFLOP/s: the burst figure (kernel timed alone) of MEASURED_PEAKS.json, else the H100 SXM data sheet's 989."""
     try:
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["bf16_tflops"]), "measured (burst)"
     except Exception:
-        return 2250.0, "nominal"
+        return 989.0, "H100 SXM data sheet"
 
 
 class ClockSampler:
-    """SM clock / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe).  In-process NVML polling
+    """SM clock / throttle reasons sampled DURING the timed region In-process NVML polling
     (nvidia_ml_py) every 10 ms; falls back to an `nvidia-smi -lms` child process.  (The first version polled nvidia-smi with
     power.draw in the query: each sample stalled kernel launches for milliseconds and the device-resident `value`, measured
     with the sampler running, came out slower than the e2e number measured without it.)"""
@@ -234,34 +237,17 @@ def gen_vector_level(level, rows, dims, device):
     return synth.gen_vectors(n, dims, 1002 * 1000 + level, device)
 
 
-KERNELS = {"ffma": (1, 16, "scan_ffma", "scan_ffma (TMA + packed FP32 FFMA2 + warp top-k)"),
-           "tc": (2, 128, "scan_tc", "scan_tc (TMA + tcgen05 3xTF32 split, TMEM accumulators, TMEM-epilogue top-k)"),
-           "tc64": (3, 64, "scan_tc", "scan_tc<64> (tcgen05 3xTF32, 64 queries per pass)"),
-           "tcb": (4, 128, "scan_tc", "scan_tc (TMA + tcgen05 3xBF16 split, TMEM accumulators, TMEM-epilogue top-k)"),
-           "tcb64": (5, 64, "scan_tc", "scan_tc<64> (tcgen05 3xBF16, 64 queries per pass)"),
-           "tcb256": (6, 256, "scan_tc", "scan_tc<256> (tcgen05 3xBF16 over bf16 planes, 256 queries per pass: half the HBM bytes per query)"),
+KERNELS = {"ffma": (1, 16, "scan_ffma", "scan_ffma (TMA + FP32 FFMA + warp top-k)"),
+           "tc": (2, 128, "scan_tc", "scan_tc (TMA + wgmma 3xTF32 split, register accumulators, warp top-k epilogue)"),
+           "tc64": (3, 64, "scan_tc", "scan_tc<64> (wgmma 3xTF32, 64 queries per pass)"),
+           "tcb": (4, 128, "scan_tc", "scan_tc (TMA + wgmma 3xBF16 split, register accumulators, warp top-k epilogue)"),
+           "tcb64": (5, 64, "scan_tc", "scan_tc<64> (wgmma 3xBF16, 64 queries per pass)"),
+           "tcb256": (6, 256, "scan_tc", "scan_tc<256> (wgmma 3xBF16 over bf16 planes, 256 queries per pass: half the HBM bytes per query)"),
            # filter scan: ONE fp16 product over the 2-byte plane selects (proven margin) the <= 32 rows that can be in the top-10, refine
            # re-scores them with the f32 dot product; the result is the exact f32 top-k (DESIGN.md 3.2c)
-           "filt": (7, 128, "scan_tc", "scan_tc<128, f16 filter> + refine_candidates (tcgen05 1xFP16 over the 2-byte plane, exact f32 re-scoring of <= 32 candidates per query)"),
+           "filt": (7, 128, "scan_tc", "scan_tc<128, f16 filter> + refine_candidates (wgmma 1xFP16 over the 2-byte plane, exact f32 re-scoring of <= 32 candidates per query)"),
            "filt256": (8, 256, "scan_tc", "scan_tc<256, f16 filter> + refine_candidates (256 queries per pass)"),
-           "filt256p": (9, 256, "scan_tc", "scan_tc2 (256-query f16 filter on CTA pairs, tcgen05 cta_group::2) + refine_candidates")}
-# DRAM traffic per corpus pass (dram__bytes_read.sum + dram__bytes_write.sum of ONE ncu --set full capture, divided by
-# the passes in that launch, 1M x 768 corpus) from the committed captures under profiles/: traffic ~= algorithmic bytes
-# (3.072 GB), i.e. no re-reads.
-NCU = {"scan_ffma": {"traffic_per_pass": 3.0770e9, "source": "profiles/r02_scan_ffma.summary.txt"},   # 3.0734 GB read + 3.6 MB written, one pass of 16 queries
-       # bf16 hi/lo corpus planes: (6.1655 GB read + 58.7 MB written) / 2 passes; 256-query tile: 3.1087 GB + 75.5 MB, one pass
-       "scan_tc": {"traffic_per_pass": 3.1121e9, "source": "profiles/r02_scan_tc_bf16_planes_v1.summary.txt", "tensor_pipe_pct": 66.1},
-       "tcb256": {"traffic_per_pass": 3.1842e9, "source": "profiles/r02_scan_tc_bf16_n256_v1.summary.txt", "tensor_pipe_pct": 84.2},
-       # filter scan (fp16 plane): 128-query tile (3.0909 GB read + 60.8 MB written) / 2 passes; 256-query tile 1.5575 GB + 59.2 MB, one pass
-       "filt": {"traffic_per_pass": 1.5759e9, "source": "profiles/r02_scan_tc_filter_v1.summary.txt", "tensor_pipe_pct": 45.2},
-       "filt256": {"traffic_per_pass": 1.6167e9, "source": "profiles/r02_scan_tc_filter_n256_v1.summary.txt", "tensor_pipe_pct": 62.1},
-       # scan_tc2 (CTA pairs, 256 queries): 1.5575 GB read + 58.9 MB written in one pass of 355.5 us under ncu
-       "filt256p": {"traffic_per_pass": 1.6164e9, "source": "profiles/r02_scan_tc2_filter_pair.summary.txt", "tensor_pipe_pct": 64.3},
-       # int8 full scan of 1M x 768, 1024 queries = 8 passes in one launch: (6.2222 GB read + 219.8 MB written) / 8
-       "scan_tc_i8": {"traffic_per_pass": 0.8052e9, "source": "profiles/r02_scan_tc_i8.summary.txt"},
-       # lex_score<OR>, C3 10M docs, 4096 queries, Topk: 6.8986 GB read + 60.6 MB written (random 32-byte sector probes of the
-       # bitmap sectors and the coarse tables on top of the 1.5 GB the algorithm names)
-       "lex_score": {"traffic": 6.9592e9, "source": "profiles/r02_lex_score_v6.summary.txt"}}
+           "filt256p": (9, 256, "scan_tc", "scan_tc<256, f16 filter, pair> (256-query f16 filter on clusters of 2 CTAs sharing the query block by TMA multicast) + refine_candidates")}
 
 
 def measure_vector_kernel(a, ix, kname, q_host, q_dev, keys, local_rows, rank, world, dev, want_clocks):
@@ -274,6 +260,7 @@ def measure_vector_kernel(a, ix, kname, q_host, q_dev, keys, local_rows, rank, w
     step_dev(); torch.cuda.synchronize()
     sampler = ClockSampler(dev.index) if want_clocks else None
     ms = timed_steps(step_dev, a.steps, a.warmup, world, sampler)
+    last_keys = keys[:, :TOPK].cpu().numpy()      # what the last timed step returned (packed top-10 keys per query)
     clocks = sampler.stop() if sampler else None
     kern_ns = []
     for _ in range(5):       # duration of the dominant kernel: CUDA events the library records around that launch
@@ -296,7 +283,6 @@ def measure_vector_kernel(a, ix, kname, q_host, q_dev, keys, local_rows, rank, w
     # algorithm only has to stream the 2-byte plane, so ITS roofline is counted on rows*dims*2 (the f32-equivalent figure is reported beside it)
     alg_bytes = float(local_rows) * a.dims * (2 if filt else 4) * passes
     achieved = alg_bytes / (kern_ms / 1e3) / 1e9 if kern_ms else None
-    ncu = NCU.get(kname, NCU.get(kshort, {}))
     tensor = None
     if kshort == "scan_tc" and kern_ms:
         # every f32 product is three bf16 MMAs (hi*hi + hi*lo + lo*hi): executed flops = 3 x the algorithmic 2*rows*dims*queries
@@ -304,7 +290,7 @@ def measure_vector_kernel(a, ix, kname, q_host, q_dev, keys, local_rows, rank, w
         alg_tf = 2.0 * local_rows * a.dims * qt * passes / (kern_ms / 1e3) / 1e12
         nprod = 1 if filt else 3
         tensor = {"algorithmic_tflops": alg_tf, "executed_tflops": nprod * alg_tf, "peak": tpeak, "peak_kind": tkind,
-                  "frac_executed": nprod * alg_tf / tpeak, "tensor_pipe_pct_ncu": ncu.get("tensor_pipe_pct")}
+                  "frac_executed": nprod * alg_tf / tpeak}
     return {
         "value": a.batch * a.steps / (ms / 1e3), "unit": "queries/s", "ms_per_step": ms / a.steps,
         "e2e": {"value": a.batch * a.steps / (ms_e2e / 1e3), "unit": "queries/s", "ms_per_step": ms_e2e / a.steps,
@@ -312,15 +298,30 @@ def measure_vector_kernel(a, ix, kname, q_host, q_dev, keys, local_rows, rank, w
         "gpu_launches": int(launches) * a.steps, "queries_per_pass": qt, "passes_per_step": passes, "kernel_desc": klong,
         "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s",
                      "frac": (achieved / peak) if achieved else None,
-                     "traffic": (ncu["traffic_per_pass"] * passes * local_rows / 1e6) if (ncu and ncu.get("traffic_per_pass") and a.dims == C2_DIMS) else None,
-                     "traffic_source": ncu.get("source"), "peak_kind": f"of {peak_kind}", "kernel": kshort, "kernel_ms": kern_ms,
+                     "peak_kind": f"of {peak_kind}", "kernel": kshort, "kernel_ms": kern_ms,
                      "algorithmic_bytes_per_launch": alg_bytes, "tensor": tensor,
                      **({"f32_equivalent_gbs": float(local_rows) * a.dims * 4 * passes / (kern_ms / 1e3) / 1e9 if kern_ms else None,
                          "note": "filter scan: streams rows*dims*2 bytes per pass (fp16 plane) + <= 32 f32 rows per query in the refine step; "
                                  "achieved/frac are counted on the 2-byte plane, f32_equivalent_gbs is the SURVEY 8(d) figure rows*dims*4/t"} if filt else {})},
         "filter_fallbacks": int(fallbacks) if filt else None,
         "clocks": clocks,
+        "last_keys": last_keys,
     }
+
+
+def dump_vector_outputs(dir_, res):
+    """DIR/vector_<kernel>_doc_ids.npy (float64) and DIR/vector_<kernel>_scores.npy (float32): [batch, 10] per measured scan, decoded
+    from the packed keys key = (ordered score bits << 32) | (0xFFFFFFFF - doc id); an empty slot (key 0) reads as doc id -1, score NaN."""
+    os.makedirs(dir_, exist_ok=True)
+    for name, r in res.items():
+        k = r["last_keys"].astype(np.uint64)
+        empty = k == 0
+        o = (k >> np.uint64(32)).astype(np.uint32)
+        bits = np.where(o & np.uint32(0x80000000), o & np.uint32(0x7FFFFFFF), ~o).astype(np.uint32)
+        scores = np.where(empty, np.float32(np.nan), bits.view(np.float32)).astype(np.float32)
+        docs = np.where(empty, -1.0, (np.uint64(0xFFFFFFFF) - (k & np.uint64(0xFFFFFFFF))).astype(np.float64))
+        np.save(os.path.join(dir_, f"vector_{name}_doc_ids.npy"), docs)
+        np.save(os.path.join(dir_, f"vector_{name}_scores.npy"), scores)
 
 
 def best_hbm_variant(kernels: dict):
@@ -358,6 +359,8 @@ def bench_vector(a, rank, world, out):
     keys = torch.zeros((a.batch, 32), dtype=torch.int64, device=dev)
     names = ["ffma", "tcb", "tcb256", "filt", "filt256", "filt256p"] if a.vector_kernel in ("both", "all") else [a.vector_kernel]
     res = {k: measure_vector_kernel(a, ix, k, q_host, q_dev, keys, local_rows, rank, world, dev, rank == 0) for k in names}
+    if a.dump_outputs and rank == 0:
+        dump_vector_outputs(a.dump_outputs, res)
     # batch-size sweep through the reference-facing call (host buffers, AUTO kernel choice): latency at batch 1 .. 256
     sweep = {}
     if world == 1:
@@ -370,8 +373,8 @@ def bench_vector(a, rank, world, out):
 
             def step_b():
                 ix.search_vector_raw(qn, TOPK, hb, nb)
-            msb = timed_steps(step_b, max(10, a.steps), 5, world)
-            per = msb / max(10, a.steps)
+            msb = timed_steps(step_b, a.steps, a.warmup, world)
+            per = msb / a.steps
             sweep[str(bs)] = {"ms_per_call": per, "queries_per_s": bs / (per / 1e3)}
     best = max(names, key=lambda k: res[k]["value"])      # headline = what SSB_VEC_KERNEL_AUTO picks for this batch size
     r = res[best]
@@ -386,7 +389,7 @@ def bench_vector(a, rank, world, out):
         "batch_sweep_e2e": sweep,
         "kernels": {{"ffma": "scan_ffma", "tc": "scan_tc_tf32", "tc64": "scan_tc_tf32_n64", "tcb": "scan_tc_bf16", "tcb64": "scan_tc_bf16_n64", "tcb256": "scan_tc_bf16_n256",
                      "filt": "scan_tc_f16_filter", "filt256": "scan_tc_f16_filter_n256", "filt256p": "scan_tc2_f16_filter_n256_pair"}[k]:
-                    {kk: vv for kk, vv in res[k].items() if kk != "kernel_desc"} for k in names},
+                    {kk: vv for kk, vv in res[k].items() if kk not in ("kernel_desc", "last_keys")} for k in names},
     })
     try:   # the same corpus pass at its most HBM-efficient tile, next to the (faster) headline kernel
         out["roofline"] = dict(out["roofline"], best_hbm_fraction_variant=best_hbm_variant(out["kernels"]))
@@ -396,7 +399,7 @@ def bench_vector(a, rank, world, out):
 
 
 def bench_vector_int8(a, rank, world):
-    """C2 corpus with Cosine + ScalarQuantizationI8 (SURVEY §8f row 2): int8 corpus, tcgen05 kind::i8 scan, exact scores."""
+    """C2 corpus with Cosine + ScalarQuantizationI8 (SURVEY §8f row 2): int8 corpus, s8 wgmma scan, exact scores."""
     from seekstorm_b200 import Index, VectorSimilarity, synth
     from seekstorm_b200.parallel import init_shard_comm
     dev = torch.device("cuda", torch.cuda.current_device())
@@ -440,7 +443,7 @@ def bench_vector_int8(a, rank, world):
 
             def step_b():
                 ix.search_vector_raw(qn, TOPK, hb, nbuf)
-            n_it = max(5, a.steps // 2)
+            n_it = a.steps
             per = timed_steps(step_b, n_it, 2, world) / n_it
             sweep[str(bs)] = {"ms_per_call": per, "queries_per_s": bs / (per / 1e3)}
     peak, peak_kind = peaks()
@@ -454,20 +457,18 @@ def bench_vector_int8(a, rank, world):
         "value": nb * a.steps / (ms / 1e3), "unit": "queries/s", "ms_per_step": ms / a.steps, "dtype": "i8 (int32 accumulate, exact)",
         "config": {"workload": f"C2 corpus quantised to int8 (Cosine + ScalarQuantizationI8): {a.rows} x {a.dims}, top-{TOPK}, "
                                f"batch {nb} queries/step ({passes} corpus passes of 128 queries)",
-                   "kernel": "scan_tc<128, i8> (tcgen05 kind::i8, TMEM s32 accumulators)"},
+                   "kernel": "scan_tc<128, i8> (wgmma s8, s32 register accumulators)"},
         "e2e": {"value": nb * a.steps / (ms_e2e / 1e3), "unit": "queries/s", "ms_per_step": ms_e2e / a.steps,
                 "h2d_bytes_per_step": nb * a.dims * 4, "d2h_bytes_per_step": nb * 32 * 8},
         "gpu_launches": int(launches) * a.steps, "batch_sweep_e2e": sweep,
         "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": (achieved / peak) if achieved else None,
-                     "traffic": (NCU["scan_tc_i8"]["traffic_per_pass"] * passes * local_rows / 1e6) if a.dims == C2_DIMS else None,
-                     "traffic_source": NCU["scan_tc_i8"]["source"],
                      "peak_kind": f"of {peak_kind}", "kernel": "scan_tc_i8", "kernel_ms": kern_ms,
                      "algorithmic_bytes_per_launch": alg_bytes},
     }
 
 
 def bench_vector_int8_variants(a, rank, world):
-    """SURVEY 8(f) row 2, the other int8 quantisers on the int8 tcgen05 scan: TurboQuantI8 (1M x 768 cosine: rows are next_power_of_two(768) =
+    """SURVEY 8(f) row 2, the other int8 quantisers on the int8 tensor-core scan: TurboQuantI8 (1M x 768 cosine: rows are next_power_of_two(768) =
     1024 code bytes) and the affine Euclidean SQ of integer-valued data (SIFT-like 1M x 128).  Device-resident QPS + the scan's roofline."""
     from seekstorm_b200 import Index, VectorSimilarity, synth
     dev = torch.device("cuda", torch.cuda.current_device())
@@ -654,7 +655,7 @@ def _bm25_filter_variants(a, ix, qk, out_keys, steps, world, dev):
     for name, rt_ in (("or_topk_facet_filter", ResultType.Topk), ("or_topkcount_facet_filter", ResultType.TopkCount)):
         def step_f():
             ix.search_lexical_keys(bf, TOPK, rt_, out_keys, cnt_dev)
-        nv = max(2, steps // 2)
+        nv = steps
         msv = timed_steps(step_f, nv, 2, world)
         step_f(); torch.cuda.synchronize()
         sv = ix.last_stats()
@@ -688,7 +689,7 @@ def bench_phrase(a, rank, world):
     cnt_dev = torch.zeros(len(qk), dtype=torch.int64, device=dev)
     res = {"config": {"workload": f"{n} docs Zipf(1) V={C3_VOCAB} with positions ({n_pos} tokens), {len(qk)} phrases/step of 2-3 terms, ranks log-uniform [1,300]",
                       "index_build_s": build_s}}
-    steps = max(3, a.steps // 2)
+    steps = a.steps
     for name, rt_ in (("topk", ResultType.Topk), ("topkcount", ResultType.TopkCount)):
         def step():
             ix.search_lexical_keys(b, TOPK, rt_, out_keys, cnt_dev)
@@ -718,7 +719,7 @@ def bench_bm25(a, rank, world, keep_index=False, vector_dims=0):
 
     def step_dev():     # N>1: collective (all-gather + merge of the packed keys inside the library)
         ix.search_lexical_keys(b_dev, TOPK, ResultType.Topk, out_keys)
-    steps = max(3, a.steps // 2)
+    steps = a.steps
     ms = timed_steps(step_dev, steps, a.warmup, world)
     kern_ns = []
     for _ in range(3):
@@ -741,7 +742,7 @@ def bench_bm25(a, rank, world, keep_index=False, vector_dims=0):
 
         def step_v():
             ix.search_lexical_keys(bv, TOPK, rt_, out_keys, cnt_dev)
-        nv = max(2, steps // 2)
+        nv = steps
         msv = timed_steps(step_v, nv, 2, world)
         step_v(); torch.cuda.synchronize()
         sv = ix.last_stats()
@@ -765,8 +766,6 @@ def bench_bm25(a, rank, world, keep_index=False, vector_dims=0):
         "gpu_launches": int(launches) * steps, "variants": variants,
         "roofline": {"bound": "hbm", "achieved": (alg / (kern_ms / 1e3) / 1e9) if (alg and kern_ms) else None, "peak": peak, "unit": "GB/s",
                      "frac": (alg / (kern_ms / 1e3) / 1e9 / peak) if (alg and kern_ms) else None,
-                     "traffic": NCU["lex_score"]["traffic"] if (a.bm25_docs == C3_DOCS and len(qk) == 4096 and world == 1) else None,
-                     "traffic_source": NCU["lex_score"]["source"],
                      "peak_kind": f"of {peak_kind}", "kernel": "lex_score (+ lex_generic)", "kernel_ms": kern_ms,
                      "algorithmic_bytes_per_launch": alg, "postings_visited": st.get("postings_visited"), "probes": st.get("probes"),
                      "items_processed": st.get("items_processed"), "items_skipped": st.get("items_skipped")},
@@ -817,7 +816,7 @@ def bench_hybrid(a, rank, world):
     nq = 1000
     qk = bm25_queries(nq, 2004)
     qv = synth.gen_vectors(nq, C2_DIMS, 2005, "cpu").numpy()
-    steps = max(3, a.steps // 4)
+    steps = a.steps
     ms, h2d, launches = _hybrid_steps(a, ix, qk, qv, world, steps)
     ix.close()
     peak, peak_kind = peaks()
@@ -846,7 +845,7 @@ def bench_c5(a, rank, world, ix):
     qk = bm25_queries(nq, 2003)
     qv_t = synth.gen_vectors(nq, C2_DIMS, 2006, "cpu").pin_memory()
     qv = qv_t.numpy()
-    steps = max(3, a.steps // 4)
+    steps = a.steps
     ms, h2d, launches = _hybrid_steps(a, ix, qk, qv, world, steps)
     # vector-only on the same shards (device-resident, batch 256): the scan at C5 size
     q_dev = qv_t[:a.batch].to(dev)
@@ -854,7 +853,7 @@ def bench_c5(a, rank, world, ix):
 
     def step_v():
         ix.search_vector_keys(q_dev, TOPK, keys)
-    msv = timed_steps(step_v, max(3, a.steps // 2), 3, world)
+    msv = timed_steps(step_v, a.steps, a.warmup, world)
     kern = []
     for _ in range(3):
         step_v(); torch.cuda.synchronize()
@@ -868,7 +867,7 @@ def bench_c5(a, rank, world, ix):
             "config": {"workload": f"C5: {n} docs + {n} x {C2_DIMS} f32 vectors over {world} GPU(s) ({local_rows} rows on this rank), {nq} hybrid queries/step, e2e through ssb_search_hybrid",
                        "vector_build_s": build_s},
             "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": nq * 32 * 16, "gpu_launches": int(launches) * steps,
-            "vector_only": {"value": a.batch * max(3, a.steps // 2) / (msv / 1e3), "unit": "queries/s", "batch": a.batch,
+            "vector_only": {"value": a.batch * a.steps / (msv / 1e3), "unit": "queries/s", "batch": a.batch,
                             "roofline": {"bound": "hbm", "achieved": (alg / (kern_ms / 1e3) / 1e9) if kern_ms else None, "peak": peak, "unit": "GB/s",
                                          "frac": (alg / (kern_ms / 1e3) / 1e9 / peak) if kern_ms else None, "peak_kind": f"of {peak_kind}",
                                          "kernel": "scan_tc<256, f16 filter>", "kernel_ms": kern_ms, "algorithmic_bytes_per_launch": alg,
@@ -1031,7 +1030,7 @@ def main():
         return 0
 
     if not torch.cuda.is_available():
-        emit({"error": "no CUDA device: bench.py measures the B200 path only (no CPU fallback)"})
+        emit({"error": "no CUDA device: bench.py measures the GPU path only (no CPU fallback)"})
         return 1
     import __graft_entry__ as g
     if not os.path.exists(g.LIB):
@@ -1080,7 +1079,13 @@ def main():
     if "bm25" in sections:
         lex_ix = None
         try:
-            want_c5 = "c5" in sections and a.c5_docs == a.bm25_docs
+            # C5 keeps f32 + two bf16 planes + the fp16 plane of every vector (10 bytes per element) next to the lexical index: it runs
+            # when this GPU's shard of the vectors takes at most 60 % of device memory (10M x 768 needs two 80 GB GPUs)
+            c5_bytes = a.c5_docs / world * C2_DIMS * 10
+            c5_fits = c5_bytes <= 0.6 * torch.cuda.get_device_properties(torch.cuda.current_device()).total_memory
+            want_c5 = "c5" in sections and a.c5_docs == a.bm25_docs and c5_fits
+            if "c5" in sections and not c5_fits:
+                out["c5"] = {"skipped": f"{c5_bytes / 1e9:.1f} GB of vectors per GPU do not fit next to the lexical index; run with --gpus >= 2"}
             out["bm25"], lex_ix = bench_bm25(a, rank, world, keep_index=True, vector_dims=C2_DIMS if want_c5 else 0)
             if want_parity:
                 try:

@@ -1,5 +1,5 @@
 /*
- * seekstorm_b200.h — C ABI of libseekstorm_b200.so, the B200 (sm_100a) drop-in for the two query-time hot
+ * seekstorm_b200.h — C ABI of libseekstorm_b200.so, the H100 (sm_90a) drop-in for the two query-time hot
  * paths behind SeekStorm's Index::search():
  *   (a) BM25 top-k over block-partitioned posting lists (AND / OR with block-max pruning), and
  *   (b) the brute-force f32 dot / cosine / Euclidean vector scan with fused top-k,
@@ -63,7 +63,7 @@ enum { SSB_SIM_DOT = 0, SSB_SIM_COSINE = 1, SSB_SIM_EUCLIDEAN = 2 };
  *              (new_scale_norm_affine, :1414-1463: codes = round(x / scale) + zero_point with scale / zero point from the running min / max
  *              of everything indexed so far; euclidean_i8_quantized_affine, :1770-1795) — so does this library: rows must then be added
  *              in the reference's ingestion order, queries are quantised with the state the index has reached.
- * All three are bit-exact with the scalar CPU arithmetic (integer accumulation on tcgen05 kind::i8, reference operation order). */
+ * All three are bit-exact with the scalar CPU arithmetic (integer accumulation on s8 wgmma, reference operation order). */
 enum { SSB_QUANT_NONE = 0, SSB_QUANT_SCALAR_I8 = 1,
        /* TurboQuantI8 (vector_similarity.rs:1825-2093): every vector (after normalize_f32 for Cosine) is zero-padded to the next power of
         * two, sign-flipped by the index's seed mask, rotated by the normalised fast Walsh-Hadamard transform and quantised with
@@ -73,7 +73,7 @@ enum { SSB_QUANT_NONE = 0, SSB_QUANT_SCALAR_I8 = 1,
         * arithmetic.  Needs ssb_vector_set_turboquant_mask before the first level. */
        SSB_QUANT_TURBO_I8 = 2 };
 /* which vector scan kernel to use */
-/* FFMA: packed-FP32 scan, 16 queries per corpus pass (HBM-bound).  TCGEN05[_N64]: tensor-core scan with the 3xTF32
+/* FFMA: FP32 scan, 16 queries per corpus pass (HBM-bound).  TCGEN05[_N64]: tensor-core scan with the 3xTF32
  * split, 128 (or 64) queries per corpus pass.  TCGEN05_BF16[_N64]: tensor-core scan with the 3xBF16 split (half the
  * operand bytes; score error ~1e-5 relative, inside the 1e-4 tolerance).  AUTO: FFMA up to 16 queries and
  * for Euclidean; above that TCGEN05_BF16, or TCGEN05_BF16_N256 when its passes take less time for the batch size. */
@@ -84,7 +84,7 @@ enum { SSB_VEC_KERNEL_AUTO = 0, SSB_VEC_KERNEL_FFMA = 1, SSB_VEC_KERNEL_TCGEN05 
         * in the top-k (k <= 16); those are re-scored with the plain f32 dot product and queries whose candidate set did not fit are re-run
         * by an exact f32 scan on the device.  Results are the exact f32 top-k.  128 / 256 queries per corpus pass. */
        SSB_VEC_KERNEL_TCGEN05_FILTER = 7, SSB_VEC_KERNEL_TCGEN05_FILTER_N256 = 8,
-       /* the 256-query filter scan on CTA pairs (tcgen05 cta_group::2, clusters of 2): the two SMs of a pair share one copy of the query block */
+       /* the 256-query filter scan on CTA pairs (clusters of 2 CTAs): the two SMs of a pair share one copy of the query block (TMA multicast) */
        SSB_VEC_KERNEL_TCGEN05_FILTER_N256_PAIR = 9 };
 
 typedef struct ssb_index ssb_index;

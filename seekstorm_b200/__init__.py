@@ -1,4 +1,4 @@
-"""seekstorm_b200 — B200-native (sm_100a) drop-in for the two query-time hot paths behind SeekStorm's
+"""seekstorm_b200 — H100-native (sm_90a) drop-in for the two query-time hot paths behind SeekStorm's
 Index::search(): BM25 AND/OR top-k and the brute-force f32 vector scan (+ RRF hybrid).
 
 The compute lives in libseekstorm_b200.so (hand-written CUDA, C-ABI in include/seekstorm_b200.h);

@@ -1,6 +1,6 @@
 """ctypes loader for libseekstorm_b200.so (the C-ABI in include/seekstorm_b200.h).
 
-There is NO CPU fallback: if the shared library is missing or no B200 is visible, calls raise.
+There is NO CPU fallback: if the shared library is missing or no H100 is visible, calls raise.
 """
 from __future__ import annotations
 

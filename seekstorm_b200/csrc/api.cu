@@ -111,7 +111,7 @@ struct ssb_index {
     uint32_t tq_dim = 0; float* tq_mask = nullptr;   // the index's seed mask (+-1), ssb_vector_set_turboquant_mask
     bool dup_docs = false;            // some doc id occurs on more than one vector row (multi-chunk documents): results are de-duplicated
     DevBuf<float> rows;
-    DevBuf<uint16_t> rows_hi, rows_lo;   // bf16 planes of `rows` (hi = bf16_rn(x), lo = bf16_rn(x - hi)): what the tcgen05 bf16 scan streams
+    DevBuf<uint16_t> rows_hi, rows_lo;   // bf16 planes of `rows` (hi = bf16_rn(x), lo = bf16_rn(x - hi)): what the tensor-core bf16 scan streams
     DevBuf<int8_t> rows_i8;
     DevBuf<float> row_scale, row_norm;   // Dot / Euclidean + ScalarQuantizationI8: per-vector scale (and norm), QuantizedVector vector_similarity.rs:1340-1371
     // Euclidean + ScalarQuantizationI8 over integer-valued 0..255 data: the AFFINE quantiser (new_scale_norm_affine, vector_similarity.rs:1414-1463)
@@ -185,26 +185,27 @@ int32_t vec_keys(ssb_index* ix, SearchCtx& c, const void* queries, bool queries_
     if (k == 0 || k > SSB_K_MAX) { set_error("k must be in 1..%u", SSB_K_MAX); return SSB_E_UNSUPPORTED; }
     if (queries_i8 && !ix->quant_i8) { set_error("int8 queries need a ScalarQuantizationI8 index"); return SSB_E_INVALID; }
     if (nq == 0) return SSB_OK;
-    // AUTO (measured, 1M x 768): one FP32 pass of 16 queries takes ~0.5 ms, one tensor-core pass of up to 128 queries
-    // ~0.6 ms -> FP32 scan for <= 16 queries, tensor-core scan above.  Euclidean always takes the FP32 scan.
+    // AUTO (measured on one H100 SXM, 700 W, 1M x 768): one FP32 pass of 16 queries takes ~0.97 ms, one 3xBF16 tensor-core pass of up
+    // to 128 queries ~1.08 ms -> FP32 scan for <= 16 queries, tensor-core scan above.  Euclidean always takes the FP32 scan.
     uint32_t kern = ix->cfg.vector_kernel;
-    if (ix->quant_i8) kern = SSB_VEC_KERNEL_TCGEN05;   // one kernel for the int8 corpus: tcgen05 kind::i8, 128-query tile
+    if (ix->quant_i8) kern = SSB_VEC_KERNEL_TCGEN05;   // one kernel for the int8 corpus: s8 wgmma, 128-query tile
     if (kern == SSB_VEC_KERNEL_AUTO) {
-        // tensor-core scan above 16 queries; the 256-query tile (0.95 ms per pass vs 0.55 ms for 128 queries, measured) when it
-        // needs fewer milliseconds for this batch: ceil(nq/256) * 0.95 < ceil(nq/128) * 0.55
+        // tensor-core scan above 16 queries; the 256-query tile (2.37 ms per pass vs 1.08 ms for 128 queries, measured) when it
+        // needs fewer milliseconds for this batch: ceil(nq/256) * 2.37 < ceil(nq/128) * 1.08
         const uint32_t p128 = (nq + 127u) / 128u, p256 = (nq + 255u) / 256u;
-        kern = nq <= 16 ? SSB_VEC_KERNEL_FFMA : (p256 * 95u < p128 * 55u ? SSB_VEC_KERNEL_TCGEN05_BF16_N256 : SSB_VEC_KERNEL_TCGEN05_BF16);
+        kern = nq <= 16 ? SSB_VEC_KERNEL_FFMA : (p256 * 237u < p128 * 108u ? SSB_VEC_KERNEL_TCGEN05_BF16_N256 : SSB_VEC_KERNEL_TCGEN05_BF16);
         // filter scan + exact refine (DESIGN.md §3.2c): half the bytes and a third of the tensor work per pass
-        // — at every batch size: one 128-query filter pass (0.25 ms on 1M x 768) also beats the FP32 scan's 0.5 ms pass for <= 16 queries
+        // — at every batch size: one 128-query filter pass (0.59 ms on 1M x 768) also beats the FP32 scan's 0.97 ms pass for <= 16 queries.
+        // Above 128 queries one 256-query pass (1.13 ms, measured; 1.52 ms on CTA pairs) beats two 128-query passes (1.18 ms)
         const uint32_t exact_kern = kern;
-        kern = nq <= 128 ? SSB_VEC_KERNEL_TCGEN05_FILTER : SSB_VEC_KERNEL_TCGEN05_FILTER_N256_PAIR;   // above 128 queries: 256 per pass on CTA pairs
+        kern = nq <= 128 ? SSB_VEC_KERNEL_TCGEN05_FILTER : SSB_VEC_KERNEL_TCGEN05_FILTER_N256;
         if (ix->quant_i8 || ix->cfg.vector_similarity == SSB_SIM_EUCLIDEAN || k > 16 || ceil_dev || !ix->rows_h16.p || !ix->vec_err.p) kern = exact_kern;
     }
     // the filter scan keeps a candidate set sized for k <= 16 in the 32-entry lists and has no paging (ceilings are exact keys): those
     // calls take the exact 3-product scan
     bool filter = (kern == SSB_VEC_KERNEL_TCGEN05_FILTER || kern == SSB_VEC_KERNEL_TCGEN05_FILTER_N256 || kern == SSB_VEC_KERNEL_TCGEN05_FILTER_N256_PAIR);
     if (filter && (ix->quant_i8 || ix->cfg.vector_similarity == SSB_SIM_EUCLIDEAN || k > 16 || ceil_dev || !ix->rows_h16.p || !ix->vec_err.p)) {
-        kern = kern != SSB_VEC_KERNEL_TCGEN05_FILTER && (nq + 255u) / 256u * 95u < (nq + 127u) / 128u * 55u ? SSB_VEC_KERNEL_TCGEN05_BF16_N256 : SSB_VEC_KERNEL_TCGEN05_BF16;
+        kern = kern != SSB_VEC_KERNEL_TCGEN05_FILTER && (nq + 255u) / 256u * 237u < (nq + 127u) / 128u * 108u ? SSB_VEC_KERNEL_TCGEN05_BF16_N256 : SSB_VEC_KERNEL_TCGEN05_BF16;
         filter = false;
         if (ix->quant_i8) kern = SSB_VEC_KERNEL_TCGEN05;
     }
@@ -482,7 +483,7 @@ int32_t ssb_create(const ssb_config* cfg, ssb_index** out) {
     SSB_CUDA_TRY(cudaSetDevice(cfg->device));
     cudaDeviceProp prop;
     SSB_CUDA_TRY(cudaGetDeviceProperties(&prop, cfg->device));
-    if (prop.major != 10) { set_error("device %d is sm_%d%d; this library is built for sm_100a (B200) only", cfg->device, prop.major, prop.minor); return SSB_E_UNSUPPORTED; }
+    if (prop.major != 9 || prop.minor != 0) { set_error("device %d is sm_%d%d; this library is built for sm_90a (H100) only", cfg->device, prop.major, prop.minor); return SSB_E_UNSUPPORTED; }
     std::unique_ptr<ssb_index> ix(new (std::nothrow) ssb_index());
     if (!ix) { set_error("out of host memory"); return SSB_E_NOMEM; }
     ix->cfg = *cfg;

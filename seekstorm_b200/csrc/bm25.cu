@@ -1,4 +1,4 @@
-// bm25.cu — BM25 AND/OR top-k over block-partitioned posting lists (sm_100a).
+// bm25.cu — BM25 AND/OR top-k over block-partitioned posting lists (sm_90a).
 //
 // Replaces, for committed data (all paths /root/reference/seekstorm/src/; the per-candidate chain — delete set, NOT lists, facet filters,
 // field filter, phrase check: add_result.rs:3435-3500, 3124-3137, 3586-3684 — runs as predicates of the scoring kernels, see lex_generic):

@@ -7,7 +7,7 @@
 // records of the selected clusters (:1395-1467).
 //
 // Here: the scan kernels are batched — 16 to 256 queries share one pass over the corpus — so the union of the clusters a batch selects is
-// (nearly) the whole corpus and skipping bytes is not where a B200 saves time.  The probe is therefore a SELECTION MASK: ivf_score_medoids
+// (nearly) the whole corpus and skipping bytes is not where the GPU saves time.  The probe is therefore a SELECTION MASK: ivf_score_medoids
 // + ivf_select write one bit per (query, cluster), the scans run unchanged and test the bit only where a row is about to become a
 // candidate (the rare path, next to the delete-set probe).  A row of an unselected cluster can therefore never enter a list or move a
 // threshold: the result is exactly the reference's result for the same AnnMode, recall loss included.

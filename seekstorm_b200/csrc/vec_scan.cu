@@ -1,4 +1,4 @@
-// vec_scan.cu — brute-force f32 vector scan with fused top-k (sm_100a).
+// vec_scan.cu — brute-force f32 vector scan with fused top-k (sm_90a).
 //
 // Replaces the record loop of search_vector_shard (vector.rs:1397-1467): for every record,
 // similarity = dot_f32 / -euclidean_f32 (vector_similarity.rs:1006-1008, 912-918, 1120-1142) and
@@ -12,7 +12,7 @@
 //   producer: cp.async.bulk.tensor.2d of two [256 rows x 32 floats] corpus boxes (SWIZZLE_128B, 64 KB) and
 //             the [16 queries x 32 floats] query box into a 3-stage mbarrier ring.
 //   consumers: warp w owns rows (w>>1)*128 + lane + 32*{0..3} of the tile and queries (w&1)*8..+8
-//             (4 x 8 register tile per lane): packed FP32x2 FFMA2 accumulation over the k-chunks
+//             (4 x 8 register tile per lane): FP32 FFMA accumulation (even-k / odd-k pairs) over the k-chunks
 //             (conflict-free swizzled LDS.128 for rows, broadcast LDS.128 for queries; the 4x8 tile
 //             keeps shared-memory wavefronts at ~55 % of the HBM-time budget), then a warp-shuffle
 //             top-k insert per finished tile.
@@ -37,17 +37,13 @@ constexpr int STAGE_TX = A_BYTES + Q_BYTES;
 constexpr int LISTS_BYTES = CWARPS * 8 * LIST * 8;   // per-warp top-k lists (8 queries x 32 keys) live in smem
 constexpr int SMEM_BYTES = STAGES * (A_BYTES + Q_BYTES) + LISTS_BYTES + 2 * STAGES * 8;
 
-// packed FP32x2 math (Blackwell FFMA2 / FADD2): two FMAs per issued instruction
+// pairs of FP32 lanes (even-k / odd-k partial sums): Hopper has no packed FP32x2 instructions, so each pair is two scalar
+// round-to-nearest operations (the same rounding per component)
 __device__ __forceinline__ void ffma2(float2& c, float2 a, float2 b) {
-    asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(reinterpret_cast<unsigned long long&>(c))
-        : "l"(reinterpret_cast<unsigned long long&>(a)), "l"(reinterpret_cast<unsigned long long&>(b)));
+    c.x = __fmaf_rn(a.x, b.x, c.x);
+    c.y = __fmaf_rn(a.y, b.y, c.y);
 }
-__device__ __forceinline__ float2 fsub2(float2 a, float2 b) {
-    float2 d;
-    asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(reinterpret_cast<unsigned long long&>(d))
-        : "l"(reinterpret_cast<unsigned long long&>(a)), "l"(reinterpret_cast<unsigned long long&>(b)));
-    return d;
-}
+__device__ __forceinline__ float2 fsub2(float2 a, float2 b) { return make_float2(__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y)); }
 
 
 template <int SIM>

@@ -10,7 +10,7 @@ constexpr int VEC_QT = 16;      // queries per corpus pass of the FFMA kernel
 
 struct ScanArgs {
     const float* rows;            // [n_rows][dpad]
-    const void* rows_hi = nullptr; const void* rows_lo = nullptr;   // bf16 planes [n_rows][dpad] of the same rows (tcgen05 bf16 scan)
+    const void* rows_hi = nullptr; const void* rows_lo = nullptr;   // bf16 planes [n_rows][dpad] of the same rows (tensor-core bf16 scan)
     const void* rows_h16 = nullptr;   // scaled fp16 plane [n_rows][dpad] (filter scan)
     const uint32_t* doc_ids;      // [n_rows] or nullptr
     uint64_t n_rows;
@@ -25,7 +25,7 @@ struct ScanArgs {
     size_t scratch_bytes;
     uint64_t* keys_out;           // [nq_pad][32]
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;   // recorded around the scan kernel when set
-    float* q_hi = nullptr; float* q_lo = nullptr;  // [nq_pad][dpad] tf32 split of the queries (tcgen05 kernel)
+    float* q_hi = nullptr; float* q_lo = nullptr;  // [nq_pad][dpad] tf32 split of the queries (tensor-core kernel)
     uint32_t* thr_buf = nullptr;                   // [nq_pad] scratch for the pre-sampled per-query thresholds
     const uint32_t* thr_init = nullptr;            // internal: initial thresholds (ordered-uint scores) or null
     const uint64_t* ceil_keys = nullptr;           // [nq_pad] exclusive key ceilings for paging beyond 32 results, or null

@@ -1,38 +1,39 @@
-// vec_scan_tc.cu — tensor-core variant of the brute-force vector scan (sm_100a, tcgen05 + TMEM + TMA).
+// vec_scan_tc.cu — tensor-core variant of the brute-force vector scan (sm_90a: wgmma + TMA + mbarrier, thread-block clusters).
 //
-// Same contract as scan_ffma (vec_scan.cu): corpus [n_rows, Dpad] f32 x a block of NQ queries -> per-warp
-// top-32 lists, but the query x corpus contraction runs on the 5th-gen tensor cores:
-//   D[128 corpus rows, NQ queries] (f32, TMEM) += A[128 x K] . B[NQ x K]^T          tcgen05.mma.cta_group::1
+// Same contract as scan_ffma (vec_scan.cu): corpus [n_rows, Dpad] f32 x a block of NQ queries -> per-warp top-32 lists, but the
+// query x corpus contraction runs on the Hopper tensor cores (warpgroup MMA, both operands in shared memory, accumulators in registers):
+//   D[64 corpus rows, NQ/2 queries] (f32) += A[64 x K] . B[NQ/2 x K]^T          wgmma.mma_async.m64nNk*
 // f32-level accuracy (north-star tolerance 1e-4 on cosine scores) comes from a 3-product split
 //   a.b ~= a_hi.b_hi + a_lo.b_hi + a_hi.b_lo                (the dropped a_lo.b_lo term is second order)
 // in one of two operand precisions, or exactly on int8 codes (template PREC):
-//   PREC_TF32 : kind::tf32, x_hi = x & 0xFFFFE000 (exactly representable in tf32, so the result does not depend on
+//   PREC_TF32 : tf32 operands, x_hi = x & 0xFFFFE000 (exactly representable in tf32, so the result does not depend on
 //               whether the tensor core truncates or rounds), x_lo = x - x_hi (exact); error ~2^-22 per product.
-//   PREC_BF16 : kind::f16 (bf16 operands, f32 accumulate), x_hi = bf16_rn(x), x_lo = bf16_rn(x - x_hi);
+//   PREC_BF16 : bf16 operands, f32 accumulate, x_hi = bf16_rn(x), x_lo = bf16_rn(x - x_hi);
 //               error ~3*2^-17 per product (random sign) -> ~1e-5 relative on a 768-d score.  Twice the MACs per MMA
-//               instruction and half the operand bytes per MAC of tf32: the faster split (measured), now within a few
-//               percent of the tensor-pipe floor of 12 MMAs per 256-row stage.
-//   PREC_I8   : kind::i8 over an int8 corpus (Cosine + ScalarQuantizationI8, quantised at load time): ONE exact product, s32
-//               accumulators; the TMA'd tile is the MMA operand (no splitters), the 128-query block stays resident in smem
-//               (template BRES) and 12 warps run the epilogue.  See DESIGN.md §3.2b.
+//               instruction and half the operand bytes per MAC of tf32: the faster split.
+//   PREC_I8   : s8 x s8 -> s32 over an int8 corpus (Cosine + ScalarQuantizationI8, quantised at load time): ONE exact product; the
+//               TMA'd tile is the MMA operand (no splitting), the 128-query block stays resident in smem (template BRES) when it
+//               leaves room for 3 corpus stages.  See DESIGN.md §3.2b.
 // The query parts are prepared once per batch in global memory.  PREC_BF16: the corpus parts are prepared ONCE AT LOAD TIME as
 // two bf16 planes (hi, lo) — together 4 bytes per element, so the algorithmic bytes of a pass stay n_rows*dims*4 — and TMA
-// delivers them straight into the MMA-ready SWIZZLE_64B tiles: no splitter warps, no generic-proxy pass over the tile, half the
-// shared-memory traffic per stage (round 1 split the f32 tile in shared memory per stage: ncu showed LSU wavefronts at 47 % of
-// peak with 49.5 M bank conflicts competing with the tensor core's operand reads for the 128 B/clk of the SM's shared memory,
-// and the pass ran at 1.35x the HBM floor).  48 KB per stage, 4 stages.  PREC_TF32 keeps the f32 corpus and the 8 splitter
-// warps (out of place, 2 stages).  Each smem stage holds MT=2 corpus tiles (256 rows) against ONE query chunk.
+// delivers them straight into the MMA-ready SWIZZLE_64B tiles: no splitting pass over the tile in shared memory.  PREC_TF32 keeps
+// the f32 corpus and splits each stage in shared memory (out of place for the lo part).
 //
-// Warp roles (512 threads, 1 CTA/SM): w0 TMA producer | w1 TMEM alloc + MMA issuer | w4-7 epilogue (TMEM lane quadrant =
-// warp%4) | w8-15 splitters (tf32) / additional epilogue warps (int8) / idle (bf16).  Pipelines: full/split/empty per smem stage,
-// tfull/tempty per TMEM accumulator buffer (double-buffered: the epilogue of tile t overlaps the MMAs of tile t+1).
-// Epilogue: tcgen05.ld 8 (int8: 16) query columns at a time; the whole chunk is tested against the per-query thresholds
-// branch-free with ONE vote, and only chunks with a candidate take the per-column path (ballot, per-warp sorted lists in the
-// CTA's slice of the output scratch, no CTA barriers).
-// Threshold seeding: the same kernel runs first in sample mode over one tile per SM and writes per-(32-row group, query)
-// score maxima; kth_from_groupmax turns them into valid lower bounds of the k-th best score.
+// Warp roles (384 threads = 3 warpgroups, 1 CTA/SM): warpgroup 0 = TMA producer (one thread), warpgroups 1-2 = consumers.  Consumer
+// warpgroup c owns the query columns [c*NQ/2, (c+1)*NQ/2) of the block and all TROWS corpus rows of a tile (TROWS/64 m64 sub-tiles,
+// at most 128 accumulator registers per thread); warp w of the warpgroup owns rows 16w..16w+15 of every sub-tile and list w of the
+// warpgroup's queries, so each (list, query) pair has exactly one writer, as in the scratch layout [4 lists][NQ][32] per CTA.
+// Per stage both consumer warpgroups wait on the full barrier, issue their MMAs as one commit group (one group kept in flight) and
+// release the stage once its group retired.  Epilogue per tile (the producer keeps streaming up to STAGES stages ahead meanwhile):
+// the accumulator fragment goes 8 query columns at a time through a small per-warp shared-memory buffer into a lane = corpus row
+// layout (one pass = 32 rows = two sub-tiles); the whole chunk is tested against the per-query thresholds branch-free with ONE vote,
+// and only chunks with a candidate take the per-column path (ballot, per-warp sorted lists in the CTA's slice of the output scratch,
+// no CTA barriers).
+// Threshold seeding: the same kernel runs first in sample mode over one tile per SM and writes per-(32-row group, query) score
+// maxima; kth_from_groupmax turns them into valid lower bounds of the k-th best score.
 #include <cuda_bf16.h>
 #include <stdlib.h>
+#include <type_traits>
 #include <cuda_fp16.h>
 
 #include "common.cuh"
@@ -43,14 +44,15 @@ namespace vec {
 
 namespace tc {
 constexpr int KC = 32;                 // floats per k-chunk = one 128-byte swizzle row of the f32 corpus tile
-constexpr int TM = 128;                // UMMA M
-constexpr int MT = 2;                  // M-tiles per stage: the query chunk is fetched once per MT*128 corpus rows
+constexpr int TM = 128;                // corpus rows per TMA tile unit
+constexpr int MT = 2;                  // tile units per stage (128-query variants): the query chunk is fetched once per MT*128 corpus rows
 constexpr int TROWS = TM * MT;         // corpus rows per stage
 constexpr int A1_BYTES = TM * KC * 4;  // one 128-row f32 tile, 16 KB
-constexpr int A_BYTES = MT * A1_BYTES; // 32 KB
-constexpr int THREADS = 512;            // 16 warps: TMA, MMA, 2 idle, 4 epilogue, 8 splitters
-constexpr int SPLIT_THREADS = 256;
+constexpr int THREADS = 384;           // 3 warpgroups: TMA producer, 2 MMA + epilogue
 constexpr int CHUNK = 8;               // query columns per epilogue step
+constexpr int XB_STRIDE = CHUNK + 1;   // per-warp transposition buffer [32 rows][CHUNK] (+1 column: conflict-free row reads)
+constexpr int XB_BYTES = 8 * 32 * XB_STRIDE * 4;
+constexpr int SMEM_MAX = 232448;       // 227 KB opt-in limit per CTA
 enum { PREC_TF32 = 0, PREC_BF16 = 1, PREC_I8 = 2, PREC_F16F = 3 };
 // PREC_F16F — the FILTER scan (DESIGN.md §3.2c): ONE product h(a).h(b) over an fp16 plane of the corpus (2 bytes per element, a third of
 // the tensor work of the 3-product split; fp16 keeps 11 significand bits, bf16 8 — the margin below is 8x tighter than with the bf16
@@ -60,22 +62,26 @@ enum { PREC_TF32 = 0, PREC_BF16 = 1, PREC_I8 = 2, PREC_F16F = 3 };
 // so every row of the exact top-k satisfies s^ >= (k-th best s^) - 2 eps_q.  The epilogue keeps exactly that candidate set (keys carry
 // the ROW index, thresholds are lowered by the per-query margin 2 eps_q), refine_candidates (vec_refine.cu) re-scores the <= 32 candidates
 // in f32 from the f32 rows and flags the queries whose candidate set may not have fitted the 32-entry list for the exact fallback scan.
+// PAIR (filter scan, 256 queries): clusters of 2 CTAs on neighbouring corpus tiles share ONE copy of the query block: each CTA loads
+// half of it per stage with TMA multicast into both CTAs' shared memory, so an SM takes in its corpus tile plus half a query block per
+// stage instead of a whole one, and a stage is refilled once the consumers of BOTH CTAs released it.
 
 constexpr int MAX_STAGES = 6;
 template <int NQ, int PREC, bool BRES = false> struct Cfg {
-    // NQ = 256 (bf16 only): ONE 128-row corpus tile per stage against 256 queries — the corpus is streamed once per 256 queries (half
-    // the HBM bytes per query) and an MMA reads 4 KB of A per 8 KB of B (6 KB per 128x128x16 instead of 8); TMEM: 2 x 1 x 256 columns
-    static constexpr int MT = NQ == 256 ? 1 : 2;
+    // at most 128 accumulator registers per consumer thread (TROWS/64 sub-tiles x NQ/4): 256 queries -> one 128-row tile per stage (the
+    // corpus is streamed once per 256 queries: half the HBM bytes per query); tf32 -> 128 rows too (its stage also holds the lo part)
+    static constexpr int MT = (NQ == 256 || PREC == PREC_TF32) ? 1 : 2;
     static constexpr int TROWS = TM * MT;
+    static constexpr int MW = TROWS / 64;      // m64 sub-tiles per consumer warpgroup
+    static constexpr int NQH = NQ / 2;         // query columns per consumer warpgroup = the MMA's N
     static constexpr int A_BYTES = MT * A1_BYTES;
     // TF32: [A (-> A_hi in place) | A_lo | B_hi | B_lo], all f32 SWIZZLE_128B tiles
     // BF16: [A1 bf16 (hi plane) | A2 bf16 (lo plane) | B1 bf16 | B2 bf16], 64-byte rows, SWIZZLE_64B, all four delivered by TMA.
-    //       48 KB per stage -> 4 stages.
-    // I8  : [A i8 | B i8]: the int8 corpus (quantised at load time) is the MMA operand as TMA delivers it — no splitter
-    //       pass, 128 dims per 128-byte swizzle row, 4 smem stages
-    static constexpr int STAGES = PREC == PREC_TF32 ? 2 : 4;
-    static constexpr int KCE = PREC == PREC_I8 ? 128 : (PREC == PREC_F16F ? 64 : KC);   // elements per k-chunk (128 bytes; bf16 3-product: 64-byte rows)
+    // I8  : [A i8 | B i8]: the int8 corpus (quantised at load time) is the MMA operand as TMA delivers it, 128 dims per 128-byte swizzle row
+    // F16F: [A f16 | B f16], 64 halves per 128-byte swizzle row
+    static constexpr int KCE = PREC == PREC_I8 ? 128 : (PREC == PREC_F16F ? 64 : KC);   // elements per k-chunk
     static constexpr int B_BYTES = PREC == PREC_BF16 ? NQ * KC * 2 : NQ * KC * 4;
+    static constexpr int B_ROW = PREC == PREC_BF16 ? 64 : 128;                 // bytes per query row of a B tile
     static constexpr int ALO_OFF = PREC == PREC_BF16 ? 0 : A_BYTES;            // TF32: A_lo   | BF16: A1 (in place)
     static constexpr int A2_OFF = A_BYTES / 2;                                 // BF16: A2 (in place)
     static constexpr int B_OFF = PREC == PREC_TF32 ? 2 * A_BYTES : A_BYTES;
@@ -83,35 +89,165 @@ template <int NQ, int PREC, bool BRES = false> struct Cfg {
     // so the per-stage L2->SM traffic is the corpus tile alone (stage count chosen at launch from what is left of 227 KB)
     static constexpr int STAGE_BYTES = BRES ? A_BYTES : ((PREC == PREC_I8 || PREC == PREC_F16F) ? A_BYTES + B_BYTES : (PREC == PREC_BF16 ? A_BYTES + 2 * B_BYTES : 2 * A_BYTES + 2 * B_BYTES));
     static constexpr int TX_BYTES = BRES ? A_BYTES : ((PREC == PREC_I8 || PREC == PREC_F16F) ? A_BYTES + B_BYTES : A_BYTES + 2 * B_BYTES);
-    static constexpr int SMEM = STAGES * STAGE_BYTES + NQ * 12 + 256;   // thresholds + (scaled int8) per-query scale / norm
-    static constexpr int TMEM_COLS = 2 * MT * NQ;                              // double-buffered MT accumulators
+    // transposition buffers + thresholds + (scaled int8) per-query scale / norm + barriers + alignment slack of the dynamic segment
+    static constexpr int FIXED = XB_BYTES + NQ * 12 + 256 + 1024;
+    static constexpr int STAGES = (SMEM_MAX - FIXED) / STAGE_BYTES > MAX_STAGES ? MAX_STAGES : (SMEM_MAX - FIXED) / STAGE_BYTES;
+    static constexpr int SMEM = STAGES * STAGE_BYTES + FIXED;
 };
+// int8: the query block stays resident when it leaves room for 3 corpus stages
+constexpr bool i8_resident(uint32_t dpad8) { return (int)dpad8 * 128 + Cfg<128, PREC_I8, true>::FIXED + 3 * Cfg<128, PREC_I8, true>::A_BYTES <= SMEM_MAX; }
 
-// K-major SWIZZLE_128B canonical layout ((8,n),2):((8,SBO),1) in 16-byte units: LBO = 1, SBO = 1024 B
-__device__ __forceinline__ uint64_t umma_desc_k128(uint32_t saddr) {
-    return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
+// wgmma shared-memory matrix descriptor for K-major swizzled tiles: start address >> 4 (bits 0-13), leading byte offset (unused by
+// swizzled K-major layouts: 1), stride byte offset = one 8-row swizzle atom >> 4 (bits 32-45), swizzle mode (bits 62-63).
+// SWIZZLE_128B: 128-byte rows, 1024-byte atom, mode 1
+__device__ __forceinline__ uint64_t gmma_desc_k128(uint32_t saddr) {
+    return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 62);
 }
-// K-major SWIZZLE_64B: 64-byte rows, 8-row atom = 512 B -> SBO = 512 B, layout type 4
-__device__ __forceinline__ uint64_t umma_desc_k64(uint32_t saddr) {
-    return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | (32ull << 32) | (1ull << 46) | (4ull << 61);
+// SWIZZLE_64B: 64-byte rows, 512-byte atom, mode 2
+__device__ __forceinline__ uint64_t gmma_desc_k64(uint32_t saddr) {
+    return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | (32ull << 32) | (2ull << 62);
 }
-template <int PREC>
-__device__ __forceinline__ void umma(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
-    if (PREC == PREC_TF32)
-        asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\ntcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n}\n"
-                     ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum) : "memory");
-    else if (PREC == PREC_I8)
-        asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\ntcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n}\n"
-                     ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum) : "memory");
-    else
-        asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\ntcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n}\n"
-                     ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum) : "memory");
+
+// wgmma.mma_async m64nNk*, D (+)= A . B^T with both operands K-major in shared memory; acc = 0 overwrites D (first product of a tile)
+__device__ __forceinline__ void wgmma_tf32_n32(float (&d)[16], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+                 "%16, %17, p, 1, 1;\n}\n"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+                   "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+                 : "l"(a), "l"(b), "r"(acc) : "memory");
 }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+__device__ __forceinline__ void wgmma_tf32_n64(float (&d)[32], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
+                 "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+                 "%32, %33, p, 1, 1;\n}\n"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+                   "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+                   "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+                   "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+                 : "l"(a), "l"(b), "r"(acc) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_bf16_n32(float (&d)[16], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+                 "%16, %17, p, 1, 1, 0, 0;\n}\n"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+                   "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+                 : "l"(a), "l"(b), "r"(acc) : "memory");
+}
+__device__ __forceinline__ void wgmma_bf16_n64(float (&d)[32], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
+                 "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+                 "%32, %33, p, 1, 1, 0, 0;\n}\n"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+                   "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+                   "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+                   "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+                 : "l"(a), "l"(b), "r"(acc) : "memory");
+}
+__device__ __forceinline__ void wgmma_bf16_n128(float (&d)[64], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
+                 "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31,"
+                 "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47,"
+                 "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+                 "%64, %65, p, 1, 1, 0, 0;\n}\n"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+                   "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+                   "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+                   "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+                   "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+                   "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+                   "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+                   "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+                 : "l"(a), "l"(b), "r"(acc) : "memory");
+}
+__device__ __forceinline__ void wgmma_f16_n64(float (&d)[32], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
+                 "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+                 "%32, %33, p, 1, 1, 0, 0;\n}\n"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+                   "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+                   "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+                   "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+                 : "l"(a), "l"(b), "r"(acc) : "memory");
+}
+__device__ __forceinline__ void wgmma_f16_n128(float (&d)[64], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
+                 "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31,"
+                 "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47,"
+                 "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+                 "%64, %65, p, 1, 1, 0, 0;\n}\n"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+                   "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+                   "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+                   "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+                   "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+                   "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+                   "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+                   "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+                 : "l"(a), "l"(b), "r"(acc) : "memory");
+}
+__device__ __forceinline__ void wgmma_s8_n64(uint32_t (&d)[32], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n64k32.s32.s8.s8 "
+                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
+                 "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+                 "%32, %33, p;\n}\n"
+                 : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]),
+                   "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]),
+                   "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]),
+                   "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31])
+                 : "l"(a), "l"(b), "r"(acc) : "memory");
+}
+template <int PREC, int N, class T>
+__device__ __forceinline__ void mma(T (&d)[N / 2], uint64_t a, uint64_t b, uint32_t acc) {
+    if constexpr (PREC == PREC_TF32 && N == 32) wgmma_tf32_n32(d, a, b, acc);
+    else if constexpr (PREC == PREC_TF32 && N == 64) wgmma_tf32_n64(d, a, b, acc);
+    else if constexpr (PREC == PREC_BF16 && N == 32) wgmma_bf16_n32(d, a, b, acc);
+    else if constexpr (PREC == PREC_BF16 && N == 64) wgmma_bf16_n64(d, a, b, acc);
+    else if constexpr (PREC == PREC_BF16 && N == 128) wgmma_bf16_n128(d, a, b, acc);
+    else if constexpr (PREC == PREC_F16F && N == 64) wgmma_f16_n64(d, a, b, acc);
+    else if constexpr (PREC == PREC_F16F && N == 128) wgmma_f16_n128(d, a, b, acc);
+    else if constexpr (PREC == PREC_I8 && N == 64) wgmma_s8_n64(d, a, b, acc);
+    else static_assert(N < 0, "no wgmma shape for this precision / query tile");
+}
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from touching accumulator registers across wgmma.wait_group (the tensor core writes them asynchronously)
+__device__ __forceinline__ void fence_reg(float& r) { asm volatile("" : "+f"(r)::"memory"); }
+__device__ __forceinline__ void fence_reg(uint32_t& r) { asm volatile("" : "+r"(r)::"memory"); }
+__device__ __forceinline__ uint32_t acc_bits(float x) { return __float_as_uint(x); }
+__device__ __forceinline__ uint32_t acc_bits(uint32_t x) { return x; }
+
+__device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
+__device__ __forceinline__ void cluster_sync_all() {
+    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
+    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+// TMA load multicast to the CTAs of `mask`: the box lands at the same shared-memory offset in each, completing on each one's `bar`
+__device__ __forceinline__ void tma_load_2d_mc(void* dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar, uint16_t mask) {
+    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;"
+                 ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(mask) : "memory");
+}
+// arrive on the barrier at the same offset in CTA `cta` of the cluster
+__device__ __forceinline__ void mbar_arrive_cta(uint64_t* bar, uint32_t cta) {
+    uint32_t r;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_u32(bar)), "r"(cta));
+    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(r) : "memory");
+}
 
 __device__ __forceinline__ uint32_t bf16x2_hi(float x, float y, float& rx, float& ry) {
     // hi = bf16_rn(x); the residual x - hi is exact in f32
@@ -124,17 +260,13 @@ __device__ __forceinline__ uint32_t bf16x2(float x, float y) {
     return *reinterpret_cast<uint32_t*>(&h);
 }
 
-// int8 path: thresholds are kept as int32 dot products (scores are integer valued, so ord_f32((float)d) is monotone in d)
-__device__ __forceinline__ int ord_to_int(uint32_t o) {
-    return o == 0u ? INT_MIN : (o == 0xFFFFFFFFu ? INT_MAX : (int)unord_f32(o));
-}
-
 // SCALED (int8 only): 0 = Cosine + ScalarQuantizationI8 (score = the int32 dot product); 1 = Dot + ScalarQuantizationI8 (per-vector
 // scale, score = dot_i32 as f32 * query_scale * row_scale, dot_i8_quantized vector_similarity.rs:1754-1758); 2 = Euclidean +
 // ScalarQuantizationI8, non-affine (score = -max(0, query_norm + row_norm - 2*dot), euclidean_i8_quantized :1721-1734); 3 = the AFFINE
 // variant (integer-valued 0..255 data, euclidean_i8_quantized_affine :1770-1795): the int32 dot product is first corrected for the two zero
 // points, dot - zp_row*sum_q(query) - zp_query*sum_q(row) + n*zp_query*zp_row, regrouped as dot - zp_row*sum_q(query) + zp_query*(n*zp_row - sum_q(row))
-template <int NQ, int PREC, bool BRES, int SCALED>
+// Unscaled int8 scores are the int32 dot products as f32 (exact below 2^24), so every variant runs the same f32-score epilogue.
+template <int NQ, int PREC, bool BRES, int SCALED, bool PAIR>
 __global__ void __launch_bounds__(THREADS, 1)
 scan_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2 /*bf16: lo plane*/,
         const __grid_constant__ CUtensorMap tmBh, const __grid_constant__ CUtensorMap tmBl, uint32_t n_rows, uint32_t n_kchunks, uint32_t n_tiles, uint32_t k,
@@ -143,62 +275,56 @@ scan_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtenso
         const uint64_t* __restrict__ ceil_keys /*[gridDim.y*NQ] or null*/, uint32_t nst_rt,
         const uint32_t* __restrict__ del_slot, const uint64_t* __restrict__ del_words /*delete set or null*/,
         const float* __restrict__ row_scale, const float* __restrict__ row_norm /*SCALED: [n_rows]*/,
-        const float* __restrict__ q_scale, const float* __restrict__ q_norm /*SCALED: [gridDim.y*NQ]*/,
+        const float* __restrict__ q_scale, const float* __restrict__ q_norm /*SCALED: [gridDim.y*NQ]; filter scan: q_scale = margins*/,
         const int2* __restrict__ row_aff /*SCALED 3: [n_rows] (zero_point, dims*zero_point - sum_q)*/, const int2* __restrict__ q_aff /*SCALED 3: [gridDim.y*NQ] (zero_point, sum_q)*/,
-        const uint32_t* __restrict__ ivf_sel, uint32_t ivf_words, const uint32_t* __restrict__ row_cluster /*IVF selection mask (f32 epilogue) or null*/,
-        uint32_t sample_mode /*int8 only: write per-(32-row group, query) score maxima instead of lists*/) {
+        const uint32_t* __restrict__ ivf_sel, uint32_t ivf_words, const uint32_t* __restrict__ row_cluster /*IVF selection mask or null*/,
+        uint32_t sample_mode /*write per-(32-row group, query) score maxima instead of lists*/) {
     using C = Cfg<NQ, PREC, BRES>;
-    constexpr int MT = C::MT, TROWS = C::TROWS, A_BYTES = C::A_BYTES;   // (shadow the namespace-level 2-tile defaults)
+    constexpr int TROWS = C::TROWS, MW = C::MW, NQH = C::NQH;
+    using AccT = typename std::conditional<PREC == PREC_I8, uint32_t, float>::type;
     const uint32_t STAGES = BRES ? nst_rt : (uint32_t)C::STAGES;
-    // no static shared memory: the dynamic segment starts at offset 0 of the CTA window (1024-aligned for the swizzled
-    // tiles) and pointers derived from it stay in the shared address space (LDS/STS instead of generic LD/ST)
-    extern __shared__ __align__(1024) uint8_t base[];
+    // the swizzled tiles need 1024-byte alignment in the shared window (the same offset in both CTAs of a pair)
+    extern __shared__ __align__(1024) uint8_t smem_raw[];
+    uint8_t* base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     uint8_t* stage0 = base;
     // per-query sorted lists live directly in this CTA's slice of the output scratch (global, L2-resident): they are
     // touched only on the rare candidate insert, and each (warp, query) list is always owned by the same warp
-    uint64_t* lists = scratch + ((size_t)blockIdx.y * gridDim.x + blockIdx.x) * 4 * NQ * LIST;   // [4 epilogue warps][NQ][32]
+    uint64_t* lists = scratch + ((size_t)blockIdx.y * gridDim.x + blockIdx.x) * 4 * NQ * LIST;   // [4 lists][NQ][32]
     uint8_t* bres = base + STAGES * C::STAGE_BYTES;                           // BRES: resident query block
-    uint32_t* thr_u = (uint32_t*)(bres + (BRES ? n_kchunks * C::B_BYTES : 0)); // [NQ] ordered-uint score thresholds
-    float* qs_sm = (float*)(thr_u + NQ);          // [NQ] SCALED: query scale
+    uint32_t* xbuf = (uint32_t*)(bres + (BRES ? n_kchunks * C::B_BYTES : 0)); // [8 consumer warps][32][XB_STRIDE]
+    uint32_t* thr_u = xbuf + XB_BYTES / 4;        // [NQ] ordered-uint score thresholds
+    float* qs_sm = (float*)(thr_u + NQ);          // [NQ] SCALED: query scale; filter scan: margin
     float* qn_sm = qs_sm + NQ;                    // [NQ] SCALED: query norm
     uint64_t* bars = (uint64_t*)(thr_u + 3 * NQ);
     uint64_t* full = bars;                     // [STAGES]
-    uint64_t* split = full + MAX_STAGES;       // [STAGES]
-    uint64_t* empty = split + MAX_STAGES;      // [STAGES]
-    uint64_t* tfull = empty + MAX_STAGES;      // [2]
-    uint64_t* tempty = tfull + 2;              // [2]
-    uint64_t* bfull = tempty + 2;              // BRES: query block landed
-    uint32_t* tmem_slot = (uint32_t*)(bfull + 1);
+    uint64_t* empty = full + MAX_STAGES;       // [STAGES]
+    uint64_t* bfull = empty + MAX_STAGES;      // BRES: query block landed
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const uint32_t group = blockIdx.y;
+    const uint32_t rank = PAIR ? cluster_ctarank() : 0u;
 
     if (threadIdx.x == 0) {
         mbar_init(bfull, 1);
-        for (uint32_t s = 0; s < STAGES; s++) { mbar_init(&full[s], 1); mbar_init(&split[s], SPLIT_THREADS / 32); mbar_init(&empty[s], 1); }
-        for (int b = 0; b < 2; b++) { mbar_init(&tfull[b], 1); mbar_init(&tempty[b], PREC == PREC_TF32 ? 4 : 12); }
+        // every consumer warp releases a stage (and in a pair also the peer's copy of it: the peer's multicast writes into this one)
+        for (uint32_t s = 0; s < STAGES; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], PAIR ? 16 : 8); }
         fence_mbar_init();
     }
     for (int i = threadIdx.x; i < NQ; i += THREADS) {  // seeded by the pre-sample pass when present
-        uint32_t t = blockIdx.y * NQ + i >= nq_valid ? 0xFFFFFFFFu   // zero-padded query slot: unreachable threshold
-                                                     : (thr_init ? __ldg(&thr_init[blockIdx.y * NQ + i]) : 0u);
-        if (PREC == PREC_I8 && !SCALED) t = (uint32_t)ord_to_int(t);   // unscaled int8 path compares the raw int32 dot products
-        thr_u[i] = t;
+        thr_u[i] = blockIdx.y * NQ + i >= nq_valid ? 0xFFFFFFFFu   // zero-padded query slot: unreachable threshold
+                                                   : (thr_init ? __ldg(&thr_init[blockIdx.y * NQ + i]) : 0u);
         if (PREC == PREC_F16F) qs_sm[i] = __ldg(&q_scale[blockIdx.y * NQ + i]);   // filter scan: per-query margin 2 eps_q
         if (SCALED) { qs_sm[i] = __ldg(&q_scale[blockIdx.y * NQ + i]); qn_sm[i] = SCALED >= 2 ? __ldg(&q_norm[blockIdx.y * NQ + i]) : 0.f; }
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"((uint32_t)C::TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *(volatile uint32_t*)tmem_slot;
+    if (PAIR) cluster_sync_all();                 // both CTAs' barriers are initialised before anything arrives on them
 
-    if (warp == 0) {
+    // a pair walks pairs of neighbouring tiles; both CTAs take the same number of steps (the peer's multicast feeds both)
+    const uint32_t tile0 = PAIR ? (blockIdx.x & ~1u) + rank : blockIdx.x;
+    if (warp < 4) {
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
         // ===================== TMA producer =====================
-        if (lane == 0) {
+        if (warp == 0 && lane == 0) {
             tma_prefetch_desc(&tmA); tma_prefetch_desc(&tmA2); tma_prefetch_desc(&tmBh); tma_prefetch_desc(&tmBl);
             uint32_t it = 0;
             if (BRES) {
@@ -206,296 +332,207 @@ scan_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtenso
                 for (uint32_t kc = 0; kc < n_kchunks; ++kc)
                     tma_load_2d(bres + kc * C::B_BYTES, &tmBh, (int)(kc * C::KCE), (int)(group * NQ), bfull);
             }
-            for (uint32_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+            for (uint32_t tile = tile0; tile - rank < n_tiles; tile += gridDim.x) {
                 for (uint32_t kc = 0; kc < n_kchunks; ++kc, ++it) {
                     uint32_t s = it % STAGES, ph = (it / STAGES) & 1u;
                     uint8_t* st = stage0 + s * C::STAGE_BYTES;
                     mbar_wait(&empty[s], ph ^ 1u);
                     mbar_arrive_expect_tx(&full[s], C::TX_BYTES);
-                    tma_load_2d(st, &tmA, (int)(kc * C::KCE), (int)(tile * TROWS), &full[s]);   // 256-row box = MT swizzled tiles
+                    tma_load_2d(st, &tmA, (int)(kc * C::KCE), (int)(tile * TROWS), &full[s]);
                     if (PREC == PREC_BF16) tma_load_2d(st + C::A2_OFF, &tmA2, (int)(kc * C::KCE), (int)(tile * TROWS), &full[s]);   // lo plane
-                    if (!BRES) tma_load_2d(st + C::B_OFF, &tmBh, (int)(kc * C::KCE), (int)(group * NQ), &full[s]);
+                    if (PAIR)   // this CTA's half of the query block, into both CTAs
+                        tma_load_2d_mc(st + C::B_OFF + rank * (C::B_BYTES / 2), &tmBh, (int)(kc * C::KCE), (int)(group * NQ + rank * NQH), &full[s], (uint16_t)3);
+                    else if (!BRES)
+                        tma_load_2d(st + C::B_OFF, &tmBh, (int)(kc * C::KCE), (int)(group * NQ), &full[s]);
                     if (PREC == PREC_TF32 || PREC == PREC_BF16) tma_load_2d(st + C::B_OFF + C::B_BYTES, &tmBl, (int)(kc * C::KCE), (int)(group * NQ), &full[s]);
                 }
             }
         }
-    } else if (warp == 1) {
-        // ===================== MMA issuer (one thread) =====================
-        if (lane == 0) {
-            // instruction descriptor: D=f32 (bit 4), A/B format at bits 7/10 (tf32 = 2, bf16 = 1, f16 = 0), both K-major,
-            // N>>3 at bit 17, M>>4 at bit 24
-            // (kind::i8: D = s32 (2 at bit 4), A/B format 1 = signed int8)
-            constexpr uint32_t fmt = PREC == PREC_TF32 ? 2u : (PREC == PREC_F16F ? 0u /*kind::f16: F16*/ : 1u);
-            constexpr uint32_t cfmt = PREC == PREC_I8 ? 2u : 1u;
-            const uint32_t idesc = (cfmt << 4) | (fmt << 7) | (fmt << 10) | ((uint32_t)(NQ >> 3) << 17) | ((uint32_t)(TM >> 4) << 24);
-            uint32_t it = 0, ti = 0;
-            if (BRES) mbar_wait(bfull, 0);
-            for (uint32_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++ti) {
-                const uint32_t buf = ti & 1u, tph = (ti >> 1) & 1u;
-                mbar_wait(&tempty[buf], tph ^ 1u);
-                tc_fence_after();
-                const uint32_t d = tmem_base + buf * (MT * NQ);
-                for (uint32_t kc = 0; kc < n_kchunks; ++kc, ++it) {
-                    uint32_t s = it % STAGES, ph = (it / STAGES) & 1u;
-                    mbar_wait(&full[s], ph);
-                    if (PREC == PREC_TF32) mbar_wait(&split[s], ph);
-                    tc_fence_after();
-                    const uint32_t sa = smem_u32(stage0 + s * C::STAGE_BYTES);
-                    if (PREC == PREC_I8 || PREC == PREC_F16F) {   // one product; 4 x (K = 32 bytes) inside the 128-byte swizzle row
-                        const uint64_t a = umma_desc_k128(sa), b = umma_desc_k128(BRES ? smem_u32(bres + kc * C::B_BYTES) : sa + C::B_OFF);
-#pragma unroll
-                        for (uint32_t m = 0; m < MT; m++) {
-                            const uint64_t am = (uint64_t)((m * A1_BYTES) >> 4);
-#pragma unroll
-                            for (uint32_t kk = 0; kk < 4; kk++)          // 4 x K=32 int8 (32 bytes) inside the 128-byte swizzle row
-                                umma<PREC>(d + m * NQ, a + am + (uint64_t)(kk * 2), b + (uint64_t)(kk * 2), idesc, (kc | kk) != 0);
-                        }
-                    } else if (PREC == PREC_TF32) {
-                        const uint64_t a_hi = umma_desc_k128(sa), a_lo = umma_desc_k128(sa + C::ALO_OFF);
-                        const uint64_t b_hi = umma_desc_k128(sa + C::B_OFF), b_lo = umma_desc_k128(sa + C::B_OFF + C::B_BYTES);
-#pragma unroll
-                        for (uint32_t m = 0; m < MT; m++) {
-                            const uint64_t am = (uint64_t)((m * A1_BYTES) >> 4);   // next 128-row tile of the stage
-#pragma unroll
-                            for (uint32_t kk = 0; kk < 4; kk++) {        // 4 x K=8 (32 bytes) inside the 128-byte swizzle row
-                                const uint64_t o = (uint64_t)(kk * 2);  // +32 bytes in 16-byte units
-                                umma<PREC>(d + m * NQ, a_hi + am + o, b_hi + o, idesc, (kc | kk) != 0);
-                                umma<PREC>(d + m * NQ, a_lo + am + o, b_hi + o, idesc, 1);
-                                umma<PREC>(d + m * NQ, a_hi + am + o, b_lo + o, idesc, 1);
-                            }
-                        }
-                    } else {
-                        const uint64_t a1 = umma_desc_k64(sa + C::ALO_OFF), a2 = umma_desc_k64(sa + C::A2_OFF);
-                        const uint64_t b1 = umma_desc_k64(sa + C::B_OFF), b2 = umma_desc_k64(sa + C::B_OFF + C::B_BYTES);
-#pragma unroll
-                        for (uint32_t m = 0; m < MT; m++) {
-                            const uint64_t am = (uint64_t)((m * (A1_BYTES / 2)) >> 4);   // bf16 tile = 8 KB
-#pragma unroll
-                            for (uint32_t kk = 0; kk < 2; kk++) {        // 2 x K=16 bf16 (32 bytes) inside the 64-byte swizzle row
-                                const uint64_t o = (uint64_t)(kk * 2);
-                                umma<PREC>(d + m * NQ, a1 + am + o, b1 + o, idesc, (kc | kk) != 0);
-                                umma<PREC>(d + m * NQ, a2 + am + o, b1 + o, idesc, 1);
-                                umma<PREC>(d + m * NQ, a1 + am + o, b2 + o, idesc, 1);
-                            }
-                        }
-                    }
-                    umma_commit(&empty[s]);                      // stage reusable once these MMAs retire
-                    if (kc + 1 == n_kchunks) umma_commit(&tfull[buf]);
-                }
-            }
-        }
-    } else if (warp >= 8 && PREC == PREC_TF32) {
-        // ===================== splitters (tf32 only): f32 corpus tile -> (hi, lo) operand tiles =====================
-        const int t = threadIdx.x - 256;   // 0..SPLIT_THREADS-1
+    } else {
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+        // ===================== consumers: MMA + epilogue =====================
+        const int cw = (warp - 4) >> 2;          // consumer warpgroup: query columns [cw*NQH, (cw+1)*NQH)
+        const int w = warp & 3;                  // rows 16w..16w+15 of every 64-row sub-tile; list w
+        const int q0 = cw * NQH;
+        uint32_t* xb = xbuf + (warp - 4) * 32 * XB_STRIDE;
+        uint64_t* mylists = lists + (size_t)w * NQ * LIST;
+        if (!sample_mode)
+            for (int i = lane; i < NQH * LIST; i += 32) mylists[q0 * LIST + i] = 0;
+        __syncwarp();
+        uint32_t* gmaxu = (uint32_t*)scratch;     // sample mode: ordered-uint group maxima [gridDim.y * NQ][n_tiles * TROWS / 32]
+        const uint32_t n_rg = n_tiles * (TROWS / 32);
+        AccT acc[MW][NQH / 2];
+        if (BRES) mbar_wait(bfull, 0);
         uint32_t it = 0;
-        for (uint32_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+        for (uint32_t tile = tile0; tile - rank < n_tiles; tile += gridDim.x) {
             for (uint32_t kc = 0; kc < n_kchunks; ++kc, ++it) {
-                uint32_t s = it % STAGES, ph = (it / STAGES) & 1u;
-                mbar_wait(&full[s], ph);
+                const uint32_t s = it % STAGES, ph = (it / STAGES) & 1u;
                 uint8_t* st = stage0 + s * C::STAGE_BYTES;
+                mbar_wait(&full[s], ph);
                 if (PREC == PREC_TF32) {
+                    // f32 corpus tile -> (hi in place, lo) operand tiles, by all 256 consumer threads, then visible to the tensor core
+                    const int t = threadIdx.x - 128;
                     uint4* A = (uint4*)st;
                     uint4* Al = (uint4*)(st + C::ALO_OFF);
 #pragma unroll
-                    for (int j = 0; j < (A_BYTES / 16) / SPLIT_THREADS; j++) {
-                        uint4 x = A[t + SPLIT_THREADS * j], h, l;
+                    for (int j = 0; j < (C::A_BYTES / 16) / 256; j++) {
+                        uint4 x = A[t + 256 * j], h, l;
                         h.x = x.x & 0xFFFFE000u; h.y = x.y & 0xFFFFE000u; h.z = x.z & 0xFFFFE000u; h.w = x.w & 0xFFFFE000u;
                         l.x = __float_as_uint(__uint_as_float(x.x) - __uint_as_float(h.x));
                         l.y = __float_as_uint(__uint_as_float(x.y) - __uint_as_float(h.y));
                         l.z = __float_as_uint(__uint_as_float(x.z) - __uint_as_float(h.z));
                         l.w = __float_as_uint(__uint_as_float(x.w) - __uint_as_float(h.w));
-                        A[t + SPLIT_THREADS * j] = h;
-                        Al[t + SPLIT_THREADS * j] = l;
+                        A[t + 256 * j] = h;
+                        Al[t + 256 * j] = l;
+                    }
+                    fence_proxy_async();          // generic-proxy smem writes -> visible to the tensor core (async proxy)
+                    asm volatile("bar.sync 1, 256;" ::: "memory");
+                }
+                const uint32_t sa = smem_u32(st);
+                const uint32_t sb = (BRES ? smem_u32(bres + kc * C::B_BYTES) : sa + C::B_OFF) + q0 * C::B_ROW;   // this warpgroup's queries
+                wg_fence();
+                if (PREC == PREC_I8 || PREC == PREC_F16F) {   // one product; 4 x 32 bytes of K inside the 128-byte swizzle row
+                    const uint64_t a = gmma_desc_k128(sa), b = gmma_desc_k128(sb);
+#pragma unroll
+                    for (int m = 0; m < MW; m++) {
+                        const uint64_t am = (uint64_t)((m * 64 * 128) >> 4);
+#pragma unroll
+                        for (uint32_t kk = 0; kk < 4; kk++)
+                            mma<PREC, NQH>(acc[m], a + am + (uint64_t)(kk * 2), b + (uint64_t)(kk * 2), (kc | kk) != 0);
+                    }
+                } else if (PREC == PREC_TF32) {
+                    const uint64_t a_hi = gmma_desc_k128(sa), a_lo = gmma_desc_k128(sa + C::ALO_OFF);
+                    const uint64_t b_hi = gmma_desc_k128(sb), b_lo = gmma_desc_k128(sb + C::B_BYTES);
+#pragma unroll
+                    for (int m = 0; m < MW; m++) {
+                        const uint64_t am = (uint64_t)((m * 64 * 128) >> 4);   // next 64-row sub-tile
+#pragma unroll
+                        for (uint32_t kk = 0; kk < 4; kk++) {        // 4 x K=8 (32 bytes) inside the 128-byte swizzle row
+                            const uint64_t o = (uint64_t)(kk * 2);  // +32 bytes in 16-byte units
+                            mma<PREC, NQH>(acc[m], a_hi + am + o, b_hi + o, (kc | kk) != 0);
+                            mma<PREC, NQH>(acc[m], a_lo + am + o, b_hi + o, 1);
+                            mma<PREC, NQH>(acc[m], a_hi + am + o, b_lo + o, 1);
+                        }
+                    }
+                } else {
+                    const uint64_t a1 = gmma_desc_k64(sa + C::ALO_OFF), a2 = gmma_desc_k64(sa + C::A2_OFF);
+                    const uint64_t b1 = gmma_desc_k64(sb), b2 = gmma_desc_k64(sb + C::B_BYTES);
+#pragma unroll
+                    for (int m = 0; m < MW; m++) {
+                        const uint64_t am = (uint64_t)((m * 64 * 64) >> 4);   // bf16 sub-tile = 4 KB
+#pragma unroll
+                        for (uint32_t kk = 0; kk < 2; kk++) {        // 2 x K=16 bf16 (32 bytes) inside the 64-byte swizzle row
+                            const uint64_t o = (uint64_t)(kk * 2);
+                            mma<PREC, NQH>(acc[m], a1 + am + o, b1 + o, (kc | kk) != 0);
+                            mma<PREC, NQH>(acc[m], a2 + am + o, b1 + o, 1);
+                            mma<PREC, NQH>(acc[m], a1 + am + o, b2 + o, 1);
+                        }
                     }
                 }
-                fence_proxy_async();          // generic-proxy smem writes -> visible to the tensor core (async proxy)
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&split[s]);
+                wg_commit();
+                wg_wait<1>();                                  // the previous stage's MMAs retired: release it
+                if (kc > 0 && lane == 0) {
+                    const uint32_t sp = (it - 1) % STAGES;
+                    mbar_arrive(&empty[sp]);
+                    if (PAIR) mbar_arrive_cta(&empty[sp], rank ^ 1u);
+                }
             }
-        }
-    } else if (warp >= 4 && PREC == PREC_I8 && !SCALED) {
-        // ===================== int8 epilogue: 12 warps = 4 TMEM lane quadrants x 3 query-column groups =====================
-        // With the int8 operands the MMA + smem side of a 128-query pass costs a fraction of the HBM time, so the epilogue
-        // (one compare + ballot per (row, query) pair) is what has to keep up: the 8 warps that are splitters in the f32
-        // variants join in.  Warp (quadrant ew, group g) owns the 16-query column chunks c = g, g+3, ... for both M tiles,
-        // and with them the lists (ew, q) of those queries — the scratch layout is the same as in the 4-warp epilogue.
-        const int ew = warp & 3, g = (warp - 4) >> 2;
-        int* thr_i = (int*)thr_u;
-        uint64_t* mylists = lists + (size_t)ew * NQ * LIST;
-        if (!sample_mode)
-            for (int c = g; c < NQ / 16; c += 3)
-                for (int i = lane; i < 16 * LIST; i += 32) mylists[c * 16 * LIST + i] = 0;
-        __syncwarp();
-        // sample mode (threshold seeding): no lists.  Every (tile, m, quadrant) is a group of 32 rows; per query the group's
-        // best score goes to gmax[query][group].  The k-th largest group maximum is a valid lower bound of the k-th best score
-        // (k groups each hold a row at least that good) and, for k << #groups, nearly as tight as an exact k-th of the sample.
-        int* gmax = (int*)scratch;                       // [gridDim.y * NQ][n_tiles * 8]
-        const uint32_t n_rg = n_tiles * (MT * 4);
-        uint32_t ti = 0;
-        for (uint32_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++ti) {
-            const uint32_t buf = ti & 1u, tph = (ti >> 1) & 1u;
-            mbar_wait(&tfull[buf], tph);
-            tc_fence_after();
-            for (int m = 0; m < MT; m++) {
-                const uint32_t row = tile * TROWS + (uint32_t)(m * TM) + (uint32_t)(ew * 32 + lane);
-                const bool valid = row < n_rows;
-                for (int c = g; c < NQ / 16; c += 3) {
-                    uint32_t v[16];
-                    const uint32_t taddr = tmem_base + ((uint32_t)(ew * 32) << 16) + buf * (MT * NQ) + m * NQ + c * 16;
-                    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                                 : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-                                   "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-                                 : "r"(taddr) : "memory");
-                    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                    if (sample_mode) {
-                        int keep = INT_MIN;
+            wg_wait<0>();
+            if (lane == 0) {
+                const uint32_t sp = (it - 1) % STAGES;
+                mbar_arrive(&empty[sp]);
+                if (PAIR) mbar_arrive_cta(&empty[sp], rank ^ 1u);
+            }
 #pragma unroll
-                        for (int j = 0; j < 16; j++) {
-                            int d = valid ? (int)v[j] : INT_MIN;
-                            if (ceil_keys && valid) {   // paging: rows already returned by an earlier page do not count
-                                const uint64_t key = ((uint64_t)ord_f32((float)d) << 32) | (uint64_t)(0xFFFFFFFFu - (doc_ids ? __ldg(&doc_ids[row]) : row));
-                                if (key >= __ldg(&ceil_keys[blockIdx.y * NQ + c * 16 + j])) d = INT_MIN;
+            for (int m = 0; m < MW; m++)
+#pragma unroll
+                for (int i = 0; i < NQH / 2; i++) fence_reg(acc[m][i]);
+
+            // ===================== epilogue: accumulators -> filter -> per-warp per-query top-k (no CTA-level barriers) =====================
+            // The per-query threshold (ordered-uint score of the best k-th entry any warp of the warpgroup has seen, seeded by the
+            // pre-sample pass) is shared through smem with atomicMax: monotone, so stale reads only cost an extra insert.
+            // Fragment of m64nN: register 4j+2h+b of sub-tile m holds row 16w + lane/4 + 8h, column 8j + 2(lane%4) + b.
+#pragma unroll
+            for (int p = 0; p < MW / 2; p++) {                        // 32 rows: lanes 0-15 sub-tile 2p, lanes 16-31 sub-tile 2p+1
+                const uint32_t row = tile * TROWS + (uint32_t)(64 * (2 * p + (lane >> 4)) + 16 * w + (lane & 15));
+                const bool valid = row < n_rows;
+                float rs = 0.f, rn = 0.f;
+                int2 ra = make_int2(0, 0);
+                if (SCALED) {
+                    rs = valid ? __ldg(&row_scale[row]) : 0.f;
+                    rn = (SCALED >= 2 && valid) ? __ldg(&row_norm[row]) : 0.f;
+                    ra = (SCALED == 3 && valid) ? __ldg(&row_aff[row]) : make_int2(0, 0);
+                }
+#pragma unroll
+                for (int jb = 0; jb < NQH / CHUNK; jb++) {
+                    const int c = q0 / CHUNK + jb;                    // 8-query chunk of the block
+                    __syncwarp();
+#pragma unroll
+                    for (int hm = 0; hm < 2; hm++)
+#pragma unroll
+                        for (int h = 0; h < 2; h++) {
+                            uint32_t* d = xb + (hm * 16 + (lane >> 2) + 8 * h) * XB_STRIDE + 2 * (lane & 3);
+                            d[0] = acc_bits(acc[2 * p + hm][4 * jb + 2 * h]);
+                            d[1] = acc_bits(acc[2 * p + hm][4 * jb + 2 * h + 1]);
+                        }
+                    __syncwarp();
+                    uint32_t v[CHUNK];
+#pragma unroll
+                    for (int j = 0; j < CHUNK; j++) {
+                        v[j] = xb[lane * XB_STRIDE + j];
+                        if (PREC == PREC_I8 && !SCALED) v[j] = __float_as_uint((float)(int)v[j]);
+                        if (SCALED) {
+                            // scaled int8: the accumulators are exact int32 dot products; the score is rebuilt with the reference's
+                            // operation order so that it is bit-identical to the CPU path, then treated like an f32 score below
+                            int di = (int)v[j];
+                            if (SCALED == 3) { const int2 qa = __ldg(&q_aff[blockIdx.y * NQ + c * CHUNK + j]); di = di - ra.x * qa.y + qa.x * ra.y; }
+                            const float dotf = __fmul_rn(__fmul_rn((float)di, qs_sm[c * CHUNK + j]), rs);
+                            const float sc = SCALED >= 2 ? -fmaxf(__fsub_rn(__fadd_rn(qn_sm[c * CHUNK + j], rn), __fmul_rn(2.0f, dotf)), 0.0f) : dotf;
+                            v[j] = __float_as_uint(sc);
+                        }
+                    }
+                    if (sample_mode) {
+                        // no lists.  Every (tile, pass, warp) is a group of 32 rows; per query the group's best score goes to
+                        // gmax[query][group].  The k-th largest group maximum is a valid lower bound of the k-th best score (k groups
+                        // each hold a row at least that good) and, for k << #groups, nearly as tight as an exact k-th of the sample.
+                        uint32_t keep = 0;
+#pragma unroll
+                        for (int j = 0; j < CHUNK; j++) {
+                            const float sc = __uint_as_float(v[j]);
+                            uint32_t so = (valid && sc == sc) ? ord_f32(sc) : 0u;
+                            if (ceil_keys && so) {   // paging: rows already returned by an earlier page do not count
+                                const uint64_t key = ((uint64_t)so << 32) | (uint64_t)(0xFFFFFFFFu - (doc_ids ? __ldg(&doc_ids[row]) : row));
+                                if (key >= __ldg(&ceil_keys[blockIdx.y * NQ + c * CHUNK + j])) so = 0u;
                             }
-                            const int mx = __reduce_max_sync(FULL, d);
+                            const uint32_t mx = __reduce_max_sync(FULL, so);
                             if (lane == j) keep = mx;
                         }
-                        if (lane < 16)
-                            gmax[(size_t)(blockIdx.y * NQ + c * 16 + lane) * n_rg + (tile * (MT * 4) + m * 4 + ew)] = keep;
+                        if (lane < CHUNK)
+                            gmaxu[(size_t)(blockIdx.y * NQ + c * CHUNK + lane) * n_rg + (tile * (TROWS / 32) + p * 4 + w)] = keep;
                         continue;
                     }
-                    {   // common case, branch-free: does ANY of the 32 x 16 scores reach its query's threshold?  (ncu: with a
-                        // ballot + branch per column this loop, not HBM, set the tile period)
-                        const int4* t4 = reinterpret_cast<const int4*>(thr_i + c * 16);
-                        const int4 t0 = t4[0], t1 = t4[1], t2 = t4[2], t3 = t4[3];
-                        bool any = ((int)v[0] >= t0.x) | ((int)v[1] >= t0.y) | ((int)v[2] >= t0.z) | ((int)v[3] >= t0.w) |
-                                   ((int)v[4] >= t1.x) | ((int)v[5] >= t1.y) | ((int)v[6] >= t1.z) | ((int)v[7] >= t1.w) |
-                                   ((int)v[8] >= t2.x) | ((int)v[9] >= t2.y) | ((int)v[10] >= t2.z) | ((int)v[11] >= t2.w) |
-                                   ((int)v[12] >= t3.x) | ((int)v[13] >= t3.y) | ((int)v[14] >= t3.z) | ((int)v[15] >= t3.w);
+                    {   // common case, branch-free: one vote per 8-query chunk instead of one per column (a NaN score maps above every
+                        // threshold here and is rejected by the per-column test below)
+                        const uint4* t4 = reinterpret_cast<const uint4*>(thr_u + c * CHUNK);
+                        const uint4 t0 = t4[0], t1 = t4[1];
+                        const bool any = (ord_f32(__uint_as_float(v[0])) >= t0.x) | (ord_f32(__uint_as_float(v[1])) >= t0.y) |
+                                         (ord_f32(__uint_as_float(v[2])) >= t0.z) | (ord_f32(__uint_as_float(v[3])) >= t0.w) |
+                                         (ord_f32(__uint_as_float(v[4])) >= t1.x) | (ord_f32(__uint_as_float(v[5])) >= t1.y) |
+                                         (ord_f32(__uint_as_float(v[6])) >= t1.z) | (ord_f32(__uint_as_float(v[7])) >= t1.w);
                         if (!__any_sync(FULL, any && valid)) continue;
                     }
+                    // rare after warm-up: per column, from the lane's own row of the buffer (a runtime loop keeps one copy of this
+                    // path per chunk)
 #pragma unroll
-                    for (int j = 0; j < 16; j++) {
-                        const int q = c * 16 + j;
-                        const int d = (int)v[j];
-                        const bool pass = valid && d >= thr_i[q];
+                    for (int j = 0; j < CHUNK; j++) xb[lane * XB_STRIDE + j] = v[j];
+#pragma unroll 1
+                    for (int j = 0; j < CHUNK; j++) {
+                        const int q = c * CHUNK + j;
+                        const float sc = __uint_as_float(xb[lane * XB_STRIDE + j]);
+                        const uint32_t so = ord_f32(sc);
+                        const bool pass = valid && sc == sc && so >= thr_u[q];
                         unsigned pm = __ballot_sync(FULL, pass);
-                        if (pm) {                                           // rare after warm-up
-                            uint64_t key = 0;
-                            if (pass) {
-                                const uint32_t doc = doc_ids ? __ldg(&doc_ids[row]) : row;
-                                key = ((uint64_t)ord_f32((float)d) << 32) | (uint64_t)(0xFFFFFFFFu - doc);   // dot_i8 as f32: exact below 2^24
-                                if (doc_deleted(del_slot, del_words, doc)) key = 0;
-                            }
-                            if (ceil_keys || del_slot) {
-                                if (ceil_keys) { const uint64_t ceil = __ldg(&ceil_keys[blockIdx.y * NQ + q]); if (key >= ceil) key = 0; }
-                                pm = __ballot_sync(FULL, key != 0);
-                                if (!pm) continue;
-                            }
-                            uint64_t L = mylists[q * LIST + lane];
-                            if (__popc(pm) > 3) {
-                                L = wl_merge(L, wl_sort_desc(key, lane), lane);
-                            } else {
-                                while (pm) { const int src = __ffs(pm) - 1; pm &= pm - 1; wl_insert(L, shfl64(key, src), lane); }
-                            }
-                            mylists[q * LIST + lane] = L;
-                            const uint32_t kth = (uint32_t)(shfl64(L, (int)k - 1) >> 32);
-                            if (lane == 0 && kth) atomicMax(&thr_i[q], ord_to_int(kth));
-                        }
-                    }
-                }
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&tempty[buf]);
-        }
-    } else if (warp >= 4 && (warp < 8 || PREC != PREC_TF32)) {
-        // ===================== epilogue: TMEM -> filter -> per-warp per-query top-k (no CTA-level barriers) =====================
-        // Each epilogue warp owns the 32 TMEM lanes (= corpus rows) of its quadrant and keeps its own sorted list per
-        // query.  The per-query threshold (ordered-uint score of the best k-th entry any warp of the CTA has seen, seeded
-        // by the pre-sample pass) is shared through smem with atomicMax: monotone, so stale reads only cost an extra
-        // insert.  (An earlier version pushed candidates into per-query buckets with two CTA-wide named barriers per
-        // 8-query chunk and inserted them one by one: the dependent-shuffle insert chain made the epilogue, not the
-        // tensor pipe, the limiter.)
-        // Except in the tf32 variant (warps 8-15 are its splitters) all 12 warps 4-15 run the epilogue: quadrant ew = warp % 4, column group
-        // g = (warp - 4) / 4 owns the 8-query chunks c = g, g + 3, ... of both M tiles and with them the lists (ew, q) of those queries —
-        // same scratch layout as with 4 warps.  A candidate insert is a dependent global (L2) load + shuffle insert + store, ~1 us of pure
-        // latency for the warp: with one warp per quadrant those inserts, not the tensor pipe or HBM, set the tile period of the filter scan.
-        constexpr int EG = PREC == PREC_TF32 ? 1 : 3;
-        constexpr int NCH3 = (NQ / CHUNK + EG - 1) / EG * EG;   // chunk slots per M tile, rounded up to a multiple of EG so that mc % EG == c % EG
-        const int ew = warp & 3, g = (warp - 4) >> 2;
-        uint64_t* mylists = lists + (size_t)ew * NQ * LIST;
-        if (!sample_mode)
-            for (int c = g; c < NQ / CHUNK; c += EG)
-                for (int i = lane; i < CHUNK * LIST; i += 32) mylists[c * CHUNK * LIST + i] = 0;
-        __syncwarp();
-        uint32_t* gmaxu = (uint32_t*)scratch;            // sample mode (see the int8 epilogue): ordered-uint group maxima
-        const uint32_t n_rg = n_tiles * (MT * 4);
-        uint32_t ti = 0;
-        for (uint32_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++ti) {
-            const uint32_t buf = ti & 1u, tph = (ti >> 1) & 1u;
-            mbar_wait(&tfull[buf], tph);
-            tc_fence_after();
-            for (int mc = g; mc < MT * NCH3; mc += EG) {             // chunk c of either M tile belongs to warp group c % EG (list ownership)
-                const int m = mc / NCH3, c = mc % NCH3;
-                if (c >= NQ / CHUNK) continue;                        // padding slot of the rounded-up chunk count
-                const uint32_t row = tile * TROWS + (uint32_t)(m * TM) + (uint32_t)(ew * 32 + lane);
-                const bool valid = row < n_rows;
-                uint32_t v[CHUNK];
-                const uint32_t taddr = tmem_base + ((uint32_t)(ew * 32) << 16) + buf * (MT * NQ) + m * NQ + c * CHUNK;
-                asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                             : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-                             : "r"(taddr) : "memory");
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                if (SCALED) {
-                    // scaled int8: the accumulators are exact int32 dot products; the score is rebuilt with the reference's
-                    // operation order so that it is bit-identical to the CPU path, then treated like an f32 score below
-                    const float rs = valid ? __ldg(&row_scale[row]) : 0.f;
-                    const float rn = (SCALED >= 2 && valid) ? __ldg(&row_norm[row]) : 0.f;
-                    const int2 ra = (SCALED == 3 && valid) ? __ldg(&row_aff[row]) : make_int2(0, 0);
-#pragma unroll
-                    for (int j = 0; j < CHUNK; j++) {
-                        int di = (int)v[j];
-                        if (SCALED == 3) { const int2 qa = __ldg(&q_aff[blockIdx.y * NQ + c * CHUNK + j]); di = di - ra.x * qa.y + qa.x * ra.y; }
-                        const float dotf = __fmul_rn(__fmul_rn((float)di, qs_sm[c * CHUNK + j]), rs);
-                        const float sc = SCALED >= 2 ? -fmaxf(__fsub_rn(__fadd_rn(qn_sm[c * CHUNK + j], rn), __fmul_rn(2.0f, dotf)), 0.0f) : dotf;
-                        v[j] = __float_as_uint(sc);
-                    }
-                }
-                if (sample_mode) {
-                    uint32_t keep = 0;
-#pragma unroll
-                    for (int j = 0; j < CHUNK; j++) {
-                        const float sc = __uint_as_float(v[j]);
-                        uint32_t so = (valid && sc == sc) ? ord_f32(sc) : 0u;
-                        if (ceil_keys && so) {
-                            const uint64_t key = ((uint64_t)so << 32) | (uint64_t)(0xFFFFFFFFu - (doc_ids ? __ldg(&doc_ids[row]) : row));
-                            if (key >= __ldg(&ceil_keys[blockIdx.y * NQ + c * CHUNK + j])) so = 0u;
-                        }
-                        const uint32_t mx = __reduce_max_sync(FULL, so);
-                        if (lane == j) keep = mx;
-                    }
-                    if (lane < CHUNK)
-                        gmaxu[(size_t)(blockIdx.y * NQ + c * CHUNK + lane) * n_rg + (tile * (MT * 4) + m * 4 + ew)] = keep;
-                    continue;
-                }
-                {   // common case, branch-free: one vote per 8-query chunk instead of one per column (a NaN score maps above every
-                    // threshold here and is rejected by the per-column test below)
-                    const uint4* t4 = reinterpret_cast<const uint4*>(thr_u + c * CHUNK);
-                    const uint4 t0 = t4[0], t1 = t4[1];
-                    const bool any = (ord_f32(__uint_as_float(v[0])) >= t0.x) | (ord_f32(__uint_as_float(v[1])) >= t0.y) |
-                                     (ord_f32(__uint_as_float(v[2])) >= t0.z) | (ord_f32(__uint_as_float(v[3])) >= t0.w) |
-                                     (ord_f32(__uint_as_float(v[4])) >= t1.x) | (ord_f32(__uint_as_float(v[5])) >= t1.y) |
-                                     (ord_f32(__uint_as_float(v[6])) >= t1.z) | (ord_f32(__uint_as_float(v[7])) >= t1.w);
-                    if (!__any_sync(FULL, any && valid)) continue;
-                }
-#pragma unroll
-                for (int j = 0; j < CHUNK; j++) {
-                    const int q = c * CHUNK + j;
-                    const float sc = __uint_as_float(v[j]);
-                    const uint32_t so = ord_f32(sc);
-                    const bool pass = valid && sc == sc && so >= thr_u[q];
-                    unsigned pm = __ballot_sync(FULL, pass);
-                    if (pm) {                                           // rare after warm-up
+                        if (!pm) continue;
                         uint64_t key = 0;
                         if (pass) {
                             const uint32_t doc = doc_ids ? __ldg(&doc_ids[row]) : row;
@@ -521,211 +558,10 @@ scan_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtenso
                     }
                 }
             }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&tempty[buf]);
         }
     }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)C::TMEM_COLS) : "memory");
-    }
-}
-
-// ------------------------------------------------------------------------------------------------------------------------------------
-// scan_tc2 — the 256-query filter scan on CTA PAIRS (tcgen05 cta_group::2, thread-block cluster of 2).
-// The one-CTA 256-query pass is bounded by what an SM can take in from L2: per 64-dim stage 16 KB of corpus + 32 KB of the query block
-// at ~64 B/clk (ncu: 374 us against an HBM time of 234 us).  A pair of SMs shares ONE copy of the query block: each CTA loads its own
-// 128 corpus rows (A, 16 KB) and HALF of the 256 queries (B, 16 KB) per stage, the leader's single thread issues M = 256 x N = 256 MMAs
-// that read both halves (the peer's through the pair's shared-memory path), and every SM takes in 32 KB per stage instead of 48.
-// Pipelines as in scan_tc; what changes: both CTAs' TMA loads complete on the LEADER's full barrier (cta_group::2 loads, peer bit of the
-// barrier address cleared), tcgen05.commit is multicast to both CTAs' empty / tfull barriers, the epilogue warps of BOTH CTAs arrive on
-// the leader's tempty barrier, TMEM is allocated with cta_group::2.  Filter precision only (PREC_F16F, NQ = 256); the threshold-seeding
-// sample pass stays on scan_tc<256, F16F>.
-constexpr uint32_t PEER_MASK = 0xFEFFFFFFu;        // shared::cluster address -> the same offset in the pair's even (leader) CTA
-struct Cfg2 {
-    static constexpr int NQ = 256, NQH = 128;
-    static constexpr int A_BYTES = TM * 128;           // 128 rows x 64 halves
-    static constexpr int B_BYTES = NQH * 128;          // this CTA's half of the query block
-    static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;   // 32 KB
-    static constexpr int STAGES = 6;
-    static constexpr int SMEM = STAGES * STAGE_BYTES + NQ * 12 + 256;
-    static constexpr int TMEM_COLS = 2 * NQ;            // double-buffered [128 lanes x 256 columns] per CTA
-};
-__device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tma_load_2d_pair(void* dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar_in_leader) {
-    asm volatile("cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-                 ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar_in_leader) & PEER_MASK), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar) {   // arrives on `bar` in BOTH CTAs once the MMAs issued so far retire
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(smem_u32(bar)), "h"((uint16_t)3) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_leader(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(smem_u32(bar) & PEER_MASK) : "memory");
-}
-
-__global__ void __launch_bounds__(THREADS, 1)
-scan_tc2(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, uint32_t n_rows, uint32_t n_kchunks, uint32_t n_pairs, uint32_t k,
-         const uint32_t* __restrict__ doc_ids, uint64_t* __restrict__ scratch /*[gridDim.y][gridDim.x*4][256][32]*/,
-         const uint32_t* __restrict__ thr_init, uint32_t nq_valid, const uint32_t* __restrict__ del_slot, const uint64_t* __restrict__ del_words,
-         const float* __restrict__ q_margin, const uint32_t* __restrict__ ivf_sel, uint32_t ivf_words, const uint32_t* __restrict__ row_cluster) {
-    using C = Cfg2;
-    constexpr int NQ = C::NQ;
-    extern __shared__ __align__(1024) uint8_t base[];
-    uint8_t* stage0 = base;
-    uint64_t* lists = scratch + ((size_t)blockIdx.y * gridDim.x + blockIdx.x) * 4 * NQ * LIST;
-    uint32_t* thr_u = (uint32_t*)(base + C::STAGES * C::STAGE_BYTES);
-    float* qs_sm = (float*)(thr_u + NQ);
-    uint64_t* bars = (uint64_t*)(thr_u + 3 * NQ);
-    uint64_t* full = bars;                     // [STAGES]  (used in the leader only)
-    uint64_t* empty = full + MAX_STAGES;       // [STAGES]
-    uint64_t* tfull = empty + MAX_STAGES;      // [2]
-    uint64_t* tempty = tfull + 2;              // [2]       (used in the leader only: 24 arrivals = 12 epilogue warps x 2 CTAs)
-    uint32_t* tmem_slot = (uint32_t*)(tempty + 2);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t rank = cluster_ctarank();
-    const uint32_t pair0 = blockIdx.x >> 1, n_clusters = gridDim.x >> 1;
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < C::STAGES; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-        for (int b = 0; b < 2; b++) { mbar_init(&tfull[b], 1); mbar_init(&tempty[b], 24); }
-        fence_mbar_init();
-    }
-    for (int i = threadIdx.x; i < NQ; i += THREADS) {
-        thr_u[i] = blockIdx.y * NQ + i >= nq_valid ? 0xFFFFFFFFu : (thr_init ? __ldg(&thr_init[blockIdx.y * NQ + i]) : 0u);
-        qs_sm[i] = __ldg(&q_margin[blockIdx.y * NQ + i]);
-    }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"((uint32_t)C::TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();                                  // both CTAs' barriers are initialised before anything arrives on them
-    tc_fence_after();
-    const uint32_t tmem_base = *(volatile uint32_t*)tmem_slot;
-
-    if (warp == 0) {
-        // ===================== TMA producer (both CTAs): own corpus rows + own half of the query block =====================
-        if (lane == 0) {
-            tma_prefetch_desc(&tmA); tma_prefetch_desc(&tmB);
-            uint32_t it = 0;
-            for (uint32_t pr = pair0; pr < n_pairs; pr += n_clusters) {
-                for (uint32_t kc = 0; kc < n_kchunks; ++kc, ++it) {
-                    const uint32_t s = it % C::STAGES, ph = (it / C::STAGES) & 1u;
-                    uint8_t* st = stage0 + s * C::STAGE_BYTES;
-                    mbar_wait(&empty[s], ph ^ 1u);
-                    if (rank == 0) mbar_arrive_expect_tx(&full[s], 2 * C::STAGE_BYTES);       // the bytes of both CTAs land on the leader's barrier
-                    tma_load_2d_pair(st, &tmA, (int)(kc * 64), (int)((pr * 2 + rank) * TM), &full[s]);
-                    tma_load_2d_pair(st + C::A_BYTES, &tmB, (int)(kc * 64), (int)(blockIdx.y * NQ + rank * C::NQH), &full[s]);
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // ===================== MMA issuer: one thread of the LEADER CTA, M = 256 (128 rows per CTA) x N = 256 =====================
-        if (lane == 0 && rank == 0) {
-            const uint32_t idesc = (1u << 4) | (0u << 7) | (0u << 10) | ((uint32_t)(NQ >> 3) << 17) | ((uint32_t)((2 * TM) >> 4) << 24);
-            uint32_t it = 0, ti = 0;
-            for (uint32_t pr = pair0; pr < n_pairs; pr += n_clusters, ++ti) {
-                const uint32_t buf = ti & 1u, tph = (ti >> 1) & 1u;
-                mbar_wait(&tempty[buf], tph ^ 1u);
-                tc_fence_after();
-                const uint32_t d = tmem_base + buf * NQ;
-                for (uint32_t kc = 0; kc < n_kchunks; ++kc, ++it) {
-                    const uint32_t s = it % C::STAGES, ph = (it / C::STAGES) & 1u;
-                    mbar_wait(&full[s], ph);
-                    tc_fence_after();
-                    const uint32_t sa = smem_u32(stage0 + s * C::STAGE_BYTES);
-                    const uint64_t a = umma_desc_k128(sa), b = umma_desc_k128(sa + C::A_BYTES);
-#pragma unroll
-                    for (uint32_t kk = 0; kk < 4; kk++)
-                        asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\ntcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n}\n"
-                                     ::"r"(d), "l"(a + (uint64_t)(kk * 2)), "l"(b + (uint64_t)(kk * 2)), "r"(idesc), "r"((uint32_t)((kc | kk) != 0)) : "memory");
-                    umma_commit_pair(&empty[s]);
-                    if (kc + 1 == n_kchunks) umma_commit_pair(&tfull[buf]);
-                }
-            }
-        }
-    } else if (warp >= 4) {
-        // ===================== epilogue (both CTAs, 12 warps each): the f32 epilogue of scan_tc for MT = 1, filter margins =====================
-        constexpr int EG = 3;
-        constexpr int NCH3 = (NQ / CHUNK + EG - 1) / EG * EG;
-        const int ew = warp & 3, g = (warp - 4) >> 2;
-        uint64_t* mylists = lists + (size_t)ew * NQ * LIST;
-        for (int c = g; c < NQ / CHUNK; c += EG)
-            for (int i = lane; i < CHUNK * LIST; i += 32) mylists[c * CHUNK * LIST + i] = 0;
-        __syncwarp();
-        uint32_t ti = 0;
-        for (uint32_t pr = pair0; pr < n_pairs; pr += n_clusters, ++ti) {
-            const uint32_t buf = ti & 1u, tph = (ti >> 1) & 1u;
-            mbar_wait(&tfull[buf], tph);
-            tc_fence_after();
-            const uint32_t row = (pr * 2 + rank) * TM + (uint32_t)(ew * 32 + lane);
-            const bool valid = row < n_rows;
-            for (int c = g; c < NCH3; c += EG) {
-                if (c >= NQ / CHUNK) continue;
-                uint32_t v[CHUNK];
-                const uint32_t taddr = tmem_base + ((uint32_t)(ew * 32) << 16) + buf * NQ + c * CHUNK;
-                asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                             : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-                             : "r"(taddr) : "memory");
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                {
-                    const uint4* t4 = reinterpret_cast<const uint4*>(thr_u + c * CHUNK);
-                    const uint4 t0 = t4[0], t1 = t4[1];
-                    const bool any = (ord_f32(__uint_as_float(v[0])) >= t0.x) | (ord_f32(__uint_as_float(v[1])) >= t0.y) |
-                                     (ord_f32(__uint_as_float(v[2])) >= t0.z) | (ord_f32(__uint_as_float(v[3])) >= t0.w) |
-                                     (ord_f32(__uint_as_float(v[4])) >= t1.x) | (ord_f32(__uint_as_float(v[5])) >= t1.y) |
-                                     (ord_f32(__uint_as_float(v[6])) >= t1.z) | (ord_f32(__uint_as_float(v[7])) >= t1.w);
-                    if (!__any_sync(FULL, any && valid)) continue;
-                }
-#pragma unroll
-                for (int j = 0; j < CHUNK; j++) {
-                    const int q = c * CHUNK + j;
-                    const float sc = __uint_as_float(v[j]);
-                    const uint32_t so = ord_f32(sc);
-                    const bool pass = valid && sc == sc && so >= thr_u[q];
-                    unsigned pm = __ballot_sync(FULL, pass);
-                    if (pm) {
-                        uint64_t key = 0;
-                        if (pass) {
-                            const uint32_t doc = doc_ids ? __ldg(&doc_ids[row]) : row;
-                            key = ((uint64_t)so << 32) | (uint64_t)(0xFFFFFFFFu - row);          // filter scan: candidates are named by row
-                            if (doc_deleted(del_slot, del_words, doc) || ivf_skipped(ivf_sel, ivf_words, blockIdx.y * NQ + q, row_cluster, row)) key = 0;
-                        }
-                        if (del_slot || ivf_sel) { pm = __ballot_sync(FULL, key != 0); if (!pm) continue; }
-                        uint64_t L = mylists[q * LIST + lane];
-                        if (__popc(pm) > 3) L = wl_merge(L, wl_sort_desc(key, lane), lane);
-                        else while (pm) { const int src = __ffs(pm) - 1; pm &= pm - 1; wl_insert(L, shfl64(key, src), lane); }
-                        mylists[q * LIST + lane] = L;
-                        uint32_t kth = (uint32_t)(shfl64(L, (int)k - 1) >> 32);
-                        if (kth) kth = ord_f32(__fsub_rd(unord_f32(kth), qs_sm[q]));
-                        if (lane == 0 && kth > thr_u[q]) atomicMax(&thr_u[q], kth);
-                    }
-                }
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive_leader(&tempty[buf]);
-        }
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();                                  // the peer may still be reading this CTA's shared memory / arriving on its barriers
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)C::TMEM_COLS) : "memory");
-    }
+    // a pair: the peer may still be multicasting into this CTA's shared memory / arriving on its barriers
+    if (PAIR) cluster_sync_all();
 }
 
 // [nq_pad][dpad] f32 -> hi / lo parts: tf32 (f32 containers) or bf16
@@ -737,7 +573,7 @@ __global__ void split_queries_tf32(const float* __restrict__ q, float* __restric
     lo[i] = __uint_as_float(x) - __uint_as_float(h);
 }
 // queries [nq][dims] f32 -> padded, (Cosine:) L2-normalised exactly like prep_queries (vec_scan.cu), split into bf16 hi / lo parts:
-// one launch instead of prep_queries + split (the per-batch launch chain is what limits small shards, SCALE_r01)
+// one launch instead of prep_queries + split
 __global__ void prep_split_queries_bf16(const float* __restrict__ q, uint32_t nq, uint32_t dims, uint64_t qstride,
                                         __nv_bfloat16* __restrict__ hi, __nv_bfloat16* __restrict__ lo, uint32_t nq_pad, uint32_t dpad, int normalize,
                                         float* __restrict__ f32_out /*filter scan: padded f32 queries for the refine step, else null*/,
@@ -876,9 +712,10 @@ kth_from_groupmax(const int* __restrict__ gmax, uint32_t n_rg, uint32_t nq, uint
 
 }  // namespace tc
 
-template <int NQ, int PREC, bool BRES = false, int SCALED = 0>
+template <int NQ, int PREC, bool BRES = false, int SCALED = 0, bool PAIR = false>
 static int32_t launch_tc_n(const ScanArgs& a, cudaStream_t st) {
     using C = tc::Cfg<NQ, PREC, BRES>;
+    static_assert(!PAIR || (NQ == 256 && PREC == tc::PREC_F16F && !BRES), "CTA pairs run the 256-query filter scan only");
     CUtensorMap tmA, tmA2, tmBh, tmBl;
     uint32_t n_tiles = (uint32_t)((a.n_rows + C::TROWS - 1) / C::TROWS);
     uint32_t n_groups = a.nq_pad / NQ;
@@ -897,47 +734,57 @@ static int32_t launch_tc_n(const ScanArgs& a, cudaStream_t st) {
         tmA2 = tmA;
         if (!a.thr_init) tc::split_queries_tf32<<<(unsigned)((nel + 255) / 256), 256, 0, st>>>(a.queries_padded, a.q_hi, a.q_lo, nel);
     } else if constexpr (PREC == tc::PREC_F16F) {
-        // filter scan: fp16 plane and fp16 queries only, 64 halves (128 bytes) per swizzle row; the box may run past dpad (zero fill)
-        if (!a.rows_h16 || !a.q_scale) { set_error("tcgen05 filter scan: the index holds no fp16 plane / no margins"); return SSB_E_STATE; }
+        // filter scan: fp16 plane and fp16 queries only, 64 halves (128 bytes) per swizzle row; the box may run past dpad (zero fill).
+        // A pair loads the query block in two halves, one per CTA.
+        if (!a.rows_h16 || !a.q_scale) { set_error("tensor-core filter scan: the index holds no fp16 plane / no margins"); return SSB_E_STATE; }
         SSB_TRY(encode_tmap_2d(&tmA, a.rows_h16, 2 /*fp16: 2-byte elements*/, a.dpad, a.n_rows, (uint64_t)a.dpad * 2, 64, C::TROWS, 128));
-        SSB_TRY(encode_tmap_2d(&tmBh, a.q_hi, 2, a.dpad, a.nq_pad, (uint64_t)a.dpad * 2, 64, NQ, 128));
+        SSB_TRY(encode_tmap_2d(&tmBh, a.q_hi, 2, a.dpad, a.nq_pad, (uint64_t)a.dpad * 2, 64, PAIR ? NQ / 2 : NQ, 128));
         tmBl = tmBh; tmA2 = tmA;
         n_kchunks = (a.dpad + 63) / 64;
     } else {
         // corpus: the two bf16 planes written at load time; queries: the two bf16 parts live in the q_hi / q_lo buffers (half of
         // each is used) and were written by prep_split_queries_bf16 (launch_prep_split_queries_bf16)
-        if (!a.rows_hi || !a.rows_lo) { set_error("tcgen05 bf16 scan: the index holds no bf16 planes"); return SSB_E_STATE; }
+        if (!a.rows_hi || !a.rows_lo) { set_error("tensor-core bf16 scan: the index holds no bf16 planes"); return SSB_E_STATE; }
         SSB_TRY(encode_tmap_2d(&tmA, a.rows_hi, 2 /*bf16*/, a.dpad, a.n_rows, (uint64_t)a.dpad * 2, tc::KC, C::TROWS, 64));
         SSB_TRY(encode_tmap_2d(&tmA2, a.rows_lo, 2 /*bf16*/, a.dpad, a.n_rows, (uint64_t)a.dpad * 2, tc::KC, C::TROWS, 64));
         SSB_TRY(encode_tmap_2d(&tmBh, a.q_hi, 2 /*bf16*/, a.dpad, a.nq_pad, (uint64_t)a.dpad * 2, tc::KC, NQ, 64));
         SSB_TRY(encode_tmap_2d(&tmBl, a.q_lo, 2 /*bf16*/, a.dpad, a.nq_pad, (uint64_t)a.dpad * 2, tc::KC, NQ, 64));
     }
+    // one CTA per SM at most; a pair per two SMs, both CTAs of a pair on the tiles of one pair of neighbouring tiles
     uint32_t gx = n_tiles < (uint32_t)a.n_sms ? n_tiles : (uint32_t)a.n_sms;
+    if (PAIR) {
+        uint32_t n_pairs = (n_tiles + 1) / 2, n_clusters = (uint32_t)a.n_sms / 2;
+        gx = 2 * (n_pairs < n_clusters ? n_pairs : n_clusters);
+    }
     if ((size_t)n_groups * gx * 4 * NQ * LIST * 8 > a.scratch_bytes) { set_error("vector scan scratch too small"); return SSB_E_STATE; }
-    constexpr int SMEM_MAX = 232448;   // 227 KB opt-in limit per CTA
     uint32_t nst = C::STAGES;
     int smem = C::SMEM;
-    if (BRES) {   // resident query block + as many corpus stages as fit (launch_scan_tc_impl guarantees >= 3)
-        const int fixed = (int)n_kchunks * C::B_BYTES + NQ * 12 + 256;
-        nst = (uint32_t)((SMEM_MAX - fixed) / C::STAGE_BYTES);
+    if (BRES) {   // resident query block + as many corpus stages as fit (tc::i8_resident guarantees >= 3)
+        const int fixed = (int)n_kchunks * C::B_BYTES + C::FIXED;
+        nst = (uint32_t)((tc::SMEM_MAX - fixed) / C::STAGE_BYTES);
         if (nst > (uint32_t)tc::MAX_STAGES) nst = tc::MAX_STAGES;
         smem = fixed + (int)nst * C::STAGE_BYTES;
     }
+    auto kern = tc::scan_tc<NQ, PREC, BRES, SCALED, PAIR>;
     // per launch, not once per process: the opt-in applies to the CURRENT device's context only (ssb_config.device allows
     // several indexes on different GPUs in one process); the call is a cheap host-side attribute write
-    SSB_CUDA_TRY(cudaFuncSetAttribute(tc::scan_tc<NQ, PREC, BRES, SCALED>, cudaFuncAttributeMaxDynamicSharedMemorySize, BRES ? SMEM_MAX : C::SMEM));
+    SSB_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, BRES ? tc::SMEM_MAX : C::SMEM));
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3(gx, n_groups); cfg.blockDim = dim3(tc::THREADS); cfg.dynamicSmemBytes = (size_t)smem; cfg.stream = st;
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = PAIR ? 2 : 1; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
+    cfg.attrs = at; cfg.numAttrs = PAIR ? 1 : 0;
     if (a.ev0) cudaEventRecord(a.ev0, st);
-    tc::scan_tc<NQ, PREC, BRES, SCALED><<<dim3(gx, n_groups), tc::THREADS, smem, st>>>(tmA, tmA2, tmBh, tmBl, (uint32_t)a.n_rows, n_kchunks, n_tiles,
-                                                                             a.k, a.doc_ids, a.scratch, a.thr_init, a.nq_valid ? a.nq_valid : a.nq_pad, a.ceil_keys, nst,
-                                                                             a.del_slot, a.del_words, a.row_scale, a.row_norm, a.q_scale, a.q_norm,
-                                                                             (const int2*)a.row_aff, (const int2*)a.q_aff,
-                                                                             PREC == tc::PREC_I8 ? nullptr : a.ivf_sel, a.ivf_words, a.row_cluster,
-                                                                             a.sample_groupmax ? 1u : 0u);
+    SSB_CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, tmA, tmA2, tmBh, tmBl, (uint32_t)a.n_rows, n_kchunks, n_tiles,
+                                    a.k, a.doc_ids, a.scratch, a.thr_init, a.nq_valid ? a.nq_valid : a.nq_pad, a.ceil_keys, nst,
+                                    a.del_slot, a.del_words, a.row_scale, a.row_norm, a.q_scale, a.q_norm,
+                                    (const int2*)a.row_aff, (const int2*)a.q_aff,
+                                    PREC == tc::PREC_I8 ? nullptr : a.ivf_sel, a.ivf_words, a.row_cluster,
+                                    a.sample_groupmax ? 1u : 0u));
     if (a.ev1) cudaEventRecord(a.ev1, st);
-    SSB_CUDA_TRY(cudaGetLastError());
-    if (a.sample_groupmax) {   // threshold seeding pass: scratch holds gmax[nq_pad][n_tiles * 8]
-        tc::kth_from_groupmax<<<a.nq_pad, 256, 0, st>>>((const int*)a.scratch, n_tiles * (C::MT * 4), a.nq_pad, a.k, a.thr_buf,
-                                                                      (PREC == tc::PREC_I8 && !SCALED) ? 1 : 0, PREC == tc::PREC_F16F ? a.q_scale : nullptr);
+    if (a.sample_groupmax) {   // threshold seeding pass: scratch holds gmax[nq_pad][n_tiles * TROWS / 32]
+        tc::kth_from_groupmax<<<a.nq_pad, 256, 0, st>>>((const int*)a.scratch, n_tiles * (C::TROWS / 32), a.nq_pad, a.k, a.thr_buf,
+                                                        0, PREC == tc::PREC_F16F ? a.q_scale : nullptr);
         SSB_CUDA_TRY(cudaGetLastError());
         if (a.launches) *a.launches += PREC == tc::PREC_TF32 ? 3 : 2;   // (tf32 query split +) scan + kth
         return SSB_OK;
@@ -949,56 +796,29 @@ static int32_t launch_tc_n(const ScanArgs& a, cudaStream_t st) {
     return SSB_OK;
 }
 
-// 256-query filter scan on CTA pairs (scan_tc2): thread-block clusters of 2, one pair per 256 corpus rows and k-chunk
-static int32_t launch_tc2(const ScanArgs& a, cudaStream_t st) {
-    using C = tc::Cfg2;
-    if (!a.rows_h16 || !a.q_scale) { set_error("tcgen05 filter scan: the index holds no fp16 plane / no margins"); return SSB_E_STATE; }
-    if (a.nq_pad % C::NQ != 0) { set_error("tcgen05 pair scan: query count must be padded to 256"); return SSB_E_INVALID; }
-    CUtensorMap tmA, tmB;
-    SSB_TRY(encode_tmap_2d(&tmA, a.rows_h16, 2, a.dpad, a.n_rows, (uint64_t)a.dpad * 2, 64, tc::TM, 128));
-    SSB_TRY(encode_tmap_2d(&tmB, a.q_hi, 2, a.dpad, a.nq_pad, (uint64_t)a.dpad * 2, 64, C::NQH, 128));
-    const uint32_t n_kchunks = (a.dpad + 63) / 64, n_groups = a.nq_pad / C::NQ;
-    const uint32_t n_pairs = (uint32_t)((a.n_rows + 2 * tc::TM - 1) / (2 * tc::TM));
-    uint32_t n_clusters = (uint32_t)a.n_sms / 2;
-    if (n_clusters > n_pairs) n_clusters = n_pairs;
-    const uint32_t gx = 2 * n_clusters;
-    if ((size_t)n_groups * gx * 4 * C::NQ * LIST * 8 > a.scratch_bytes) { set_error("vector scan scratch too small"); return SSB_E_STATE; }
-    SSB_CUDA_TRY(cudaFuncSetAttribute(tc::scan_tc2, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM));
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(gx, n_groups); cfg.blockDim = dim3(tc::THREADS); cfg.dynamicSmemBytes = C::SMEM; cfg.stream = st;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-    cfg.attrs = at; cfg.numAttrs = 1;
-    if (a.ev0) cudaEventRecord(a.ev0, st);
-    SSB_CUDA_TRY(cudaLaunchKernelEx(&cfg, tc::scan_tc2, tmA, tmB, (uint32_t)a.n_rows, n_kchunks, n_pairs, a.k, a.doc_ids, a.scratch, a.thr_init,
-                                    a.nq_valid ? a.nq_valid : a.nq_pad, a.del_slot, a.del_words, a.q_scale, a.ivf_sel, a.ivf_words, a.row_cluster));
-    if (a.ev1) cudaEventRecord(a.ev1, st);
-    merge_lists_generic(a.scratch, gx * 4, C::NQ, a.nq_pad, a.keys_out, st);
-    SSB_CUDA_TRY(cudaGetLastError());
-    if (a.launches) *a.launches += 2;
-    return SSB_OK;
-}
-
 static int32_t launch_scan_tc_impl(const ScanArgs& a, uint32_t nq_tile, int prec /*0 tf32, 1 bf16, 2 int8, 3 fp16 filter, 4 fp16 filter on CTA pairs*/, cudaStream_t st) {
     if (a.n_rows == 0 || a.nq_pad == 0) return SSB_OK;
-    if (prec == 4) return a.sample_groupmax ? launch_tc_n<256, tc::PREC_F16F>(a, st) : launch_tc2(a, st);   // the seeding pass stays on one CTA per SM
+    if (prec == 4) {   // the seeding pass stays on one CTA per SM
+        if (a.nq_pad % 256 != 0) { set_error("tensor-core pair scan: query count must be padded to 256"); return SSB_E_INVALID; }
+        return a.sample_groupmax ? launch_tc_n<256, tc::PREC_F16F>(a, st) : launch_tc_n<256, tc::PREC_F16F, false, 0, true>(a, st);
+    }
     if (prec == 2) {
         if (nq_tile != 128 || a.nq_pad % 128 != 0 || !a.rows_i8 || !a.queries_i8 || a.dpad8 % 128) { set_error("int8 scan: bad arguments"); return SSB_E_INVALID; }
-        // query block resident in smem when it leaves room for >= 3 corpus stages (dims <= 1024), else streamed per stage
+        const bool res = tc::i8_resident(a.dpad8);   // query block resident in smem when it leaves room for >= 3 corpus stages, else streamed per stage
         if (a.i8_scaled) {
             if (!a.row_scale || !a.q_scale || (a.i8_scaled >= 2 && (!a.row_norm || !a.q_norm)) || (a.i8_scaled == 3 && (!a.row_aff || !a.q_aff))) { set_error("scaled int8 scan: missing scale / norm arrays"); return SSB_E_INVALID; }
-            if (a.i8_scaled == 3) return a.dpad8 <= 1024 ? launch_tc_n<128, tc::PREC_I8, true, 3>(a, st) : launch_tc_n<128, tc::PREC_I8, false, 3>(a, st);
-            if (a.i8_scaled == 1) return a.dpad8 <= 1024 ? launch_tc_n<128, tc::PREC_I8, true, 1>(a, st) : launch_tc_n<128, tc::PREC_I8, false, 1>(a, st);
-            return a.dpad8 <= 1024 ? launch_tc_n<128, tc::PREC_I8, true, 2>(a, st) : launch_tc_n<128, tc::PREC_I8, false, 2>(a, st);
+            if (a.i8_scaled == 3) return res ? launch_tc_n<128, tc::PREC_I8, true, 3>(a, st) : launch_tc_n<128, tc::PREC_I8, false, 3>(a, st);
+            if (a.i8_scaled == 1) return res ? launch_tc_n<128, tc::PREC_I8, true, 1>(a, st) : launch_tc_n<128, tc::PREC_I8, false, 1>(a, st);
+            return res ? launch_tc_n<128, tc::PREC_I8, true, 2>(a, st) : launch_tc_n<128, tc::PREC_I8, false, 2>(a, st);
         }
-        return a.dpad8 <= 1024 ? launch_tc_n<128, tc::PREC_I8, true>(a, st) : launch_tc_n<128, tc::PREC_I8, false>(a, st);
+        return res ? launch_tc_n<128, tc::PREC_I8, true>(a, st) : launch_tc_n<128, tc::PREC_I8, false>(a, st);
     }
-    if (a.similarity == SSB_SIM_EUCLIDEAN) { set_error("tcgen05 scan supports Dot/Cosine only"); return SSB_E_UNSUPPORTED; }
+    if (a.similarity == SSB_SIM_EUCLIDEAN) { set_error("tensor-core scan supports Dot/Cosine only"); return SSB_E_UNSUPPORTED; }
     if (prec == 3) {
-        if ((nq_tile != 128 && nq_tile != 256) || a.nq_pad % nq_tile != 0) { set_error("tcgen05 filter scan: query count must be padded to the 128/256 query tile"); return SSB_E_INVALID; }
+        if ((nq_tile != 128 && nq_tile != 256) || a.nq_pad % nq_tile != 0) { set_error("tensor-core filter scan: query count must be padded to the 128/256 query tile"); return SSB_E_INVALID; }
         return nq_tile == 256 ? launch_tc_n<256, tc::PREC_F16F>(a, st) : launch_tc_n<128, tc::PREC_F16F>(a, st);
     }
-    if ((nq_tile != 64 && nq_tile != 128 && !(nq_tile == 256 && prec == 1)) || a.nq_pad % nq_tile != 0) { set_error("tcgen05 scan: query count must be padded to the 64/128(/256 bf16) query tile"); return SSB_E_INVALID; }
+    if ((nq_tile != 64 && nq_tile != 128 && !(nq_tile == 256 && prec == 1)) || a.nq_pad % nq_tile != 0) { set_error("tensor-core scan: query count must be padded to the 64/128(/256 bf16) query tile"); return SSB_E_INVALID; }
     if (prec == 1) return nq_tile == 64 ? launch_tc_n<64, tc::PREC_BF16>(a, st) : (nq_tile == 256 ? launch_tc_n<256, tc::PREC_BF16>(a, st) : launch_tc_n<128, tc::PREC_BF16>(a, st));
     return nq_tile == 64 ? launch_tc_n<64, tc::PREC_TF32>(a, st) : launch_tc_n<128, tc::PREC_TF32>(a, st);
 }

@@ -152,13 +152,13 @@ def _hits_array(n):
 
 
 class Index:
-    """One shard's GPU-resident mirror: committed lexical levels + vector levels on one B200."""
+    """One shard's GPU-resident mirror: committed lexical levels + vector levels on one H100."""
 
     def __init__(self, device: int = 0, vector_dims: int = 0,
                  vector_similarity: VectorSimilarity = VectorSimilarity.Cosine, max_batch: int = 4096,
                  term_key_fn: Callable[[str], int] = synthetic_term_key, vector_kernel: int = 0,
                  vector_quantization: int = 0):
-        """vector_kernel: SSB_VEC_KERNEL_* (0 = auto, 1 = FP32 FFMA scan, 2/3 = tcgen05 3xTF32, 4/5/6 = tcgen05 3xBF16 with 128/64/256
+        """vector_kernel: SSB_VEC_KERNEL_* (0 = auto, 1 = FP32 FFMA scan, 2/3 = wgmma 3xTF32, 4/5/6 = wgmma 3xBF16 with 128/64/256
         queries per pass, 7/8 = bf16 filter scan + exact f32 refine with 128/256 queries per pass)."""
         self._h = C.c_void_p()
         cfg = SsbConfig(device, max_batch, vector_dims, int(vector_similarity), vector_kernel, int(vector_quantization),
@@ -352,7 +352,7 @@ class Index:
             self.add_vector_level(first_level + s // 65536, rows[s:min(n, s + 65536)])
 
     def set_vector_kernel(self, kernel: int):
-        """0 = auto, 1 = FP32 FFMA2 scan, 2/3 = tcgen05 3xTF32 (128/64 queries per pass), 4/5/6 = tcgen05 3xBF16 (128/64/256)."""
+        """0 = auto, 1 = FP32 FFMA scan, 2/3 = wgmma 3xTF32 (128/64 queries per pass), 4/5/6 = wgmma 3xBF16 (128/64/256)."""
         check(lib().ssb_set_vector_kernel(self._h, kernel))
 
     @property

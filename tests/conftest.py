@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs a real H100 (run with -m gpu on the GPU box)")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -21,7 +21,7 @@ def pytest_collection_modifyitems(config, items):
         have = False
     if have:
         return
-    skip = pytest.mark.skip(reason="needs a CUDA device (B200)")
+    skip = pytest.mark.skip(reason="needs a CUDA device (H100)")
     for it in items:
         if "gpu" in it.keywords:
             it.add_marker(skip)

@@ -25,7 +25,7 @@ def test_stats_and_kernel_selection():
         assert st["kernel_launches"] == {1: 5, 2: 6, 3: 6, 4: 5, 5: 5, 0: 8}[kern]   # FP32: prep + sample(scan, kth) + scan + merge; tf32: prep + split + sample(scan, kth) + scan + merge; bf16: fused prep/split + sample(scan, kth) + scan + merge; AUTO (50 queries) -> filter scan: + refine + fallback scan / merge (both exit at once)
         assert st["dominant_kernel_ns"] > 0
         assert st["h2d_bytes"] == 50 * 64 * 4 and st["d2h_bytes"] == 50 * 32 * 8
-        passes = {1: 4, 2: 1, 3: 1, 4: 1, 5: 1, 0: 1}[kern]   # 50 queries: 4 x 16, 1 x 128, 1 x 64, AUTO -> tcgen05
+        passes = {1: 4, 2: 1, 3: 1, 4: 1, 5: 1, 0: 1}[kern]   # 50 queries: 4 x 16, 1 x 128, 1 x 64, AUTO -> tensor-core scan
         assert st["algorithmic_bytes"] == passes * 70000 * 64 * 4
     for kern in (2, 3, 4, 5, 0):                            # all kernels agree on the ids (scores within tolerance)
         for a, b in zip(outs[1], outs[kern]):

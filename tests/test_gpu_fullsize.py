@@ -25,7 +25,7 @@ def test_c2_full_size_vector():
     for j, p in enumerate(planted.tolist()):
         assert got[3 * j][0][0] == p
     # property: results do not depend on batch composition / padding.  AUTO switches kernel with the batch size
-    # (48 queries -> tcgen05, 7 -> FP32 scan): same ids, scores within the 1e-4 tolerance; with the kernel pinned the
+    # (48 queries -> tensor-core scan, 7 -> FP32 scan): same ids, scores within the 1e-4 tolerance; with the kernel pinned the
     # scores are bit-identical.
     again = ix.search_vector_batch(q[5:12].cpu().numpy(), 10)
     for a_, g_ in zip(again, got[5:12]):
@@ -112,9 +112,13 @@ def _build_full_lexical(n_docs, seed, want_oracle=True, **index_kw):
     return ix, orc
 
 
+_c3_open = []   # the module's 10 M-doc index while it is alive
+
+
 @pytest.fixture(scope="module")
 def c3_index():
     ix, orc = _build_full_lexical(10_000_000, 1003)
+    _c3_open.append(ix)
     yield ix, orc
     ix.close()
 
@@ -205,6 +209,10 @@ def test_c4_full_size_hybrid_identity():
     (lexical list bit-exact; the vector list is checked to 1e-4 and must agree on ids for the RRF ranks to agree)."""
     from seekstorm_b200 import QueryType, VectorSimilarity
     n, d = 5_000_000, 768
+    # an 80 GB GPU holds this index (5 M docs + 5 M x 768 vectors as f32, two bf16 planes and an fp16 plane: 38 GB of vectors) but not
+    # next to the C3 index of the tests above, which have run by now: it is released first (its fixture's own close() is then a no-op)
+    while _c3_open:
+        _c3_open.pop().close()
     ix, orc = _build_full_lexical(n, 1004, vector_dims=d, vector_similarity=VectorSimilarity.Cosine)
     host_rows = np.empty((n, d), dtype=np.float32)
     ix.reserve_vectors(n)

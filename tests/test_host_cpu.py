@@ -105,7 +105,7 @@ def test_lex_bound_inflation_covers_rounding():
 
 
 def test_group_maximum_threshold_is_a_valid_lower_bound():
-    """Threshold seeding of the tcgen05 scans (vec_scan_tc.cu, sample mode): the k-th largest of the per-32-row-group maxima is
+    """Threshold seeding of the tensor-core scans (vec_scan_tc.cu, sample mode): the k-th largest of the per-32-row-group maxima is
     never above the true k-th best score (k disjoint groups each hold a row at least that good), and for k << #groups it is
     close to the exact k-th of the sample."""
     rng = np.random.default_rng(12)

@@ -1,10 +1,10 @@
 #!/usr/bin/env python
-"""SASS evidence of the built library: per kernel, how many tcgen05 / TMEM / TMA / packed-FP32 instructions it contains.
+"""SASS evidence of the built library: per kernel, how many warpgroup-MMA / TMA / FP32 instructions it contains.
 
-  python tools/sass_opcodes.py > profiles/sass_opcodes.txt
+  python tools/sass_opcodes.py
 
-(PTX names never appear in SASS: tcgen05.mma -> UTC*MMA, tcgen05.ld -> LDTM, cp.async.bulk.tensor -> UTMALDG, fma.rn.f32x2 -> FFMA2;
-HMMA / HGMMA would be the legacy tensor paths — none is expected.)"""
+(PTX names never appear in SASS: wgmma.mma_async -> HGMMA (f16 / bf16 / tf32) or IGMMA (s8), cp.async.bulk.tensor -> UTMALDG;
+HMMA / IMMA would be the warp-level tensor paths — none is expected.)"""
 import collections
 import os
 import re
@@ -13,8 +13,8 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "seekstorm_b200", "libseekstorm_b200.so")
-PAT = ["UTCHMMA", "UTCIMMA", "UTCQMMA", "UTCMXQMMA", "UTCBAR", "LDTM", "STTM", "UTMALDG", "UTMASTG", "UBLKCP", "UTMAPF", "SYNCS", "FFMA2", "FFMA",
-       "HMMA", "HGMMA", "IMMA", "LDL", "STL", "LDG", "LDS", "STS", "ATOM", "RED", "SHFL", "VOTE", "POPC", "F2F", "HADD2", "MUFU", "BAR"]
+PAT = ["HGMMA", "IGMMA", "WARPGROUP", "UTMALDG", "UTMASTG", "UBLKCP", "UTMAPF", "SYNCS", "FFMA",
+       "HMMA", "IMMA", "LDL", "STL", "LDG", "LDS", "STS", "ATOM", "RED", "SHFL", "VOTE", "POPC", "F2F", "HADD2", "MUFU", "BAR"]
 
 
 def main():
@@ -35,7 +35,7 @@ def main():
             counts[fn][op] += 1
             counts[fn]["_total"] += 1
     demangled = subprocess.run(["c++filt"], input="\n".join(counts.keys()), capture_output=True, text=True).stdout.splitlines()
-    print(f"# {os.path.relpath(LIB, ROOT)}: SASS opcode counts per kernel (cuobjdump -sass, sm_100a)")
+    print(f"# {os.path.relpath(LIB, ROOT)}: SASS opcode counts per kernel (cuobjdump -sass, sm_90a)")
     print("# kernel | total | " + " ".join(PAT))
     for (fn, c), dn in zip(counts.items(), demangled):
         name = re.sub(r"\(.*", "", dn)[:70]
