@@ -46,7 +46,9 @@ enum { SSB_OK = 0, SSB_E_INVALID = -1, SSB_E_CUDA = -2, SSB_E_NOMEM = -3, SSB_E_
 /* QueryType (search.rs, enum QueryType): Union / Intersection / Phrase.  A PHRASE batch lists every query's terms in phrase order,
  * repeated terms included ("to be or not to be" = 6 keys); a doc matches when it contains all of them and token i occurs at position
  * p + i for some p (add_result.rs:3586-3684); scores and counts as for an intersection of the unique terms.  Needs levels loaded with
- * ssb_level_desc.positions (one indexed field); NOT terms are not accepted in a phrase batch. */
+ * ssb_level_desc.positions; NOT terms are not accepted in a phrase batch.  Several indexed fields (add_result.rs:3247-3389): positions
+ * restart in every field and the phrase must occur inside ONE field; with a field filter (ssb_lex_batch.field_masks) only the fields of
+ * the filter are searched. */
 enum { SSB_QUERY_UNION = 0, SSB_QUERY_INTERSECTION = 1, SSB_QUERY_PHRASE = 2 };
 /* ResultType (search.rs:150-175): Count / Topk / TopkCount (default) */
 enum { SSB_RESULT_COUNT = 0, SSB_RESULT_TOPK = 1, SSB_RESULT_TOPKCOUNT = 2 };
@@ -123,11 +125,14 @@ typedef struct {
     const uint64_t* term_keys;        /* [n_terms] 64-bit term hash (reference key_hash), any order       */
     const uint32_t* posting_offsets;  /* [n_terms+1]                                                      */
     const uint16_t* doc_ids;          /* [n_postings] ascending within a term                            */
-    const uint16_t* tfs;              /* [n_postings]; F fields: [n_postings][F], 0 = the term does not occur in that field           */
+    const uint16_t* tfs;              /* [n_postings]; F fields: [n_postings][F], 0 = the term does not occur in that field; the     */
+                                      /* per-field tfs also give the lengths of a posting's per-field position runs (positions)      */
     const uint8_t*  doc_len_bytes;    /* [n_docs];     F fields: [F][n_docs] (document_length_compressed_array[field], index.rs:770-776) */
     const uint16_t* positions;        /* [sum of tfs] or NULL: the term positions of every posting, in posting order, ascending inside a   */
                                       /* posting (what get_next_position_singlefield decodes, add_result.rs:2036-2197); needed by          */
-                                      /* SSB_QUERY_PHRASE only; either every level carries them or none; one indexed field                  */
+                                      /* SSB_QUERY_PHRASE only; either every level carries them or none.  F fields: a posting holds        */
+                                      /* Σ_f tfs[p][f] positions, one run per field in field order (field 0's tfs[p][0] first), each run   */
+                                      /* strictly ascending and starting again from 0 (add_result.rs:3258-3283)                             */
 } ssb_level_desc;
 
 /* ---- facets and facet filters (SURVEY.md §8f row 4) ---------------------------------------------------- */

@@ -1,7 +1,8 @@
 // bm25.cu — BM25 AND/OR top-k over block-partitioned posting lists (sm_90a).
 //
 // Replaces, for committed data (all paths /root/reference/seekstorm/src/; the per-candidate chain — delete set, NOT lists, facet filters,
-// field filter, phrase check: add_result.rs:3435-3500, 3124-3137, 3586-3684 — runs as predicates of the scoring kernels, see lex_generic):
+// field filter, phrase check: add_result.rs:3435-3500, 3124-3137, 3586-3684, multi-field phrase 3247-3389 — runs as predicates of the scoring
+// kernels, see lex_generic):
 //   intersection_blockid / intersection_docid   intersection.rs:2023-2301 / 112-2013   (AND)
 //   intersection_bitmap_2                       intersection.rs:33-108                 (dense x dense: bitmap-word AND + popcount)
 //   union_docid_2 / union_docid_3 / single_blockid  union.rs:1168-1479, single.rs:292-417 (OR + block-max)
@@ -87,16 +88,27 @@ __global__ void validate_level(const uint16_t* __restrict__ ids, const uint16_t*
     if (!ok) atomicAdd(bad, 1u);
 }
 
-// positions of one level: the posting's tf positions must ascend strictly (get_next_position_singlefield decodes ascending deltas)
-__global__ void validate_positions(const uint16_t* __restrict__ pos, const uint32_t* __restrict__ off, const uint16_t* __restrict__ tfs, uint32_t n, uint32_t* bad) {
+// positions of one level: the posting's tf positions must ascend strictly (get_next_position_singlefield decodes ascending deltas).
+// Several fields: the posting holds one run per field (field 0's tfs[0] positions, then field 1's, ...), each run ascends strictly and
+// restarts from 0 (add_result.rs:3258-3283 reads them field by field).
+__global__ void validate_positions(const uint16_t* __restrict__ pos, const uint32_t* __restrict__ off, const uint16_t* __restrict__ tfs, uint32_t n,
+                                   uint32_t nf, uint32_t* bad) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const uint32_t o = off[i], tf = tfs[i];
-    for (uint32_t j = 1; j < tf; j++) if (pos[o + j] <= pos[o + j - 1]) { atomicAdd(bad, 1u); return; }
+    uint32_t o = off[i];
+    for (uint32_t f = 0; f < nf; f++) {
+        const uint32_t tf = tfs[(size_t)i * nf + f];
+        for (uint32_t j = 1; j < tf; j++) if (pos[o + j] <= pos[o + j - 1]) { atomicAdd(bad, 1u); return; }
+        o += tf;
+    }
 }
-__global__ void widen_tf(const uint16_t* __restrict__ tfs, uint32_t* __restrict__ out, uint32_t n) {
+// positions of one posting: Σ_f tf_f
+__global__ void widen_tf(const uint16_t* __restrict__ tfs, uint32_t* __restrict__ out, uint32_t n, uint32_t nf) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) out[i] = tfs[i];
+    if (i >= n) return;
+    uint32_t s = 0;
+    for (uint32_t f = 0; f < nf; f++) s += tfs[(size_t)i * nf + f];
+    out[i] = s;
 }
 
 __global__ void build_postings(const uint16_t* __restrict__ ids, const uint16_t* __restrict__ tfs, const uint8_t* __restrict__ len_bytes,
@@ -638,11 +650,79 @@ __device__ __noinline__ bool phrase_rejects_impl(PhraseArgs v, const QueryPlan* 
     }
     return true;
 }
-// facet filters and the field filter of one query on one doc: true = filtered OUT
+// Several indexed fields (add_result.rs:3247-3389): a posting's positions are one run per field, field 0 first, each restarting from 0, of
+// the posting's per-field tfs (v.pay = payf here).  The same merge as above runs field by field on those runs only — a phrase never spans two
+// fields: field f is searched when every unique term occurs in it and, if the query has a field filter (pl->field_mask != 0), when f is in
+// the filter (field_filter_set.contains).  The doc matches on the first field that holds the phrase.  Out of line like the single-field
+// check and only in lex_generic<true>, so that the single-field kernel keeps its code.
+__device__ __noinline__ bool phrase_rejects_fields_impl(PhraseArgs v, const QueryPlan* pl, uint32_t n_live, uint32_t lv, uint32_t d, uint32_t n_fields) {
+    uint64_t ubase[SSB_MAX_QUERY_TERMS], ftf[SSB_MAX_QUERY_TERMS];       // per unique term: its first position in field 0, its tfs (16 bits per field)
+    uint32_t utf[SSB_MAX_QUERY_TERMS];
+    const uint64_t lbase = __ldg(&v.lvl_pos_base[lv]);
+    for (uint32_t t = 0; t < n_live; t++) {
+        const QTerm qt = pl->t[t];
+        uint32_t a = 0, b = qt.n;
+        while (a < b) { const uint32_t m = (a + b) >> 1; if (__ldg(&v.e_level[qt.first + m]) < lv) a = m + 1; else b = m; }
+        if (a >= qt.n || __ldg(&v.e_level[qt.first + a]) != lv) return true;
+        const uint32_t e = qt.first + a;
+        const uint32_t cnt = __ldg(&v.e_count[e]), bmi = __ldg(&v.e_bitmap[e]); const uint64_t off = __ldg(&v.e_off[e]);
+        uint32_t rank; bool found;
+        if (bmi != NONE) {
+            const BmSec* sec = v.bm + (size_t)bmi * 512 + (d >> 7);
+            const uint64_t w = __ldg(&sec->w[(d >> 6) & 1u]);
+            rank = (__ldg(&sec->meta[(d >> 6) & 1u]) & 0xFFFFu) + (uint32_t)__popcll(w & ((1ull << (d & 63)) - 1ull));
+            found = ((w >> (d & 63)) & 1ull) != 0;
+        } else {
+            uint32_t lo = 0, hi = cnt;
+            const uint32_t* p = v.post + off;
+            while (lo < hi) { const uint32_t m = (lo + hi) >> 1; if ((__ldg(&p[m]) & 0xFFFFu) < d) lo = m + 1; else hi = m; }
+            rank = lo; found = lo < cnt && (__ldg(&p[lo]) & 0xFFFFu) == d;
+        }
+        if (!found) return true;
+        ubase[t] = lbase + __ldg(&v.pos_off[off + rank]);
+        uint64_t tfs = 0;
+        for (uint32_t f = 0; f < n_fields; f++) tfs |= (uint64_t)(__ldg(&v.pay[(off + rank) * n_fields + f]) & 0xFFFFu) << (16 * f);
+        ftf[t] = tfs;
+    }
+    const uint32_t m = pl->n_phr, u0 = pl->phr[0], field_mask = pl->field_mask;
+    uint32_t cur[SSB_MAX_QUERY_TERMS];
+    for (uint32_t f = 0; f < n_fields; f++) {
+        bool in_all = true;
+        for (uint32_t t = 0; t < n_live; t++) {
+            if (f) ubase[t] += utf[t];                                       // field f's run follows the run of field f - 1
+            utf[t] = (uint32_t)(ftf[t] >> (16 * f)) & 0xFFFFu;
+            in_all = in_all && utf[t] != 0;
+        }
+        if (!in_all || (field_mask && !((field_mask >> f) & 1u))) continue;
+        for (uint32_t i = 0; i < m; i++) cur[i] = 0;
+        bool exhausted = false;
+        while (!exhausted && cur[0] < utf[u0]) {
+            const uint32_t s = __ldg(&v.positions[ubase[u0] + cur[0]]);
+            bool all = true; uint32_t next_s = s;
+            for (uint32_t i = 1; i < m; i++) {
+                const uint32_t u = pl->phr[i];
+                while (cur[i] < utf[u] && (uint32_t)__ldg(&v.positions[ubase[u] + cur[i]]) < s + i) cur[i]++;
+                if (cur[i] >= utf[u]) { exhausted = true; break; }          // a token's positions in this field are exhausted
+                const uint32_t p = __ldg(&v.positions[ubase[u] + cur[i]]);
+                if (p != s + i) { all = false; next_s = p - i; break; }
+            }
+            if (exhausted) break;
+            if (all) return false;                                           // phrasematch_count >= 1
+            while (cur[0] < utf[u0] && (uint32_t)__ldg(&v.positions[ubase[u0] + cur[0]]) < next_s) cur[0]++;
+        }
+    }
+    return true;
+}
+// facet filters, the field filter and the phrase check of one query on one doc: true = filtered OUT.  FIELD_RUNS: the index has several
+// fields and a phrase batch is running (positions in per-field runs) — its own instantiation of lex_generic, so that the single-field kernel
+// keeps its code and register allocation
+template <bool FIELD_RUNS>
 __device__ __forceinline__ bool filters_reject(const LexView& v, const QueryPlan* pl, uint32_t f0, uint32_t nf, uint32_t field_mask, uint32_t n_live, uint32_t lv, uint32_t d, uint32_t doc) {
     if (nf && facet_rejects(v, f0, nf, doc)) return true;
     if (field_mask && field_rejects_impl(FieldArgs{v.e_level, v.e_count, v.e_bitmap, v.post, v.e_off, v.bm, v.payf, v.n_fields}, pl, n_live, lv, d, field_mask)) return true;
-    if (pl->n_phr && phrase_rejects_impl(PhraseArgs{v.e_level, v.e_count, v.e_bitmap, v.post, v.e_off, v.bm, v.pay, v.positions, v.pos_off, v.lvl_pos_base}, pl, n_live, lv, d)) return true;
+    if (!FIELD_RUNS && pl->n_phr && phrase_rejects_impl(PhraseArgs{v.e_level, v.e_count, v.e_bitmap, v.post, v.e_off, v.bm, v.pay, v.positions, v.pos_off, v.lvl_pos_base}, pl, n_live, lv, d)) return true;
+    if (FIELD_RUNS && pl->n_phr && phrase_rejects_fields_impl(PhraseArgs{v.e_level, v.e_count, v.e_bitmap, v.post, v.e_off, v.bm, v.payf, v.positions, v.pos_off,
+                                                                         v.lvl_pos_base}, pl, n_live, lv, d, v.n_fields)) return true;
     return false;
 }
 
@@ -1125,6 +1205,7 @@ __device__ __forceinline__ void score_records(const LexView& v, WarpSm& w, uint3
 }
 
 // ---- generic path: up to SSB_MAX_QUERY_TERMS live terms, lane t holds term t, values broadcast by shuffles ----
+template <bool FIELD_RUNS>
 __device__ __forceinline__ void process_item_generic(const LexView& v, const QueryPlan* pl, const ItemCtx& c, int lane,
                                                   uint64_t& L, uint32_t& thr, bool& dirty, uint32_t& matches_out,
                                                   uint32_t& st_visited, uint32_t& st_probes) {
@@ -1167,7 +1248,7 @@ __device__ __forceinline__ void process_item_generic(const LexView& v, const Que
             }
             if (c.n_filt) {
                 // a filtered query is counted here doc by doc: filter, delete set and NOT lists at once (the correction kernels skip it)
-                ok = ok && !filters_reject(v, pl, c.filt_first, c.n_facet_filt, c.field_mask, c.n, c.lv, d, c.docbase | d) && !is_deleted(v, c.docbase | d) && !(c.n_not && in_not_lists(v, pl, c.n_not, c.lv, d));
+                ok = ok && !filters_reject<FIELD_RUNS>(v, pl, c.filt_first, c.n_facet_filt, c.field_mask, c.n, c.lv, d, c.docbase | d) && !is_deleted(v, c.docbase | d) && !(c.n_not && in_not_lists(v, pl, c.n_not, c.lv, d));
                 matches += __popc(__ballot_sync(FULL, ok));
                 if (c.scoring) insert_candidates(L, thr, ok && ord_f32(score) >= thr, score, c.docbase | d, c.k, lane, dirty, c.ceil);
                 continue;
@@ -1218,7 +1299,7 @@ __device__ __forceinline__ void process_item_generic(const LexView& v, const Que
                     }
                 }
                 insert_candidates(L, thr, active && !dup && ord_f32(score) >= thr && !is_deleted(v, c.docbase | d) && !(c.n_not && in_not_lists(v, pl, c.n_not, c.lv, d))
-                                              && !(c.n_filt && filters_reject(v, pl, c.filt_first, c.n_facet_filt, c.field_mask, c.n, c.lv, d, c.docbase | d)), score, c.docbase | d, c.k, lane, dirty, c.ceil);
+                                              && !(c.n_filt && filters_reject<FIELD_RUNS>(v, pl, c.filt_first, c.n_facet_filt, c.field_mask, c.n, c.lv, d, c.docbase | d)), score, c.docbase | d, c.k, lane, dirty, c.ceil);
             }
         }
     }
@@ -1250,7 +1331,7 @@ __device__ __forceinline__ void process_item_generic(const LexView& v, const Que
                 }
                 bool cnt_ok = active && !dup;
                 if (c.n_filt && cnt_ok)      // filtered query: every match is tested here (filter, delete set, NOT lists; the correction kernels skip it)
-                    cnt_ok = !filters_reject(v, pl, c.filt_first, c.n_facet_filt, c.field_mask, c.n, c.lv, d, c.docbase | d) && !is_deleted(v, c.docbase | d) && !(c.n_not && in_not_lists(v, pl, c.n_not, c.lv, d));
+                    cnt_ok = !filters_reject<FIELD_RUNS>(v, pl, c.filt_first, c.n_facet_filt, c.field_mask, c.n, c.lv, d, c.docbase | d) && !is_deleted(v, c.docbase | d) && !(c.n_not && in_not_lists(v, pl, c.n_not, c.lv, d));
                 matches += __popc(__ballot_sync(FULL, cnt_ok));
             }
         }
@@ -1400,6 +1481,8 @@ __global__ void __launch_bounds__(128, 6) lex_count(LexView v, const QueryPlan* 
 }
 
 // ---- queries with 5..16 live terms: one level per item, per-term state in lanes (scoring and counting) ----
+// FIELD_RUNS: phrase batch on an index with several fields (the phrase check walks per-field position runs)
+template <bool FIELD_RUNS>
 __global__ void __launch_bounds__(256) lex_generic(LexView v, const QueryPlan* __restrict__ plans, const LvRec* __restrict__ recs,
                                                   const uint16_t* __restrict__ item_start, uint32_t nq, uint32_t query_type, uint32_t result_type,
                                                   uint32_t k, uint32_t* ctr, uint64_t* theta, int* lock, uint64_t* count, uint64_t* glist,
@@ -1432,7 +1515,7 @@ __global__ void __launch_bounds__(256) lex_generic(LexView v, const QueryPlan* _
             c.need_count = need_count; c.is_and = query_type == SSB_QUERY_INTERSECTION; c.docbase = w.recs[ri].docbase;
             if (!c.scoring && !need_count) { st_skipped++; continue; }
             st_done++;
-            process_item_generic(v, pl, c, lane, L, thr, dirty, matches, st_visited, st_probes);
+            process_item_generic<FIELD_RUNS>(v, pl, c, lane, L, thr, dirty, matches, st_visited, st_probes);
         }
         if (dirty) publish(L, q, k, lane, theta, lock, glist);
         if (need_count && lane == 0 && matches) atomicAdd((unsigned long long*)&count[q], (unsigned long long)matches);
@@ -1650,13 +1733,12 @@ int32_t LexIndex::add_level(const ssb_level_desc* d) {
     const int has_pos = d->positions ? 1 : 0;
     if (np) {
         if (has_positions_ >= 0 && has_positions_ != has_pos) { set_error("add_level %u: either every level carries positions or none", d->level_id); return SSB_E_INVALID; }
-        if (has_pos && nf > 1) { set_error("add_level: positions (phrase queries) are supported for one indexed field"); return SSB_E_UNSUPPORTED; }
     }
     uint64_t level_positions = 0;
     if (np && has_pos) {
         SSB_TRY(pos_off_.reserve(n_post_ + np, n_post_, st_));
         uint32_t* off = pos_off_.p + n_post_;
-        widen_tf<<<(np + 255) / 256, 256, 0, st_>>>(d_tfs, off, np);
+        widen_tf<<<(np + 255) / 256, 256, 0, st_>>>(d_tfs, off, np, nf);          // a posting's positions: Σ_f tf_f, field by field
         SSB_CUDA_TRY(cudaGetLastError());
         uint32_t last_tf = 0, last_off = 0;
         SSB_CUDA_TRY(cudaMemcpyAsync(&last_tf, off + np - 1, 4, cudaMemcpyDeviceToHost, st_));
@@ -1668,11 +1750,15 @@ int32_t LexIndex::add_level(const ssb_level_desc* d) {
         SSB_TRY(positions_.reserve(n_positions_ + level_positions + 8, n_positions_, st_));
         SSB_CUDA_TRY(to_device(positions_.p + n_positions_, d->positions, (size_t)level_positions * 2, st_));
         SSB_CUDA_TRY(cudaMemsetAsync(t_bad.p, 0, 4, st_));
-        validate_positions<<<(np + 255) / 256, 256, 0, st_>>>(positions_.p + n_positions_, off, d_tfs, np, t_bad.p);
+        validate_positions<<<(np + 255) / 256, 256, 0, st_>>>(positions_.p + n_positions_, off, d_tfs, np, nf, t_bad.p);
         SSB_CUDA_TRY(cudaGetLastError());
         SSB_CUDA_TRY(cudaMemcpyAsync(&bad, t_bad.p, 4, cudaMemcpyDeviceToHost, st_));
         SSB_CUDA_TRY(cudaStreamSynchronize(st_));
-        if (bad) { set_error("add_level %u: %u postings whose positions do not ascend strictly", d->level_id, bad); return SSB_E_INVALID; }
+        if (bad) {
+            if (nf > 1) set_error("add_level %u: %u postings whose positions do not ascend strictly inside one field's run", d->level_id, bad);
+            else set_error("add_level %u: %u postings whose positions do not ascend strictly", d->level_id, bad);
+            return SSB_E_INVALID;
+        }
     }
     if (np) has_positions_ = has_pos;
     h_lvl_pos_base_.push_back(n_positions_);
@@ -2067,7 +2153,8 @@ int32_t LexIndex::search_keys(LexWorkspace& ws, cudaStream_t st, const ssb_lex_b
         if (launches) *launches += 1;
     }
     // queries with 5..16 live terms (the kernel returns at once when the batch has none)
-    lex_generic<<<n_sms_ * 2, 256, 0, st>>>(v, ws.plans, ws.recs, ws.item_start, nq, qt_eff, result_type, kk, ws.ctr, ws.theta, ws.lock, ws.count, glist, ws.stats, ceil_dev);
+    auto generic = (phrase && n_fields_ > 1) ? lex_generic<true> : lex_generic<false>;
+    generic<<<n_sms_ * 2, 256, 0, st>>>(v, ws.plans, ws.recs, ws.item_start, nq, qt_eff, result_type, kk, ws.ctr, ws.theta, ws.lock, ws.count, glist, ws.stats, ceil_dev);
     SSB_CUDA_TRY(cudaGetLastError());
     if (need_count) {     // returns at once unless some query of the batch carries NOT terms
         lex_not_count<<<n_sms_ * 4, 256, 0, st>>>(v, ws.plans, nq, qt_eff, ws.ctr, ws.count);

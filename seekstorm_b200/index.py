@@ -193,7 +193,14 @@ class Index:
 
     def add_lexical_level(self, level_id: int, n_docs: int, term_keys, posting_offsets, doc_ids, tfs, doc_len_bytes, positions=None):
         """One committed 64K-doc level in the neutral layout (arrays: numpy on host or torch on the device).  positions: u16 [sum of tfs], the
-        term positions of every posting in posting order (phrase queries), or None."""
+        term positions of every posting in posting order (phrase queries), or None.  With several indexed fields (tfs [n_postings, F]) a
+        posting holds the sum of its F tfs positions, one run per field in field order (field 0's first), each run ascending and starting
+        again from 0 in every field; a phrase matches inside one field only."""
+        if positions is not None:
+            n_pos = positions.size if isinstance(positions, np.ndarray) else positions.numel()
+            want = int(tfs.astype(np.int64).sum()) if isinstance(tfs, np.ndarray) else int((tfs.long() & 0xFFFF).sum())
+            if n_pos != want:
+                raise _lib.SsbError(f"add_lexical_level {level_id}: positions holds {n_pos} values, the postings' tfs add up to {want}")
         n_terms = int(term_keys.shape[0])
         d = SsbLevelDesc(level_id, n_docs, n_terms, getattr(self, "_n_fields", 1), _addr(term_keys), _addr(posting_offsets), _addr(doc_ids),
                          _addr(tfs), _addr(doc_len_bytes), _addr(positions))
