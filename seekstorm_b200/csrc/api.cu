@@ -196,7 +196,7 @@ int32_t vec_keys(ssb_index* ix, SearchCtx& c, const void* queries, bool queries_
         kern = nq <= 16 ? SSB_VEC_KERNEL_FFMA : (p256 * 237u < p128 * 108u ? SSB_VEC_KERNEL_TCGEN05_BF16_N256 : SSB_VEC_KERNEL_TCGEN05_BF16);
         // filter scan + exact refine (DESIGN.md §3.2c): half the bytes and a third of the tensor work per pass
         // — at every batch size: one 128-query filter pass (0.59 ms on 1M x 768) also beats the FP32 scan's 0.97 ms pass for <= 16 queries.
-        // Above 128 queries one 256-query pass (1.13 ms, measured; 1.52 ms on CTA pairs) beats two 128-query passes (1.18 ms)
+        // Above 128 queries one 256-query pass (0.88 ms, measured; 1.2 ms on CTA pairs) beats two 128-query passes (1.17-1.20 ms)
         const uint32_t exact_kern = kern;
         kern = nq <= 128 ? SSB_VEC_KERNEL_TCGEN05_FILTER : SSB_VEC_KERNEL_TCGEN05_FILTER_N256;
         if (ix->quant_i8 || ix->cfg.vector_similarity == SSB_SIM_EUCLIDEAN || k > 16 || ceil_dev || !ix->rows_h16.p || !ix->vec_err.p) kern = exact_kern;

@@ -28,7 +28,8 @@
 // the accumulator fragment goes 8 query columns at a time through a small per-warp shared-memory buffer into a lane = corpus row
 // layout (one pass = 32 rows = two sub-tiles); the whole chunk is tested against the per-query thresholds branch-free with ONE vote,
 // and only chunks with a candidate take the per-column path (ballot, per-warp sorted lists in the CTA's slice of the output scratch,
-// no CTA barriers).
+// no CTA barriers).  The 256-query kernels take that vote on the fragment itself, before the transposition, so that a chunk without
+// a candidate costs no shared-memory traffic.
 // Threshold seeding: the same kernel runs first in sample mode over one tile per SM and writes per-(32-row group, query) score
 // maxima; kth_from_groupmax turns them into valid lower bounds of the k-th best score.
 #include <cuda_bf16.h>
@@ -53,6 +54,7 @@ constexpr int CHUNK = 8;               // query columns per epilogue step
 constexpr int XB_STRIDE = CHUNK + 1;   // per-warp transposition buffer [32 rows][CHUNK] (+1 column: conflict-free row reads)
 constexpr int XB_BYTES = 8 * 32 * XB_STRIDE * 4;
 constexpr int SMEM_MAX = 232448;       // 227 KB opt-in limit per CTA
+constexpr uint32_t ORD_NEG_INF = 0x007FFFFFu;   // ord_f32(-inf)
 enum { PREC_TF32 = 0, PREC_BF16 = 1, PREC_I8 = 2, PREC_F16F = 3 };
 // PREC_F16F — the FILTER scan (DESIGN.md §3.2c): ONE product h(a).h(b) over an fp16 plane of the corpus (2 bytes per element, a third of
 // the tensor work of the 3-product split; fp16 keeps 11 significand bits, bf16 8 — the margin below is 8x tighter than with the bf16
@@ -229,8 +231,11 @@ template <int N> __device__ __forceinline__ void wg_wait() { asm volatile("wgmma
 // keeps the compiler from touching accumulator registers across wgmma.wait_group (the tensor core writes them asynchronously)
 __device__ __forceinline__ void fence_reg(float& r) { asm volatile("" : "+f"(r)::"memory"); }
 __device__ __forceinline__ void fence_reg(uint32_t& r) { asm volatile("" : "+r"(r)::"memory"); }
-__device__ __forceinline__ uint32_t acc_bits(float x) { return __float_as_uint(x); }
-__device__ __forceinline__ uint32_t acc_bits(uint32_t x) { return x; }
+// an accumulator into the transposition buffer in its own type.  Reading an f32 accumulator as bits (__float_as_uint) makes the compiler
+// carry the accumulators through the stage loop as integer values: the copies between the two register types then read accumulators
+// between an MMA and its wait, and ptxas serialises the whole wgmma chain (remark C7514; 256-query kernels).
+__device__ __forceinline__ void xb_put(uint32_t* d, float x) { *reinterpret_cast<float*>(d) = x; }
+__device__ __forceinline__ void xb_put(uint32_t* d, uint32_t x) { *d = x; }
 
 __device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
 __device__ __forceinline__ void cluster_sync_all() {
@@ -281,6 +286,9 @@ scan_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtenso
         uint32_t sample_mode /*write per-(32-row group, query) score maxima instead of lists*/) {
     using C = Cfg<NQ, PREC, BRES>;
     constexpr int TROWS = C::TROWS, MW = C::MW, NQH = C::NQH;
+    // 256 queries: the tensor pipe, not HBM, sets the pass time, and the epilogue stalls it -> the common-case test runs on the
+    // accumulator fragment, without the shared-memory transposition
+    constexpr bool FRAG_VOTE = NQ == 256;
     using AccT = typename std::conditional<PREC == PREC_I8, uint32_t, float>::type;
     const uint32_t STAGES = BRES ? nst_rt : (uint32_t)C::STAGES;
     // the swizzled tiles need 1024-byte alignment in the shared window (the same offset in both CTAs of a pair)
@@ -466,14 +474,29 @@ scan_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtenso
 #pragma unroll
                 for (int jb = 0; jb < NQH / CHUNK; jb++) {
                     const int c = q0 / CHUNK + jb;                    // 8-query chunk of the block
+                    if (FRAG_VOTE && !sample_mode) {
+                        // common case, in the fragment layout: the lane's 8 scores of the chunk (2 sub-tiles x 2 rows x its 2 columns)
+                        // against the thresholds of its 2 columns, one vote.  A superset of the exact per-column test below: float
+                        // compare treats -0 = +0 and rejects NaN scores; ord values at or below ord(-inf) (0 = no threshold yet) accept
+                        // every score; rows past n_rows are left to the exact test.
+                        const uint2 t = *reinterpret_cast<const uint2*>(thr_u + c * CHUNK + 2 * (lane & 3));
+                        const float t0 = unord_f32(max(t.x, ORD_NEG_INF)), t1 = unord_f32(max(t.y, ORD_NEG_INF));
+                        bool any = false;
+#pragma unroll
+                        for (int hm = 0; hm < 2; hm++)
+#pragma unroll
+                            for (int h = 0; h < 2; h++)
+                                any |= (acc[2 * p + hm][4 * jb + 2 * h] >= t0) | (acc[2 * p + hm][4 * jb + 2 * h + 1] >= t1);
+                        if (!__any_sync(FULL, any)) continue;
+                    }
                     __syncwarp();
 #pragma unroll
                     for (int hm = 0; hm < 2; hm++)
 #pragma unroll
                         for (int h = 0; h < 2; h++) {
                             uint32_t* d = xb + (hm * 16 + (lane >> 2) + 8 * h) * XB_STRIDE + 2 * (lane & 3);
-                            d[0] = acc_bits(acc[2 * p + hm][4 * jb + 2 * h]);
-                            d[1] = acc_bits(acc[2 * p + hm][4 * jb + 2 * h + 1]);
+                            xb_put(&d[0], acc[2 * p + hm][4 * jb + 2 * h]);
+                            xb_put(&d[1], acc[2 * p + hm][4 * jb + 2 * h + 1]);
                         }
                     __syncwarp();
                     uint32_t v[CHUNK];
@@ -511,8 +534,8 @@ scan_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtenso
                             gmaxu[(size_t)(blockIdx.y * NQ + c * CHUNK + lane) * n_rg + (tile * (TROWS / 32) + p * 4 + w)] = keep;
                         continue;
                     }
-                    {   // common case, branch-free: one vote per 8-query chunk instead of one per column (a NaN score maps above every
-                        // threshold here and is rejected by the per-column test below)
+                    if (!FRAG_VOTE) {   // common case, branch-free: one vote per 8-query chunk instead of one per column (a NaN score maps
+                        // above every threshold here and is rejected by the per-column test below)
                         const uint4* t4 = reinterpret_cast<const uint4*>(thr_u + c * CHUNK);
                         const uint4 t0 = t4[0], t1 = t4[1];
                         const bool any = (ord_f32(__uint_as_float(v[0])) >= t0.x) | (ord_f32(__uint_as_float(v[1])) >= t0.y) |
