@@ -74,20 +74,18 @@ enum { SSB_QUANT_NONE = 0, SSB_QUANT_SCALAR_I8 = 1,
         * -max(0, query_norm + row_norm - 2 * dot_i32 as f32 * query_scale * row_scale) (:2058-2069).  Bit-exact with the scalar CPU
         * arithmetic.  Needs ssb_vector_set_turboquant_mask before the first level. */
        SSB_QUANT_TURBO_I8 = 2 };
-/* which vector scan kernel to use */
-/* FFMA: FP32 scan, 16 queries per corpus pass (HBM-bound).  TCGEN05[_N64]: tensor-core scan with the 3xTF32
- * split, 128 (or 64) queries per corpus pass.  TCGEN05_BF16[_N64]: tensor-core scan with the 3xBF16 split (half the
- * operand bytes; score error ~1e-5 relative, inside the 1e-4 tolerance).  AUTO: FFMA up to 16 queries and
- * for Euclidean; above that TCGEN05_BF16, or TCGEN05_BF16_N256 when its passes take less time for the batch size. */
+/* which vector scan kernel to use.  FFMA: FP32 scan, 16 queries per corpus pass (HBM-bound).  TCGEN05[_N64]: tensor-core scan with
+ * the 3xTF32 split, 128 (64) queries per pass.  TCGEN05_BF16[_N64|_N256]: the 3xBF16 split (half the operand bytes; score error ~1e-5
+ * relative, inside the 1e-4 tolerance), 128 (64, 256) queries per pass.  FILTER[_N256]: one fp16 product over a 2-byte plane of the
+ * corpus selects, with a proven error margin, the <= 32 rows that can be in the top-k; those are re-scored with the plain f32 dot product
+ * and queries whose candidate set did not fit are re-run by an exact f32 scan on the device: the exact f32 top-k, 128 (256) queries per
+ * pass; FILTER_N256_PAIR: the 256-query filter scan on CTA pairs sharing one copy of the query block (TMA multicast).  The filter scans
+ * run for k <= 16 without paging; other calls take TCGEN05_BF16 (FILTER) or the cheaper of TCGEN05_BF16 and _N256 (the 256-query ones).
+ * AUTO: the filter scan whenever it can run (FILTER up to 128 queries, FILTER_N256 above), else FFMA up to 16 queries and the cheaper of
+ * TCGEN05_BF16 and _N256 above.  Euclidean f32 indexes always take FFMA, int8 indexes the s8 tensor-core scan (128 queries per pass). */
 enum { SSB_VEC_KERNEL_AUTO = 0, SSB_VEC_KERNEL_FFMA = 1, SSB_VEC_KERNEL_TCGEN05 = 2, SSB_VEC_KERNEL_TCGEN05_N64 = 3,
-       SSB_VEC_KERNEL_TCGEN05_BF16 = 4, SSB_VEC_KERNEL_TCGEN05_BF16_N64 = 5,
-       SSB_VEC_KERNEL_TCGEN05_BF16_N256 = 6 /* 256 queries per corpus pass: half the HBM bytes per query, tensor / shared-memory bound */,
-       /* FILTER: one bf16 product over the 2-byte hi plane of the corpus selects, with a proven error margin, the <= 32 rows that can be
-        * in the top-k (k <= 16); those are re-scored with the plain f32 dot product and queries whose candidate set did not fit are re-run
-        * by an exact f32 scan on the device.  Results are the exact f32 top-k.  128 / 256 queries per corpus pass. */
-       SSB_VEC_KERNEL_TCGEN05_FILTER = 7, SSB_VEC_KERNEL_TCGEN05_FILTER_N256 = 8,
-       /* the 256-query filter scan on CTA pairs (clusters of 2 CTAs): the two SMs of a pair share one copy of the query block (TMA multicast) */
-       SSB_VEC_KERNEL_TCGEN05_FILTER_N256_PAIR = 9 };
+       SSB_VEC_KERNEL_TCGEN05_BF16 = 4, SSB_VEC_KERNEL_TCGEN05_BF16_N64 = 5, SSB_VEC_KERNEL_TCGEN05_BF16_N256 = 6,
+       SSB_VEC_KERNEL_TCGEN05_FILTER = 7, SSB_VEC_KERNEL_TCGEN05_FILTER_N256 = 8, SSB_VEC_KERNEL_TCGEN05_FILTER_N256_PAIR = 9 };
 
 typedef struct ssb_index ssb_index;
 

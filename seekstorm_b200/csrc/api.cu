@@ -185,36 +185,13 @@ int32_t vec_keys(ssb_index* ix, SearchCtx& c, const void* queries, bool queries_
     if (k == 0 || k > SSB_K_MAX) { set_error("k must be in 1..%u", SSB_K_MAX); return SSB_E_UNSUPPORTED; }
     if (queries_i8 && !ix->quant_i8) { set_error("int8 queries need a ScalarQuantizationI8 index"); return SSB_E_INVALID; }
     if (nq == 0) return SSB_OK;
-    // AUTO (measured on one H100 SXM, 700 W, 1M x 768): one FP32 pass of 16 queries takes ~0.97 ms, one 3xBF16 tensor-core pass of up
-    // to 128 queries ~1.08 ms -> FP32 scan for <= 16 queries, tensor-core scan above.  Euclidean always takes the FP32 scan.
-    uint32_t kern = ix->cfg.vector_kernel;
-    if (ix->quant_i8) kern = SSB_VEC_KERNEL_TCGEN05;   // one kernel for the int8 corpus: s8 wgmma, 128-query tile
-    if (kern == SSB_VEC_KERNEL_AUTO) {
-        // tensor-core scan above 16 queries; the 256-query tile (2.37 ms per pass vs 1.08 ms for 128 queries, measured) when it
-        // needs fewer milliseconds for this batch: ceil(nq/256) * 2.37 < ceil(nq/128) * 1.08
-        const uint32_t p128 = (nq + 127u) / 128u, p256 = (nq + 255u) / 256u;
-        kern = nq <= 16 ? SSB_VEC_KERNEL_FFMA : (p256 * 237u < p128 * 108u ? SSB_VEC_KERNEL_TCGEN05_BF16_N256 : SSB_VEC_KERNEL_TCGEN05_BF16);
-        // filter scan + exact refine (DESIGN.md §3.2c): half the bytes and a third of the tensor work per pass
-        // — at every batch size: one 128-query filter pass (0.59 ms on 1M x 768) also beats the FP32 scan's 0.97 ms pass for <= 16 queries.
-        // Above 128 queries one 256-query pass (0.88 ms, measured; 1.2 ms on CTA pairs) beats two 128-query passes (1.17-1.20 ms)
-        const uint32_t exact_kern = kern;
-        kern = nq <= 128 ? SSB_VEC_KERNEL_TCGEN05_FILTER : SSB_VEC_KERNEL_TCGEN05_FILTER_N256;
-        if (ix->quant_i8 || ix->cfg.vector_similarity == SSB_SIM_EUCLIDEAN || k > 16 || ceil_dev || !ix->rows_h16.p || !ix->vec_err.p) kern = exact_kern;
-    }
-    // the filter scan keeps a candidate set sized for k <= 16 in the 32-entry lists and has no paging (ceilings are exact keys): those
-    // calls take the exact 3-product scan
-    bool filter = (kern == SSB_VEC_KERNEL_TCGEN05_FILTER || kern == SSB_VEC_KERNEL_TCGEN05_FILTER_N256 || kern == SSB_VEC_KERNEL_TCGEN05_FILTER_N256_PAIR);
-    if (filter && (ix->quant_i8 || ix->cfg.vector_similarity == SSB_SIM_EUCLIDEAN || k > 16 || ceil_dev || !ix->rows_h16.p || !ix->vec_err.p)) {
-        kern = kern != SSB_VEC_KERNEL_TCGEN05_FILTER && (nq + 255u) / 256u * 237u < (nq + 127u) / 128u * 108u ? SSB_VEC_KERNEL_TCGEN05_BF16_N256 : SSB_VEC_KERNEL_TCGEN05_BF16;
-        filter = false;
-        if (ix->quant_i8) kern = SSB_VEC_KERNEL_TCGEN05;
-    }
-    const bool use_tc = ix->quant_i8 || (kern >= SSB_VEC_KERNEL_TCGEN05 && ix->cfg.vector_similarity != SSB_SIM_EUCLIDEAN);   // the int8 index is always scanned on the tensor cores
-    const bool tc_bf16 = filter || kern == SSB_VEC_KERNEL_TCGEN05_BF16 || kern == SSB_VEC_KERNEL_TCGEN05_BF16_N64 || kern == SSB_VEC_KERNEL_TCGEN05_BF16_N256;
-    const uint32_t qt = !use_tc ? vec::VEC_QT : (ix->quant_i8 ? 128u : (kern == SSB_VEC_KERNEL_TCGEN05_N64 || kern == SSB_VEC_KERNEL_TCGEN05_BF16_N64) ? 64u : ((kern == SSB_VEC_KERNEL_TCGEN05_BF16_N256 || kern == SSB_VEC_KERNEL_TCGEN05_FILTER_N256 || kern == SSB_VEC_KERNEL_TCGEN05_FILTER_N256_PAIR) ? 256u : 128u));
-    const uint32_t nq_pad = (nq + qt - 1) / qt * qt;
+    const vec::Scan scan = vec::plan_scan(ix->cfg.vector_kernel, ix->cfg.vector_similarity, ix->quant_i8, ix->rows_h16.p && ix->vec_err.p, nq, k,
+                                          ceil_dev != nullptr);
+    const bool filter = vec::is_filter(scan);
+    const uint32_t passes = (nq + vec::queries_per_pass(scan) - 1) / vec::queries_per_pass(scan);   // corpus passes of the scan
+    const uint32_t nq_pad = passes * vec::queries_per_pass(scan);
     cudaStream_t st = c.st;
-    if (!ix->quant_i8) SSB_TRY(c.qpad.reserve((size_t)nq_pad * ix->dpad, 0, st));
+    if (scan != vec::Scan::I8_128) SSB_TRY(c.qpad.reserve((size_t)nq_pad * ix->dpad, 0, st));
     const size_t qbytes = (size_t)nq * ix->dims * (queries_i8 ? 1 : 4);
     const void* qsrc = queries;
     if (!dev_ptr(queries)) {
@@ -223,7 +200,7 @@ int32_t vec_keys(ssb_index* ix, SearchCtx& c, const void* queries, bool queries_
         c.stats.h2d_bytes += qbytes;
         qsrc = c.qstage.p;
     }
-    if (ix->quant_i8) {
+    if (scan == vec::Scan::I8_128) {
         SSB_TRY(c.q_i8.reserve((size_t)nq_pad * ix->dpad8, 0, st));
         if (queries_i8 && (ix->turbo || ix->cfg.vector_similarity != SSB_SIM_COSINE)) { set_error("int8 query codes are accepted for Cosine + ScalarQuantizationI8 only (the other quantisers need the query scale)"); return SSB_E_UNSUPPORTED; }
         if (ix->turbo) {
@@ -250,7 +227,7 @@ int32_t vec_keys(ssb_index* ix, SearchCtx& c, const void* queries, bool queries_
             // the query is normalised and quantised exactly like the corpus (search.rs:1464-1475, vector_similarity.rs:1226-1232)
             SSB_TRY(vec::launch_quantize_rows_i8((const float*)qsrc, ix->dims, nq, nq_pad, ix->dims, c.q_i8.p, ix->dpad8, st));
         }
-    } else if (use_tc && tc_bf16) {
+    } else if (filter || scan == vec::Scan::Bf16_64 || scan == vec::Scan::Bf16_128 || scan == vec::Scan::Bf16_256) {
         // one launch: pad + normalise + bf16 hi/lo split (the scan reads only the split parts)
         SSB_TRY(c.qhi.reserve((size_t)nq_pad * ix->dpad, 0, st));
         SSB_TRY(c.qlo.reserve((size_t)nq_pad * ix->dpad, 0, st));
@@ -263,7 +240,7 @@ int32_t vec_keys(ssb_index* ix, SearchCtx& c, const void* queries, bool queries_
                                      ix->cfg.vector_similarity == SSB_SIM_COSINE, st));
     c.stats.kernel_launches += 1;
     if (ix->n_rows == 0) { SSB_CUDA_TRY(cudaMemsetAsync(keys_out_dev, 0, (size_t)nq * LIST * 8, st)); return SSB_OK; }
-    size_t sb = use_tc ? vec::scan_tc_scratch_bytes(ix->n_sms, nq_pad) : vec::scan_scratch_bytes(ix->n_sms, nq_pad);
+    size_t sb = vec::is_tensor_core(scan) ? vec::scan_tc_scratch_bytes(ix->n_sms, nq_pad) : vec::scan_scratch_bytes(ix->n_sms, nq_pad);
     const size_t head_words = sb / 8 + (size_t)nq_pad * LIST + (nq_pad + 1) / 2;
     SSB_TRY(c.scratch.reserve(head_words + (filter ? vec::refine_scratch_words(ix->n_sms, nq_pad) : 0), 0, st));
     vec::ScanArgs a{};
@@ -291,39 +268,38 @@ int32_t vec_keys(ssb_index* ix, SearchCtx& c, const void* queries, bool queries_
         SSB_TRY(vec::launch_ivf_select(v, st));
         a.ivf_sel = c.ivf_sel.p; a.ivf_words = v.words; a.row_cluster = ix->row_cluster.p;
     }
-    if (ix->quant_i8) {
+    if (scan == vec::Scan::I8_128) {
         a.rows_i8 = ix->rows_i8.p; a.queries_i8 = c.q_i8.p; a.dpad8 = ix->dpad8;
         if (ix->turbo || ix->cfg.vector_similarity != SSB_SIM_COSINE) {
             a.i8_scaled = ix->cfg.vector_similarity == SSB_SIM_EUCLIDEAN ? (ix->affine ? 3 : 2) : 1;
             a.row_aff = ix->row_aff.p; a.q_aff = c.q_aff.p;
             a.row_scale = ix->row_scale.p; a.row_norm = ix->row_norm.p; a.q_scale = c.q_scale.p; a.q_norm = c.q_norm.p;
         }
-        SSB_TRY(vec::launch_scan_tc(a, 128, 2, st));
-    } else if (use_tc) {
+    } else if (vec::is_tensor_core(scan)) {
         SSB_TRY(c.qhi.reserve((size_t)nq_pad * ix->dpad, 0, st));
         SSB_TRY(c.qlo.reserve((size_t)nq_pad * ix->dpad, 0, st));
         a.q_hi = c.qhi.p; a.q_lo = c.qlo.p;
         if (filter) a.q_scale = c.q_scale.p;
-        SSB_TRY(vec::launch_scan_tc(a, qt, filter ? (kern == SSB_VEC_KERNEL_TCGEN05_FILTER_N256_PAIR ? 4 : 3) : (tc_bf16 ? 1 : 0), st));
-        if (filter) {
-            vec::RefineArgs r{};
-            r.rows = ix->rows.p; r.doc_ids = ix->doc_ids.p; r.n_rows = ix->n_rows; r.dpad = ix->dpad; r.queries_padded = c.qpad.p; r.margin = c.q_scale.p;
-            r.keys = merged; r.keys_out = keys_out_dev;   // the refine step writes the caller's buffer directly
-            r.nq = nq; r.nq_pad = nq_pad; r.k = k;
-            r.fb_lists = c.scratch.p + head_words;
-            r.fb_state = reinterpret_cast<uint32_t*>(r.fb_lists + (size_t)nq_pad * ix->n_sms * LIST);
-            r.del_slot = a.del_slot; r.del_words = a.del_words; r.ivf_sel = a.ivf_sel; r.ivf_words = a.ivf_words; r.row_cluster = a.row_cluster; r.n_sms = ix->n_sms; r.launches = &c.stats.kernel_launches;
-            SSB_TRY(vec::launch_refine(r, st));
-            c.fb_state = r.fb_state;
-        }
-    } else {
-        SSB_TRY(vec::launch_scan_ffma(a, st));
     }
-    if (!filter) SSB_CUDA_TRY(cudaMemcpyAsync(keys_out_dev, merged, (size_t)nq * LIST * 8, cudaMemcpyDeviceToDevice, st));
-    c.stats.algorithmic_bytes += (uint64_t)(nq_pad / qt) * ix->n_rows * ix->dims * (ix->quant_i8 ? 1 : 4);
-    // bytes the scan kernel actually streams per call: the filter scan reads the 2-byte hi plane, the refine step <= 32 f32 rows per query
-    c.stats.scan_bytes_read += filter ? (uint64_t)(nq_pad / qt) * ix->n_rows * ix->dims * 2 + (uint64_t)nq * LIST * ix->dims * 4
-                                      : (uint64_t)(nq_pad / qt) * ix->n_rows * ix->dims * (ix->quant_i8 ? 1 : 4);
+    SSB_TRY(vec::is_tensor_core(scan) ? vec::launch_scan_tc(a, scan, st) : vec::launch_scan_ffma(a, st));
+    if (filter) {
+        vec::RefineArgs r{};
+        r.rows = ix->rows.p; r.doc_ids = ix->doc_ids.p; r.n_rows = ix->n_rows; r.dpad = ix->dpad; r.queries_padded = c.qpad.p; r.margin = c.q_scale.p;
+        r.keys = merged; r.keys_out = keys_out_dev;   // the refine step writes the caller's buffer directly
+        r.nq = nq; r.nq_pad = nq_pad; r.k = k;
+        r.fb_lists = c.scratch.p + head_words;
+        r.fb_state = reinterpret_cast<uint32_t*>(r.fb_lists + (size_t)nq_pad * ix->n_sms * LIST);
+        r.del_slot = a.del_slot; r.del_words = a.del_words; r.ivf_sel = a.ivf_sel; r.ivf_words = a.ivf_words; r.row_cluster = a.row_cluster; r.n_sms = ix->n_sms; r.launches = &c.stats.kernel_launches;
+        SSB_TRY(vec::launch_refine(r, st));
+        c.fb_state = r.fb_state;
+    } else {
+        SSB_CUDA_TRY(cudaMemcpyAsync(keys_out_dev, merged, (size_t)nq * LIST * 8, cudaMemcpyDeviceToDevice, st));
+    }
+    const uint64_t pass_bytes = ix->n_rows * ix->dims * (scan == vec::Scan::I8_128 ? 1 : 4);   // algorithmic bytes of one corpus pass
+    c.stats.algorithmic_bytes += passes * pass_bytes;
+    // bytes the scan kernel actually streams per call: the filter scan reads the 2-byte fp16 plane (half the f32 bytes), the refine step
+    // <= 32 f32 rows per query
+    c.stats.scan_bytes_read += filter ? passes * pass_bytes / 2 + (uint64_t)nq * LIST * ix->dims * 4 : passes * pass_bytes;
     return SSB_OK;
 }
 
@@ -478,6 +454,7 @@ int32_t ssb_create(const ssb_config* cfg, ssb_index** out) {
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); set_error("no CUDA device visible: libseekstorm_b200 has no CPU fallback"); return SSB_E_NO_DEVICE; }
     if (cfg->device < 0 || cfg->device >= ndev) { set_error("device %d out of range (%d visible)", cfg->device, ndev); return SSB_E_INVALID; }
     if (cfg->vector_similarity > SSB_SIM_EUCLIDEAN) { set_error("bad vector_similarity"); return SSB_E_INVALID; }
+    if (cfg->vector_kernel > SSB_VEC_KERNEL_TCGEN05_FILTER_N256_PAIR) { set_error("bad vector kernel"); return SSB_E_INVALID; }
     if (cfg->vector_quantization > SSB_QUANT_TURBO_I8) { set_error("bad vector_quantization"); return SSB_E_INVALID; }
     if (cfg->vector_quantization == SSB_QUANT_TURBO_I8 && cfg->vector_dims > 16384) { set_error("TurboQuantI8: vector_dims above 16384 unsupported"); return SSB_E_UNSUPPORTED; }
     SSB_CUDA_TRY(cudaSetDevice(cfg->device));

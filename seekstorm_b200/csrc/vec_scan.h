@@ -3,10 +3,11 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "common.cuh"
+#include "scan_plan.h"
+
 namespace ssb {
 namespace vec {
-
-constexpr int VEC_QT = 16;      // queries per corpus pass of the FFMA kernel
 
 struct ScanArgs {
     const float* rows;            // [n_rows][dpad]
@@ -15,7 +16,7 @@ struct ScanArgs {
     const uint32_t* doc_ids;      // [n_rows] or nullptr
     uint64_t n_rows;
     uint32_t dpad;                // multiple of 32
-    const float* queries_padded;  // [nq_pad][dpad], nq_pad multiple of VEC_QT
+    const float* queries_padded;  // [nq_pad][dpad], nq_pad a multiple of the scan's queries_per_pass
     uint32_t nq_pad;
     uint32_t nq_valid = 0;         // real queries; rows >= nq_valid are zero padding and must never collect candidates
     uint32_t k;
@@ -44,21 +45,26 @@ struct ScanArgs {
     const uint32_t* ivf_sel = nullptr; uint32_t ivf_words = 0; const uint32_t* row_cluster = nullptr;
 };
 
-// rows scanned first to seed the per-query top-k thresholds (0 = shard too small to bother).  With S sample rows the full
-// scan sees ~k*N/S threshold passes per query in total, while in the sample pass itself every row passes at first.
-// Measured on 1M x 768: the FP32 scan (inserts stall the FFMA warps) is best at ~N/32 (94-95 % of HBM peak vs 89 % at
-// N/128); the tensor-core scan (inserts run in separate epilogue warps) is best at ~N/128.
-inline uint64_t vec_presample_rows(uint64_t n_rows, bool tensor_core) {
-    if (n_rows < 65536) return 0;
-    uint64_t s = tensor_core ? n_rows / 128 : n_rows / 32;
-    const uint64_t lo = tensor_core ? 2048 : 4096, hi = tensor_core ? 8192 : 32768;
-    s = s < lo ? lo : (s > hi ? hi : s);
-    return s / 512 * 512;
+// Threshold seeding: `launch` first scans the first `sample_rows` rows keeping only each 32-row group's best score per query (no
+// lists, no merge); the k-th largest of those group maxima (kth_from_groupmax) is a valid lower bound of the final k-th best score —
+// k different groups each hold a row at least that good — and, written to thr_buf, seeds the threshold of the full scan: results are
+// unchanged, but the expected number of list insertions per query drops from ~k*ln(rows/k) PER LIST to ~k*N/S in total.  Skipped
+// below 64 K rows, and with a delete set or an IVF mask: a deleted or unselected row must never seed a threshold.
+template <class F>
+int32_t with_threshold_seed(const ScanArgs& a, uint64_t sample_rows, F launch) {
+    if (a.thr_init || !a.thr_buf || a.del_slot || a.ivf_sel || a.n_rows < 65536) return launch(a);
+    ScanArgs pre = a;
+    pre.n_rows = sample_rows; pre.ev0 = nullptr; pre.ev1 = nullptr;
+    pre.sample_groupmax = true;   // the sample launch writes the thresholds (thr_buf) itself
+    SSB_TRY(launch(pre));
+    ScanArgs full = a;
+    full.thr_init = a.thr_buf;
+    return launch(full);
 }
 
 int32_t launch_scan_ffma(const ScanArgs& a, cudaStream_t st);
 size_t scan_scratch_bytes(int n_sms, uint32_t nq_pad);
-int32_t launch_scan_tc(const ScanArgs& a, uint32_t nq_tile /*64|128|256*/, int prec /*0: 3xTF32, 1: 3xBF16, 2: int8 (exact), 3: fp16 filter (q_scale = margins)*/, cudaStream_t st);
+int32_t launch_scan_tc(const ScanArgs& a, Scan s /*any but Scan::Ffma*/, cudaStream_t st);
 size_t scan_tc_scratch_bytes(int n_sms, uint32_t nq_pad);
 // fused query preparation of the bf16 tensor-core scan: pad + (Cosine) normalise + hi/lo split in one launch
 int32_t launch_prep_split_queries_bf16(const float* q, uint32_t nq, uint32_t dims, uint64_t qstride, void* hi, void* lo, uint32_t nq_pad,

@@ -819,14 +819,22 @@ static int32_t launch_tc_n(const ScanArgs& a, cudaStream_t st) {
     return SSB_OK;
 }
 
-static int32_t launch_scan_tc_impl(const ScanArgs& a, uint32_t nq_tile, int prec /*0 tf32, 1 bf16, 2 int8, 3 fp16 filter, 4 fp16 filter on CTA pairs*/, cudaStream_t st) {
+static int32_t launch_scan_tc_impl(const ScanArgs& a, Scan s, cudaStream_t st) {
     if (a.n_rows == 0 || a.nq_pad == 0) return SSB_OK;
-    if (prec == 4) {   // the seeding pass stays on one CTA per SM
-        if (a.nq_pad % 256 != 0) { set_error("tensor-core pair scan: query count must be padded to 256"); return SSB_E_INVALID; }
+    if (a.nq_pad % queries_per_pass(s) != 0) { set_error("tensor-core scan: query count must be padded to the %u-query tile", queries_per_pass(s)); return SSB_E_INVALID; }
+    if (s != Scan::I8_128 && a.similarity == SSB_SIM_EUCLIDEAN) { set_error("tensor-core scan supports Dot/Cosine only"); return SSB_E_UNSUPPORTED; }
+    switch (s) {
+    case Scan::Tf32_64: return launch_tc_n<64, tc::PREC_TF32>(a, st);
+    case Scan::Tf32_128: return launch_tc_n<128, tc::PREC_TF32>(a, st);
+    case Scan::Bf16_64: return launch_tc_n<64, tc::PREC_BF16>(a, st);
+    case Scan::Bf16_128: return launch_tc_n<128, tc::PREC_BF16>(a, st);
+    case Scan::Bf16_256: return launch_tc_n<256, tc::PREC_BF16>(a, st);
+    case Scan::F16f_128: return launch_tc_n<128, tc::PREC_F16F>(a, st);
+    case Scan::F16f_256: return launch_tc_n<256, tc::PREC_F16F>(a, st);
+    case Scan::F16f_256Pair:   // the seeding pass stays on one CTA per SM
         return a.sample_groupmax ? launch_tc_n<256, tc::PREC_F16F>(a, st) : launch_tc_n<256, tc::PREC_F16F, false, 0, true>(a, st);
-    }
-    if (prec == 2) {
-        if (nq_tile != 128 || a.nq_pad % 128 != 0 || !a.rows_i8 || !a.queries_i8 || a.dpad8 % 128) { set_error("int8 scan: bad arguments"); return SSB_E_INVALID; }
+    case Scan::I8_128: {
+        if (!a.rows_i8 || !a.queries_i8 || a.dpad8 % 128) { set_error("int8 scan: bad arguments"); return SSB_E_INVALID; }
         const bool res = tc::i8_resident(a.dpad8);   // query block resident in smem when it leaves room for >= 3 corpus stages, else streamed per stage
         if (a.i8_scaled) {
             if (!a.row_scale || !a.q_scale || (a.i8_scaled >= 2 && (!a.row_norm || !a.q_norm)) || (a.i8_scaled == 3 && (!a.row_aff || !a.q_aff))) { set_error("scaled int8 scan: missing scale / norm arrays"); return SSB_E_INVALID; }
@@ -836,39 +844,25 @@ static int32_t launch_scan_tc_impl(const ScanArgs& a, uint32_t nq_tile, int prec
         }
         return res ? launch_tc_n<128, tc::PREC_I8, true>(a, st) : launch_tc_n<128, tc::PREC_I8, false>(a, st);
     }
-    if (a.similarity == SSB_SIM_EUCLIDEAN) { set_error("tensor-core scan supports Dot/Cosine only"); return SSB_E_UNSUPPORTED; }
-    if (prec == 3) {
-        if ((nq_tile != 128 && nq_tile != 256) || a.nq_pad % nq_tile != 0) { set_error("tensor-core filter scan: query count must be padded to the 128/256 query tile"); return SSB_E_INVALID; }
-        return nq_tile == 256 ? launch_tc_n<256, tc::PREC_F16F>(a, st) : launch_tc_n<128, tc::PREC_F16F>(a, st);
+    case Scan::Ffma: break;
     }
-    if ((nq_tile != 64 && nq_tile != 128 && !(nq_tile == 256 && prec == 1)) || a.nq_pad % nq_tile != 0) { set_error("tensor-core scan: query count must be padded to the 64/128(/256 bf16) query tile"); return SSB_E_INVALID; }
-    if (prec == 1) return nq_tile == 64 ? launch_tc_n<64, tc::PREC_BF16>(a, st) : (nq_tile == 256 ? launch_tc_n<256, tc::PREC_BF16>(a, st) : launch_tc_n<128, tc::PREC_BF16>(a, st));
-    return nq_tile == 64 ? launch_tc_n<64, tc::PREC_TF32>(a, st) : launch_tc_n<128, tc::PREC_TF32>(a, st);
+    set_error("tensor-core scan: the FP32 scan is launch_scan_ffma"); return SSB_E_INVALID;
 }
 
-int32_t launch_scan_tc(const ScanArgs& a, uint32_t nq_tile, int prec, cudaStream_t st) {
-    // threshold pre-sampling (see vec_scan.cu): scan the first rows, seed the thresholds, then the full scan
-    // (with a delete set the sample pass is skipped: a deleted row must never seed a threshold)
-    if (a.thr_init || !a.thr_buf || a.del_slot || a.ivf_sel || vec_presample_rows(a.n_rows, true) == 0) return launch_scan_tc_impl(a, nq_tile, prec, st);
-    ScanArgs pre = a;
+int32_t launch_scan_tc(const ScanArgs& a, Scan s, cudaStream_t st) {
     // The sample pass writes per-(32-row group, query) score maxima instead of lists (no insert storm) and costs the same for one
     // 256-row tile per CTA as for a handful of tiles: sample one tile per SM.  (An earlier version ran the normal list epilogue
     // over N/128 rows: ~90 us per pass, and ncu showed the full scan's epilogue warps waiting on list loads for candidates that
     // a better seed rejects.)
-    const uint64_t trows = nq_tile == 256 ? 128 : tc::TROWS;      // rows per stage of the variant that will run
+    const uint64_t trows = queries_per_pass(s) == 256 ? 128 : tc::TROWS;   // rows per stage of the variant that will run
     // sample tiles per SM: the seed is the k-th best of S sampled rows, the full scan then sees ~k*N/S candidates per query, each a
     // ~1 us latency-bound list insert for an epilogue warp.  The filter scan streams a pass in half the time of the 3-product scan, so the
     // same insert load weighs twice as much: it samples more (SSB_TC_SAMPLE_TILES overrides; measured in DESIGN.md §3.2c)
     static const int env_tiles = [] { const char* e = getenv("SSB_TC_SAMPLE_TILES"); return e ? atoi(e) : 0; }();
-    const int sample_tiles = env_tiles > 0 ? (env_tiles > 16 ? 16 : env_tiles) : ((prec >= 3 && nq_tile == 256) ? 2 : 1);
-    uint64_t s = (uint64_t)a.n_sms * trows * sample_tiles;
-    if (s > a.n_rows / 4) s = a.n_rows / 4 / trows * trows;
-    pre.n_rows = s; pre.ev0 = nullptr; pre.ev1 = nullptr;
-    pre.sample_groupmax = true;                          // writes the thresholds straight into thr_buf
-    SSB_TRY(launch_scan_tc_impl(pre, nq_tile, prec, st));
-    ScanArgs full = a;
-    full.thr_init = a.thr_buf;
-    return launch_scan_tc_impl(full, nq_tile, prec, st);
+    const int sample_tiles = env_tiles > 0 ? (env_tiles > 16 ? 16 : env_tiles) : ((s == Scan::F16f_256 || s == Scan::F16f_256Pair) ? 2 : 1);
+    uint64_t rows = (uint64_t)a.n_sms * trows * sample_tiles;
+    if (rows > a.n_rows / 4) rows = a.n_rows / 4 / trows * trows;
+    return with_threshold_seed(a, rows, [s, st](const ScanArgs& x) { return launch_scan_tc_impl(x, s, st); });
 }
 
 void launch_kth_from_groupmax(const void* gmax, uint32_t n_groups, uint32_t nq, uint32_t k, uint32_t* thr, int is_int, cudaStream_t st) {

@@ -159,7 +159,8 @@ class Index:
                  term_key_fn: Callable[[str], int] = synthetic_term_key, vector_kernel: int = 0,
                  vector_quantization: int = 0):
         """vector_kernel: SSB_VEC_KERNEL_* (0 = auto, 1 = FP32 FFMA scan, 2/3 = wgmma 3xTF32, 4/5/6 = wgmma 3xBF16 with 128/64/256
-        queries per pass, 7/8 = bf16 filter scan + exact f32 refine with 128/256 queries per pass)."""
+        queries per pass, 7/8 = fp16 filter scan + exact f32 refine with 128/256 queries per pass, 9 = the 256-query filter scan on
+        CTA pairs).  include/seekstorm_b200.h states what AUTO picks and when the filter scans fall back."""
         self._h = C.c_void_p()
         cfg = SsbConfig(device, max_batch, vector_dims, int(vector_similarity), vector_kernel, int(vector_quantization),
                         (C.c_uint32 * 2)(0, 0))
@@ -359,7 +360,7 @@ class Index:
             self.add_vector_level(first_level + s // 65536, rows[s:min(n, s + 65536)])
 
     def set_vector_kernel(self, kernel: int):
-        """0 = auto, 1 = FP32 FFMA scan, 2/3 = wgmma 3xTF32 (128/64 queries per pass), 4/5/6 = wgmma 3xBF16 (128/64/256)."""
+        """SSB_VEC_KERNEL_*, as `vector_kernel` of the constructor."""
         check(lib().ssb_set_vector_kernel(self._h, kernel))
 
     @property
