@@ -19,17 +19,20 @@
 // delivers them straight into the MMA-ready SWIZZLE_64B tiles: no splitting pass over the tile in shared memory.  PREC_TF32 keeps
 // the f32 corpus and splits each stage in shared memory (out of place for the lo part).
 //
-// Warp roles (384 threads = 3 warpgroups, 1 CTA/SM): warpgroup 0 = TMA producer (one thread), warpgroups 1-2 = consumers.  Consumer
+// Warp roles (384 threads = 3 warpgroups, 1 CTA/SM): warpgroup 0 = TMA producer (one thread; 256 queries: + 3 list warps), warpgroups 1-2 = consumers.  Consumer
 // warpgroup c owns the query columns [c*NQ/2, (c+1)*NQ/2) of the block and all TROWS corpus rows of a tile (TROWS/64 m64 sub-tiles,
-// at most 128 accumulator registers per thread); warp w of the warpgroup owns rows 16w..16w+15 of every sub-tile and list w of the
-// warpgroup's queries, so each (list, query) pair has exactly one writer, as in the scratch layout [4 lists][NQ][32] per CTA.
+// at most 128 accumulator registers per thread); warp w of the warpgroup owns rows 16w..16w+15 of every sub-tile and (64/128 queries)
+// list w of the warpgroup's queries, so each (list, query) pair has exactly one writer, as in the scratch layout [4 lists][NQ][32] per CTA.
 // Per stage both consumer warpgroups wait on the full barrier, issue their MMAs as one commit group (one group kept in flight) and
 // release the stage once its group retired.  Epilogue per tile (the producer keeps streaming up to STAGES stages ahead meanwhile):
 // the accumulator fragment goes 8 query columns at a time through a small per-warp shared-memory buffer into a lane = corpus row
 // layout (one pass = 32 rows = two sub-tiles); the whole chunk is tested against the per-query thresholds branch-free with ONE vote,
 // and only chunks with a candidate take the per-column path (ballot, per-warp sorted lists in the CTA's slice of the output scratch,
 // no CTA barriers).  The 256-query kernels take that vote on the fragment itself, before the transposition, so that a chunk without
-// a candidate costs no shared-memory traffic.
+// a candidate costs no shared-memory traffic.  When the scan is seeded they do no list work in the consumer warps: a chunk that passes is written as a
+// record into a shared-memory queue, and warps 1-3 of warpgroup 0 (idle otherwise: one thread issues the TMA loads) run the exact test
+// and the inserts into one list per query per CTA ([NQ][32]), each warp for a fixed third of the 8-query chunks.  An insert is ~1 us of
+// latency-bound work; in the consumer warps it held both warpgroups, and with them the tensor pipe, at the end of every tile.
 // Threshold seeding: the same kernel runs first in sample mode over one tile per SM and writes per-(32-row group, query) score
 // maxima; kth_from_groupmax turns them into valid lower bounds of the k-th best score.
 #include <cuda_bf16.h>
@@ -52,7 +55,13 @@ constexpr int A1_BYTES = TM * KC * 4;  // one 128-row f32 tile, 16 KB
 constexpr int THREADS = 384;           // 3 warpgroups: TMA producer, 2 MMA + epilogue
 constexpr int CHUNK = 8;               // query columns per epilogue step
 constexpr int XB_STRIDE = CHUNK + 1;   // per-warp transposition buffer [32 rows][CHUNK] (+1 column: conflict-free row reads)
-constexpr int XB_BYTES = 8 * 32 * XB_STRIDE * 4;
+constexpr int REC_WORDS = 32 * XB_STRIDE;     // one warp's buffer: 32 rows x CHUNK scores
+constexpr int XB_BYTES = 8 * REC_WORDS * 4;
+// QUEUE kernels (seeded 256-query scans): the buffers form a queue of chunk records (one chunk = 32 rows x 8 queries that passed the
+// vote) from the consumer warps to the list warps, plus per slot a state word (0 free, 1 being written, 2 + chunk = ready) and the
+// record's (tile, warp), and a count of finished consumer warps.  26 slots keep the 256-query configurations at 4 stages.
+constexpr int QSLOTS = 26;
+constexpr int QUEUE_BYTES = QSLOTS * REC_WORDS * 4 + (3 * QSLOTS + 2) * 4;
 constexpr int SMEM_MAX = 232448;       // 227 KB opt-in limit per CTA
 constexpr uint32_t ORD_NEG_INF = 0x007FFFFFu;   // ord_f32(-inf)
 enum { PREC_TF32 = 0, PREC_BF16 = 1, PREC_I8 = 2, PREC_F16F = 3 };
@@ -69,7 +78,7 @@ enum { PREC_TF32 = 0, PREC_BF16 = 1, PREC_I8 = 2, PREC_F16F = 3 };
 // stage instead of a whole one, and a stage is refilled once the consumers of BOTH CTAs released it.
 
 constexpr int MAX_STAGES = 6;
-template <int NQ, int PREC, bool BRES = false> struct Cfg {
+template <int NQ, int PREC, bool BRES = false, bool QUEUE = false> struct Cfg {
     // at most 128 accumulator registers per consumer thread (TROWS/64 sub-tiles x NQ/4): 256 queries -> one 128-row tile per stage (the
     // corpus is streamed once per 256 queries: half the HBM bytes per query); tf32 -> 128 rows too (its stage also holds the lo part)
     static constexpr int MT = (NQ == 256 || PREC == PREC_TF32) ? 1 : 2;
@@ -91,10 +100,15 @@ template <int NQ, int PREC, bool BRES = false> struct Cfg {
     // so the per-stage L2->SM traffic is the corpus tile alone (stage count chosen at launch from what is left of 227 KB)
     static constexpr int STAGE_BYTES = BRES ? A_BYTES : ((PREC == PREC_I8 || PREC == PREC_F16F) ? A_BYTES + B_BYTES : (PREC == PREC_BF16 ? A_BYTES + 2 * B_BYTES : 2 * A_BYTES + 2 * B_BYTES));
     static constexpr int TX_BYTES = BRES ? A_BYTES : ((PREC == PREC_I8 || PREC == PREC_F16F) ? A_BYTES + B_BYTES : A_BYTES + 2 * B_BYTES);
-    // transposition buffers + thresholds + (scaled int8) per-query scale / norm + barriers + alignment slack of the dynamic segment
-    static constexpr int FIXED = XB_BYTES + NQ * 12 + 256 + 1024;
+    // transposition buffers (QUEUE: the record queue) + thresholds + (scaled int8) per-query scale / norm + barriers + alignment
+    // slack of the dynamic segment
+    static constexpr int XB_REGION = QUEUE ? QUEUE_BYTES : XB_BYTES;
+    static constexpr int FIXED = XB_REGION + NQ * 12 + 256 + 1024;
     static constexpr int STAGES = (SMEM_MAX - FIXED) / STAGE_BYTES > MAX_STAGES ? MAX_STAGES : (SMEM_MAX - FIXED) / STAGE_BYTES;
     static constexpr int SMEM = STAGES * STAGE_BYTES + FIXED;
+    static_assert(!QUEUE || (NQ == 256 && !BRES && STAGES >= 4), "the record queue is for the 256-query kernels and must leave them 4 stages");
+    // a record names its rows by (tile, consumer warp): one pair of m64 sub-tiles per tile
+    static_assert(!QUEUE || MW == 2, "queue records hold the one 32-row pass of a 128-row tile");
 };
 // int8: the query block stays resident when it leaves room for 3 corpus stages
 constexpr bool i8_resident(uint32_t dpad8) { return (int)dpad8 * 128 + Cfg<128, PREC_I8, true>::FIXED + 3 * Cfg<128, PREC_I8, true>::A_BYTES <= SMEM_MAX; }
@@ -271,7 +285,7 @@ __device__ __forceinline__ uint32_t bf16x2(float x, float y) {
 // variant (integer-valued 0..255 data, euclidean_i8_quantized_affine :1770-1795): the int32 dot product is first corrected for the two zero
 // points, dot - zp_row*sum_q(query) - zp_query*sum_q(row) + n*zp_query*zp_row, regrouped as dot - zp_row*sum_q(query) + zp_query*(n*zp_row - sum_q(row))
 // Unscaled int8 scores are the int32 dot products as f32 (exact below 2^24), so every variant runs the same f32-score epilogue.
-template <int NQ, int PREC, bool BRES, int SCALED, bool PAIR>
+template <int NQ, int PREC, bool BRES, int SCALED, bool PAIR, bool QUEUE>
 __global__ void __launch_bounds__(THREADS, 1)
 scan_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2 /*bf16: lo plane*/,
         const __grid_constant__ CUtensorMap tmBh, const __grid_constant__ CUtensorMap tmBl, uint32_t n_rows, uint32_t n_kchunks, uint32_t n_tiles, uint32_t k,
@@ -284,7 +298,7 @@ scan_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtenso
         const int2* __restrict__ row_aff /*SCALED 3: [n_rows] (zero_point, dims*zero_point - sum_q)*/, const int2* __restrict__ q_aff /*SCALED 3: [gridDim.y*NQ] (zero_point, sum_q)*/,
         const uint32_t* __restrict__ ivf_sel, uint32_t ivf_words, const uint32_t* __restrict__ row_cluster /*IVF selection mask or null*/,
         uint32_t sample_mode /*write per-(32-row group, query) score maxima instead of lists*/) {
-    using C = Cfg<NQ, PREC, BRES>;
+    using C = Cfg<NQ, PREC, BRES, QUEUE>;
     constexpr int TROWS = C::TROWS, MW = C::MW, NQH = C::NQH;
     // 256 queries: the tensor pipe, not HBM, sets the pass time, and the epilogue stalls it -> the common-case test runs on the
     // accumulator fragment, without the shared-memory transposition
@@ -295,12 +309,19 @@ scan_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtenso
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     uint8_t* stage0 = base;
+    // QUEUE (256 queries, seeded scan; chosen at launch): chunks with a candidate go through the record queue to the list warps, one
+    // list per query per CTA.  Unseeded (no sample pass: delete set, IVF mask, < 65536 rows) the first tiles are an insert storm that the
+    // 8 consumer warps clear faster than 3 list warps, so the other instantiation keeps the per-warp lists, inserts in the consumers and
+    // gives the producer warpgroup's registers to them, as in the 64/128-query kernels.
     // per-query sorted lists live directly in this CTA's slice of the output scratch (global, L2-resident): they are
-    // touched only on the rare candidate insert, and each (warp, query) list is always owned by the same warp
-    uint64_t* lists = scratch + ((size_t)blockIdx.y * gridDim.x + blockIdx.x) * 4 * NQ * LIST;   // [4 lists][NQ][32]
+    // touched only on the rare candidate insert, and each list is always owned by the same warp
+    uint64_t* lists = scratch + ((size_t)blockIdx.y * gridDim.x + blockIdx.x) * (QUEUE ? 1 : 4) * NQ * LIST;   // [QUEUE ? 1 : 4][NQ][32]
     uint8_t* bres = base + STAGES * C::STAGE_BYTES;                           // BRES: resident query block
-    uint32_t* xbuf = (uint32_t*)(bres + (BRES ? n_kchunks * C::B_BYTES : 0)); // [8 consumer warps][32][XB_STRIDE]
-    uint32_t* thr_u = xbuf + XB_BYTES / 4;        // [NQ] ordered-uint score thresholds
+    uint32_t* xbuf = (uint32_t*)(bres + (BRES ? n_kchunks * C::B_BYTES : 0)); // [8 consumer warps | QSLOTS records][32][XB_STRIDE]
+    volatile uint32_t* qstate = xbuf + QSLOTS * REC_WORDS;                    // 256 queries: [QSLOTS] slot states
+    volatile uint32_t* qmeta = qstate + QSLOTS;                               //              [QSLOTS][2] (tile, consumer warp 0-3)
+    volatile uint32_t* qdone = qmeta + 2 * QSLOTS;                            //              consumer warps finished
+    uint32_t* thr_u = xbuf + C::XB_REGION / 4;    // [NQ] ordered-uint score thresholds
     float* qs_sm = (float*)(thr_u + NQ);          // [NQ] SCALED: query scale; filter scan: margin
     float* qn_sm = qs_sm + NQ;                    // [NQ] SCALED: query norm
     uint64_t* bars = (uint64_t*)(thr_u + 3 * NQ);
@@ -324,13 +345,56 @@ scan_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtenso
         if (PREC == PREC_F16F) qs_sm[i] = __ldg(&q_scale[blockIdx.y * NQ + i]);   // filter scan: per-query margin 2 eps_q
         if (SCALED) { qs_sm[i] = __ldg(&q_scale[blockIdx.y * NQ + i]); qn_sm[i] = SCALED >= 2 ? __ldg(&q_norm[blockIdx.y * NQ + i]) : 0.f; }
     }
+    if (QUEUE && threadIdx.x < QSLOTS) qstate[threadIdx.x] = 0u;
+    if (QUEUE && threadIdx.x == 0) *qdone = 0u;
     __syncthreads();
     if (PAIR) cluster_sync_all();                 // both CTAs' barriers are initialised before anything arrives on them
 
     // a pair walks pairs of neighbouring tiles; both CTAs take the same number of steps (the peer's multicast feeds both)
     const uint32_t tile0 = PAIR ? (blockIdx.x & ~1u) + rank : blockIdx.x;
+
+    // The exact candidate test and list insert for one 8-query chunk c of 32 rows: lane = corpus row `row`, its CHUNK scores (f32 bits)
+    // at xr[0..CHUNK).  Per column: ballot of the rows at or above the query's threshold, delete set / IVF mask / paging ceiling, then
+    // one insert per key or (warm-up tiles: many rows pass) a bulk sort + merge into the list, and the threshold rises to its k-th
+    // best (filter scan: lowered by the query's margin).  A runtime loop keeps one copy of this path.  QUEUE kernels run only seeded,
+    // and a delete set or an IVF mask turns the seed off (the launcher checks it): they have no delete / IVF test.
+    auto insert_chunk = [&](const uint32_t* xr, uint32_t row, bool valid, int c, uint64_t* qlists) {
+#pragma unroll 1
+        for (int j = 0; j < CHUNK; j++) {
+            const int q = c * CHUNK + j;
+            const float sc = __uint_as_float(xr[j]);
+            const uint32_t so = ord_f32(sc);
+            const bool pass = valid && sc == sc && so >= thr_u[q];
+            unsigned pm = __ballot_sync(FULL, pass);
+            if (!pm) continue;
+            uint64_t key = 0;
+            if (pass) {
+                const uint32_t doc = doc_ids ? __ldg(&doc_ids[row]) : row;
+                key = ((uint64_t)so << 32) | (uint64_t)(0xFFFFFFFFu - (PREC == PREC_F16F ? row : doc));   // filter scan: candidates are named by row
+                if (!QUEUE && (doc_deleted(del_slot, del_words, doc) || ivf_skipped(ivf_sel, ivf_words, blockIdx.y * NQ + q, row_cluster, row))) key = 0;
+            }
+            if (ceil_keys || (!QUEUE && (del_slot || ivf_sel))) {   // paging: keys >= ceil were returned by an earlier page (0 = exhausted)
+                if (ceil_keys) { const uint64_t ceil = __ldg(&ceil_keys[blockIdx.y * NQ + q]); if (key >= ceil) key = 0; }
+                pm = __ballot_sync(FULL, key != 0);
+                if (!pm) continue;
+            }
+            uint64_t L = qlists[q * LIST + lane];
+            if (__popc(pm) > 3) {
+                L = wl_merge(L, wl_sort_desc(key, lane), lane);
+            } else {
+                while (pm) { const int src = __ffs(pm) - 1; pm &= pm - 1; wl_insert(L, shfl64(key, src), lane); }
+            }
+            qlists[q * LIST + lane] = L;
+            uint32_t kth = (uint32_t)(shfl64(L, (int)k - 1) >> 32);
+            if (PREC == PREC_F16F && kth) kth = ord_f32(__fsub_rd(unord_f32(kth), qs_sm[q]));   // candidates: s^ >= k-th best s^ - 2 eps_q
+            if (lane == 0 && kth > thr_u[q]) atomicMax(&thr_u[q], kth);
+        }
+    };
+
     if (warp < 4) {
-        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+        // QUEUE: warps 1-3 run the list inserts and need more than the producer's registers
+        if constexpr (QUEUE) asm volatile("setmaxnreg.dec.sync.aligned.u32 64;");
+        else asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
         // ===================== TMA producer =====================
         if (warp == 0 && lane == 0) {
             tma_prefetch_desc(&tmA); tma_prefetch_desc(&tmA2); tma_prefetch_desc(&tmBh); tma_prefetch_desc(&tmBl);
@@ -355,16 +419,48 @@ scan_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtenso
                     if (PREC == PREC_TF32 || PREC == PREC_BF16) tma_load_2d(st + C::B_OFF + C::B_BYTES, &tmBl, (int)(kc * C::KCE), (int)(group * NQ), &full[s]);
                 }
             }
+        } else if (QUEUE && warp > 0) {
+            // ===================== list warps (QUEUE): drain the record queue =====================
+            // List warp r owns the 8-query chunks c with c % 3 == r, so every (CTA, query) list has one writer.  It exits once all
+            // 8 consumer warps have finished and no record of its chunks is left.
+            const uint32_t r = (uint32_t)warp - 1u;
+            for (uint32_t c = r; c < NQ / CHUNK; c += 3)
+                for (int i = lane; i < CHUNK * LIST; i += 32) lists[c * CHUNK * LIST + i] = 0;
+            __syncwarp();
+            for (;;) {
+                const bool fin = *qdone == 8u;   // read before the states: every record published before the count is seen below
+                __threadfence_block();
+                const uint32_t f = lane < QSLOTS ? qstate[lane] : 0u;
+                unsigned ready = __ballot_sync(FULL, f >= 2u && (f - 2u) % 3u == r);
+                if (!ready) {
+                    if (fin) break;
+                    __nanosleep(128);
+                    continue;
+                }
+                __threadfence_block();
+                while (ready) {
+                    const int s = __ffs(ready) - 1; ready &= ready - 1;
+                    const uint32_t tile = qmeta[2 * s], w = qmeta[2 * s + 1];
+                    const int c = (int)__shfl_sync(FULL, f, s) - 2;
+                    const uint32_t row = tile * TROWS + (uint32_t)(64 * (lane >> 4) + 16 * w + (lane & 15));
+                    insert_chunk(xbuf + s * REC_WORDS + lane * XB_STRIDE, row, row < n_rows, c, lists);
+                    __syncwarp();
+                    if (lane == 0) { __threadfence_block(); qstate[s] = 0u; }
+                }
+            }
         }
     } else {
-        asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+        // the warpgroups trade registers within the CTA's allocation, 384 x 168 = 64512: 128 x 40 + 256 x 232, or with the list warps
+        // 128 x 64 + 256 x 216 (an inc beyond what the decs released never returns)
+        if constexpr (QUEUE) asm volatile("setmaxnreg.inc.sync.aligned.u32 216;");
+        else asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
         // ===================== consumers: MMA + epilogue =====================
         const int cw = (warp - 4) >> 2;          // consumer warpgroup: query columns [cw*NQH, (cw+1)*NQH)
         const int w = warp & 3;                  // rows 16w..16w+15 of every 64-row sub-tile; list w
         const int q0 = cw * NQH;
         uint32_t* xb = xbuf + (warp - 4) * 32 * XB_STRIDE;
-        uint64_t* mylists = lists + (size_t)w * NQ * LIST;
-        if (!sample_mode)
+        uint64_t* mylists = lists + (size_t)w * NQ * LIST;   // no queue: list w of the warpgroup's queries
+        if (!QUEUE && !sample_mode)
             for (int i = lane; i < NQH * LIST; i += 32) mylists[q0 * LIST + i] = 0;
         __syncwarp();
         uint32_t* gmaxu = (uint32_t*)scratch;     // sample mode: ordered-uint group maxima [gridDim.y * NQ][n_tiles * TROWS / 32]
@@ -489,6 +585,37 @@ scan_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtenso
                                 any |= (acc[2 * p + hm][4 * jb + 2 * h] >= t0) | (acc[2 * p + hm][4 * jb + 2 * h + 1] >= t1);
                         if (!__any_sync(FULL, any)) continue;
                     }
+                    if (QUEUE) {
+                        // a candidate: the chunk goes to the list warp that owns it as a record in lane = row layout.  Claim a free
+                        // slot (wait while the queue is full: the list warps drain it whatever the consumers do), write, publish.
+                        int s;
+                        for (;;) {
+                            unsigned fr = __ballot_sync(FULL, lane < QSLOTS && qstate[lane] == 0u);
+                            int got = -1;
+                            if (lane == 0)
+                                while (fr) {
+                                    const int i = __ffs(fr) - 1; fr &= fr - 1;
+                                    if (atomicCAS((uint32_t*)&qstate[i], 0u, 1u) == 0u) { got = i; break; }
+                                }
+                            s = __shfl_sync(FULL, got, 0);
+                            if (s >= 0) break;
+                            __nanosleep(64);
+                        }
+                        uint32_t* rec = xbuf + s * REC_WORDS;
+#pragma unroll
+                        for (int hm = 0; hm < 2; hm++)
+#pragma unroll
+                            for (int h = 0; h < 2; h++) {
+                                uint32_t* d = rec + (hm * 16 + (lane >> 2) + 8 * h) * XB_STRIDE + 2 * (lane & 3);
+                                xb_put(&d[0], acc[2 * p + hm][4 * jb + 2 * h]);
+                                xb_put(&d[1], acc[2 * p + hm][4 * jb + 2 * h + 1]);
+                            }
+                        if (lane == 0) { qmeta[2 * s] = tile; qmeta[2 * s + 1] = (uint32_t)w; }
+                        __threadfence_block();
+                        __syncwarp();
+                        if (lane == 0) qstate[s] = 2u + (uint32_t)c;
+                        continue;
+                    }
                     __syncwarp();
 #pragma unroll
                     for (int hm = 0; hm < 2; hm++)
@@ -544,43 +671,16 @@ scan_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtenso
                                          (ord_f32(__uint_as_float(v[6])) >= t1.z) | (ord_f32(__uint_as_float(v[7])) >= t1.w);
                         if (!__any_sync(FULL, any && valid)) continue;
                     }
-                    // rare after warm-up: per column, from the lane's own row of the buffer (a runtime loop keeps one copy of this
-                    // path per chunk)
+                    // rare after warm-up: per column, from the lane's own row of the buffer
 #pragma unroll
                     for (int j = 0; j < CHUNK; j++) xb[lane * XB_STRIDE + j] = v[j];
-#pragma unroll 1
-                    for (int j = 0; j < CHUNK; j++) {
-                        const int q = c * CHUNK + j;
-                        const float sc = __uint_as_float(xb[lane * XB_STRIDE + j]);
-                        const uint32_t so = ord_f32(sc);
-                        const bool pass = valid && sc == sc && so >= thr_u[q];
-                        unsigned pm = __ballot_sync(FULL, pass);
-                        if (!pm) continue;
-                        uint64_t key = 0;
-                        if (pass) {
-                            const uint32_t doc = doc_ids ? __ldg(&doc_ids[row]) : row;
-                            key = ((uint64_t)so << 32) | (uint64_t)(0xFFFFFFFFu - (PREC == PREC_F16F ? row : doc));   // filter scan: candidates are named by row
-                            if (doc_deleted(del_slot, del_words, doc) || ivf_skipped(ivf_sel, ivf_words, blockIdx.y * NQ + q, row_cluster, row)) key = 0;
-                        }
-                        if (ceil_keys || del_slot || ivf_sel) {   // paging: keys >= ceil were returned by an earlier page (0 = exhausted)
-                            if (ceil_keys) { const uint64_t ceil = __ldg(&ceil_keys[blockIdx.y * NQ + q]); if (key >= ceil) key = 0; }
-                            pm = __ballot_sync(FULL, key != 0);
-                            if (!pm) continue;
-                        }
-                        uint64_t L = mylists[q * LIST + lane];
-                        if (__popc(pm) > 3) {
-                            // bulk (warm-up tiles: many rows pass): sort the 32 keys, bitonic-merge into the list
-                            L = wl_merge(L, wl_sort_desc(key, lane), lane);
-                        } else {
-                            while (pm) { const int src = __ffs(pm) - 1; pm &= pm - 1; wl_insert(L, shfl64(key, src), lane); }
-                        }
-                        mylists[q * LIST + lane] = L;
-                        uint32_t kth = (uint32_t)(shfl64(L, (int)k - 1) >> 32);
-                        if (PREC == PREC_F16F && kth) kth = ord_f32(__fsub_rd(unord_f32(kth), qs_sm[q]));   // candidates: s^ >= k-th best s^ - 2 eps_q
-                        if (lane == 0 && kth > thr_u[q]) atomicMax(&thr_u[q], kth);
-                    }
+                    insert_chunk(xb + lane * XB_STRIDE, row, valid, c, mylists);
                 }
             }
+        }
+        if (QUEUE) {   // every record of this warp is published before the list warps can see the count
+            __syncwarp();
+            if (lane == 0) { __threadfence_block(); atomicAdd((uint32_t*)qdone, 1u); }
         }
     }
     // a pair: the peer may still be multicasting into this CTA's shared memory / arriving on its barriers
@@ -779,19 +879,24 @@ static int32_t launch_tc_n(const ScanArgs& a, cudaStream_t st) {
         uint32_t n_pairs = (n_tiles + 1) / 2, n_clusters = (uint32_t)a.n_sms / 2;
         gx = 2 * (n_pairs < n_clusters ? n_pairs : n_clusters);
     }
-    if ((size_t)n_groups * gx * 4 * NQ * LIST * 8 > a.scratch_bytes) { set_error("vector scan scratch too small"); return SSB_E_STATE; }
-    uint32_t nst = C::STAGES;
-    int smem = C::SMEM;
+    // the seeded 256-query scan runs the record-queue instantiation (no delete / IVF test in it: either turns the seed off anyway).
+    // Lists per CTA: one per consumer warp of a warpgroup, or with the queue one per query.
+    const bool queue = NQ == 256 && a.thr_init && !a.sample_groupmax && !a.del_slot && !a.ivf_sel;
+    using CQ = tc::Cfg<NQ, PREC, BRES, NQ == 256>;
+    const uint32_t n_lists = queue ? 1u : 4u;
+    if ((size_t)n_groups * gx * n_lists * NQ * LIST * 8 > a.scratch_bytes) { set_error("vector scan scratch too small"); return SSB_E_STATE; }
+    uint32_t nst = queue ? CQ::STAGES : C::STAGES;
+    int smem = queue ? CQ::SMEM : C::SMEM;
     if (BRES) {   // resident query block + as many corpus stages as fit (tc::i8_resident guarantees >= 3)
         const int fixed = (int)n_kchunks * C::B_BYTES + C::FIXED;
         nst = (uint32_t)((tc::SMEM_MAX - fixed) / C::STAGE_BYTES);
         if (nst > (uint32_t)tc::MAX_STAGES) nst = tc::MAX_STAGES;
         smem = fixed + (int)nst * C::STAGE_BYTES;
     }
-    auto kern = tc::scan_tc<NQ, PREC, BRES, SCALED, PAIR>;
+    auto kern = queue ? tc::scan_tc<NQ, PREC, BRES, SCALED, PAIR, NQ == 256> : tc::scan_tc<NQ, PREC, BRES, SCALED, PAIR, false>;
     // per launch, not once per process: the opt-in applies to the CURRENT device's context only (ssb_config.device allows
     // several indexes on different GPUs in one process); the call is a cheap host-side attribute write
-    SSB_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, BRES ? tc::SMEM_MAX : C::SMEM));
+    SSB_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, BRES ? tc::SMEM_MAX : smem));
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = dim3(gx, n_groups); cfg.blockDim = dim3(tc::THREADS); cfg.dynamicSmemBytes = (size_t)smem; cfg.stream = st;
     cudaLaunchAttribute at[1];
@@ -813,7 +918,7 @@ static int32_t launch_tc_n(const ScanArgs& a, cudaStream_t st) {
         return SSB_OK;
     }
     // scratch layout [group][list][q in NQ][32] -> generic merge with qt = NQ
-    merge_lists_generic(a.scratch, gx * 4, NQ, a.nq_pad, a.keys_out, st);
+    merge_lists_generic(a.scratch, gx * n_lists, NQ, a.nq_pad, a.keys_out, st);
     SSB_CUDA_TRY(cudaGetLastError());
     if (a.launches) *a.launches += 2;   // scan + merge (the tf32 query split is counted with the sample pass)
     return SSB_OK;
@@ -856,7 +961,7 @@ int32_t launch_scan_tc(const ScanArgs& a, Scan s, cudaStream_t st) {
     // a better seed rejects.)
     const uint64_t trows = queries_per_pass(s) == 256 ? 128 : tc::TROWS;   // rows per stage of the variant that will run
     // sample tiles per SM: the seed is the k-th best of S sampled rows, the full scan then sees ~k*N/S candidates per query, each a
-    // ~1 us latency-bound list insert for an epilogue warp.  The filter scan streams a pass in half the time of the 3-product scan, so the
+    // ~1 us latency-bound list insert (256 queries: for a list warp, beside the MMAs).  The filter scan streams a pass in half the time of the 3-product scan, so the
     // same insert load weighs twice as much: it samples more (SSB_TC_SAMPLE_TILES overrides; measured in DESIGN.md §3.2c)
     static const int env_tiles = [] { const char* e = getenv("SSB_TC_SAMPLE_TILES"); return e ? atoi(e) : 0; }();
     const int sample_tiles = env_tiles > 0 ? (env_tiles > 16 ? 16 : env_tiles) : ((s == Scan::F16f_256 || s == Scan::F16f_256Pair) ? 2 : 1);
