@@ -469,8 +469,25 @@ struct TermRegs {   // generic path: lane t holds query term t of the current it
     uint32_t cnt; uint64_t off; uint32_t bmi; float idf; float ub;
 };
 
+// The term directory and the list arenas, by value for the out-of-line predicates: a LexView reference would force the whole view
+// onto the thread stack.  The helpers below take either this or a LexView (V).
+struct ListView { const uint32_t* e_level; const uint32_t* e_count; const uint32_t* e_bitmap; const uint32_t* post; const uint64_t* e_off;
+                  const BmSec* bm; const uint64_t* bm_words; };
+__device__ __forceinline__ ListView list_view(const LexView& v) { return ListView{v.e_level, v.e_count, v.e_bitmap, v.post, v.e_off, v.bm, v.bm_words}; }
+
+// directory entry e of term qt at local level lv (a term's entries ascend by level); false = the term has no list there.  qt by value:
+// its fields are loaded once up front, as the callers' copies did.  A bool, not an index-or-NONE, so that callers branch on the search.
+template <class V>
+__device__ __forceinline__ bool find_entry(const V& v, QTerm qt, uint32_t lv, uint32_t& e) {
+    uint32_t a = 0, b = qt.n;
+    while (a < b) { const uint32_t m = (a + b) >> 1; if (__ldg(&v.e_level[qt.first + m]) < lv) a = m + 1; else b = m; }
+    if (a < qt.n && __ldg(&v.e_level[qt.first + a]) == lv) { e = qt.first + a; return true; }
+    return false;
+}
+
 // membership + rank probe of doc d in the list described by (cnt, off, bmi)
-__device__ __forceinline__ bool probe(const LexView& v, uint32_t cnt, uint64_t off, uint32_t bmi, uint32_t d, uint32_t& rank) {
+template <class V>
+__device__ __forceinline__ bool probe(const V& v, uint32_t cnt, uint64_t off, uint32_t bmi, uint32_t d, uint32_t& rank) {
     if (bmi != NONE) {
         // word + rank sit in the same 32-byte sector: one DRAM access, two independent loads
         const BmSec* sec = v.bm + (size_t)bmi * 512 + (d >> 7);
@@ -486,12 +503,31 @@ __device__ __forceinline__ bool probe(const LexView& v, uint32_t cnt, uint64_t o
     return lo < cnt && (__ldg(&a[lo]) & 0xFFFFu) == d;
 }
 // membership only
-__device__ __forceinline__ bool present_in(const LexView& v, uint32_t cnt, uint64_t off, uint32_t bmi, uint32_t d) {
+template <class V>
+__device__ __forceinline__ bool present_in(const V& v, uint32_t cnt, uint64_t off, uint32_t bmi, uint32_t d) {
     if (bmi != NONE) return ((__ldg(&v.bm_words[(size_t)bmi * 1024 + (d >> 6)]) >> (d & 63)) & 1ull) != 0;
     uint32_t lo = 0, hi = cnt;
     const uint32_t* a = v.post + off;
     while (lo < hi) { uint32_t m = (lo + hi) >> 1; if ((__ldg(&a[m]) & 0xFFFFu) < d) lo = m + 1; else hi = m; }
     return lo < cnt && (__ldg(&a[lo]) & 0xFFFFu) == d;
+}
+// is doc d in term qt's list at local level lv?
+template <class V>
+__device__ __forceinline__ bool term_has(const V& v, QTerm qt, uint32_t lv, uint32_t d) {
+    uint32_t e;
+    if (!find_entry(v, qt, lv, e)) return false;
+    const uint32_t cnt = __ldg(&v.e_count[e]), bmi = __ldg(&v.e_bitmap[e]); const uint64_t off = __ldg(&v.e_off[e]);
+    return present_in(v, cnt, off, bmi, d);
+}
+// the posting of doc d in term qt's list at local level lv: false when the term has no list there or d is not in it
+__device__ __forceinline__ bool find_posting(const ListView& v, QTerm qt, uint32_t lv, uint32_t d, uint64_t& pos) {
+    uint32_t e;
+    if (!find_entry(v, qt, lv, e)) return false;
+    const uint32_t cnt = __ldg(&v.e_count[e]), bmi = __ldg(&v.e_bitmap[e]); const uint64_t off = __ldg(&v.e_off[e]);
+    uint32_t rank;
+    if (!probe(v, cnt, off, bmi, d, rank)) return false;
+    pos = off + rank;
+    return true;
 }
 
 __device__ __forceinline__ float term_score(const LexView& v, float idf, uint64_t pos) {
@@ -519,28 +555,13 @@ __device__ __forceinline__ bool is_deleted(const LexView& v, uint32_t doc) {
 }
 
 // not_query_list (add_result.rs:3440-3496): is doc d of local level lv in one of the query's NOT lists?  Out of line and fed by
-// value (no LexView reference: that would force the whole view onto the thread stack) — the call sits on the rare survivor path.
-struct NotView { const uint32_t* e_level; const uint32_t* e_count; const uint32_t* e_bitmap; const uint32_t* post; const uint64_t* e_off; const uint64_t* bm_words; };
-__device__ __forceinline__ NotView not_view(const LexView& v) { return NotView{v.e_level, v.e_count, v.e_bitmap, v.post, v.e_off, v.bm_words}; }
-__device__ __noinline__ bool in_not_lists_impl(NotView v, const QueryPlan* pl, uint32_t n_not, uint32_t lv, uint32_t d) {
-    for (uint32_t i = 0; i < n_not; i++) {
-        const QTerm qt = pl->tn[i];
-        uint32_t a = 0, b = qt.n;
-        while (a < b) { const uint32_t m = (a + b) >> 1; if (__ldg(&v.e_level[qt.first + m]) < lv) a = m + 1; else b = m; }
-        if (a < qt.n && __ldg(&v.e_level[qt.first + a]) == lv) {
-            const uint32_t e = qt.first + a;
-            const uint32_t cnt = __ldg(&v.e_count[e]), bmi = __ldg(&v.e_bitmap[e]); const uint64_t off = __ldg(&v.e_off[e]);
-            if (bmi != NONE) { if ((__ldg(&v.bm_words[(size_t)bmi * 1024 + (d >> 6)]) >> (d & 63)) & 1ull) return true; continue; }
-            uint32_t lo = 0, hi = cnt;
-            const uint32_t* p = v.post + off;
-            while (lo < hi) { const uint32_t m = (lo + hi) >> 1; if ((__ldg(&p[m]) & 0xFFFFu) < d) lo = m + 1; else hi = m; }
-            if (lo < cnt && (__ldg(&p[lo]) & 0xFFFFu) == d) return true;
-        }
-    }
+// value (ListView) — the call sits on the rare survivor path.
+__device__ __noinline__ bool in_not_lists_impl(ListView v, const QueryPlan* pl, uint32_t n_not, uint32_t lv, uint32_t d) {
+    for (uint32_t i = 0; i < n_not; i++) if (term_has(v, pl->tn[i], lv, d)) return true;
     return false;
 }
 __device__ __forceinline__ bool in_not_lists(const LexView& v, const QueryPlan* pl, uint32_t n_not, uint32_t lv, uint32_t d) {
-    return in_not_lists_impl(not_view(v), pl, n_not, lv, d);
+    return in_not_lists_impl(list_view(v), pl, n_not, lv, d);
 }
 
 // is_facet_filter (add_result.rs:340-478): true = the doc is filtered OUT.  The typed range / set tests of the reference run on the
@@ -569,122 +590,74 @@ __device__ __forceinline__ bool facet_rejects(const LexView& v, uint32_t f0, uin
 // field_filter (`field_filter_set`, add_result.rs:3124-3137, 3558-3571): every query term the doc contains must occur in at least one
 // field of the filter — tested only when (fields the term occurs in) + (fields of the filter) <= indexed fields, otherwise they overlap for
 // certain.  The score still sums every field.  true = the doc is filtered OUT.  Out of line, on the filtered path of lex_generic only.
-struct FieldArgs { const uint32_t* e_level; const uint32_t* e_count; const uint32_t* e_bitmap; const uint32_t* post; const uint64_t* e_off; const BmSec* bm;
-                   const uint32_t* payf; uint32_t n_fields; };
-__device__ __noinline__ bool field_rejects_impl(FieldArgs v, const QueryPlan* pl, uint32_t n_live, uint32_t lv, uint32_t d, uint32_t field_mask) {
+__device__ __noinline__ bool field_rejects_impl(ListView v, const uint32_t* payf, uint32_t n_fields, const QueryPlan* pl, uint32_t n_live, uint32_t lv,
+                                                uint32_t d, uint32_t field_mask) {
     const uint32_t n_filter = (uint32_t)__popc(field_mask);
     for (uint32_t t = 0; t < n_live; t++) {
-        const QTerm qt = pl->t[t];
-        uint32_t a = 0, b = qt.n;
-        while (a < b) { const uint32_t m = (a + b) >> 1; if (__ldg(&v.e_level[qt.first + m]) < lv) a = m + 1; else b = m; }
-        if (a >= qt.n || __ldg(&v.e_level[qt.first + a]) != lv) continue;
-        const uint32_t e = qt.first + a;
-        const uint32_t cnt = __ldg(&v.e_count[e]), bmi = __ldg(&v.e_bitmap[e]); const uint64_t off = __ldg(&v.e_off[e]);
-        uint32_t rank; bool found;
-        if (bmi != NONE) {
-            const BmSec* sec = v.bm + (size_t)bmi * 512 + (d >> 7);
-            const uint64_t w = __ldg(&sec->w[(d >> 6) & 1u]);
-            rank = (__ldg(&sec->meta[(d >> 6) & 1u]) & 0xFFFFu) + (uint32_t)__popcll(w & ((1ull << (d & 63)) - 1ull));
-            found = ((w >> (d & 63)) & 1ull) != 0;
-        } else {
-            uint32_t lo = 0, hi = cnt;
-            const uint32_t* p = v.post + off;
-            while (lo < hi) { const uint32_t m = (lo + hi) >> 1; if ((__ldg(&p[m]) & 0xFFFFu) < d) lo = m + 1; else hi = m; }
-            rank = lo; found = lo < cnt && (__ldg(&p[lo]) & 0xFFFFu) == d;
-        }
-        if (!found) continue;                                            // the doc does not contain this term (OR)
+        uint64_t pos;
+        if (!find_posting(v, pl->t[t], lv, d, pos)) continue;           // the doc does not contain this term (OR)
         uint32_t present = 0;
-        for (uint32_t f = 0; f < v.n_fields; f++) if (__ldg(&v.payf[(off + rank) * v.n_fields + f]) & 0xFFFFu) present |= 1u << f;
-        if ((uint32_t)__popc(present) + n_filter <= v.n_fields && !(present & field_mask)) return true;
+        for (uint32_t f = 0; f < n_fields; f++) if (__ldg(&payf[pos * n_fields + f]) & 0xFFFFu) present |= 1u << f;
+        if ((uint32_t)__popc(present) + n_filter <= n_fields && !(present & field_mask)) return true;
     }
     return false;
 }
 // Phrase check (add_result.rs:3586-3684): the doc (already known to contain every term) matches iff some start position p has token i of
 // the phrase at p + i for every i — the reference finds it by a k-way merge of the tokens' position lists aligned by their index in the
-// phrase (term_index_nonunique); the same merge here, one thread per candidate doc, cursors on the thread's stack (rare path, out of line).
-struct PhraseArgs { const uint32_t* e_level; const uint32_t* e_count; const uint32_t* e_bitmap; const uint32_t* post; const uint64_t* e_off; const BmSec* bm;
-                    const uint32_t* pay; const uint16_t* positions; const uint32_t* pos_off; const uint64_t* lvl_pos_base; };
-__device__ __noinline__ bool phrase_rejects_impl(PhraseArgs v, const QueryPlan* pl, uint32_t n_live, uint32_t lv, uint32_t d) {
-    uint64_t ubase[SSB_MAX_QUERY_TERMS]; uint32_t utf[SSB_MAX_QUERY_TERMS];
-    const uint64_t lbase = __ldg(&v.lvl_pos_base[lv]);
-    for (uint32_t t = 0; t < n_live; t++) {
-        const QTerm qt = pl->t[t];
-        uint32_t a = 0, b = qt.n;
-        while (a < b) { const uint32_t m = (a + b) >> 1; if (__ldg(&v.e_level[qt.first + m]) < lv) a = m + 1; else b = m; }
-        if (a >= qt.n || __ldg(&v.e_level[qt.first + a]) != lv) return true;
-        const uint32_t e = qt.first + a;
-        const uint32_t cnt = __ldg(&v.e_count[e]), bmi = __ldg(&v.e_bitmap[e]); const uint64_t off = __ldg(&v.e_off[e]);
-        uint32_t rank; bool found;
-        if (bmi != NONE) {
-            const BmSec* sec = v.bm + (size_t)bmi * 512 + (d >> 7);
-            const uint64_t w = __ldg(&sec->w[(d >> 6) & 1u]);
-            rank = (__ldg(&sec->meta[(d >> 6) & 1u]) & 0xFFFFu) + (uint32_t)__popcll(w & ((1ull << (d & 63)) - 1ull));
-            found = ((w >> (d & 63)) & 1ull) != 0;
-        } else {
-            uint32_t lo = 0, hi = cnt;
-            const uint32_t* p = v.post + off;
-            while (lo < hi) { const uint32_t m = (lo + hi) >> 1; if ((__ldg(&p[m]) & 0xFFFFu) < d) lo = m + 1; else hi = m; }
-            rank = lo; found = lo < cnt && (__ldg(&p[lo]) & 0xFFFFu) == d;
-        }
-        if (!found) return true;
-        ubase[t] = lbase + __ldg(&v.pos_off[off + rank]);
-        utf[t] = __ldg(&v.pay[off + rank]) & 0xFFFFu;
-    }
-    const uint32_t m = pl->n_phr;
-    uint32_t cur[SSB_MAX_QUERY_TERMS];
+// phrase (term_index_nonunique); the same merge here, one thread per candidate doc (rare path, out of line).  Unique term u's positions
+// are positions[ubase[u] .. + utf[u]); true = some start s has token i at s + i for every i (phrasematch_count >= 1).  The cursors `cur`
+// (one per token) are an array of the calling check, on the thread's stack: declared there, after its own arrays, they keep that
+// function's frame layout and with it the register allocation of lex_generic<true>.
+__device__ __forceinline__ bool phrase_in_runs(const uint16_t* positions, const QueryPlan* pl, const uint64_t* ubase, const uint32_t* utf, uint32_t* cur) {
+    const uint32_t m = pl->n_phr, u0 = pl->phr[0];
     for (uint32_t i = 0; i < m; i++) cur[i] = 0;
-    // anchor = token 0; value searched: a start position s with positions(token i) containing s + i for every i
-    const uint32_t u0 = pl->phr[0];
-    while (cur[0] < utf[u0]) {
-        const uint32_t s = __ldg(&v.positions[ubase[u0] + cur[0]]);
+    while (cur[0] < utf[u0]) {                                               // anchor = token 0
+        const uint32_t s = __ldg(&positions[ubase[u0] + cur[0]]);
         bool all = true; uint32_t next_s = s;
         for (uint32_t i = 1; i < m; i++) {
             const uint32_t u = pl->phr[i];
-            while (cur[i] < utf[u] && (uint32_t)__ldg(&v.positions[ubase[u] + cur[i]]) < s + i) cur[i]++;
-            if (cur[i] >= utf[u]) return true;                              // a token's positions are exhausted: no (further) match
-            const uint32_t p = __ldg(&v.positions[ubase[u] + cur[i]]);
+            while (cur[i] < utf[u] && (uint32_t)__ldg(&positions[ubase[u] + cur[i]]) < s + i) cur[i]++;
+            if (cur[i] >= utf[u]) return false;                             // a token's positions are exhausted: no (further) match
+            const uint32_t p = __ldg(&positions[ubase[u] + cur[i]]);
             if (p != s + i) { all = false; next_s = p - i; break; }          // p > s + i: the start must move up to at least p - i
         }
-        if (all) return false;                                               // phrasematch_count >= 1
-        while (cur[0] < utf[u0] && (uint32_t)__ldg(&v.positions[ubase[u0] + cur[0]]) < next_s) cur[0]++;
+        if (all) return true;
+        while (cur[0] < utf[u0] && (uint32_t)__ldg(&positions[ubase[u0] + cur[0]]) < next_s) cur[0]++;
     }
-    return true;
+    return false;
+}
+struct PhraseArgs { const uint32_t* pay; const uint16_t* positions; const uint32_t* pos_off; const uint64_t* lvl_pos_base; };
+__device__ __noinline__ bool phrase_rejects_impl(ListView v, PhraseArgs a, const QueryPlan* pl, uint32_t n_live, uint32_t lv, uint32_t d) {
+    uint64_t ubase[SSB_MAX_QUERY_TERMS]; uint32_t utf[SSB_MAX_QUERY_TERMS];
+    const uint64_t lbase = __ldg(&a.lvl_pos_base[lv]);
+    for (uint32_t t = 0; t < n_live; t++) {
+        uint64_t pos;
+        if (!find_posting(v, pl->t[t], lv, d, pos)) return true;
+        ubase[t] = lbase + __ldg(&a.pos_off[pos]);
+        utf[t] = __ldg(&a.pay[pos]) & 0xFFFFu;
+    }
+    uint32_t cur[SSB_MAX_QUERY_TERMS];
+    return !phrase_in_runs(a.positions, pl, ubase, utf, cur);
 }
 // Several indexed fields (add_result.rs:3247-3389): a posting's positions are one run per field, field 0 first, each restarting from 0, of
-// the posting's per-field tfs (v.pay = payf here).  The same merge as above runs field by field on those runs only — a phrase never spans two
+// the posting's per-field tfs (a.pay = payf here).  The same merge as above runs field by field on those runs only — a phrase never spans two
 // fields: field f is searched when every unique term occurs in it and, if the query has a field filter (pl->field_mask != 0), when f is in
 // the filter (field_filter_set.contains).  The doc matches on the first field that holds the phrase.  Out of line like the single-field
 // check and only in lex_generic<true>, so that the single-field kernel keeps its code.
-__device__ __noinline__ bool phrase_rejects_fields_impl(PhraseArgs v, const QueryPlan* pl, uint32_t n_live, uint32_t lv, uint32_t d, uint32_t n_fields) {
+__device__ __noinline__ bool phrase_rejects_fields_impl(ListView v, PhraseArgs a, const QueryPlan* pl, uint32_t n_live, uint32_t lv, uint32_t d,
+                                                        uint32_t n_fields) {
     uint64_t ubase[SSB_MAX_QUERY_TERMS], ftf[SSB_MAX_QUERY_TERMS];       // per unique term: its first position in field 0, its tfs (16 bits per field)
     uint32_t utf[SSB_MAX_QUERY_TERMS];
-    const uint64_t lbase = __ldg(&v.lvl_pos_base[lv]);
+    const uint64_t lbase = __ldg(&a.lvl_pos_base[lv]);
     for (uint32_t t = 0; t < n_live; t++) {
-        const QTerm qt = pl->t[t];
-        uint32_t a = 0, b = qt.n;
-        while (a < b) { const uint32_t m = (a + b) >> 1; if (__ldg(&v.e_level[qt.first + m]) < lv) a = m + 1; else b = m; }
-        if (a >= qt.n || __ldg(&v.e_level[qt.first + a]) != lv) return true;
-        const uint32_t e = qt.first + a;
-        const uint32_t cnt = __ldg(&v.e_count[e]), bmi = __ldg(&v.e_bitmap[e]); const uint64_t off = __ldg(&v.e_off[e]);
-        uint32_t rank; bool found;
-        if (bmi != NONE) {
-            const BmSec* sec = v.bm + (size_t)bmi * 512 + (d >> 7);
-            const uint64_t w = __ldg(&sec->w[(d >> 6) & 1u]);
-            rank = (__ldg(&sec->meta[(d >> 6) & 1u]) & 0xFFFFu) + (uint32_t)__popcll(w & ((1ull << (d & 63)) - 1ull));
-            found = ((w >> (d & 63)) & 1ull) != 0;
-        } else {
-            uint32_t lo = 0, hi = cnt;
-            const uint32_t* p = v.post + off;
-            while (lo < hi) { const uint32_t m = (lo + hi) >> 1; if ((__ldg(&p[m]) & 0xFFFFu) < d) lo = m + 1; else hi = m; }
-            rank = lo; found = lo < cnt && (__ldg(&p[lo]) & 0xFFFFu) == d;
-        }
-        if (!found) return true;
-        ubase[t] = lbase + __ldg(&v.pos_off[off + rank]);
+        uint64_t pos;
+        if (!find_posting(v, pl->t[t], lv, d, pos)) return true;
+        ubase[t] = lbase + __ldg(&a.pos_off[pos]);
         uint64_t tfs = 0;
-        for (uint32_t f = 0; f < n_fields; f++) tfs |= (uint64_t)(__ldg(&v.pay[(off + rank) * n_fields + f]) & 0xFFFFu) << (16 * f);
+        for (uint32_t f = 0; f < n_fields; f++) tfs |= (uint64_t)(__ldg(&a.pay[pos * n_fields + f]) & 0xFFFFu) << (16 * f);
         ftf[t] = tfs;
     }
-    const uint32_t m = pl->n_phr, u0 = pl->phr[0], field_mask = pl->field_mask;
+    const uint32_t field_mask = pl->field_mask;
     uint32_t cur[SSB_MAX_QUERY_TERMS];
     for (uint32_t f = 0; f < n_fields; f++) {
         bool in_all = true;
@@ -694,22 +667,7 @@ __device__ __noinline__ bool phrase_rejects_fields_impl(PhraseArgs v, const Quer
             in_all = in_all && utf[t] != 0;
         }
         if (!in_all || (field_mask && !((field_mask >> f) & 1u))) continue;
-        for (uint32_t i = 0; i < m; i++) cur[i] = 0;
-        bool exhausted = false;
-        while (!exhausted && cur[0] < utf[u0]) {
-            const uint32_t s = __ldg(&v.positions[ubase[u0] + cur[0]]);
-            bool all = true; uint32_t next_s = s;
-            for (uint32_t i = 1; i < m; i++) {
-                const uint32_t u = pl->phr[i];
-                while (cur[i] < utf[u] && (uint32_t)__ldg(&v.positions[ubase[u] + cur[i]]) < s + i) cur[i]++;
-                if (cur[i] >= utf[u]) { exhausted = true; break; }          // a token's positions in this field are exhausted
-                const uint32_t p = __ldg(&v.positions[ubase[u] + cur[i]]);
-                if (p != s + i) { all = false; next_s = p - i; break; }
-            }
-            if (exhausted) break;
-            if (all) return false;                                           // phrasematch_count >= 1
-            while (cur[0] < utf[u0] && (uint32_t)__ldg(&v.positions[ubase[u0] + cur[0]]) < next_s) cur[0]++;
-        }
+        if (phrase_in_runs(a.positions, pl, ubase, utf, cur)) return false;
     }
     return true;
 }
@@ -719,10 +677,10 @@ __device__ __noinline__ bool phrase_rejects_fields_impl(PhraseArgs v, const Quer
 template <bool FIELD_RUNS>
 __device__ __forceinline__ bool filters_reject(const LexView& v, const QueryPlan* pl, uint32_t f0, uint32_t nf, uint32_t field_mask, uint32_t n_live, uint32_t lv, uint32_t d, uint32_t doc) {
     if (nf && facet_rejects(v, f0, nf, doc)) return true;
-    if (field_mask && field_rejects_impl(FieldArgs{v.e_level, v.e_count, v.e_bitmap, v.post, v.e_off, v.bm, v.payf, v.n_fields}, pl, n_live, lv, d, field_mask)) return true;
-    if (!FIELD_RUNS && pl->n_phr && phrase_rejects_impl(PhraseArgs{v.e_level, v.e_count, v.e_bitmap, v.post, v.e_off, v.bm, v.pay, v.positions, v.pos_off, v.lvl_pos_base}, pl, n_live, lv, d)) return true;
-    if (FIELD_RUNS && pl->n_phr && phrase_rejects_fields_impl(PhraseArgs{v.e_level, v.e_count, v.e_bitmap, v.post, v.e_off, v.bm, v.payf, v.positions, v.pos_off,
-                                                                         v.lvl_pos_base}, pl, n_live, lv, d, v.n_fields)) return true;
+    if (field_mask && field_rejects_impl(list_view(v), v.payf, v.n_fields, pl, n_live, lv, d, field_mask)) return true;
+    if (!FIELD_RUNS && pl->n_phr && phrase_rejects_impl(list_view(v), PhraseArgs{v.pay, v.positions, v.pos_off, v.lvl_pos_base}, pl, n_live, lv, d)) return true;
+    if (FIELD_RUNS && pl->n_phr && phrase_rejects_fields_impl(list_view(v), PhraseArgs{v.payf, v.positions, v.pos_off, v.lvl_pos_base}, pl, n_live, lv, d,
+                                                              v.n_fields)) return true;
     return false;
 }
 
@@ -1214,10 +1172,8 @@ __device__ __forceinline__ void process_item_generic(const LexView& v, const Que
     TermRegs tr; tr.cnt = 0; tr.off = 0; tr.bmi = NONE; tr.idf = 0.f; tr.ub = 0.f;
     if ((uint32_t)lane < n) {
         QTerm qt = pl->t[lane];
-        uint32_t lo = 0, hi = qt.n;
-        while (lo < hi) { uint32_t m = (lo + hi) >> 1; if (__ldg(&v.e_level[qt.first + m]) < lv) lo = m + 1; else hi = m; }
-        if (lo < qt.n && __ldg(&v.e_level[qt.first + lo]) == lv) {
-            uint32_t e = qt.first + lo;
+        uint32_t e;
+        if (find_entry(v, qt, lv, e)) {
             tr.cnt = __ldg(&v.e_count[e]); tr.off = __ldg(&v.e_off[e]); tr.bmi = __ldg(&v.e_bitmap[e]);
             tr.ub = __fmul_rn(qt.idf, __ldg(&v.e_maxcomp[e]));
         }
@@ -1530,6 +1486,16 @@ __global__ void __launch_bounds__(256) lex_generic(LexView v, const QueryPlan* _
     }
 }
 
+// does doc d of local level lv match the query's n positive terms (AND: all of them, OR: any)?
+__device__ __forceinline__ bool matches_terms(const LexView& v, const QueryPlan* pl, uint32_t n, bool is_and, uint32_t lv, uint32_t d) {
+    bool any = false, all = true;
+    for (uint32_t t = 0; t < n; t++) {
+        const bool pres = term_has(v, pl->t[t], lv, d);
+        any = any || pres; all = all && pres;
+    }
+    return is_and ? all : any;
+}
+
 // ---- exact counts with NOT lists: the count kernels count every match of the positive terms; the matches that sit in a NOT list are
 // subtracted here.  One warp per (query, local level); a NOT list's postings are enumerated (each doc once: docs already seen in an
 // earlier NOT list are skipped), deleted docs are left to lex_del_count. ----
@@ -1548,28 +1514,13 @@ __global__ void __launch_bounds__(256) lex_not_count(LexView v, const QueryPlan*
         const uint32_t docbase = __ldg(&v.level_ids[lv]) << 16;
         uint32_t sub = 0;
         for (uint32_t i = 0; i < n_not; i++) {
-            const QTerm qt = pl->tn[i];
-            uint32_t a = 0, b = qt.n;
-            while (a < b) { const uint32_t m = (a + b) >> 1; if (__ldg(&v.e_level[qt.first + m]) < lv) a = m + 1; else b = m; }
-            if (a >= qt.n || __ldg(&v.e_level[qt.first + a]) != lv) continue;
-            const uint32_t e = qt.first + a;
+            uint32_t e;
+            if (!find_entry(v, pl->tn[i], lv, e)) continue;
             for_each_posting(v, __ldg(&v.e_off[e]), __ldg(&v.e_count[e]), lane, [&](uint32_t d, bool valid) {
                 if (!valid) return;
                 if (i && in_not_lists(v, pl, i, lv, d)) return;          // counted with an earlier NOT list
                 if (is_deleted(v, docbase | d)) return;
-                bool any = false, all = true;
-                for (uint32_t t = 0; t < n; t++) {
-                    const QTerm pt = pl->t[t];
-                    uint32_t x = 0, y = pt.n;
-                    while (x < y) { const uint32_t m = (x + y) >> 1; if (__ldg(&v.e_level[pt.first + m]) < lv) x = m + 1; else y = m; }
-                    bool pres = false;
-                    if (x < pt.n && __ldg(&v.e_level[pt.first + x]) == lv) {
-                        const uint32_t pe = pt.first + x;
-                        pres = present_in(v, __ldg(&v.e_count[pe]), __ldg(&v.e_off[pe]), __ldg(&v.e_bitmap[pe]), d);
-                    }
-                    any = any || pres; all = all && pres;
-                }
-                sub += (is_and ? all : any) ? 1u : 0u;
+                sub += matches_terms(v, pl, n, is_and, lv, d) ? 1u : 0u;
             });
         }
         for (int s = 16; s; s >>= 1) sub += __shfl_xor_sync(FULL, sub, s);
@@ -1590,21 +1541,7 @@ __global__ void lex_del_count(LexView v, const QueryPlan* __restrict__ plans, ui
     const uint32_t lid = doc >> 16, d = doc & 0xFFFFu;
     while (lo < hi) { const uint32_t m = (lo + hi) >> 1; if (__ldg(&v.level_ids[m]) < lid) lo = m + 1; else hi = m; }
     if (lo >= v.n_levels || __ldg(&v.level_ids[lo]) != lid) return;  // level not on this shard
-    const uint32_t lv = lo;
-    const bool is_and = query_type == SSB_QUERY_INTERSECTION;
-    bool any = false, all = true;
-    for (uint32_t t = 0; t < n; t++) {
-        const QTerm qt = pl->t[t];
-        uint32_t a = 0, b = qt.n;
-        while (a < b) { const uint32_t m = (a + b) >> 1; if (__ldg(&v.e_level[qt.first + m]) < lv) a = m + 1; else b = m; }
-        bool pres = false;
-        if (a < qt.n && __ldg(&v.e_level[qt.first + a]) == lv) {
-            const uint32_t e = qt.first + a;
-            pres = present_in(v, __ldg(&v.e_count[e]), __ldg(&v.e_off[e]), __ldg(&v.e_bitmap[e]), d);
-        }
-        any = any || pres; all = all && pres;
-    }
-    if (is_and ? all : any) atomicAdd((unsigned long long*)&count[q], ~0ull);   // -1
+    if (matches_terms(v, pl, n, query_type == SSB_QUERY_INTERSECTION, lo, d)) atomicAdd((unsigned long long*)&count[q], ~0ull);   // -1
 }
 
 __global__ void copy_out(const uint64_t* __restrict__ glist, const uint64_t* __restrict__ count, uint32_t nq, uint32_t k,
