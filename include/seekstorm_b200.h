@@ -239,6 +239,10 @@ int32_t ssb_set_deleted(ssb_index* ix, const uint64_t* doc_ids, uint64_t n);
  * facet); a doc outside the covered range fails every filter.  Replaces the current facets; n_docs = 0 clears them.  Exclusive. */
 int32_t ssb_set_facets(ssb_index* ix, const void* rows, uint64_t first_doc_id, uint64_t n_docs, uint32_t row_bytes,
                        const ssb_facet_field* fields, uint32_t n_fields);
+/* String16 / String32 facets sort by the value's STRING (result_ordering_shard, min_heap.rs:861-898, `values.get_index(id)`; Rust
+ * String order = byte-wise lexicographic), which the library does not hold: rank_of_id[id] = position of id's string in that order
+ * (equal strings, equal rank), computed by the host.  HOST array [n_ids].  ssb_set_facets clears it.  Needed by sorted searches only. */
+int32_t ssb_set_facet_value_order(ssb_index* ix, uint32_t facet, const uint32_t* rank_of_id, uint32_t n_ids);
 
 /* ---- vector index -------------------------------------------------------------------------------- */
 /* rows: [n, dims] row-major f32 (row_stride_floats >= dims, 0 = dims); local_ids: [n] u16 or NULL (= 0..n-1).
@@ -267,6 +271,22 @@ int32_t ssb_set_vector_kernel(ssb_index* ix, uint32_t vector_kernel);
  * NULL (result_count_total: exact for Count/TopkCount, unspecified for Topk — search.rs:196-198). */
 int32_t ssb_search_lexical(ssb_index* ix, const ssb_lex_batch* q, uint32_t k, uint32_t result_type,
                            ssb_hit* hits, uint32_t* n_hits, uint64_t* count_total);
+/* `result_sort: Vec<ResultSort>` of Search::search (search.rs:1004-1013, ResultSort :893-901, resolved by ResultSortIndex :2497-2525):
+ * the same search with the hits ordered by the criteria, compared left to right (result_ordering_shard, min_heap.rs:574-1051): a facet
+ * in its own type (String16 / String32 by the value order of ssb_set_facet_value_order), the doc id (SSB_SORT_ID) or the score
+ * (SSB_SORT_SCORE).  _id and _score end the comparison (min_heap.rs:580-604): criteria after them are ignored.  Ties on every criterion
+ * fall back to score desc (:1043-1050), then doc id asc.  Deviations: a NaN facet value orders above +inf (descending puts it first), the
+ * reference's partial_cmp makes it equal to everything; -0.0 == +0.0 as in the reference.  Hits carry the BM25 score; counts are those
+ * of ssb_search_lexical (Count ignores the sort, search.rs:2498).  One sort for the whole batch; n_sort = 0, or criteria that reduce to
+ * "_score desc", is ssb_search_lexical.  The facet criteria with their natural widths (8 bits U8 / I8, 16 bits U16 / I16 / String16,
+ * 32 bits U32 / I32 / F32 / String32 / _id, 64 bits U64 / I64 / Timestamp / F64) must fit 64 bits in total (else SSB_E_UNSUPPORTED).
+ * Needs ssb_set_facets rows for every doc of the lexical levels.  Not on a handle with a communicator (SSB_E_UNSUPPORTED). */
+enum { SSB_SORT_FACET = 0, SSB_SORT_ID = 1, SSB_SORT_SCORE = 2 };
+enum { SSB_SORT_ASCENDING = 0, SSB_SORT_DESCENDING = 1 };          /* SortOrder, search.rs:885-890 */
+typedef struct { uint32_t source, facet, order, pad; } ssb_sort_criterion;   /* facet: index into ssb_set_facets' fields (SSB_SORT_FACET) */
+#define SSB_MAX_SORT_CRITERIA 4u
+int32_t ssb_search_lexical_sorted(ssb_index* ix, const ssb_lex_batch* q, const ssb_sort_criterion* sort, uint32_t n_sort,
+                                  uint32_t k, uint32_t result_type, ssb_hit* hits, uint32_t* n_hits, uint64_t* count_total);
 /* queries: [n_queries, dims] f32; Cosine: normalised by the callee (search.rs:1464-1475).  score = dot
  * (Dot/Cosine) or -Σ(q-x)² (Euclidean) exactly as Result.score in vector.rs:1489. */
 int32_t ssb_search_vector(ssb_index* ix, const float* queries, uint32_t n_queries, uint32_t k,

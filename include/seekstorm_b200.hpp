@@ -87,6 +87,18 @@ struct FacetFilter {
     static FacetFilter set(uint32_t facet, std::vector<uint64_t> ids) { FacetFilter f; f.facet = facet; f.values = std::move(ids); return f; }
 };
 
+// `ResultSort` (search.rs:893-901) resolved against the schema (ResultSortIndex, search.rs:2497-2525): a facet field (index in the order
+// of set_facets; a String16 / String32 facet needs set_facet_value_order), the doc id ("_id") or the score ("_score").  Geo proximity
+// sorting (a FacetValue::Point base) is not built.
+enum class SortOrder : uint32_t { Ascending = SSB_SORT_ASCENDING, Descending = SSB_SORT_DESCENDING };   // search.rs:885-890
+struct ResultSort {
+    uint32_t source = SSB_SORT_FACET, facet = 0;
+    SortOrder order = SortOrder::Descending;
+    static ResultSort facet_field(uint32_t facet, SortOrder o) { ResultSort r; r.facet = facet; r.order = o; return r; }
+    static ResultSort id(SortOrder o) { ResultSort r; r.source = SSB_SORT_ID; r.order = o; return r; }
+    static ResultSort score(SortOrder o) { ResultSort r; r.source = SSB_SORT_SCORE; r.order = o; return r; }
+};
+
 class Index {
 public:
     using TermKeyFn = std::function<uint64_t(const std::string&)>;
@@ -120,6 +132,10 @@ public:
     void set_facets(const void* rows, uint64_t first_doc_id, uint64_t n_docs, uint32_t row_bytes, const std::vector<ssb_facet_field>& fields) {
         check(ssb_set_facets(h_, rows, first_doc_id, n_docs, row_bytes, fields.data(), static_cast<uint32_t>(fields.size())));
     }
+    // String16 / String32 facet: rank_of_id[id] = position of the id's string in byte-wise order (what sorting by the facet compares)
+    void set_facet_value_order(uint32_t facet, const std::vector<uint32_t>& rank_of_id) {
+        check(ssb_set_facet_value_order(h_, facet, rank_of_id.data(), static_cast<uint32_t>(rank_of_id.size())));
+    }
     // several indexed fields: boosts (before the first level) and the fields' names in schema order (for field_filter)
     void set_field_boosts(const std::vector<float>& boosts) { check(ssb_lexical_set_field_boosts(h_, static_cast<uint32_t>(boosts.size()), boosts.data())); }
     void set_field_names(std::vector<std::string> names) { field_names_ = std::move(names); }
@@ -133,10 +149,12 @@ public:
                         QueryType query_type_default, const SearchMode& search_mode, bool enable_empty_query, size_t offset,
                         size_t length, ResultType result_type, bool include_uncommitted = false,
                         const std::vector<std::string>& field_filter = {}, size_t n_query_facets = 0,
-                        const std::vector<FacetFilter>& facet_filter = {}, size_t n_result_sort = 0) const {
+                        const std::vector<FacetFilter>& facet_filter = {}, const std::vector<ResultSort>& result_sort = {}) const {
         (void)enable_empty_query;
-        if (include_uncommitted || n_query_facets || n_result_sort)
-            throw Error(SSB_E_UNSUPPORTED, "facet counts / sort / uncommitted search are outside the GPU hot path");
+        if (include_uncommitted || n_query_facets)
+            throw Error(SSB_E_UNSUPPORTED, "facet counts / uncommitted search are outside the GPU hot path");
+        if (!result_sort.empty() && search_mode.kind != SearchMode::Lexical)
+            throw Error(SSB_E_UNSUPPORTED, "result_sort on vector / hybrid search is not built");
         // field_filter: names of indexed fields (set_field_names, schema order) -> field_filter_set as a bitmask
         uint32_t field_mask = 0;
         for (auto& name : field_filter) {
@@ -206,7 +224,10 @@ public:
             const uint32_t k = rt == ResultType::Count ? 0u : static_cast<uint32_t>(heap);
             lex.resize(k ? k : 1);
             uint32_t n = 0;
-            check(ssb_search_lexical(h_, &b, k, static_cast<uint32_t>(rt), lex.data(), &n, &total));
+            std::vector<ssb_sort_criterion> sc;
+            for (auto& r : result_sort) sc.push_back(ssb_sort_criterion{r.source, r.facet, static_cast<uint32_t>(r.order), 0});
+            if (sc.empty()) check(ssb_search_lexical(h_, &b, k, static_cast<uint32_t>(rt), lex.data(), &n, &total));
+            else check(ssb_search_lexical_sorted(h_, &b, sc.data(), static_cast<uint32_t>(sc.size()), k, static_cast<uint32_t>(rt), lex.data(), &n, &total));
             lex.resize(n);
         }
         if (want_vec) {

@@ -343,36 +343,43 @@ int32_t shard_sum_counts(ssb_index* ix, SearchCtx& c, uint64_t* counts_dev, uint
     return SSB_OK;
 }
 
-// Paging state of the host-facing search calls (k > SSB_K_MAX, or de-duplication of multi-chunk documents).
+// Paging state of the host-facing search calls (k > SSB_K_MAX, or de-duplication of multi-chunk documents).  W = words per key:
+// 1 = the 64-bit (score, doc) keys, 2 = the 128-bit keys {hi, lo} of a sorted lexical search, lo = pack_key(score, doc) with its score
+// half inverted when score_inv (`_score` ascending).
+template <int W>
 struct PageState {
-    SearchCtx& c; uint32_t nq, k; ssb_hit* hits; uint32_t* n_hits; std::vector<uint32_t> cnt; std::vector<uint8_t> open; bool dedup;
-    PageState(SearchCtx& c_, uint32_t nq_, uint32_t k_, ssb_hit* h, uint32_t* n, bool dedup_ = false)
-        : c(c_), nq(nq_), k(k_), hits(h), n_hits(n), cnt(nq_, 0), open(nq_, 1), dedup(dedup_) {
-        c.h_ceil.assign((size_t)nq_ + 256, 0);
+    SearchCtx& c; uint32_t nq, k; ssb_hit* hits; uint32_t* n_hits; std::vector<uint32_t> cnt; std::vector<uint8_t> open; bool dedup, score_inv;
+    PageState(SearchCtx& c_, uint32_t nq_, uint32_t k_, ssb_hit* h, uint32_t* n, bool dedup_ = false, bool score_inv_ = false)
+        : c(c_), nq(nq_), k(k_), hits(h), n_hits(n), cnt(nq_, 0), open(nq_, 1), dedup(dedup_), score_inv(score_inv_) {
+        c.h_ceil.assign(((size_t)nq_ + 256) * W, 0);
     }
     // consume one [nq][32] page that was fetched with `kk` results per query; returns true if any query wants another page
     bool append(const uint64_t* keys, uint32_t kk) {
         bool more = false;
         for (uint32_t q = 0; q < nq; q++) {
-            if (!open[q]) { c.h_ceil[q] = 0; continue; }                    // exhausted or complete on an earlier page
-            uint32_t seen = 0; uint64_t last = 0;
+            uint64_t* ceil = &c.h_ceil[(size_t)q * W];
+            if (!open[q]) { for (int w = 0; w < W; w++) ceil[w] = 0; continue; }   // exhausted or complete on an earlier page
+            uint32_t seen = 0; const uint64_t* last = nullptr;
             for (uint32_t j = 0; j < kk && cnt[q] < k; j++) {
-                const uint64_t key = keys[(size_t)q * LIST + j];
-                if (!key) break;
+                const uint64_t* key = keys + ((size_t)q * LIST + j) * W;
+                bool empty = true;
+                for (int w = 0; w < W; w++) empty = empty && key[w] == 0;
+                if (empty) break;
                 seen++; last = key;
-                const uint64_t doc = key_doc(key);
+                const uint64_t lo = key[W - 1];
+                const uint64_t doc = key_doc(lo);
                 if (dedup) {
                     bool dup = false;
                     for (uint32_t i = 0; i < cnt[q]; i++) dup = dup || hits[(size_t)q * k + i].doc_id == doc;
                     if (dup) continue;
                 }
                 ssb_hit& h = hits[(size_t)q * k + cnt[q]];
-                h.doc_id = doc; h.score = key_score(key); h.pad = 0;
+                h.doc_id = doc; h.score = key_score(score_inv ? lo ^ 0xFFFFFFFF00000000ull : lo); h.pad = 0;
                 cnt[q]++;
             }
             // another page only if this one was full (else the list is exhausted) and the query still lacks results
             open[q] = seen == kk && cnt[q] < k;
-            c.h_ceil[q] = open[q] ? last : 0;                                // 0 = nothing left below
+            for (int w = 0; w < W; w++) ceil[w] = open[q] ? last[w] : 0;        // 0 = nothing left below
             more = more || open[q];
         }
         return more;
@@ -384,9 +391,9 @@ struct PageState {
         return need < SSB_K_MAX ? need : SSB_K_MAX;
     }
     int32_t upload_ceilings() {
-        SSB_TRY(c.ceil.reserve((size_t)nq + 256, 0, c.st));
-        SSB_CUDA_TRY(cudaMemcpyAsync(c.ceil.p, c.h_ceil.data(), ((size_t)nq + 256) * 8, cudaMemcpyHostToDevice, c.st));
-        c.stats.h2d_bytes += (uint64_t)nq * 8;
+        SSB_TRY(c.ceil.reserve(((size_t)nq + 256) * W, 0, c.st));
+        SSB_CUDA_TRY(cudaMemcpyAsync(c.ceil.p, c.h_ceil.data(), ((size_t)nq + 256) * W * 8, cudaMemcpyHostToDevice, c.st));
+        c.stats.h2d_bytes += (uint64_t)nq * W * 8;
         return SSB_OK;
     }
     void finish() {
@@ -413,7 +420,7 @@ int32_t search_vector_host(ssb_index* ix, SearchCtx& c, const void* queries, boo
                            const IvfQuery* ivf = nullptr) {
     SSB_TRY(c.keys_a.reserve((size_t)nq * LIST, 0, c.st));
     c.h_keys_a.resize((size_t)nq * LIST);
-    PageState ps(c, nq, k, hits, n_hits, ix->dup_docs);
+    PageState<1> ps(c, nq, k, hits, n_hits, ix->dup_docs);
     // the fused kernels keep 32 results per query; longer result lists are produced page by page, each page restricted to
     // keys strictly below the last key of the previous one (keys are a total order on (score desc, doc id asc))
     uint32_t kk = ix->dup_docs ? SSB_K_MAX : (k < SSB_K_MAX ? k : SSB_K_MAX);
@@ -436,6 +443,53 @@ int32_t search_vector_host(ssb_index* ix, SearchCtx& c, const void* queries, boo
         SSB_TRY(ps.upload_ceilings());
     }
     ps.finish();
+    return SSB_OK;
+}
+
+// host-facing lexical search: the first page of <= SSB_K_MAX hits with the counts, then Topk pages below the previous page's last key.
+// W = 2: a sorted batch (sort), 128-bit keys.
+template <int W>
+int32_t search_lexical_host(ssb_index* ix, SearchCtx& c, const ssb_lex_batch* q, uint32_t k, uint32_t result_type, ssb_hit* hits, uint32_t* n_hits,
+                            uint64_t* count_total, const SortDev* sort) {
+    const uint32_t nq = q->n_queries;
+    SSB_TRY(c.keys_a.reserve((size_t)nq * LIST * W, 0, c.st));
+    SSB_TRY(c.counts.reserve(nq, 0, c.st));
+    c.h_keys_a.resize((size_t)nq * LIST * W); c.h_counts.resize(nq);
+    const bool want_hits = hits && k && result_type != SSB_RESULT_COUNT;
+    const uint32_t k1 = k < SSB_K_MAX ? k : SSB_K_MAX;
+    SSB_TRY(ix->lex->search_keys(c.lex, c.st, q, k1, result_type, c.keys_a.p, c.counts.p, &c.stats.kernel_launches, nullptr, sort));
+    if (W == 1) SSB_TRY(shard_merge(ix, c, c.keys_a.p, nq));         // (sorted searches refuse a communicator)
+    SSB_TRY(shard_sum_counts(ix, c, c.counts.p, nq));
+    SSB_CUDA_TRY(cudaMemcpyAsync(c.h_keys_a.data(), c.keys_a.p, (size_t)nq * LIST * W * 8, cudaMemcpyDeviceToHost, c.st));
+    SSB_CUDA_TRY(cudaMemcpyAsync(c.h_counts.data(), c.counts.p, (size_t)nq * 8, cudaMemcpyDeviceToHost, c.st));
+    SSB_CUDA_TRY(cudaStreamSynchronize(c.st));
+    c.stats.d2h_bytes += (uint64_t)nq * (LIST * W * 8 + 8);
+    c.ev_used = true;
+    finish_stats(ix, c);                                        // the first page's scoring kernel is the one reported
+    const LexStats ls = LexIndex::read_stats(c.lex, c.st);
+    if (want_hits) {
+        PageState<W> ps(c, nq, k, hits, n_hits, false, sort && sort->score_asc);
+        bool more = ps.append(c.h_keys_a.data(), k1);
+        // pages beyond the first 32 results: Topk search restricted to keys below the previous page's last key
+        while (more) {
+            const uint32_t kk = ps.next_page_k();
+            SSB_TRY(ps.upload_ceilings());
+            SSB_TRY(ix->lex->search_keys(c.lex, c.st, q, kk, SSB_RESULT_TOPK, c.keys_a.p, nullptr, &c.stats.kernel_launches, c.ceil.p, sort));
+            if (W == 1) SSB_TRY(shard_merge(ix, c, c.keys_a.p, nq));
+            SSB_CUDA_TRY(cudaMemcpyAsync(c.h_keys_a.data(), c.keys_a.p, (size_t)nq * LIST * W * 8, cudaMemcpyDeviceToHost, c.st));
+            SSB_CUDA_TRY(cudaStreamSynchronize(c.st));
+            c.stats.d2h_bytes += (uint64_t)nq * LIST * W * 8;
+            more = ps.append(c.h_keys_a.data(), kk);
+        }
+        ps.finish();
+    } else if (n_hits) for (uint32_t i = 0; i < nq; i++) n_hits[i] = 0;
+    if (count_total) for (uint32_t i = 0; i < nq; i++) count_total[i] = c.h_counts[i];
+    c.stats.postings_visited = ls.postings_visited;
+    // SURVEY.md §8(d) accounting with this layout's sizes: 4 B per streamed posting word, 16 B per probe (8 B bitmap word + 4 B
+    // rank / word bound + 4 B component), 128 B per (query, level) record read, 8 B per bitmap word of the word-wise count paths;
+    // the 1-byte coarse-table lookups of the stream filter are not counted
+    c.stats.algorithmic_bytes = ls.postings_visited * 4 + ls.probes * 16 + ls.recs_processed * 128 + ls.dense_words * 8;
+    c.stats.probes = ls.probes; c.stats.items_processed = ls.items_processed; c.stats.items_skipped = ls.items_skipped;
     return SSB_OK;
 }
 
@@ -851,7 +905,37 @@ int32_t ssb_set_facets(ssb_index* ix, const void* rows, uint64_t first_doc_id, u
     SSB_CUDA_TRY(cudaMalloc(&ix->facets.d_keys, keys.size() * 8));
     SSB_CUDA_TRY(cudaMemcpy(ix->facets.d_keys, keys.data(), keys.size() * 8, cudaMemcpyHostToDevice));
     ix->facets.n_rows = n_docs; ix->facets.first_doc = (uint32_t)first_doc_id; ix->facets.n_facets = n_fields;
-    for (uint32_t f = 0; f < n_fields; f++) ix->facets.types[f] = (uint8_t)fields[f].type;
+    for (uint32_t f = 0; f < n_fields; f++) {
+        ix->facets.types[f] = (uint8_t)fields[f].type;
+        const uint64_t* col = keys.data() + (size_t)f * n_docs;
+        ix->facets.max_key[f] = *std::max_element(col, col + n_docs);
+        SSB_TRY(facet_zones(ix->facets, f, ix->load_st));           // per-level bounds of sorted searches
+    }
+    SSB_CUDA_TRY(cudaStreamSynchronize(ix->load_st));
+    return SSB_OK;
+    SSB_API_END
+}
+
+int32_t ssb_set_facet_value_order(ssb_index* ix, uint32_t facet, const uint32_t* rank_of_id, uint32_t n_ids) {
+    SSB_API_BEGIN
+    if (!ix || (n_ids && !rank_of_id)) { set_error("ssb_set_facet_value_order: null argument"); return SSB_E_INVALID; }
+    std::unique_lock<std::shared_mutex> g(ix->rw);
+    SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
+    FacetSet& fs = ix->facets;
+    if (!fs.n_facets) { set_error("ssb_set_facet_value_order: no facets (ssb_set_facets)"); return SSB_E_STATE; }
+    if (facet >= fs.n_facets) { set_error("ssb_set_facet_value_order: facet %u of %u", facet, fs.n_facets); return SSB_E_INVALID; }
+    const uint32_t type = fs.types[facet];
+    if (type != SSB_FACET_STRING16 && type != SSB_FACET_STRING32) { set_error("ssb_set_facet_value_order: facet %u is not a String16 / String32 facet", facet); return SSB_E_INVALID; }
+    const uint64_t lim = type == SSB_FACET_STRING16 ? 65536ull : (1ull << 32);
+    if (n_ids == 0 || n_ids > lim) { set_error("ssb_set_facet_value_order: n_ids must be in 1..%llu", (unsigned long long)lim); return SSB_E_INVALID; }
+    for (uint32_t i = 0; i < n_ids; i++) if (rank_of_id[i] >= n_ids) { set_error("ssb_set_facet_value_order: rank %u of id %u is not below n_ids", rank_of_id[i], i); return SSB_E_INVALID; }
+    SSB_CUDA_TRY(cudaDeviceSynchronize());        // searches on a caller-owned stream may still read the old order
+    cudaFree(fs.d_rank[facet]); fs.d_rank[facet] = nullptr; fs.n_rank[facet] = 0;
+    SSB_CUDA_TRY(cudaMalloc(&fs.d_rank[facet], (size_t)n_ids * 4));
+    SSB_CUDA_TRY(cudaMemcpy(fs.d_rank[facet], rank_of_id, (size_t)n_ids * 4, cudaMemcpyHostToDevice));
+    fs.n_rank[facet] = n_ids;
+    SSB_TRY(facet_zones(fs, facet, ix->load_st));                   // the level bounds of this facet are ranks from now on
+    SSB_CUDA_TRY(cudaStreamSynchronize(ix->load_st));
     return SSB_OK;
     SSB_API_END
 }
@@ -982,50 +1066,29 @@ int32_t ssb_search_lexical(ssb_index* ix, const ssb_lex_batch* q, uint32_t k, ui
     if (!ix || !q || (q->n_queries && k && result_type != SSB_RESULT_COUNT && !hits)) { set_error("ssb_search_lexical: null argument"); return SSB_E_INVALID; }
     std::shared_lock<std::shared_mutex> g(ix->rw);
     SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
-    const uint32_t nq = q->n_queries;
-    if (nq == 0) return SSB_OK;
+    if (q->n_queries == 0) return SSB_OK;
     if (k > SSB_K_LIMIT) { set_error("k=%u exceeds SSB_K_LIMIT=%u", k, SSB_K_LIMIT); return SSB_E_UNSUPPORTED; }
     CtxLease l(ix); SSB_TRY(l.acquire());
-    SearchCtx& c = *l.c;
-    SSB_TRY(c.keys_a.reserve((size_t)nq * LIST, 0, c.st));
-    SSB_TRY(c.counts.reserve(nq, 0, c.st));
-    c.h_keys_a.resize((size_t)nq * LIST); c.h_counts.resize(nq);
-    const bool want_hits = hits && k && result_type != SSB_RESULT_COUNT;
-    const uint32_t k1 = k < SSB_K_MAX ? k : SSB_K_MAX;
-    SSB_TRY(ix->lex->search_keys(c.lex, c.st, q, k1, result_type, c.keys_a.p, c.counts.p, &c.stats.kernel_launches));
-    SSB_TRY(shard_merge(ix, c, c.keys_a.p, nq));
-    SSB_TRY(shard_sum_counts(ix, c, c.counts.p, nq));
-    SSB_CUDA_TRY(cudaMemcpyAsync(c.h_keys_a.data(), c.keys_a.p, (size_t)nq * LIST * 8, cudaMemcpyDeviceToHost, c.st));
-    SSB_CUDA_TRY(cudaMemcpyAsync(c.h_counts.data(), c.counts.p, (size_t)nq * 8, cudaMemcpyDeviceToHost, c.st));
-    SSB_CUDA_TRY(cudaStreamSynchronize(c.st));
-    c.stats.d2h_bytes += (uint64_t)nq * (LIST * 8 + 8);
-    c.ev_used = true;
-    finish_stats(ix, c);                                        // the first page's scoring kernel is the one reported
-    const LexStats ls = LexIndex::read_stats(c.lex, c.st);
-    if (want_hits) {
-        PageState ps(c, nq, k, hits, n_hits);
-        bool more = ps.append(c.h_keys_a.data(), k1);
-        // pages beyond the first 32 results: Topk search restricted to keys below the previous page's last key
-        while (more) {
-            const uint32_t kk = ps.next_page_k();
-            SSB_TRY(ps.upload_ceilings());
-            SSB_TRY(ix->lex->search_keys(c.lex, c.st, q, kk, SSB_RESULT_TOPK, c.keys_a.p, nullptr, &c.stats.kernel_launches, c.ceil.p));
-            SSB_TRY(shard_merge(ix, c, c.keys_a.p, nq));
-            SSB_CUDA_TRY(cudaMemcpyAsync(c.h_keys_a.data(), c.keys_a.p, (size_t)nq * LIST * 8, cudaMemcpyDeviceToHost, c.st));
-            SSB_CUDA_TRY(cudaStreamSynchronize(c.st));
-            c.stats.d2h_bytes += (uint64_t)nq * LIST * 8;
-            more = ps.append(c.h_keys_a.data(), kk);
-        }
-        ps.finish();
-    } else if (n_hits) for (uint32_t i = 0; i < nq; i++) n_hits[i] = 0;
-    if (count_total) for (uint32_t i = 0; i < nq; i++) count_total[i] = c.h_counts[i];
-    c.stats.postings_visited = ls.postings_visited;
-    // SURVEY.md §8(d) accounting with this layout's sizes: 4 B per streamed posting word, 16 B per probe (8 B bitmap word + 4 B
-    // rank / word bound + 4 B component), 128 B per (query, level) record read, 8 B per bitmap word of the word-wise count paths;
-    // the 1-byte coarse-table lookups of the stream filter are not counted
-    c.stats.algorithmic_bytes = ls.postings_visited * 4 + ls.probes * 16 + ls.recs_processed * 128 + ls.dense_words * 8;
-    c.stats.probes = ls.probes; c.stats.items_processed = ls.items_processed; c.stats.items_skipped = ls.items_skipped;
-    return SSB_OK;
+    return search_lexical_host<1>(ix, *l.c, q, k, result_type, hits, n_hits, count_total, nullptr);
+    SSB_API_END
+}
+
+int32_t ssb_search_lexical_sorted(ssb_index* ix, const ssb_lex_batch* q, const ssb_sort_criterion* sort, uint32_t n_sort, uint32_t k, uint32_t result_type,
+                                  ssb_hit* hits, uint32_t* n_hits, uint64_t* count_total) {
+    SSB_API_BEGIN
+    // ResultType::Count ignores the sort (search.rs:2498); k = 0 is Count (search.rs:2472-2478)
+    if (result_type == SSB_RESULT_COUNT || k == 0) return ssb_search_lexical(ix, q, k, result_type, hits, n_hits, count_total);
+    if (!ix || !q || (q->n_queries && !hits)) { set_error("ssb_search_lexical_sorted: null argument"); return SSB_E_INVALID; }
+    std::shared_lock<std::shared_mutex> g(ix->rw);
+    SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
+    SortDev sd{}; bool sorted = false;
+    SSB_TRY(ix->lex->prepare_sort(sort, n_sort, &sd, &sorted));
+    if (sorted && ix->comm.active()) { set_error("ssb_search_lexical_sorted: sorted search across shards is not built"); return SSB_E_UNSUPPORTED; }
+    if (q->n_queries == 0) return SSB_OK;
+    if (k > SSB_K_LIMIT) { set_error("k=%u exceeds SSB_K_LIMIT=%u", k, SSB_K_LIMIT); return SSB_E_UNSUPPORTED; }
+    CtxLease l(ix); SSB_TRY(l.acquire());
+    if (!sorted) return search_lexical_host<1>(ix, *l.c, q, k, result_type, hits, n_hits, count_total, nullptr);   // "_score desc" = the default order
+    return search_lexical_host<2>(ix, *l.c, q, k, result_type, hits, n_hits, count_total, &sd);
     SSB_API_END
 }
 

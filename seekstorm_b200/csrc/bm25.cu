@@ -263,10 +263,17 @@ __device__ __forceinline__ uint32_t meta_cperm(uint32_t m, uint32_t c) { return 
 // would otherwise derive per item with warp-uniform code: directory entries of every term, MAXSCORE order (terms by
 // block bound), the in-query-order suffix sums S[p] / R[p], the count order, the AND driver — and writes them as one
 // 128-byte record.  Thread 0 finally cuts the sorted record list into work items.
+// SORTED (ssb_search_lexical_sorted): every query takes lex_generic, theta / glist are the 128-bit θ and lists, and the levels are ordered
+// by the upper bound of the sort key instead of the score bound (its top 32 bits: the order only decides how early θ rises; the exact
+// bound goes into the record, rec_sort_bound, for the skip test).
+__device__ __forceinline__ uint64_t level_sort_bound(const SortDev& s, uint32_t level_id);
+__device__ __forceinline__ void rec_set_sort_bound(LvRec& r, uint64_t b) { r.S[0] = __uint_as_float((uint32_t)b); r.S[1] = __uint_as_float((uint32_t)(b >> 32)); }
+__device__ __forceinline__ uint64_t rec_sort_bound(const LvRec& r) { return ((uint64_t)__float_as_uint(r.S[1]) << 32) | __float_as_uint(r.S[0]); }
+template <bool SORTED>
 __global__ void __launch_bounds__(128) lex_plan(LexView v, const uint32_t* __restrict__ q_off, const uint64_t* __restrict__ q_keys,
                                                 const uint8_t* __restrict__ q_flags /*or null*/, const uint32_t* __restrict__ f_off /*or null*/, const uint32_t* __restrict__ f_mask /*or null*/, uint32_t flags /* bit 0 phrase batch, bit 1 no counts wanted */, uint32_t query_type, QueryPlan* plans, LvRec* recs, uint16_t* item_start, uint32_t* ctr,
                                                 uint64_t* theta, int* lock, uint64_t* count, uint64_t* glist, uint32_t n_pow2,
-                                                uint32_t item_w, uint32_t first_lim, uint32_t gmax) {
+                                                uint32_t item_w, uint32_t first_lim, uint32_t gmax, SortDev sort) {
     extern __shared__ __align__(16) uint8_t sm_raw[];
     float* bound = (float*)sm_raw;                                     // [n_levels]
     uint32_t* cnt = (uint32_t*)(bound + v.n_levels);                   // [n_levels]; after the sort: item weights by sorted position
@@ -281,8 +288,13 @@ __global__ void __launch_bounds__(128) lex_plan(LexView v, const uint32_t* __res
     const uint32_t nlv = v.n_levels;
     const uint32_t t0 = q_off[q], nt_raw = q_off[q + 1] - t0;
     const uint32_t nt = nt_raw > SSB_MAX_QUERY_TERMS + SSB_MAX_NOT_TERMS ? SSB_MAX_QUERY_TERMS + SSB_MAX_NOT_TERMS : nt_raw;
+    if constexpr (SORTED) {
+        if (threadIdx.x < 2 * LIST) glist[(size_t)q * 2 * LIST + threadIdx.x] = 0;
+        if (threadIdx.x == 0) { theta[2 * q] = 0; theta[2 * q + 1] = 0; lock[q] = 0; count[q] = 0; n_valid = 0; }
+    } else {
     if (threadIdx.x < 32) glist[(size_t)q * LIST + threadIdx.x] = 0;
     if (threadIdx.x == 0) { theta[q] = 0; lock[q] = 0; count[q] = 0; n_valid = 0; }
+    }
     if (threadIdx.x < nt) {
         uint64_t key = q_keys[t0 + threadIdx.x];
         uint32_t lo = 0, hi = v.n_terms;
@@ -325,6 +337,7 @@ __global__ void __launch_bounds__(128) lex_plan(LexView v, const uint32_t* __res
         // facet-filtered queries stay on the record path when nothing has to be counted (flags bit 1): lex_score tests the filter on the
         // exact-score survivors; with counts every match must be tested -> lex_generic
         pl.fast = (nl <= v.fast_t && (pl.n_filt == 0 || (flags & 2u)) && pl.field_mask == 0 && pl.n_phr == 0) ? 1u : 0u;
+        if constexpr (SORTED) pl.fast = 0;
     }
     for (uint32_t b = threadIdx.x; b < nlv; b += blockDim.x) {
         bound[b] = 0.f; cnt[b] = 0;
@@ -347,6 +360,9 @@ __global__ void __launch_bounds__(128) lex_plan(LexView v, const uint32_t* __res
         uint64_t key = 0;
         if (b < nlv) {
             bool ok = query_type == SSB_QUERY_INTERSECTION ? (nl > 0 && cnt[b] == nl) : (cnt[b] > 0);
+            if constexpr (SORTED) {
+                if (ok) { key = (level_sort_bound(sort, v.level_ids[b]) & 0xFFFFFFFF00000000ull) | (uint64_t)(0xFFFFFFFFu - b); atomicAdd(&n_valid, 1u); }
+            } else
             if (ok) { key = ((uint64_t)ord_f32(bound[b]) << 32) | (uint64_t)(0xFFFFFFFFu - b); atomicAdd(&n_valid, 1u); }
         }
         skey[b] = key;
@@ -434,6 +450,9 @@ __global__ void __launch_bounds__(128) lex_plan(LexView v, const uint32_t* __res
             meta = (nl < 7u ? nl : 7u) << 29;
 #pragma unroll
             for (int p = 0; p < 4; p++) { r.S[p] = 0.f; r.R[p] = 0.f; }
+            // lex_generic does not read S[].  A sorted query's items take up to gmax levels whatever their lists' lengths: the warp's own
+            // list then bounds the later (lower-bound) levels of its item, which it skips without waiting for θ
+            if constexpr (SORTED) { rec_set_sort_bound(r, level_sort_bound(sort, v.level_ids[lv])); weight = 0; }
         }
         r.meta = meta;
         const uint4* src = reinterpret_cast<const uint4*>(&r);
@@ -701,9 +720,79 @@ __device__ __forceinline__ void insert_candidates(uint64_t& L, uint32_t& thr, bo
     if (kth > thr) thr = kth;
 }
 
+// ---- sorted batches: 128-bit top-k keys (hi = packed sort key, lo = pack_key(score, doc)), warp lists descending like wl_* ----
+__device__ __forceinline__ bool gt128(uint64_t ah, uint64_t al, uint64_t bh, uint64_t bl) { return ah > bh || (ah == bh && al > bl); }
+__device__ __forceinline__ void wl_insert128(uint64_t& Lh, uint64_t& Ll, uint64_t ch, uint64_t cl, int lane) {
+    const int pos = __popc(__ballot_sync(FULL, !gt128(ch, cl, Lh, Ll)));   // entries >= cand stay in front
+    if (__any_sync(FULL, Lh == ch && Ll == cl)) return;
+    const uint64_t uh = shfl64_up1(Lh), ul = shfl64_up1(Ll);
+    if (lane == pos) { Lh = ch; Ll = cl; }
+    else if (lane > pos) { Lh = uh; Ll = ul; }
+}
+__device__ __forceinline__ void wl_merge128(uint64_t& Ah, uint64_t& Al, uint64_t Bh, uint64_t Bl, int lane) {
+    const uint64_t rh = shfl64(Bh, 31 - lane), rl = shfl64(Bl, 31 - lane);
+    if (gt128(rh, rl, Ah, Al)) { Ah = rh; Al = rl; }                   // bitonic, holds the top 32 of the union
+#pragma unroll
+    for (int s = 16; s >= 1; s >>= 1) {
+        const uint64_t ph = shfl64_xor(Ah, s), pl = shfl64_xor(Al, s);
+        const bool keep_max = (lane & s) == 0;
+        if (keep_max == gt128(ph, pl, Ah, Al)) { Ah = ph; Al = pl; }
+    }
+}
+// the warp's list of one sorted item; thr = a lower bound of θ.hi (global θ.hi, or the local list's k-th hi once it is full)
+struct SortTop { uint64_t h, l, thr; };
+// doc's packed sort key: the facet column keys of its row (a String facet's id through its value order), or its id
+__device__ __forceinline__ uint64_t sort_pack_hi(const SortDev& s, const uint64_t* v);
+__device__ __forceinline__ uint64_t doc_sort_hi(const LexView& v, const SortDev& s, uint32_t doc) {
+    const uint64_t row = (uint64_t)(doc - v.facet_first_doc);          // prepare_sort: the facet rows cover every doc of the levels
+    uint64_t val[SSB_MAX_SORT_CRITERIA];
+#pragma unroll
+    for (uint32_t i = 0; i < SSB_MAX_SORT_CRITERIA; i++) {
+        val[i] = doc;
+        if (i < s.n && s.src[i] == SORT_SRC_FACET) {
+            val[i] = __ldg(&v.facet_keys[(size_t)s.facet[i] * v.facet_rows + row]);
+            if (s.rank[i]) val[i] = __ldg(&s.rank[i][val[i]]);          // prepare_sort: every id of the column has a rank
+        }
+    }
+    return sort_pack_hi(s, val);
+}
+// insert the lanes' candidates (cand) below the paging ceiling (ch, cl) into the warp list; raise thr from the k-th entry
+__device__ __forceinline__ void insert_sorted(SortTop& T, bool cand, uint64_t hi, float score, uint32_t doc, bool score_asc,
+                                              uint32_t k, int lane, bool& dirty, uint64_t ch, uint64_t cl) {
+    const uint64_t lo = pack_key(score, doc) ^ (score_asc ? 0xFFFFFFFF00000000ull : 0ull);
+    unsigned m = __ballot_sync(FULL, cand && gt128(ch, cl, hi, lo));
+    if (!m) return;
+    while (m) {
+        const int src = __ffs(m) - 1; m &= m - 1;
+        wl_insert128(T.h, T.l, shfl64(hi, src), shfl64(lo, src), lane);
+    }
+    dirty = true;
+    const uint64_t kth = shfl64(T.h, (int)k - 1);
+    if (kth > T.thr) T.thr = kth;
+}
+// merge the warp's list into the query's global list (glist [q][32][2], theta [q][2]) under the per-query lock.  Readers outside the lock
+// load θ.hi alone — the pair can tear, θ.hi never decreases — and prune only docs with hi < θ.hi.
+__device__ __forceinline__ void publish_sorted(const SortTop& T, uint32_t q, uint32_t k, int lane, uint64_t* theta, int* lock, uint64_t* glist) {
+    if (lane == 0) { while (atomicCAS(&lock[q], 0, 1) != 0) __nanosleep(40); }
+    __syncwarp();
+    __threadfence();
+    uint64_t* g = glist + ((size_t)q * LIST + lane) * 2;
+    uint64_t Mh = T.h, Ml = T.l;
+    wl_merge128(Mh, Ml, __ldcg(&g[0]), __ldcg(&g[1]), lane);
+    __stcg(&g[0], Mh); __stcg(&g[1], Ml);
+    const uint64_t nh = shfl64(Mh, (int)k - 1), nl = shfl64(Ml, (int)k - 1);
+    __threadfence();
+    __syncwarp();
+    if (lane == 0) {
+        if (gt128(nh, nl, __ldcg(&theta[2 * q]), __ldcg(&theta[2 * q + 1]))) { __stcg(&theta[2 * q + 1], nl); __stcg(&theta[2 * q], nh); }
+        __threadfence();
+        atomicExch(&lock[q], 0);
+    }
+}
+
 struct ItemCtx {
     uint32_t q, lv, n, k, docbase, bound_ord, n_not, n_filt /* facet filters + (field filter ? 1 : 0): 0 = unfiltered query */, n_facet_filt, filt_first, field_mask;
-    uint64_t ceil;
+    uint64_t ceil, ceil_lo /* sorted batches: the ceiling is the 128-bit key (ceil, ceil_lo) */;
     bool scoring, need_count, is_and;
 };
 
@@ -1163,10 +1252,13 @@ __device__ __forceinline__ void score_records(const LexView& v, WarpSm& w, uint3
 }
 
 // ---- generic path: up to SSB_MAX_QUERY_TERMS live terms, lane t holds term t, values broadcast by shuffles ----
-template <bool FIELD_RUNS>
+// SORTED: the top-k key is (sort key, score, doc) in T (L / thr unused).  θ is not a score there, so none of the score bounds prunes
+// (MAXSCORE driver break, score test of the insert); a candidate whose sort key is below T.thr is dropped before its score loads and,
+// on the OR path, before its probes (AND, Topk: before its probes as well — nothing is counted).
+template <bool FIELD_RUNS, bool SORTED = false>
 __device__ __forceinline__ void process_item_generic(const LexView& v, const QueryPlan* pl, const ItemCtx& c, int lane,
                                                   uint64_t& L, uint32_t& thr, bool& dirty, uint32_t& matches_out,
-                                                  uint32_t& st_visited, uint32_t& st_probes) {
+                                                  uint32_t& st_visited, uint32_t& st_probes, SortTop& T, const SortDev& sd) {
     const uint32_t n = c.n, lv = c.lv;
     uint32_t matches = 0;
     TermRegs tr; tr.cnt = 0; tr.off = 0; tr.bmi = NONE; tr.idf = 0.f; tr.ub = 0.f;
@@ -1194,22 +1286,34 @@ __device__ __forceinline__ void process_item_generic(const LexView& v, const Que
             const bool active = p < dcnt;
             const uint32_t d = active ? (__ldg(&v.post[doff + p]) & 0xFFFFu) : 0u;
             bool ok = active; float score = 0.f;
+            uint64_t hi = 0; bool keep = true;
+            if constexpr (SORTED) {
+                if (active && c.scoring) hi = doc_sort_hi(v, sd, c.docbase | d);
+                keep = c.scoring && !(hi < T.thr);
+                ok = active && (keep || c.need_count);
+            }
             for (uint32_t t = 0; t < n; t++) {          // query order
                 const uint32_t tc = __shfl_sync(FULL, tr.cnt, t); const uint64_t to = shfl64(tr.off, t);
                 const uint32_t tb = __shfl_sync(FULL, tr.bmi, t); const float ti = __shfl_sync(FULL, tr.idf, t);
                 uint32_t rank = p; bool found = true;
                 if ((int)t != drv) { found = ok && probe(v, tc, to, tb, d, rank); st_probes += ok ? 1 : 0; }
                 ok = ok && found;
-                if (ok && c.scoring) score = acc_term(v, score, ti, to + rank);
+                if (ok && c.scoring && (!SORTED || keep)) score = acc_term(v, score, ti, to + rank);
             }
             if (c.n_filt) {
                 // a filtered query is counted here doc by doc: filter, delete set and NOT lists at once (the correction kernels skip it)
                 ok = ok && !filters_reject<FIELD_RUNS>(v, pl, c.filt_first, c.n_facet_filt, c.field_mask, c.n, c.lv, d, c.docbase | d) && !is_deleted(v, c.docbase | d) && !(c.n_not && in_not_lists(v, pl, c.n_not, c.lv, d));
                 matches += __popc(__ballot_sync(FULL, ok));
+                if constexpr (SORTED) { if (c.scoring) insert_sorted(T, ok && keep, hi, score, c.docbase | d, sd.score_asc, c.k, lane, dirty, c.ceil, c.ceil_lo); }
+                else
                 if (c.scoring) insert_candidates(L, thr, ok && ord_f32(score) >= thr, score, c.docbase | d, c.k, lane, dirty, c.ceil);
                 continue;
             }
             matches += __popc(__ballot_sync(FULL, ok));
+            if constexpr (SORTED) {
+                if (c.scoring) insert_sorted(T, ok && keep && !is_deleted(v, c.docbase | d) && !(c.n_not && in_not_lists(v, pl, c.n_not, c.lv, d)), hi, score, c.docbase | d,
+                                             sd.score_asc, c.k, lane, dirty, c.ceil, c.ceil_lo);
+            } else
             if (c.scoring) insert_candidates(L, thr, ok && ord_f32(score) >= thr && !is_deleted(v, c.docbase | d) && !(c.n_not && in_not_lists(v, pl, c.n_not, c.lv, d)), score, c.docbase | d, c.k, lane, dirty, c.ceil);
         }
         if (lane == 0) matches_out += matches;
@@ -1233,7 +1337,7 @@ __device__ __forceinline__ void process_item_generic(const LexView& v, const Que
                 float ou = __shfl_sync(FULL, tr.ub, t); uint32_t orr = __shfl_sync(FULL, rk, t);
                 if (orr >= p) S = __fadd_rn(S, ou);
             }
-            if (ord_f32(S) < thr) break;
+            if (!SORTED && ord_f32(S) < thr) break;
             const uint64_t doff = shfl64(tr.off, drv);
             const float didf = __shfl_sync(FULL, tr.idf, drv);
             st_visited += dcnt;
@@ -1242,18 +1346,28 @@ __device__ __forceinline__ void process_item_generic(const LexView& v, const Que
                 const bool active = pp < dcnt;
                 const uint32_t d = active ? (__ldg(&v.post[doff + pp]) & 0xFFFFu) : 0u;
                 bool dup = false; float score = 0.f;
+                uint64_t hi = 0; bool live = active;
+                if constexpr (SORTED) {
+                    if (active) hi = doc_sort_hi(v, sd, c.docbase | d);
+                    live = active && !(hi < T.thr);
+                }
                 for (uint32_t t = 0; t < n; t++) {      // query order
                     const uint32_t tc = __shfl_sync(FULL, tr.cnt, t); const uint64_t to = shfl64(tr.off, t);
                     const uint32_t tb = __shfl_sync(FULL, tr.bmi, t); const float ti = __shfl_sync(FULL, tr.idf, t);
                     const uint32_t trk = __shfl_sync(FULL, rk, t);
-                    if ((int)t == drv) { if (active) score = acc_term(v, score, didf, doff + pp); continue; }
-                    if (tc == 0 || !active || dup) continue;
+                    if ((int)t == drv) { if (live) score = acc_term(v, score, didf, doff + pp); continue; }
+                    if (tc == 0 || !live || dup) continue;
                     uint32_t rank; st_probes++;
                     if (probe(v, tc, to, tb, d, rank)) {
                         if (trk < p) dup = true;
                         else score = acc_term(v, score, ti, to + rank);
                     }
                 }
+                if constexpr (SORTED) {
+                    insert_sorted(T, live && !dup && !is_deleted(v, c.docbase | d) && !(c.n_not && in_not_lists(v, pl, c.n_not, c.lv, d))
+                                     && !(c.n_filt && filters_reject<FIELD_RUNS>(v, pl, c.filt_first, c.n_facet_filt, c.field_mask, c.n, c.lv, d, c.docbase | d)),
+                                  hi, score, c.docbase | d, sd.score_asc, c.k, lane, dirty, c.ceil, c.ceil_lo);
+                } else
                 insert_candidates(L, thr, active && !dup && ord_f32(score) >= thr && !is_deleted(v, c.docbase | d) && !(c.n_not && in_not_lists(v, pl, c.n_not, c.lv, d))
                                               && !(c.n_filt && filters_reject<FIELD_RUNS>(v, pl, c.filt_first, c.n_facet_filt, c.field_mask, c.n, c.lv, d, c.docbase | d)), score, c.docbase | d, c.k, lane, dirty, c.ceil);
             }
@@ -1438,11 +1552,13 @@ __global__ void __launch_bounds__(128, 6) lex_count(LexView v, const QueryPlan* 
 
 // ---- queries with 5..16 live terms: one level per item, per-term state in lanes (scoring and counting) ----
 // FIELD_RUNS: phrase batch on an index with several fields (the phrase check walks per-field position runs)
-template <bool FIELD_RUNS>
+// SORTED: a sorted batch (every query is here; theta / glist / ceil_keys hold 128-bit keys).  The score bound of a level means nothing
+// there; under Topk a level is skipped when its sort-key bound is below θ.hi (strictly: ties in hi go through the exact insert).
+template <bool FIELD_RUNS, bool SORTED>
 __global__ void __launch_bounds__(256) lex_generic(LexView v, const QueryPlan* __restrict__ plans, const LvRec* __restrict__ recs,
                                                   const uint16_t* __restrict__ item_start, uint32_t nq, uint32_t query_type, uint32_t result_type,
                                                   uint32_t k, uint32_t* ctr, uint64_t* theta, int* lock, uint64_t* count, uint64_t* glist,
-                                                  LexStats* stats, const uint64_t* __restrict__ ceil_keys) {
+                                                  LexStats* stats, const uint64_t* __restrict__ ceil_keys, SortDev sort) {
     if (*(volatile uint32_t*)&ctr[4] == 0) return;       // no query of this batch has more than FAST_T live terms
     __shared__ __align__(16) WarpSm wsm[8];
     WarpSm& w = wsm[(threadIdx.x >> 5) & 7];
@@ -1457,11 +1573,35 @@ __global__ void __launch_bounds__(256) lex_generic(LexView v, const QueryPlan* _
     while (next_item<false>(w, &ctr[3], total, nq, plans, lane, j, q)) {
         const QueryPlan* pl = &plans[q];
         const uint32_t n_live = __ldg(&pl->n_live);
+        if constexpr (SORTED) {
+            const uint64_t ch = ceil_keys ? __ldg(&ceil_keys[2 * q]) : ~0ull, cl = ceil_keys ? __ldg(&ceil_keys[2 * q + 1]) : ~0ull;
+            if (ch == 0 && cl == 0) continue;
+            const uint32_t nrec = stage_item(w, recs, item_start, v.n_levels, q, j, lane);
+            SortTop T{0, 0, 0};
+            uint64_t L = 0; uint32_t thr = 0; bool dirty = false; uint32_t matches = 0;
+            for (uint32_t ri = 0; ri < nrec; ri++) {
+                const uint64_t th = __ldcg(&theta[2 * q]);
+                if (th > T.thr) T.thr = th;
+                ItemCtx c;
+                c.ceil = ch; c.ceil_lo = cl; c.q = q; c.n = n_live; c.k = k; c.lv = w.recs[ri].lv; c.bound_ord = 0; c.n_not = __ldg(&pl->n_not);
+                c.n_facet_filt = __ldg(&pl->n_filt); c.filt_first = __ldg(&pl->filt_first); c.field_mask = __ldg(&pl->field_mask);
+                c.n_filt = c.n_facet_filt + (c.field_mask ? 1u : 0u) + (__ldg(&pl->n_phr) ? 1u : 0u);
+                c.scoring = want_topk && !(rec_sort_bound(w.recs[ri]) < T.thr);
+                c.need_count = need_count; c.is_and = query_type == SSB_QUERY_INTERSECTION; c.docbase = w.recs[ri].docbase;
+                if (!c.scoring && !need_count) { st_skipped++; continue; }
+                st_done++;
+                process_item_generic<FIELD_RUNS, true>(v, pl, c, lane, L, thr, dirty, matches, st_visited, st_probes, T, sort);
+            }
+            if (dirty) publish_sorted(T, q, k, lane, theta, lock, glist);
+            if (need_count && lane == 0 && matches) atomicAdd((unsigned long long*)&count[q], (unsigned long long)matches);
+            continue;
+        }
         const uint64_t ceil = ceil_keys ? __ldg(&ceil_keys[q]) : ~0ull;
         if (ceil == 0) continue;
         const uint32_t nrec = stage_item(w, recs, item_start, v.n_levels, q, j, lane);
         uint32_t thr = (uint32_t)(__ldcg(&theta[q]) >> 32);
         uint64_t L = 0; bool dirty = false; uint32_t matches = 0;
+        SortTop T;
         for (uint32_t ri = 0; ri < nrec; ri++) {
             ItemCtx c;
             c.ceil = ceil; c.q = q; c.n = n_live; c.k = k; c.lv = w.recs[ri].lv; c.bound_ord = ord_f32(w.recs[ri].bound); c.n_not = __ldg(&pl->n_not);
@@ -1471,7 +1611,7 @@ __global__ void __launch_bounds__(256) lex_generic(LexView v, const QueryPlan* _
             c.need_count = need_count; c.is_and = query_type == SSB_QUERY_INTERSECTION; c.docbase = w.recs[ri].docbase;
             if (!c.scoring && !need_count) { st_skipped++; continue; }
             st_done++;
-            process_item_generic<FIELD_RUNS>(v, pl, c, lane, L, thr, dirty, matches, st_visited, st_probes);
+            process_item_generic<FIELD_RUNS>(v, pl, c, lane, L, thr, dirty, matches, st_visited, st_probes, T, sort);
         }
         if (dirty) publish(L, q, k, lane, theta, lock, glist);
         if (need_count && lane == 0 && matches) atomicAdd((unsigned long long*)&count[q], (unsigned long long)matches);
@@ -1572,6 +1712,7 @@ void LexWorkspace::release() {
     cudaFree(plans); cudaFree(recs); cudaFree(item_start); cudaFree(theta); cudaFree(lock); cudaFree(count); cudaFree(ctr);
     cudaFree(qoff); cudaFree(qkeys); cudaFree(qflags); cudaFree(stats); cudaFree(foff); cudaFree(filt); cudaFree(fsets); cudaFree(fmask);
     foff = nullptr; filt = nullptr; fsets = nullptr; fmask = nullptr; cap_filt = cap_fsets = 0;
+    cudaFree(theta2); theta2 = nullptr;
     qflags = nullptr; plans = nullptr; recs = nullptr; item_start = nullptr; theta = nullptr; lock = nullptr; count = nullptr; ctr = nullptr;
     qoff = nullptr; qkeys = nullptr; stats = nullptr; cap_q = cap_terms = cap_levels = 0;
 }
@@ -1959,6 +2100,144 @@ uint32_t facet_type_bytes(uint32_t type) {
     return 0;
 }
 
+// ---- sort keys (ssb_search_lexical_sorted; result_ordering_shard, min_heap.rs:574-1051) ----
+// The packed sort key `hi` — the one place that knows its layout.  v[i] is criterion i's value: the facet's column key (facet_value_key;
+// for a String facet already replaced by the rank of its id in the value order) or the doc id (_id).  Each is narrowed to its natural
+// width (sort_width) keeping its order: unsigned values and ranks as they are, signed ones with the sign bit flipped within the width,
+// F32 by the IEEE order trick on 32 bits (-0.0 already folded into +0.0, NaN = all ones: above +inf), 64-bit keys as they are; inverted
+// within the width when ascending; concatenated with the first criterion most significant, left-aligned at bit 63.  Compared as one
+// unsigned word, hi orders docs like the criteria compared left to right.  The 128-bit top-k key is (hi, lo), lo = pack_key(score, doc)
+// with its score half inverted for `_score` ascending: ties on every criterion fall back to score desc (min_heap.rs:1043-1050), then
+// doc id asc.  hi is monotone in every v[i]: packing per-criterion upper bounds bounds the key of every doc (level_sort_bound).
+__host__ __device__ __forceinline__ uint32_t sort_width(uint32_t src, uint32_t type) {
+    if (src == SORT_SRC_ID) return 32;
+    switch (type) {
+        case SSB_FACET_U8: case SSB_FACET_I8: return 8;
+        case SSB_FACET_U16: case SSB_FACET_I16: case SSB_FACET_STRING16: return 16;
+        case SSB_FACET_U32: case SSB_FACET_I32: case SSB_FACET_F32: case SSB_FACET_STRING32: return 32;
+    }
+    return 64;
+}
+__device__ __forceinline__ uint64_t sort_pack_hi(const SortDev& s, const uint64_t* v) {
+    uint64_t hi = 0; uint32_t used = 0;
+#pragma unroll
+    for (uint32_t i = 0; i < SSB_MAX_SORT_CRITERIA; i++) {
+        if (i >= s.n) break;
+        const uint32_t w = sort_width(s.src[i], s.type[i]);
+        const uint64_t mask = w == 64 ? ~0ull : (1ull << w) - 1ull;
+        uint64_t x = v[i];
+        if (s.src[i] == SORT_SRC_FACET) {
+            const uint32_t t = s.type[i];
+            if (t == SSB_FACET_I8 || t == SSB_FACET_I16 || t == SSB_FACET_I32) x = (x & mask) ^ (1ull << (w - 1));
+            else if (t == SSB_FACET_F32) {        // column key = the f64 order key of the value (key_of_f64): back to the float, 32-bit order key
+                if (x == ~0ull) x = 0xFFFFFFFFull;
+                else x = ord_f32(__double2float_rn(__longlong_as_double((long long)((x >> 63) ? (x & 0x7FFFFFFFFFFFFFFFull) : ~x))));
+            }
+        }
+        x &= mask;
+        if (!s.desc[i]) x ^= mask;
+        used += w;
+        hi |= x << (64 - used);
+    }
+    return hi;
+}
+// upper bound of hi over the docs of a level: per criterion the level's largest value (descending) or smallest (ascending, inverted by
+// the packing) — the block's zone for a facet, level << 16 | 0xFFFF or level << 16 for _id
+__device__ __forceinline__ uint64_t level_sort_bound(const SortDev& s, uint32_t level_id) {
+    uint64_t val[SSB_MAX_SORT_CRITERIA];
+    const uint32_t b = level_id - s.zone_block0;                       // prepare_sort: the zones cover every level
+#pragma unroll
+    for (uint32_t i = 0; i < SSB_MAX_SORT_CRITERIA; i++) {
+        val[i] = s.desc[i] ? ((uint64_t)level_id << 16 | 0xFFFFu) : ((uint64_t)level_id << 16);
+        if (i < s.n && s.src[i] == SORT_SRC_FACET) val[i] = s.zones[((size_t)s.facet[i] * s.n_zone_blocks + b) * 2 + (s.desc[i] ? 1 : 0)];
+    }
+    return sort_pack_hi(s, val);
+}
+
+// one CTA per zone block: min / max of the block's column keys (or ranks) -> zone[2 * block]
+__global__ void __launch_bounds__(256) facet_zone_minmax(const uint64_t* __restrict__ col, uint64_t rows, uint32_t first_doc, uint32_t block0,
+                                                         const uint32_t* __restrict__ rank, uint32_t n_rank, uint64_t* __restrict__ zone) {
+    __shared__ uint64_t smin[8], smax[8];
+    const uint64_t d0 = (uint64_t)(block0 + blockIdx.x) << 16;
+    const uint64_t lo = d0 > first_doc ? d0 - first_doc : 0, hi = (d0 + 65536 - first_doc) < rows ? d0 + 65536 - first_doc : rows;
+    uint64_t mn = ~0ull, mx = 0;
+    for (uint64_t r = lo + threadIdx.x; r < hi; r += blockDim.x) {
+        uint64_t x = col[r];
+        if (rank) x = x < n_rank ? rank[x] : ~0ull;
+        mn = x < mn ? x : mn; mx = x > mx ? x : mx;
+    }
+    for (int s = 16; s; s >>= 1) {
+        const uint64_t a = shfl64_xor(mn, s), b = shfl64_xor(mx, s);
+        mn = a < mn ? a : mn; mx = b > mx ? b : mx;
+    }
+    if ((threadIdx.x & 31) == 0) { smin[threadIdx.x >> 5] = mn; smax[threadIdx.x >> 5] = mx; }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        for (int i = 1; i < 8; i++) { mn = smin[i] < mn ? smin[i] : mn; mx = smax[i] > mx ? smax[i] : mx; }
+        zone[2 * blockIdx.x] = mn; zone[2 * blockIdx.x + 1] = mx;
+    }
+}
+int32_t facet_zones(FacetSet& fs, uint32_t f, cudaStream_t st) {
+    if (!fs.n_facets || !fs.n_rows) return SSB_OK;
+    if (!fs.d_zones) {
+        fs.zone_block0 = fs.first_doc >> 16;
+        fs.n_zone_blocks = (uint32_t)(((uint64_t)fs.first_doc + fs.n_rows - 1) >> 16) - fs.zone_block0 + 1;
+        SSB_CUDA_TRY(cudaMalloc(&fs.d_zones, (size_t)fs.n_facets * fs.n_zone_blocks * 16));
+    }
+    facet_zone_minmax<<<fs.n_zone_blocks, 256, 0, st>>>(fs.d_keys + (size_t)f * fs.n_rows, fs.n_rows, fs.first_doc, fs.zone_block0, fs.d_rank[f], fs.n_rank[f],
+                                                        fs.d_zones + (size_t)f * fs.n_zone_blocks * 2);
+    SSB_CUDA_TRY(cudaGetLastError());
+    return SSB_OK;
+}
+
+int32_t LexIndex::prepare_sort(const ssb_sort_criterion* crit, uint32_t n, SortDev* out, bool* sorted) const {
+    if (n && !crit) { set_error("search_lexical_sorted: null criteria"); return SSB_E_INVALID; }
+    if (n > SSB_MAX_SORT_CRITERIA) { set_error("search_lexical_sorted: more than %u criteria", SSB_MAX_SORT_CRITERIA); return SSB_E_UNSUPPORTED; }
+    const uint32_t nf = facets_ ? facets_->n_facets : 0;
+    for (uint32_t i = 0; i < n; i++) {
+        if (crit[i].source > SSB_SORT_SCORE || crit[i].order > SSB_SORT_DESCENDING) { set_error("sort criterion %u: bad source / order", i); return SSB_E_INVALID; }
+        if (crit[i].source == SSB_SORT_FACET && nf && crit[i].facet >= nf) { set_error("sort criterion %u: facet %u of %u", i, crit[i].facet, nf); return SSB_E_INVALID; }
+    }
+    SortDev s{};
+    uint32_t bits = 0;
+    bool any_facet = false, ended = false;
+    for (uint32_t i = 0; i < n && !ended; i++) {                   // _id / _score end the comparison (min_heap.rs:580-604)
+        const ssb_sort_criterion& c = crit[i];
+        if (c.source == SSB_SORT_SCORE) { s.score_asc = c.order == SSB_SORT_ASCENDING; ended = true; continue; }
+        ended = c.source == SSB_SORT_ID;
+        const uint32_t j = s.n++;
+        s.src[j] = c.source == SSB_SORT_ID ? SORT_SRC_ID : SORT_SRC_FACET; s.desc[j] = c.order == SSB_SORT_DESCENDING;
+        if (s.src[j] == SORT_SRC_FACET) { s.facet[j] = c.facet; any_facet = true; }
+        s.type[j] = s.src[j] == SORT_SRC_FACET && nf ? facets_->types[c.facet] : 0u;
+        bits += sort_width(s.src[j], s.type[j]);
+    }
+    *sorted = s.n > 0 || s.score_asc;
+    if (!*sorted) return SSB_OK;
+    if (any_facet && !nf) { set_error("search_lexical_sorted: sorting by a facet needs ssb_set_facets"); return SSB_E_STATE; }
+    if (bits > 64) { set_error("search_lexical_sorted: the criteria take %u bits (at most 64)", bits); return SSB_E_UNSUPPORTED; }
+    if (any_facet) {
+        for (const LexLevel& l : levels_) {                           // a sorted doc must have a facet value
+            const uint64_t d0 = (uint64_t)l.level_id << 16;
+            if (l.n_docs && (d0 < facets_->first_doc || d0 + l.n_docs > (uint64_t)facets_->first_doc + facets_->n_rows)) {
+                set_error("search_lexical_sorted: the facet rows do not cover level %u", l.level_id); return SSB_E_STATE;
+            }
+        }
+        for (uint32_t j = 0; j < s.n; j++) {
+            if (s.src[j] != SORT_SRC_FACET) continue;
+            const uint32_t f = s.facet[j];
+            if (s.type[j] == SSB_FACET_STRING16 || s.type[j] == SSB_FACET_STRING32) {
+                if (!facets_->d_rank[f] || facets_->max_key[f] >= facets_->n_rank[f]) {
+                    set_error("search_lexical_sorted: String facet %u needs a value order covering its ids (ssb_set_facet_value_order)", f); return SSB_E_STATE;
+                }
+                s.rank[j] = facets_->d_rank[f];
+            }
+        }
+        s.zones = facets_->d_zones; s.zone_block0 = facets_->zone_block0; s.n_zone_blocks = facets_->n_zone_blocks;
+    }
+    *out = s;
+    return SSB_OK;
+}
+
 int32_t LexIndex::stage_filters(LexWorkspace& ws, cudaStream_t st, const ssb_lex_batch* q, LexView& v, bool* any) const {
     const uint32_t nq = q->n_queries;
     if (is_device_ptr(q->filter_offsets) || (q->filters && is_device_ptr(q->filters))) { set_error("search_lexical: filter arrays must be host arrays"); return SSB_E_INVALID; }
@@ -2007,7 +2286,7 @@ int32_t LexIndex::stage_filters(LexWorkspace& ws, cudaStream_t st, const ssb_lex
 }
 
 int32_t LexIndex::search_keys(LexWorkspace& ws, cudaStream_t st, const ssb_lex_batch* q, uint32_t k, uint32_t result_type,
-                              uint64_t* keys_out_dev, uint64_t* count_dev, uint64_t* launches, const uint64_t* ceil_dev) const {
+                              uint64_t* keys_out_dev, uint64_t* count_dev, uint64_t* launches, const uint64_t* ceil_dev, const SortDev* sort) const {
     if (!committed_) { set_error("search before ssb_lexical_commit"); return SSB_E_STATE; }
     if (!q || (q->n_queries && (!q->term_offsets || !keys_out_dev))) { set_error("search_lexical: null argument"); return SSB_E_INVALID; }
     if (k > SSB_K_MAX) { set_error("k=%u exceeds SSB_K_MAX=%u", k, SSB_K_MAX); return SSB_E_UNSUPPORTED; }
@@ -2059,17 +2338,45 @@ int32_t LexIndex::search_keys(LexWorkspace& ws, cudaStream_t st, const ssb_lex_b
     size_t plan_smem = (size_t)v.n_levels * (8 + 2 * FAST_T) + 16 + (size_t)n_pow2 * 8;
     // keys_out_dev doubles as the per-query global list (32 u64 per query); copy_out masks the entries >= k afterwards
     uint64_t* glist = keys_out_dev;
-    if (plan_smem > 48 * 1024) SSB_CUDA_TRY(cudaFuncSetAttribute(lex_plan, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan_smem));
     // item shape (tunable for experiments; defaults measured on C3): target postings per item, levels of a query's first item, levels per item
     static const uint32_t item_w = env_u32("SSB_LEX_ITEM_W", ITEM_W, 64, 1u << 20), first_lim = env_u32("SSB_LEX_FIRST", 2, 1, GMAX),
                           gmax = env_u32("SSB_LEX_GMAX", GMAX, 1, GMAX), grid_mult = env_u32("SSB_LEX_GRID", SSB_LEX_MINB, 1, 16);
-    lex_plan<<<nq, 128, plan_smem, st>>>(v, ws.qoff, ws.qkeys, q->term_flags ? ws.qflags : nullptr, filtered ? ws.foff : nullptr, fmask_dev, phrase | (result_type == SSB_RESULT_TOPK ? 2u : 0u), qt_eff, ws.plans, ws.recs, ws.item_start, ws.ctr, ws.theta, ws.lock, ws.count, glist, n_pow2,
-                                         item_w, first_lim, gmax);
-    SSB_CUDA_TRY(cudaGetLastError());
     const bool is_and = qt_eff == SSB_QUERY_INTERSECTION;
     const bool want_topk = result_type != SSB_RESULT_COUNT && k > 0;
     const bool need_count = result_type != SSB_RESULT_TOPK;
     const uint32_t kk = k ? k : 1;
+    if (sort) {
+        // sorted batch: every query takes lex_generic with 128-bit keys; keys_out_dev is its [nq][32][2] global list, left unmasked (callers
+        // read the first k entries), counted as usual
+        if (!ws.theta2) SSB_CUDA_TRY(cudaMalloc(&ws.theta2, (size_t)ws.cap_q * 16));
+        if (plan_smem > 48 * 1024) SSB_CUDA_TRY(cudaFuncSetAttribute(lex_plan<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan_smem));
+        lex_plan<true><<<nq, 128, plan_smem, st>>>(v, ws.qoff, ws.qkeys, q->term_flags ? ws.qflags : nullptr, filtered ? ws.foff : nullptr, fmask_dev, phrase | (result_type == SSB_RESULT_TOPK ? 2u : 0u), qt_eff, ws.plans, ws.recs, ws.item_start, ws.ctr, ws.theta2, ws.lock, ws.count, glist, n_pow2,
+                                                   item_w, first_lim, gmax, *sort);
+        SSB_CUDA_TRY(cudaGetLastError());
+        if (ws.ev0) cudaEventRecord(ws.ev0, st);
+        auto generic = (phrase && n_fields_ > 1) ? lex_generic<true, true> : lex_generic<false, true>;
+        generic<<<n_sms_ * 2, 256, 0, st>>>(v, ws.plans, ws.recs, ws.item_start, nq, qt_eff, result_type, kk, ws.ctr, ws.theta2, ws.lock, ws.count, glist, ws.stats, ceil_dev, *sort);
+        SSB_CUDA_TRY(cudaGetLastError());
+        if (need_count) {
+            lex_not_count<<<n_sms_ * 4, 256, 0, st>>>(v, ws.plans, nq, qt_eff, ws.ctr, ws.count);
+            SSB_CUDA_TRY(cudaGetLastError());
+            if (v.n_del) {
+                const uint64_t pairs = (uint64_t)nq * v.n_del;
+                lex_del_count<<<(unsigned)((pairs + 255) / 256), 256, 0, st>>>(v, ws.plans, nq, qt_eff, ws.count);
+                SSB_CUDA_TRY(cudaGetLastError());
+                if (launches) *launches += 1;
+            }
+            if (launches) *launches += 1;
+        }
+        if (ws.ev1) cudaEventRecord(ws.ev1, st);
+        if (count_dev) SSB_CUDA_TRY(cudaMemcpyAsync(count_dev, ws.count, (size_t)nq * 8, cudaMemcpyDeviceToDevice, st));
+        if (launches) *launches += 2;   // plan + generic
+        return SSB_OK;
+    }
+    if (plan_smem > 48 * 1024) SSB_CUDA_TRY(cudaFuncSetAttribute(lex_plan<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan_smem));
+    lex_plan<false><<<nq, 128, plan_smem, st>>>(v, ws.qoff, ws.qkeys, q->term_flags ? ws.qflags : nullptr, filtered ? ws.foff : nullptr, fmask_dev, phrase | (result_type == SSB_RESULT_TOPK ? 2u : 0u), qt_eff, ws.plans, ws.recs, ws.item_start, ws.ctr, ws.theta, ws.lock, ws.count, glist, n_pow2,
+                                                item_w, first_lim, gmax, SortDev{});
+    SSB_CUDA_TRY(cudaGetLastError());
     if (ws.ev0) cudaEventRecord(ws.ev0, st);
     if (want_topk) {
         const int grid = n_sms_ * (int)grid_mult;
@@ -2090,8 +2397,8 @@ int32_t LexIndex::search_keys(LexWorkspace& ws, cudaStream_t st, const ssb_lex_b
         if (launches) *launches += 1;
     }
     // queries with 5..16 live terms (the kernel returns at once when the batch has none)
-    auto generic = (phrase && n_fields_ > 1) ? lex_generic<true> : lex_generic<false>;
-    generic<<<n_sms_ * 2, 256, 0, st>>>(v, ws.plans, ws.recs, ws.item_start, nq, qt_eff, result_type, kk, ws.ctr, ws.theta, ws.lock, ws.count, glist, ws.stats, ceil_dev);
+    auto generic = (phrase && n_fields_ > 1) ? lex_generic<true, false> : lex_generic<false, false>;
+    generic<<<n_sms_ * 2, 256, 0, st>>>(v, ws.plans, ws.recs, ws.item_start, nq, qt_eff, result_type, kk, ws.ctr, ws.theta, ws.lock, ws.count, glist, ws.stats, ceil_dev, SortDev{});
     SSB_CUDA_TRY(cudaGetLastError());
     if (need_count) {     // returns at once unless some query of the batch carries NOT terms
         lex_not_count<<<n_sms_ * 4, 256, 0, st>>>(v, ws.plans, nq, qt_eff, ws.ctr, ws.count);

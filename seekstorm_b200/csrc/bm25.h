@@ -122,9 +122,30 @@ struct LexView {
 };
 
 // device-resident facet columns of an index (api.cu owns it, the lexical view borrows it)
+// zones: per facet and 65536-doc block of doc ids (block b = doc ids (zone_block0 + b) << 16 ..), the min and the max key of the block's rows
+// — the column key, or for a String facet with a value order the rank of the id; sorted searches bound a level's sort key with them.
+// rank / n_rank: the value order of a String facet (ssb_set_facet_value_order); max_key: the largest column key (host copy)
 struct FacetSet {
     uint64_t* d_keys = nullptr; uint64_t n_rows = 0; uint32_t first_doc = 0; uint32_t n_facets = 0; uint8_t types[16] = {0};
-    void release() { cudaFree(d_keys); d_keys = nullptr; n_rows = 0; n_facets = 0; }
+    uint64_t* d_zones = nullptr; uint32_t zone_block0 = 0, n_zone_blocks = 0;   // [n_facets][n_zone_blocks][2] {min, max}
+    uint32_t* d_rank[16] = {}; uint32_t n_rank[16] = {}; uint64_t max_key[16] = {};
+    void release() {
+        cudaFree(d_keys); d_keys = nullptr; n_rows = 0; n_facets = 0;
+        cudaFree(d_zones); d_zones = nullptr; n_zone_blocks = 0;
+        for (int f = 0; f < 16; f++) { cudaFree(d_rank[f]); d_rank[f] = nullptr; n_rank[f] = 0; }
+    }
+};
+// per-block min / max of facet f's column (through its value order when it has one) -> d_zones; asynchronous on st
+int32_t facet_zones(FacetSet& fs, uint32_t f, cudaStream_t st);
+
+// The sort of one sorted batch (ssb_search_lexical_sorted), validated and reduced by LexIndex::prepare_sort.  Criteria 0..n-1 are the
+// facet / _id criteria that make up the packed key `hi` (sort_pack_hi in bm25.cu); a `_score` criterion ends the list and only sets score_asc.
+enum { SORT_SRC_FACET = 0, SORT_SRC_ID = 1 };
+struct SortDev {
+    uint32_t n; uint32_t score_asc;                    // score_asc: `_score` ascending — the score half of the 128-bit top-k key is inverted
+    uint32_t src[4], facet[4], type[4], desc[4];      // per criterion (type: SSB_FACET_* of a facet criterion)
+    const uint32_t* rank[4];                           // String facets: rank_of_id (ssb_set_facet_value_order), else null
+    const uint64_t* zones; uint32_t zone_block0, n_zone_blocks;   // FacetSet zones (level bounds)
 };
 
 // device-resident delete set shared by the lexical and the vector path
@@ -171,6 +192,7 @@ struct LexWorkspace {
     uint64_t* theta = nullptr; int* lock = nullptr; uint64_t* count = nullptr; uint32_t* ctr = nullptr; /* [0] score / [2] count / [3] generic work counters, [1] max_items, [4] any query with > 4 live terms */
     uint32_t* qoff = nullptr; uint64_t* qkeys = nullptr; uint8_t* qflags = nullptr; LexStats* stats = nullptr;
     uint32_t* foff = nullptr; uint32_t* fmask = nullptr; FiltDev* filt = nullptr; uint64_t* fsets = nullptr; uint32_t cap_filt = 0, cap_fsets = 0;   // facet filters of the batch
+    uint64_t* theta2 = nullptr;   // sorted batches: [cap_q][2] 128-bit θ {hi, lo}
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;   // recorded around lex_score when set
     void release();
     ~LexWorkspace() { release(); }
@@ -192,8 +214,13 @@ public:
     // keys_out_dev: [n_queries][32]; count_dev: [n_queries] or null.  Asynchronous on `st`; thread-safe for concurrent
     // calls with distinct workspaces (the committed index is immutable).
     // ceil_dev: optional [n_queries] exclusive key ceilings (paging: only hits ranked after that key; 0 = none left)
+    // sort: a sorted batch (prepare_sort); keys_out_dev then holds [n_queries][32] 128-bit keys {hi, lo} (not masked: entries >= k may
+    // hold further candidates, callers read the first k) and ceil_dev [n_queries][2]
     int32_t search_keys(LexWorkspace& ws, cudaStream_t st, const ssb_lex_batch* q, uint32_t k, uint32_t result_type,
-                        uint64_t* keys_out_dev, uint64_t* count_dev, uint64_t* launches, const uint64_t* ceil_dev = nullptr) const;
+                        uint64_t* keys_out_dev, uint64_t* count_dev, uint64_t* launches, const uint64_t* ceil_dev = nullptr,
+                        const SortDev* sort = nullptr) const;
+    // validates ssb_search_lexical_sorted's criteria against the facets and the levels; *sorted = false: they reduce to "_score desc"
+    int32_t prepare_sort(const ssb_sort_criterion* crit, uint32_t n, SortDev* out, bool* sorted) const;
     bool committed() const { return committed_; }
     void set_stream(cudaStream_t st) { st_ = st; }   // load-time stream (add_level / commit)
     void set_deleted(const DeleteSet* d) { del_ = d; }

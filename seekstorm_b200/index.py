@@ -102,6 +102,22 @@ class FacetFilter:
     values: Optional[Sequence[int]] = None
 
 
+class SortOrder(enum.IntEnum):
+    """search.rs:885-890."""
+    Ascending = 0
+    Descending = 1
+
+
+@dataclass(frozen=True)
+class ResultSort:
+    """`ResultSort` (search.rs:893-901): sort the hits by a facet field (name given to set_facets), "_id" or "_score".  base: the
+    `FacetValue` of geo proximity sorting — only a Point facet reads it, and Point facets are not built: any base other than None
+    raises NotImplementedError."""
+    field: str
+    order: SortOrder = SortOrder.Descending
+    base: object = None
+
+
 @dataclass
 class Result:
     """min_heap.rs:17-40."""
@@ -279,10 +295,13 @@ class Index:
         a = np.ascontiguousarray(np.asarray(list(doc_ids), dtype=np.uint64))
         check(lib().ssb_set_deleted(self._h, a.ctypes.data if a.size else None, a.size))
 
-    def set_facets(self, columns: dict, first_doc_id: int = 0, string_facets: Sequence[str] = (), timestamp_facets: Sequence[str] = ()):
+    def set_facets(self, columns: dict, first_doc_id: int = 0, string_facets: Sequence[str] = (), timestamp_facets: Sequence[str] = (),
+                   string_values: Optional[dict] = None):
         """The shard's facet file (`facets_file_mmap`, add_result.rs:343-347): one typed value per doc and facet field.  columns: name ->
         numpy array [n_docs] (dtype = the facet's FieldType; names in string_facets are String16 / String32 value ids, names in
-        timestamp_facets Timestamp); rows are packed field after field like the reference's facet file and handed to ssb_set_facets."""
+        timestamp_facets Timestamp); rows are packed field after field like the reference's facet file and handed to ssb_set_facets.
+        string_values: name -> the String facet's value strings by id (`facet.values`); sorting by that facet orders by the strings
+        (result_ordering_shard, min_heap.rs:861-898), so their byte-wise order is sent along (ssb_set_facet_value_order)."""
         from ._lib import SsbFacetField
         kinds = {"uint8": _lib.FACET_U8, "uint16": _lib.FACET_U16, "uint32": _lib.FACET_U32, "uint64": _lib.FACET_U64, "int8": _lib.FACET_I8,
                  "int16": _lib.FACET_I16, "int32": _lib.FACET_I32, "int64": _lib.FACET_I64, "float32": _lib.FACET_F32, "float64": _lib.FACET_F64}
@@ -305,6 +324,32 @@ class Index:
             rows[:n, fields[i].offset:fields[i].offset + a.dtype.itemsize] = a.view(np.uint8).reshape(n, a.dtype.itemsize)
         self._facet_rows = (rows, fields, int(first_doc_id), n, off)      # also what the tests hand to the oracle
         check(lib().ssb_set_facets(self._h, rows.ctypes.data, int(first_doc_id), n, off, fields, len(names)))
+        for name, values in (string_values or {}).items():
+            t = self._facet_schema.get(name, (None, None))[1]
+            if t not in (_lib.FACET_STRING16, _lib.FACET_STRING32):
+                raise ValueError(f"string_values: {name!r} is not a String16 / String32 facet (facets: {list(self._facet_schema)})")
+            enc = [str(v).encode("utf-8") for v in values]
+            order = sorted(set(enc))                                        # Rust String order: byte-wise lexicographic
+            pos = {b: i for i, b in enumerate(order)}
+            rank = np.ascontiguousarray([pos[b] for b in enc], dtype=np.uint32)
+            check(lib().ssb_set_facet_value_order(self._h, self._facet_schema[name][0], rank.ctypes.data, rank.size))
+
+    def _sort_criteria(self, result_sort):
+        """ResultSort list -> ssb_sort_criterion array (ResultSortIndex, search.rs:2497-2525): "_id" / "_score", facet names resolved to
+        their index; unknown names are dropped like the reference does (facets_map.get, :2517)."""
+        from ._lib import SsbSortCriterion
+        out = []
+        for rs in result_sort:
+            if rs.base is not None:
+                raise NotImplementedError("geo proximity sorting (FacetValue::Point base) is not built")
+            order = _lib.SORT_DESCENDING if SortOrder(rs.order) == SortOrder.Descending else _lib.SORT_ASCENDING
+            if rs.field == "_id":
+                out.append(SsbSortCriterion(_lib.SORT_ID, 0, order, 0))
+            elif rs.field == "_score":
+                out.append(SsbSortCriterion(_lib.SORT_SCORE, 0, order, 0))
+            elif rs.field in getattr(self, "_facet_schema", {}):
+                out.append(SsbSortCriterion(_lib.SORT_FACET, self._facet_schema[rs.field][0], order, 0))
+        return (SsbSortCriterion * max(len(out), 1))(*out), len(out)
 
     def _encode_filters(self, filters):
         """filters: per query a list of FacetFilter -> (filter_offsets, ssb_facet_filter array, set values)"""
@@ -405,16 +450,21 @@ class Index:
         return b, tuple(keep)
 
     def search_lexical_batch(self, queries_keys, query_type: QueryType, k: int,
-                             result_type: ResultType = ResultType.TopkCount, not_keys=None, filters=None, field_masks=None):
+                             result_type: ResultType = ResultType.TopkCount, not_keys=None, filters=None, field_masks=None, sort=None):
         """Batched search_lexical_shard.  Returns (list of [(doc_id, score)...], counts ndarray).  not_keys: '-' terms per query;
-        filters: FacetFilter list per query (needs set_facets)."""
+        filters: FacetFilter list per query (needs set_facets); sort: ResultSort list for the whole batch (ssb_search_lexical_sorted)."""
         nq = len(queries_keys)
         b, keep = self._lex_batch(queries_keys, query_type, not_keys, filters, field_masks)
         hits = _hits_array(max(nq * max(k, 1), 1))
         n_hits = np.zeros(max(nq, 1), dtype=np.uint32)
         counts = np.zeros(max(nq, 1), dtype=np.uint64)
-        check(lib().ssb_search_lexical(self._h, C.byref(b), k, int(result_type), hits.ctypes.data, n_hits.ctypes.data,
-                                       counts.ctypes.data))
+        if sort is not None:
+            crit, n_crit = self._sort_criteria(sort)
+            check(lib().ssb_search_lexical_sorted(self._h, C.byref(b), C.addressof(crit), n_crit, k, int(result_type), hits.ctypes.data,
+                                                  n_hits.ctypes.data, counts.ctypes.data))
+        else:
+            check(lib().ssb_search_lexical(self._h, C.byref(b), k, int(result_type), hits.ctypes.data, n_hits.ctypes.data,
+                                           counts.ctypes.data))
         out = []
         for i in range(nq):
             h = hits[i * k: i * k + int(n_hits[i])]
@@ -538,10 +588,16 @@ class Index:
 
         facet_filter: FacetFilter objects (range / value-set filters on the facet fields given to set_facets) — applied to the lexical
         search like the reference does (the vector search takes no facet filter, vector.rs:1105-1115).
-        Unsupported reference features (facet counting, field filters, sort, uncommitted, rewriting, phrase) raise
+        result_sort: ResultSort objects — lexical search only (the hits in sort order, ssb_search_lexical_sorted).
+        Unsupported reference features (facet counting, sorting vector / hybrid results or by geo distance, uncommitted, rewriting) raise
         NotImplementedError rather than being silently ignored."""
-        if query_facets or result_sort or include_uncommitted:
-            raise NotImplementedError("facet counts / sort / uncommitted search are outside the GPU hot path")
+        if query_facets or include_uncommitted:
+            raise NotImplementedError("facet counts / uncommitted search are outside the GPU hot path")
+        search_mode = search_mode or SearchMode.Lexical()
+        if result_sort and search_mode.kind != "Lexical":
+            raise NotImplementedError("result_sort on vector / hybrid search is not built")
+        if result_sort:
+            self._sort_criteria(result_sort)                     # a FacetValue::Point base raises before any search runs
         # field_filter: names of indexed fields (self.field_names, in schema order) or their indices -> one bitmask
         fmask = 0
         for f in field_filter:
@@ -549,7 +605,6 @@ class Index:
             if isinstance(f, str) and f not in names:
                 raise ValueError(f"field_filter: unknown indexed field {f!r} (indexed fields: {names})")
             fmask |= 1 << (names.index(f) if isinstance(f, str) else int(f))
-        search_mode = search_mode or SearchMode.Lexical()
         ro = ResultObject(original_query=query_string, query=query_string)
         heap = offset + length                       # search.rs:1708 per-shard length = offset+length
         # tokenizer stand-in: whitespace, '+' = mandatory (tokenizer.rs:546-563); unique terms (search.rs:3023-3039)
@@ -586,7 +641,8 @@ class Index:
             rt = ResultType.Count
         if want_lex:
             res, counts = self.search_lexical_batch([keys], qt, heap if rt != ResultType.Count else 0, rt, [nkeys] if nkeys else None,
-                                                    [list(facet_filter)] if facet_filter else None, [fmask] if fmask else None)
+                                                    [list(facet_filter)] if facet_filter else None, [fmask] if fmask else None,
+                                                    list(result_sort) if result_sort else None)
             lex, total = res[0], int(counts[0])
         if want_vec:
             qv = np.asarray(query_vector, dtype=np.float32).reshape(1, -1)
