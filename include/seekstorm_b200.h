@@ -134,22 +134,39 @@ typedef struct {
 } ssb_level_desc;
 
 /* ---- facets and facet filters (SURVEY.md §8f row 4) ---------------------------------------------------- */
-/* FieldType of a facet field (index.rs `FieldType`; FilterSparse search.rs:863-881).  Point (geo) filters are not built. */
+/* FieldType of a facet field (index.rs `FieldType`; FilterSparse search.rs:863-881).  POINT (geo, index.rs:5803-5819): the row holds
+ * the u64 Morton code encode_morton_2_d([lat, lon]) (geo_search.rs:27-42): x = ((lat * 1e7) as i32) as u32 in the even bits, y = the
+ * same of lon in the odd bits, Rust's saturating `as i32` (NaN -> 0).  The reference writes no code for a coordinate outside
+ * [-90, 90] x [-180, 180]: that row stays 0, which decodes to (0.0, 0.0).  Decode: (x as i32) as f64 / 1e7 (geo_search.rs:58-79). */
 enum { SSB_FACET_U8 = 0, SSB_FACET_U16 = 1, SSB_FACET_U32 = 2, SSB_FACET_U64 = 3, SSB_FACET_I8 = 4, SSB_FACET_I16 = 5,
        SSB_FACET_I32 = 6, SSB_FACET_I64 = 7, SSB_FACET_TIMESTAMP = 8, SSB_FACET_F32 = 9, SSB_FACET_F64 = 10,
-       SSB_FACET_STRING16 = 11, SSB_FACET_STRING32 = 12 };
+       SSB_FACET_STRING16 = 11, SSB_FACET_STRING32 = 12, SSB_FACET_POINT = 13 };
+/* DistanceUnit (index.rs) of a POINT filter */
+enum { SSB_UNIT_KILOMETERS = 0, SSB_UNIT_MILES = 1 };
 /* one facet field of the shard's facet file: its type and its byte offset inside a doc's row (`facet.offset`, add_result.rs:345) */
 typedef struct { uint32_t type; uint32_t offset; } ssb_facet_field;
 /* One filter of one query.  RANGE = Rust `Range<T>::contains`: start <= value < end, compared in the facet's own type (floats by
  * PartialOrd: NaN is never inside).  start / end carry the bound widened to 8 bytes: unsigned types as u64, signed types and
  * Timestamp as i64 (two's complement), F32 / F64 as the bits of the f64 value.  SET (String16 / String32) = `values.contains(id)`
- * over filter_set_values[set_first .. set_first + set_count).  A facet without a filter entry is FilterSparse::None. */
-enum { SSB_FILTER_RANGE = 0, SSB_FILTER_SET = 1 };
+ * over filter_set_values[set_first .. set_first + set_count).  A facet without a filter entry is FilterSparse::None.
+ * POINT (POINT facets only; FacetFilter::Point {field, (base, start..end, unit)} -> FilterSparse::Point, search.rs:2712-2723,
+ * add_result.rs:462-478): start / end are the distance range as f64 bits; set_count = 3 values at filter_set_values[set_first ..]: the
+ * base's lat and lon as f64 bits, then the unit (SSB_UNIT_*).  A doc passes when morton_min <= code < morton_max, the interval of
+ * point_distance_to_morton_range(base, end, unit) (geo_search.rs:109-144, computed by the host), AND start <= euclidian_distance(base,
+ * decode(code), unit) < end: the equirectangular R * sqrt(x*x + y*y), R = 6371.0087714 km or 3958.761315801475 mi.  The reference's
+ * quirks are kept: the interval is a Z-order range of u32-cast signed coordinates, so a box that crosses latitude 0 or longitude 0
+ * usually has min > max and no doc passes; near the poles the longitude delta explodes and the encode saturates; a NaN in the base or
+ * the bounds rejects every doc.
+ * Precision: the integer decode, /1e7, + - * and sqrt are IEEE round-to-nearest in the reference's operation order without FMA
+ * contraction, bit for bit; the Morton interval is computed on the host with the C library's cos.  The device evaluates the distance's
+ * cos with CUDA's double cos (within 2 ulp, not guaranteed equal to the host libm): a filter decision can differ from the reference only
+ * for a distance within a few ulp of a bound. */
+enum { SSB_FILTER_RANGE = 0, SSB_FILTER_SET = 1, SSB_FILTER_POINT = 2 };
 typedef struct ssb_facet_filter {
     uint32_t facet;                   /* index into the fields given to ssb_set_facets                    */
     uint32_t kind;                    /* SSB_FILTER_*                                                     */
     uint64_t start, end;              /* RANGE bounds (see above)                                         */
-    uint32_t set_first, set_count;    /* SET: slice of ssb_lex_batch.filter_set_values                    */
+    uint32_t set_first, set_count;    /* SET / POINT: slice of ssb_lex_batch.filter_set_values            */
 } ssb_facet_filter;
 #define SSB_MAX_FACETS 16u
 #define SSB_MAX_FILTERS_PER_QUERY 16u
@@ -172,7 +189,8 @@ typedef struct {
     /* every filter of its query accepts its facet value (is_facet_filter, add_result.rs:340-478).  Needs ssb_set_facets.          */
     const uint32_t* filter_offsets;           /* [n_queries+1] or NULL (no query is filtered)                                      */
     const struct ssb_facet_filter* filters;   /* [filter_offsets[n_queries]]                                                       */
-    const uint64_t* filter_set_values;        /* value ids of the SSB_FILTER_SET filters (String16 / String32), or NULL            */
+    const uint64_t* filter_set_values;        /* value ids of the SSB_FILTER_SET filters (String16 / String32), the payloads of    */
+                                              /* the SSB_FILTER_POINT filters, or NULL                                              */
     /* field filter (`field_filter: Vec<String>` -> field_filter_set, add_result.rs:3124-3137, 3558-3571): HOST array [n_queries] or   */
     /* NULL; bit f = indexed field f is in the query's filter, 0 = no field filter.  A doc is dropped when a query term it contains    */
     /* occurs in none of the filter's fields (tested like the reference only when term fields + filter fields <= indexed fields);      */
@@ -287,6 +305,17 @@ typedef struct { uint32_t source, facet, order, pad; } ssb_sort_criterion;   /* 
 #define SSB_MAX_SORT_CRITERIA 4u
 int32_t ssb_search_lexical_sorted(ssb_index* ix, const ssb_lex_batch* q, const ssb_sort_criterion* sort, uint32_t n_sort,
                                   uint32_t k, uint32_t result_type, ssb_hit* hits, uint32_t* n_hits, uint64_t* count_total);
+/* The same with the bases of a POINT criterion (ResultSort on a Point facet with a FacetValue::Point base, min_heap.rs:510-529,
+ * 1017-1037): bases is a HOST array [n_queries][2] (lat, lon), one base per query.  The criterion compares simplified_distance(decode(code),
+ * base) = ((base.lon - p.lon) * cos(DEG2RAD * (p.lat + base.lat) / 2))^2 + (base.lat - p.lat)^2 in degrees (geo_search.rs:82-107):
+ * ascending = nearest first.  A NaN distance orders like a NaN F64 value.  bases = NULL: a POINT criterion has no base and is dropped, as
+ * the reference skips it; the bases are ignored by every other criterion.  A POINT criterion takes 64 bits, so only `_score` may follow it
+ * (else SSB_E_UNSUPPORTED).  Precision: as for SSB_FILTER_POINT, every operation but cos is IEEE bit-exact; with CUDA's cos two docs at
+ * DIFFERENT coordinates whose distances lie within a few ulp may order differently from the host libm; equal coordinates always tie.
+ * ssb_search_lexical_sorted is this call with bases = NULL. */
+int32_t ssb_search_lexical_sorted_ex(ssb_index* ix, const ssb_lex_batch* q, const ssb_sort_criterion* sort, uint32_t n_sort,
+                                     const double* bases, uint32_t k, uint32_t result_type, ssb_hit* hits, uint32_t* n_hits,
+                                     uint64_t* count_total);
 /* queries: [n_queries, dims] f32; Cosine: normalised by the callee (search.rs:1464-1475).  score = dot
  * (Dot/Cosine) or -Σ(q-x)² (Euclidean) exactly as Result.score in vector.rs:1489. */
 int32_t ssb_search_vector(ssb_index* ix, const float* queries, uint32_t n_queries, uint32_t k,

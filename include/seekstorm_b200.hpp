@@ -76,25 +76,34 @@ inline uint64_t fnv1a64(const std::string& term) {
 
 // `FacetFilter` (search.rs:735-860) resolved against the schema: facet = index of the facet field (order of set_facets), a Rust
 // `Range<T>` as start <= value < end with the bounds widened to 8 bytes (u64 / i64 two's complement / f64 bits — see ssb_facet_filter),
-// or the value ids of a String16 / String32 filter
+// or the value ids of a String16 / String32 filter, or a geo distance range on a Point facet (`FacetFilter::Point`: base (lat, lon),
+// start <= distance < end in unit — SSB_FILTER_POINT)
 struct FacetFilter {
     uint32_t facet = 0;
     uint64_t start = 0, end = 0;
     std::vector<uint64_t> values;
+    bool point = false; double lat = 0.0, lon = 0.0; uint32_t unit = SSB_UNIT_KILOMETERS;
     static FacetFilter range_u(uint32_t facet, uint64_t a, uint64_t b) { FacetFilter f; f.facet = facet; f.start = a; f.end = b; return f; }
     static FacetFilter range_i(uint32_t facet, int64_t a, int64_t b) { return range_u(facet, static_cast<uint64_t>(a), static_cast<uint64_t>(b)); }
     static FacetFilter range_f(uint32_t facet, double a, double b) { uint64_t x, y; std::memcpy(&x, &a, 8); std::memcpy(&y, &b, 8); return range_u(facet, x, y); }
     static FacetFilter set(uint32_t facet, std::vector<uint64_t> ids) { FacetFilter f; f.facet = facet; f.values = std::move(ids); return f; }
+    static FacetFilter geo(uint32_t facet, double lat, double lon, double start, double end, uint32_t unit = SSB_UNIT_KILOMETERS) {
+        FacetFilter f = range_f(facet, start, end); f.point = true; f.lat = lat; f.lon = lon; f.unit = unit; return f;
+    }
 };
 
 // `ResultSort` (search.rs:893-901) resolved against the schema (ResultSortIndex, search.rs:2497-2525): a facet field (index in the order
-// of set_facets; a String16 / String32 facet needs set_facet_value_order), the doc id ("_id") or the score ("_score").  Geo proximity
-// sorting (a FacetValue::Point base) is not built.
+// of set_facets; a String16 / String32 facet needs set_facet_value_order), the doc id ("_id") or the score ("_score").  A Point facet
+// sorts by the distance to its base (FacetValue::Point: has_base, lat, lon; ascending = nearest first); without a base it is skipped.
 enum class SortOrder : uint32_t { Ascending = SSB_SORT_ASCENDING, Descending = SSB_SORT_DESCENDING };   // search.rs:885-890
 struct ResultSort {
     uint32_t source = SSB_SORT_FACET, facet = 0;
     SortOrder order = SortOrder::Descending;
+    bool has_base = false; double lat = 0.0, lon = 0.0;
     static ResultSort facet_field(uint32_t facet, SortOrder o) { ResultSort r; r.facet = facet; r.order = o; return r; }
+    static ResultSort geo(uint32_t facet, SortOrder o, double lat, double lon) {
+        ResultSort r = facet_field(facet, o); r.has_base = true; r.lat = lat; r.lon = lon; return r;
+    }
     static ResultSort id(SortOrder o) { ResultSort r; r.source = SSB_SORT_ID; r.order = o; return r; }
     static ResultSort score(SortOrder o) { ResultSort r; r.source = SSB_SORT_SCORE; r.order = o; return r; }
 };
@@ -214,9 +223,16 @@ public:
             uint32_t foffs[2] = {0, static_cast<uint32_t>(facet_filter.size())};
             for (auto& f : facet_filter) {
                 ssb_facet_filter c{};
-                c.facet = f.facet; c.kind = f.values.empty() ? SSB_FILTER_RANGE : SSB_FILTER_SET; c.start = f.start; c.end = f.end;
-                c.set_first = static_cast<uint32_t>(set_values.size()); c.set_count = static_cast<uint32_t>(f.values.size());
-                set_values.insert(set_values.end(), f.values.begin(), f.values.end());
+                c.facet = f.facet; c.kind = f.point ? SSB_FILTER_POINT : f.values.empty() ? SSB_FILTER_RANGE : SSB_FILTER_SET; c.start = f.start; c.end = f.end;
+                c.set_first = static_cast<uint32_t>(set_values.size());
+                if (f.point) {                // payload: base lat / lon as f64 bits, the unit
+                    uint64_t la, lo; std::memcpy(&la, &f.lat, 8); std::memcpy(&lo, &f.lon, 8);
+                    set_values.insert(set_values.end(), {la, lo, static_cast<uint64_t>(f.unit)});
+                    c.set_count = 3;
+                } else {
+                    c.set_count = static_cast<uint32_t>(f.values.size());
+                    set_values.insert(set_values.end(), f.values.begin(), f.values.end());
+                }
                 ff.push_back(c);
             }
             if (!ff.empty()) { b.filter_offsets = foffs; b.filters = ff.data(); b.filter_set_values = set_values.data(); }
@@ -225,9 +241,14 @@ public:
             lex.resize(k ? k : 1);
             uint32_t n = 0;
             std::vector<ssb_sort_criterion> sc;
-            for (auto& r : result_sort) sc.push_back(ssb_sort_criterion{r.source, r.facet, static_cast<uint32_t>(r.order), 0});
+            double base[2] = {0.0, 0.0}; bool has_base = false;   // the Point criterion's FacetValue::Point base (one query: one base)
+            for (auto& r : result_sort) {
+                sc.push_back(ssb_sort_criterion{r.source, r.facet, static_cast<uint32_t>(r.order), 0});
+                if (r.has_base && !has_base) { base[0] = r.lat; base[1] = r.lon; has_base = true; }
+            }
             if (sc.empty()) check(ssb_search_lexical(h_, &b, k, static_cast<uint32_t>(rt), lex.data(), &n, &total));
-            else check(ssb_search_lexical_sorted(h_, &b, sc.data(), static_cast<uint32_t>(sc.size()), k, static_cast<uint32_t>(rt), lex.data(), &n, &total));
+            else check(ssb_search_lexical_sorted_ex(h_, &b, sc.data(), static_cast<uint32_t>(sc.size()), has_base ? base : nullptr, k,
+                                                    static_cast<uint32_t>(rt), lex.data(), &n, &total));
             lex.resize(n);
         }
         if (want_vec) {

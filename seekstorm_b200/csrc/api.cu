@@ -892,7 +892,7 @@ int32_t ssb_set_facets(ssb_index* ix, const void* rows, uint64_t first_doc_id, u
     if (first_doc_id + n_docs > (1ull << 32)) { set_error("ssb_set_facets: doc ids must be < 2^32"); return SSB_E_INVALID; }
     for (uint32_t f = 0; f < n_fields; f++) {
         const uint32_t w = facet_type_bytes(fields[f].type);
-        if (!w) { set_error("ssb_set_facets: field %u has unsupported type %u (Point facets are not built)", f, fields[f].type); return SSB_E_UNSUPPORTED; }
+        if (!w) { set_error("ssb_set_facets: field %u has unsupported type %u", f, fields[f].type); return SSB_E_UNSUPPORTED; }
         if ((uint64_t)fields[f].offset + w > row_bytes) { set_error("ssb_set_facets: field %u does not fit a %u-byte row", f, row_bytes); return SSB_E_INVALID; }
     }
     std::vector<uint64_t> keys((size_t)n_fields * n_docs);
@@ -1075,6 +1075,12 @@ int32_t ssb_search_lexical(ssb_index* ix, const ssb_lex_batch* q, uint32_t k, ui
 
 int32_t ssb_search_lexical_sorted(ssb_index* ix, const ssb_lex_batch* q, const ssb_sort_criterion* sort, uint32_t n_sort, uint32_t k, uint32_t result_type,
                                   ssb_hit* hits, uint32_t* n_hits, uint64_t* count_total) {
+    return ssb_search_lexical_sorted_ex(ix, q, sort, n_sort, nullptr, k, result_type, hits, n_hits, count_total);
+}
+
+// bases: per-query (lat, lon) of a Point criterion (ResultSort.base = FacetValue::Point); NULL drops that criterion
+int32_t ssb_search_lexical_sorted_ex(ssb_index* ix, const ssb_lex_batch* q, const ssb_sort_criterion* sort, uint32_t n_sort, const double* bases,
+                                     uint32_t k, uint32_t result_type, ssb_hit* hits, uint32_t* n_hits, uint64_t* count_total) {
     SSB_API_BEGIN
     // ResultType::Count ignores the sort (search.rs:2498); k = 0 is Count (search.rs:2472-2478)
     if (result_type == SSB_RESULT_COUNT || k == 0) return ssb_search_lexical(ix, q, k, result_type, hits, n_hits, count_total);
@@ -1082,12 +1088,13 @@ int32_t ssb_search_lexical_sorted(ssb_index* ix, const ssb_lex_batch* q, const s
     std::shared_lock<std::shared_mutex> g(ix->rw);
     SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
     SortDev sd{}; bool sorted = false;
-    SSB_TRY(ix->lex->prepare_sort(sort, n_sort, &sd, &sorted));
+    SSB_TRY(ix->lex->prepare_sort(sort, n_sort, bases != nullptr, &sd, &sorted));
     if (sorted && ix->comm.active()) { set_error("ssb_search_lexical_sorted: sorted search across shards is not built"); return SSB_E_UNSUPPORTED; }
     if (q->n_queries == 0) return SSB_OK;
     if (k > SSB_K_LIMIT) { set_error("k=%u exceeds SSB_K_LIMIT=%u", k, SSB_K_LIMIT); return SSB_E_UNSUPPORTED; }
     CtxLease l(ix); SSB_TRY(l.acquire());
     if (!sorted) return search_lexical_host<1>(ix, *l.c, q, k, result_type, hits, n_hits, count_total, nullptr);   // "_score desc" = the default order
+    SSB_TRY(LexIndex::stage_sort_bases(l.c->lex, l.c->st, bases, q->n_queries, &sd));
     return search_lexical_host<2>(ix, *l.c, q, k, result_type, hits, n_hits, count_total, &sd);
     SSB_API_END
 }

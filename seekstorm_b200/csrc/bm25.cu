@@ -587,6 +587,53 @@ __device__ __forceinline__ bool in_not_lists(const LexView& v, const QueryPlan* 
 // order-preserving 64-bit keys ssb_set_facets stored per doc and facet (bounds converted the same way by the host), so one unsigned
 // compare pair covers every FilterSparse range type.  Out of line, by value, on the rare candidate / count path of lex_generic only.
 struct FacetArgs { const uint64_t* keys; uint64_t rows; const FiltDev* filt; const uint64_t* sets; uint32_t first_doc; };
+
+// ---- geo (Point facets, geo_search.rs): Morton decode and the two distances, every f64 operation individually rounded in the reference's
+// order (Rust does not contract into FMA); cos is CUDA's double cos (documented within 2 ulp of the exact value, not bit-equal to glibc's)
+#define SSB_DEG2RAD 0.017453292519943295
+// decode_morton_64_bit (geo_search.rs:44-52): the even bits of code, compacted
+__device__ __forceinline__ uint32_t morton_even_bits(uint64_t code) {
+    uint64_t x = code & 0x5555555555555555ull;
+    x = (x ^ (x >> 1)) & 0x3333333333333333ull;
+    x = (x ^ (x >> 2)) & 0x0F0F0F0F0F0F0F0Full;
+    x = (x ^ (x >> 4)) & 0x00FF00FF00FF00FFull;
+    x = (x ^ (x >> 8)) & 0x0000FFFF0000FFFFull;
+    x = (x ^ (x >> 16)) & 0x00000000FFFFFFFFull;
+    return (uint32_t)x;
+}
+// decode_morton_2_d (geo_search.rs:58-79): (x_u32 as i32) as f64 / 1e7 — lat from the even bits, lon from the odd bits
+__device__ __forceinline__ double morton_lat(uint64_t code) { return __ddiv_rn((double)(int32_t)morton_even_bits(code), 10000000.0); }
+__device__ __forceinline__ double morton_lon(uint64_t code) { return __ddiv_rn((double)(int32_t)morton_even_bits(code >> 1), 10000000.0); }
+// FilterSparse::Point (add_result.rs:462-478): true = the doc is filtered OUT.  range.contains(code) on the Morton interval staged in
+// [lo, hi), then distance_range.contains(euclidian_distance(base, decode(code), unit)) (geo_search.rs:95-107).  g: the staged payload
+// (GEO_* words, f64 bits).  Out of line: only POINT filters reach it.
+__device__ __noinline__ bool geo_rejects_impl(uint64_t code, uint64_t lo, uint64_t hi, const uint64_t* g) {
+    if (!(code >= lo && code < hi)) return true;
+    const double blat = __longlong_as_double((long long)__ldg(&g[GEO_LAT])), blon = __longlong_as_double((long long)__ldg(&g[GEO_LON]));
+    const double plat = morton_lat(code), plon = morton_lon(code);
+    const double c = cos(__ddiv_rn(__dmul_rn(SSB_DEG2RAD, __dadd_rn(blat, plat)), 2.0));
+    const double x = __dmul_rn(__dmul_rn(SSB_DEG2RAD, __dsub_rn(plon, blon)), c);
+    const double y = __dmul_rn(SSB_DEG2RAD, __dsub_rn(plat, blat));
+    const double d = __dmul_rn(__longlong_as_double((long long)__ldg(&g[GEO_RADIUS])), __dsqrt_rn(__dadd_rn(__dmul_rn(x, x), __dmul_rn(y, y))));
+    const double start = __longlong_as_double((long long)__ldg(&g[GEO_START])), end = __longlong_as_double((long long)__ldg(&g[GEO_END]));
+    return !(start <= d && d < end);
+}
+// the sort key of a POINT criterion (morton_ordering, geo_search.rs:82-93): the order key of simplified_distance(decode(code), base) — the
+// F64 column key (key_of_f64: NaN = all ones, above +inf).  base: the query's (lat, lon).  Out of line: only POINT criteria reach it.
+__device__ __noinline__ uint64_t point_sort_key(uint64_t code, const double* base) {
+    const double blat = __ldg(&base[0]), blon = __ldg(&base[1]);
+    const double plat = morton_lat(code), plon = morton_lon(code);
+    const double x = __dmul_rn(__dsub_rn(blon, plon), cos(__ddiv_rn(__dmul_rn(SSB_DEG2RAD, __dadd_rn(plat, blat)), 2.0)));
+    const double y = __dsub_rn(blat, plat);
+    double d = __dadd_rn(__dmul_rn(x, x), __dmul_rn(y, y));
+    if (d != d) return ~0ull;
+    if (d == 0.0) d = 0.0;                                               // -0.0 == +0.0
+    const uint64_t b = (uint64_t)__double_as_longlong(d);
+    return (b >> 63) ? ~b : (b | 0x8000000000000000ull);
+}
+
+// GEO: the batch holds a POINT filter — its own instantiation, so that the common one keeps its code and its callers their registers
+template <bool GEO>
 __device__ __noinline__ bool facet_rejects_impl(FacetArgs a, uint32_t f0, uint32_t nf, uint32_t doc) {
     const uint64_t row = (uint64_t)doc - a.first_doc;
     if (doc < a.first_doc || row >= a.rows) return true;             // no facet row for this doc
@@ -598,12 +645,14 @@ __device__ __noinline__ bool facet_rejects_impl(FacetArgs a, uint32_t f0, uint32
             bool in = false;
             for (uint32_t s = 0; s < f.set_n; s++) in = in || __ldg(&a.sets[f.set_first + s]) == key;
             if (!in) return true;
-        } else return true;
+        } else if (GEO && f.kind == FILT_POINT) { if (geo_rejects_impl(key, f.lo, f.hi, a.sets + f.set_first)) return true; }
+        else return true;
     }
     return false;
 }
+template <bool GEO = false>
 __device__ __forceinline__ bool facet_rejects(const LexView& v, uint32_t f0, uint32_t nf, uint32_t doc) {
-    return facet_rejects_impl(FacetArgs{v.facet_keys, v.facet_rows, v.filt, v.filt_sets, v.facet_first_doc}, f0, nf, doc);
+    return facet_rejects_impl<GEO>(FacetArgs{v.facet_keys, v.facet_rows, v.filt, v.filt_sets, v.facet_first_doc}, f0, nf, doc);
 }
 
 // field_filter (`field_filter_set`, add_result.rs:3124-3137, 3558-3571): every query term the doc contains must occur in at least one
@@ -693,9 +742,9 @@ __device__ __noinline__ bool phrase_rejects_fields_impl(ListView v, PhraseArgs a
 // facet filters, the field filter and the phrase check of one query on one doc: true = filtered OUT.  FIELD_RUNS: the index has several
 // fields and a phrase batch is running (positions in per-field runs) — its own instantiation of lex_generic, so that the single-field kernel
 // keeps its code and register allocation
-template <bool FIELD_RUNS>
+template <bool FIELD_RUNS, bool GEO>
 __device__ __forceinline__ bool filters_reject(const LexView& v, const QueryPlan* pl, uint32_t f0, uint32_t nf, uint32_t field_mask, uint32_t n_live, uint32_t lv, uint32_t d, uint32_t doc) {
-    if (nf && facet_rejects(v, f0, nf, doc)) return true;
+    if (nf && facet_rejects<GEO>(v, f0, nf, doc)) return true;
     if (field_mask && field_rejects_impl(list_view(v), v.payf, v.n_fields, pl, n_live, lv, d, field_mask)) return true;
     if (!FIELD_RUNS && pl->n_phr && phrase_rejects_impl(list_view(v), PhraseArgs{v.pay, v.positions, v.pos_off, v.lvl_pos_base}, pl, n_live, lv, d)) return true;
     if (FIELD_RUNS && pl->n_phr && phrase_rejects_fields_impl(list_view(v), PhraseArgs{v.payf, v.positions, v.pos_off, v.lvl_pos_base}, pl, n_live, lv, d,
@@ -741,9 +790,11 @@ __device__ __forceinline__ void wl_merge128(uint64_t& Ah, uint64_t& Al, uint64_t
 }
 // the warp's list of one sorted item; thr = a lower bound of θ.hi (global θ.hi, or the local list's k-th hi once it is full)
 struct SortTop { uint64_t h, l, thr; };
-// doc's packed sort key: the facet column keys of its row (a String facet's id through its value order), or its id
+// doc's packed sort key for query q: the facet column keys of its row (a String facet's id through its value order, a Point facet's code
+// through its distance to the query's base), or its id
 __device__ __forceinline__ uint64_t sort_pack_hi(const SortDev& s, const uint64_t* v);
-__device__ __forceinline__ uint64_t doc_sort_hi(const LexView& v, const SortDev& s, uint32_t doc) {
+template <bool GEO>
+__device__ __forceinline__ uint64_t doc_sort_hi(const LexView& v, const SortDev& s, uint32_t doc, uint32_t q) {
     const uint64_t row = (uint64_t)(doc - v.facet_first_doc);          // prepare_sort: the facet rows cover every doc of the levels
     uint64_t val[SSB_MAX_SORT_CRITERIA];
 #pragma unroll
@@ -752,6 +803,7 @@ __device__ __forceinline__ uint64_t doc_sort_hi(const LexView& v, const SortDev&
         if (i < s.n && s.src[i] == SORT_SRC_FACET) {
             val[i] = __ldg(&v.facet_keys[(size_t)s.facet[i] * v.facet_rows + row]);
             if (s.rank[i]) val[i] = __ldg(&s.rank[i][val[i]]);          // prepare_sort: every id of the column has a rank
+            else if (GEO && s.type[i] == SSB_FACET_POINT) val[i] = point_sort_key(val[i], s.bases + 2 * (size_t)q);
         }
     }
     return sort_pack_hi(s, val);
@@ -1255,7 +1307,7 @@ __device__ __forceinline__ void score_records(const LexView& v, WarpSm& w, uint3
 // SORTED: the top-k key is (sort key, score, doc) in T (L / thr unused).  θ is not a score there, so none of the score bounds prunes
 // (MAXSCORE driver break, score test of the insert); a candidate whose sort key is below T.thr is dropped before its score loads and,
 // on the OR path, before its probes (AND, Topk: before its probes as well — nothing is counted).
-template <bool FIELD_RUNS, bool SORTED = false>
+template <bool FIELD_RUNS, bool SORTED, bool GEO>
 __device__ __forceinline__ void process_item_generic(const LexView& v, const QueryPlan* pl, const ItemCtx& c, int lane,
                                                   uint64_t& L, uint32_t& thr, bool& dirty, uint32_t& matches_out,
                                                   uint32_t& st_visited, uint32_t& st_probes, SortTop& T, const SortDev& sd) {
@@ -1288,7 +1340,7 @@ __device__ __forceinline__ void process_item_generic(const LexView& v, const Que
             bool ok = active; float score = 0.f;
             uint64_t hi = 0; bool keep = true;
             if constexpr (SORTED) {
-                if (active && c.scoring) hi = doc_sort_hi(v, sd, c.docbase | d);
+                if (active && c.scoring) hi = doc_sort_hi<GEO>(v, sd, c.docbase | d, c.q);
                 keep = c.scoring && !(hi < T.thr);
                 ok = active && (keep || c.need_count);
             }
@@ -1302,7 +1354,7 @@ __device__ __forceinline__ void process_item_generic(const LexView& v, const Que
             }
             if (c.n_filt) {
                 // a filtered query is counted here doc by doc: filter, delete set and NOT lists at once (the correction kernels skip it)
-                ok = ok && !filters_reject<FIELD_RUNS>(v, pl, c.filt_first, c.n_facet_filt, c.field_mask, c.n, c.lv, d, c.docbase | d) && !is_deleted(v, c.docbase | d) && !(c.n_not && in_not_lists(v, pl, c.n_not, c.lv, d));
+                ok = ok && !filters_reject<FIELD_RUNS, GEO>(v, pl, c.filt_first, c.n_facet_filt, c.field_mask, c.n, c.lv, d, c.docbase | d) && !is_deleted(v, c.docbase | d) && !(c.n_not && in_not_lists(v, pl, c.n_not, c.lv, d));
                 matches += __popc(__ballot_sync(FULL, ok));
                 if constexpr (SORTED) { if (c.scoring) insert_sorted(T, ok && keep, hi, score, c.docbase | d, sd.score_asc, c.k, lane, dirty, c.ceil, c.ceil_lo); }
                 else
@@ -1348,7 +1400,7 @@ __device__ __forceinline__ void process_item_generic(const LexView& v, const Que
                 bool dup = false; float score = 0.f;
                 uint64_t hi = 0; bool live = active;
                 if constexpr (SORTED) {
-                    if (active) hi = doc_sort_hi(v, sd, c.docbase | d);
+                    if (active) hi = doc_sort_hi<GEO>(v, sd, c.docbase | d, c.q);
                     live = active && !(hi < T.thr);
                 }
                 for (uint32_t t = 0; t < n; t++) {      // query order
@@ -1365,11 +1417,11 @@ __device__ __forceinline__ void process_item_generic(const LexView& v, const Que
                 }
                 if constexpr (SORTED) {
                     insert_sorted(T, live && !dup && !is_deleted(v, c.docbase | d) && !(c.n_not && in_not_lists(v, pl, c.n_not, c.lv, d))
-                                     && !(c.n_filt && filters_reject<FIELD_RUNS>(v, pl, c.filt_first, c.n_facet_filt, c.field_mask, c.n, c.lv, d, c.docbase | d)),
+                                     && !(c.n_filt && filters_reject<FIELD_RUNS, GEO>(v, pl, c.filt_first, c.n_facet_filt, c.field_mask, c.n, c.lv, d, c.docbase | d)),
                                   hi, score, c.docbase | d, sd.score_asc, c.k, lane, dirty, c.ceil, c.ceil_lo);
                 } else
                 insert_candidates(L, thr, active && !dup && ord_f32(score) >= thr && !is_deleted(v, c.docbase | d) && !(c.n_not && in_not_lists(v, pl, c.n_not, c.lv, d))
-                                              && !(c.n_filt && filters_reject<FIELD_RUNS>(v, pl, c.filt_first, c.n_facet_filt, c.field_mask, c.n, c.lv, d, c.docbase | d)), score, c.docbase | d, c.k, lane, dirty, c.ceil);
+                                              && !(c.n_filt && filters_reject<FIELD_RUNS, GEO>(v, pl, c.filt_first, c.n_facet_filt, c.field_mask, c.n, c.lv, d, c.docbase | d)), score, c.docbase | d, c.k, lane, dirty, c.ceil);
             }
         }
     }
@@ -1401,7 +1453,7 @@ __device__ __forceinline__ void process_item_generic(const LexView& v, const Que
                 }
                 bool cnt_ok = active && !dup;
                 if (c.n_filt && cnt_ok)      // filtered query: every match is tested here (filter, delete set, NOT lists; the correction kernels skip it)
-                    cnt_ok = !filters_reject<FIELD_RUNS>(v, pl, c.filt_first, c.n_facet_filt, c.field_mask, c.n, c.lv, d, c.docbase | d) && !is_deleted(v, c.docbase | d) && !(c.n_not && in_not_lists(v, pl, c.n_not, c.lv, d));
+                    cnt_ok = !filters_reject<FIELD_RUNS, GEO>(v, pl, c.filt_first, c.n_facet_filt, c.field_mask, c.n, c.lv, d, c.docbase | d) && !is_deleted(v, c.docbase | d) && !(c.n_not && in_not_lists(v, pl, c.n_not, c.lv, d));
                 matches += __popc(__ballot_sync(FULL, cnt_ok));
             }
         }
@@ -1554,7 +1606,8 @@ __global__ void __launch_bounds__(128, 6) lex_count(LexView v, const QueryPlan* 
 // FIELD_RUNS: phrase batch on an index with several fields (the phrase check walks per-field position runs)
 // SORTED: a sorted batch (every query is here; theta / glist / ceil_keys hold 128-bit keys).  The score bound of a level means nothing
 // there; under Topk a level is skipped when its sort-key bound is below θ.hi (strictly: ties in hi go through the exact insert).
-template <bool FIELD_RUNS, bool SORTED>
+// GEO: the batch has a POINT filter or sorts by a POINT criterion (geo_rejects_impl / point_sort_key in the call graph)
+template <bool FIELD_RUNS, bool SORTED, bool GEO = false>
 __global__ void __launch_bounds__(256) lex_generic(LexView v, const QueryPlan* __restrict__ plans, const LvRec* __restrict__ recs,
                                                   const uint16_t* __restrict__ item_start, uint32_t nq, uint32_t query_type, uint32_t result_type,
                                                   uint32_t k, uint32_t* ctr, uint64_t* theta, int* lock, uint64_t* count, uint64_t* glist,
@@ -1590,7 +1643,7 @@ __global__ void __launch_bounds__(256) lex_generic(LexView v, const QueryPlan* _
                 c.need_count = need_count; c.is_and = query_type == SSB_QUERY_INTERSECTION; c.docbase = w.recs[ri].docbase;
                 if (!c.scoring && !need_count) { st_skipped++; continue; }
                 st_done++;
-                process_item_generic<FIELD_RUNS, true>(v, pl, c, lane, L, thr, dirty, matches, st_visited, st_probes, T, sort);
+                process_item_generic<FIELD_RUNS, true, GEO>(v, pl, c, lane, L, thr, dirty, matches, st_visited, st_probes, T, sort);
             }
             if (dirty) publish_sorted(T, q, k, lane, theta, lock, glist);
             if (need_count && lane == 0 && matches) atomicAdd((unsigned long long*)&count[q], (unsigned long long)matches);
@@ -1611,7 +1664,7 @@ __global__ void __launch_bounds__(256) lex_generic(LexView v, const QueryPlan* _
             c.need_count = need_count; c.is_and = query_type == SSB_QUERY_INTERSECTION; c.docbase = w.recs[ri].docbase;
             if (!c.scoring && !need_count) { st_skipped++; continue; }
             st_done++;
-            process_item_generic<FIELD_RUNS>(v, pl, c, lane, L, thr, dirty, matches, st_visited, st_probes, T, sort);
+            process_item_generic<FIELD_RUNS, false, GEO>(v, pl, c, lane, L, thr, dirty, matches, st_visited, st_probes, T, sort);
         }
         if (dirty) publish(L, q, k, lane, theta, lock, glist);
         if (need_count && lane == 0 && matches) atomicAdd((unsigned long long*)&count[q], (unsigned long long)matches);
@@ -2080,7 +2133,7 @@ uint64_t facet_value_key(uint32_t type, const uint8_t* p) {
         case SSB_FACET_U8: return p[0];
         case SSB_FACET_U16: case SSB_FACET_STRING16: { uint16_t x; memcpy(&x, p, 2); return x; }
         case SSB_FACET_U32: case SSB_FACET_STRING32: { uint32_t x; memcpy(&x, p, 4); return x; }
-        case SSB_FACET_U64: { uint64_t x; memcpy(&x, p, 8); return x; }
+        case SSB_FACET_U64: case SSB_FACET_POINT: { uint64_t x; memcpy(&x, p, 8); return x; }   // Point: the Morton code itself
         case SSB_FACET_I8: { int8_t x; memcpy(&x, p, 1); return (uint64_t)(int64_t)x ^ 0x8000000000000000ull; }
         case SSB_FACET_I16: { int16_t x; memcpy(&x, p, 2); return (uint64_t)(int64_t)x ^ 0x8000000000000000ull; }
         case SSB_FACET_I32: { int32_t x; memcpy(&x, p, 4); return (uint64_t)(int64_t)x ^ 0x8000000000000000ull; }
@@ -2095,10 +2148,32 @@ uint32_t facet_type_bytes(uint32_t type) {
         case SSB_FACET_U8: case SSB_FACET_I8: return 1;
         case SSB_FACET_U16: case SSB_FACET_I16: case SSB_FACET_STRING16: return 2;
         case SSB_FACET_U32: case SSB_FACET_I32: case SSB_FACET_F32: case SSB_FACET_STRING32: return 4;
-        case SSB_FACET_U64: case SSB_FACET_I64: case SSB_FACET_TIMESTAMP: case SSB_FACET_F64: return 8;
+        case SSB_FACET_U64: case SSB_FACET_I64: case SSB_FACET_TIMESTAMP: case SSB_FACET_F64: case SSB_FACET_POINT: return 8;
     }
     return 0;
 }
+
+// ---- geo on the host: encode_morton_2_d and point_distance_to_morton_range (geo_search.rs:27-42, 109-144) for the filter interval.  The
+// host code is compiled without FMA contraction (-ffp-contract=off); the expressions hold no multiply-add anyway.
+static inline int32_t rust_as_i32(double v) {                      // Rust `f64 as i32`: truncation, saturating, NaN -> 0
+    if (v != v) return 0;
+    if (v >= 2147483648.0) return INT32_MAX;
+    if (v <= -2147483648.0) return INT32_MIN;
+    return (int32_t)v;
+}
+static inline uint64_t morton_spread(uint32_t v) {                  // encode_morton_64_bit (geo_search.rs:11-20)
+    uint64_t x = v;
+    x = (x | (x << 16)) & 0x0000FFFF0000FFFFull;
+    x = (x | (x << 8)) & 0x00FF00FF00FF00FFull;
+    x = (x | (x << 4)) & 0x0F0F0F0F0F0F0F0Full;
+    x = (x | (x << 2)) & 0x3333333333333333ull;
+    x = (x | (x << 1)) & 0x5555555555555555ull;
+    return x;
+}
+static inline uint64_t encode_morton_2d(double lat, double lon) {
+    return morton_spread((uint32_t)rust_as_i32(lat * 10000000.0)) | (morton_spread((uint32_t)rust_as_i32(lon * 10000000.0)) << 1);
+}
+static inline double earth_radius(uint64_t unit) { return unit == SSB_UNIT_MILES ? 3958.761315801475 : 6371.0087714; }
 
 // ---- sort keys (ssb_search_lexical_sorted; result_ordering_shard, min_heap.rs:574-1051) ----
 // The packed sort key `hi` — the one place that knows its layout.  v[i] is criterion i's value: the facet's column key (facet_value_key;
@@ -2142,14 +2217,16 @@ __device__ __forceinline__ uint64_t sort_pack_hi(const SortDev& s, const uint64_
     return hi;
 }
 // upper bound of hi over the docs of a level: per criterion the level's largest value (descending) or smallest (ascending, inverted by
-// the packing) — the block's zone for a facet, level << 16 | 0xFFFF or level << 16 for _id
+// the packing) — the block's zone for a facet, level << 16 | 0xFFFF or level << 16 for _id.  A Point criterion takes the trivial bound
+// (the largest key after packing): its zones hold Morton codes, not distances, and no level is skipped.
 __device__ __forceinline__ uint64_t level_sort_bound(const SortDev& s, uint32_t level_id) {
     uint64_t val[SSB_MAX_SORT_CRITERIA];
     const uint32_t b = level_id - s.zone_block0;                       // prepare_sort: the zones cover every level
 #pragma unroll
     for (uint32_t i = 0; i < SSB_MAX_SORT_CRITERIA; i++) {
         val[i] = s.desc[i] ? ((uint64_t)level_id << 16 | 0xFFFFu) : ((uint64_t)level_id << 16);
-        if (i < s.n && s.src[i] == SORT_SRC_FACET) val[i] = s.zones[((size_t)s.facet[i] * s.n_zone_blocks + b) * 2 + (s.desc[i] ? 1 : 0)];
+        if (i < s.n && s.src[i] == SORT_SRC_FACET)
+            val[i] = s.type[i] == SSB_FACET_POINT ? (s.desc[i] ? ~0ull : 0ull) : s.zones[((size_t)s.facet[i] * s.n_zone_blocks + b) * 2 + (s.desc[i] ? 1 : 0)];
     }
     return sort_pack_hi(s, val);
 }
@@ -2190,7 +2267,7 @@ int32_t facet_zones(FacetSet& fs, uint32_t f, cudaStream_t st) {
     return SSB_OK;
 }
 
-int32_t LexIndex::prepare_sort(const ssb_sort_criterion* crit, uint32_t n, SortDev* out, bool* sorted) const {
+int32_t LexIndex::prepare_sort(const ssb_sort_criterion* crit, uint32_t n, bool has_bases, SortDev* out, bool* sorted) const {
     if (n && !crit) { set_error("search_lexical_sorted: null criteria"); return SSB_E_INVALID; }
     if (n > SSB_MAX_SORT_CRITERIA) { set_error("search_lexical_sorted: more than %u criteria", SSB_MAX_SORT_CRITERIA); return SSB_E_UNSUPPORTED; }
     const uint32_t nf = facets_ ? facets_->n_facets : 0;
@@ -2204,6 +2281,8 @@ int32_t LexIndex::prepare_sort(const ssb_sort_criterion* crit, uint32_t n, SortD
     for (uint32_t i = 0; i < n && !ended; i++) {                   // _id / _score end the comparison (min_heap.rs:580-604)
         const ssb_sort_criterion& c = crit[i];
         if (c.source == SSB_SORT_SCORE) { s.score_asc = c.order == SSB_SORT_ASCENDING; ended = true; continue; }
+        // a Point facet without a FacetValue::Point base is skipped (min_heap.rs:510-529: `if let FacetValue::Point(base)`)
+        if (c.source == SSB_SORT_FACET && nf && facets_->types[c.facet] == SSB_FACET_POINT && !has_bases) continue;
         ended = c.source == SSB_SORT_ID;
         const uint32_t j = s.n++;
         s.src[j] = c.source == SSB_SORT_ID ? SORT_SRC_ID : SORT_SRC_FACET; s.desc[j] = c.order == SSB_SORT_DESCENDING;
@@ -2238,15 +2317,30 @@ int32_t LexIndex::prepare_sort(const ssb_sort_criterion* crit, uint32_t n, SortD
     return SSB_OK;
 }
 
-int32_t LexIndex::stage_filters(LexWorkspace& ws, cudaStream_t st, const ssb_lex_batch* q, LexView& v, bool* any) const {
+int32_t LexIndex::stage_sort_bases(LexWorkspace& ws, cudaStream_t st, const double* bases, uint32_t nq, SortDev* sort) {
+    bool point = false;
+    for (uint32_t j = 0; j < sort->n; j++) point = point || (sort->src[j] == SORT_SRC_FACET && sort->type[j] == SSB_FACET_POINT);
+    if (!point || nq == 0) return SSB_OK;
+    if (is_device_ptr(bases)) { set_error("search_lexical_sorted: bases must be a host array"); return SSB_E_INVALID; }
+    if (nq > ws.cap_bases) {
+        cudaFree(ws.bases); ws.bases = nullptr; ws.cap_bases = 0;
+        SSB_CUDA_TRY(cudaMalloc(&ws.bases, (size_t)nq * 16)); ws.cap_bases = nq;
+    }
+    SSB_CUDA_TRY(cudaMemcpyAsync(ws.bases, bases, (size_t)nq * 16, cudaMemcpyHostToDevice, st));
+    sort->bases = ws.bases;
+    return SSB_OK;
+}
+
+int32_t LexIndex::stage_filters(LexWorkspace& ws, cudaStream_t st, const ssb_lex_batch* q, LexView& v, bool* any, bool* geo_any) const {
     const uint32_t nq = q->n_queries;
-    if (is_device_ptr(q->filter_offsets) || (q->filters && is_device_ptr(q->filters))) { set_error("search_lexical: filter arrays must be host arrays"); return SSB_E_INVALID; }
+    if (is_device_ptr(q->filter_offsets) || (q->filters && is_device_ptr(q->filters)) || (q->filter_set_values && is_device_ptr(q->filter_set_values))) { set_error("search_lexical: filter arrays must be host arrays"); return SSB_E_INVALID; }
     const uint32_t nf = q->filter_offsets[nq];
-    *any = false;
+    *any = false; *geo_any = false;
     if (nf == 0) return SSB_OK;
     if (!q->filters) { set_error("search_lexical: null filters"); return SSB_E_INVALID; }
     if (!facets_ || !facets_->n_facets) { set_error("search_lexical: facet filters need ssb_set_facets"); return SSB_E_STATE; }
     std::vector<FiltDev> fd(nf);
+    std::vector<uint64_t> geo;                                       // POINT payloads (GEO_WORDS each), staged behind the SET values
     uint32_t n_sets = 0;
     for (uint32_t i = 0; i < nq; i++) {
         if (q->filter_offsets[i + 1] < q->filter_offsets[i] || q->filter_offsets[i + 1] > nf) { set_error("query %u: filter_offsets must ascend", i); return SSB_E_INVALID; }
@@ -2257,7 +2351,26 @@ int32_t LexIndex::stage_filters(LexWorkspace& ws, cudaStream_t st, const ssb_lex
         if (f.facet >= facets_->n_facets) { set_error("facet filter %u: facet %u of %u", i, f.facet, facets_->n_facets); return SSB_E_INVALID; }
         const uint32_t type = facets_->types[f.facet];
         FiltDev d{}; d.facet = f.facet;
-        if (f.kind == SSB_FILTER_RANGE) {
+        if ((f.kind == SSB_FILTER_POINT) != (type == SSB_FACET_POINT)) { set_error("facet filter %u: a Point facet takes SSB_FILTER_POINT and only it", i); return SSB_E_INVALID; }
+        if (f.kind == SSB_FILTER_POINT) {
+            // FilterSparse::Point(base, start..end, unit, point_distance_to_morton_range(base, end, unit)) (search.rs:2712-2723)
+            if (f.set_count != 3) { set_error("facet filter %u: SSB_FILTER_POINT takes 3 filter_set_values (lat, lon, unit), not %u", i, f.set_count); return SSB_E_INVALID; }
+            if (!q->filter_set_values) { set_error("facet filter %u: null filter_set_values", i); return SSB_E_INVALID; }
+            const uint64_t* p = q->filter_set_values + f.set_first;
+            if (p[2] > SSB_UNIT_MILES) { set_error("facet filter %u: bad distance unit %llu", i, (unsigned long long)p[2]); return SSB_E_INVALID; }
+            double lat, lon, start, end; memcpy(&lat, &p[0], 8); memcpy(&lon, &p[1], 8); memcpy(&start, &f.start, 8); memcpy(&end, &f.end, 8);
+            const double r = earth_radius(p[2]);
+            const double lat_delta = end / (SSB_DEG2RAD * r);
+            const double lon_delta = end / (SSB_DEG2RAD * r * cos(SSB_DEG2RAD * lat));
+            d.lo = encode_morton_2d(lat - lat_delta, lon - lon_delta);
+            d.hi = encode_morton_2d(lat + lat_delta, lon + lon_delta);
+            // an empty interval (a box across latitude / longitude 0, a NaN anywhere) or a NaN start: no doc passes
+            d.kind = d.lo < d.hi && start == start ? FILT_POINT : FILT_NEVER;
+            *geo_any = *geo_any || d.kind == FILT_POINT;
+            d.set_first = (uint32_t)geo.size();                     // relative to the payloads; rebased behind the SET values below
+            uint64_t rb; memcpy(&rb, &r, 8);
+            for (uint64_t w : {p[0], p[1], f.start, f.end, rb}) geo.push_back(w);
+        } else if (f.kind == SSB_FILTER_RANGE) {
             if (type == SSB_FACET_STRING16 || type == SSB_FACET_STRING32) { set_error("facet filter %u: a String facet takes SSB_FILTER_SET", i); return SSB_E_INVALID; }
             d.kind = FILT_RANGE;
             if (facet_is_float(type)) {
@@ -2273,13 +2386,16 @@ int32_t LexIndex::stage_filters(LexWorkspace& ws, cudaStream_t st, const ssb_lex
         } else { set_error("facet filter %u: bad kind %u", i, f.kind); return SSB_E_INVALID; }
         fd[i] = d;
     }
+    for (uint32_t i = 0; i < nf; i++) if (q->filters[i].kind == SSB_FILTER_POINT) fd[i].set_first += n_sets;
+    const uint32_t n_staged = n_sets + (uint32_t)geo.size();
     if (!ws.foff) SSB_CUDA_TRY(cudaMalloc(&ws.foff, ((size_t)ws.cap_q + 1) * 4));
     if (nf > ws.cap_filt) { cudaFree(ws.filt); ws.filt = nullptr; ws.cap_filt = 0; const uint32_t c = nf + nf / 2 + 64; SSB_CUDA_TRY(cudaMalloc(&ws.filt, (size_t)c * sizeof(FiltDev))); ws.cap_filt = c; }
-    if (n_sets > ws.cap_fsets) { cudaFree(ws.fsets); ws.fsets = nullptr; ws.cap_fsets = 0; const uint32_t c = n_sets + n_sets / 2 + 64; SSB_CUDA_TRY(cudaMalloc(&ws.fsets, (size_t)c * 8)); ws.cap_fsets = c; }
+    if (n_staged > ws.cap_fsets) { cudaFree(ws.fsets); ws.fsets = nullptr; ws.cap_fsets = 0; const uint32_t c = n_staged + n_staged / 2 + 64; SSB_CUDA_TRY(cudaMalloc(&ws.fsets, (size_t)c * 8)); ws.cap_fsets = c; }
     // pageable host sources: cudaMemcpyAsync returns after staging them, the vectors may go out of scope
     SSB_CUDA_TRY(cudaMemcpyAsync(ws.foff, q->filter_offsets, ((size_t)nq + 1) * 4, cudaMemcpyHostToDevice, st));
     SSB_CUDA_TRY(cudaMemcpyAsync(ws.filt, fd.data(), (size_t)nf * sizeof(FiltDev), cudaMemcpyHostToDevice, st));
     if (n_sets) SSB_CUDA_TRY(cudaMemcpyAsync(ws.fsets, q->filter_set_values, (size_t)n_sets * 8, cudaMemcpyHostToDevice, st));
+    if (!geo.empty()) SSB_CUDA_TRY(cudaMemcpyAsync(ws.fsets + n_sets, geo.data(), geo.size() * 8, cudaMemcpyHostToDevice, st));
     v.filt = ws.filt; v.filt_sets = ws.fsets;
     *any = true;
     return SSB_OK;
@@ -2321,8 +2437,12 @@ int32_t LexIndex::search_keys(LexWorkspace& ws, cudaStream_t st, const ssb_lex_b
     SSB_CUDA_TRY(to_device(ws.qkeys, q->term_keys, (size_t)total_terms * 8, st));
     if (q->term_flags) SSB_CUDA_TRY(to_device(ws.qflags, q->term_flags, (size_t)total_terms, st));
     LexView v = view();
-    bool filtered = false;
-    if (q->filter_offsets) SSB_TRY(stage_filters(ws, st, q, v, &filtered));
+    bool filtered = false, geo = false;
+    if (q->filter_offsets) SSB_TRY(stage_filters(ws, st, q, v, &filtered, &geo));
+    for (uint32_t j = 0; sort && j < sort->n; j++) geo = geo || (sort->src[j] == SORT_SRC_FACET && sort->type[j] == SSB_FACET_POINT);
+    // a batch with a POINT filter plans without flag bit 1: EVERY filtered query of that batch (its range / set filters too) leaves the
+    // lex_score record path for lex_generic<.., GEO>, so that lex_score keeps its code and registers; unfiltered queries stay on it
+    const uint32_t topk_flag = result_type == SSB_RESULT_TOPK && !geo ? 2u : 0u;
     const uint32_t* fmask_dev = nullptr;
     if (q->field_masks && n_fields_ > 1) {                   // field_filter: one bitmask of indexed fields per query (host array)
         if (is_device_ptr(q->field_masks)) { set_error("search_lexical: field_masks must be a host array"); return SSB_E_INVALID; }
@@ -2350,11 +2470,12 @@ int32_t LexIndex::search_keys(LexWorkspace& ws, cudaStream_t st, const ssb_lex_b
         // read the first k entries), counted as usual
         if (!ws.theta2) SSB_CUDA_TRY(cudaMalloc(&ws.theta2, (size_t)ws.cap_q * 16));
         if (plan_smem > 48 * 1024) SSB_CUDA_TRY(cudaFuncSetAttribute(lex_plan<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan_smem));
-        lex_plan<true><<<nq, 128, plan_smem, st>>>(v, ws.qoff, ws.qkeys, q->term_flags ? ws.qflags : nullptr, filtered ? ws.foff : nullptr, fmask_dev, phrase | (result_type == SSB_RESULT_TOPK ? 2u : 0u), qt_eff, ws.plans, ws.recs, ws.item_start, ws.ctr, ws.theta2, ws.lock, ws.count, glist, n_pow2,
+        lex_plan<true><<<nq, 128, plan_smem, st>>>(v, ws.qoff, ws.qkeys, q->term_flags ? ws.qflags : nullptr, filtered ? ws.foff : nullptr, fmask_dev, phrase | topk_flag, qt_eff, ws.plans, ws.recs, ws.item_start, ws.ctr, ws.theta2, ws.lock, ws.count, glist, n_pow2,
                                                    item_w, first_lim, gmax, *sort);
         SSB_CUDA_TRY(cudaGetLastError());
         if (ws.ev0) cudaEventRecord(ws.ev0, st);
-        auto generic = (phrase && n_fields_ > 1) ? lex_generic<true, true> : lex_generic<false, true>;
+        auto generic = (phrase && n_fields_ > 1) ? (geo ? lex_generic<true, true, true> : lex_generic<true, true>)
+                                                 : (geo ? lex_generic<false, true, true> : lex_generic<false, true>);
         generic<<<n_sms_ * 2, 256, 0, st>>>(v, ws.plans, ws.recs, ws.item_start, nq, qt_eff, result_type, kk, ws.ctr, ws.theta2, ws.lock, ws.count, glist, ws.stats, ceil_dev, *sort);
         SSB_CUDA_TRY(cudaGetLastError());
         if (need_count) {
@@ -2374,7 +2495,7 @@ int32_t LexIndex::search_keys(LexWorkspace& ws, cudaStream_t st, const ssb_lex_b
         return SSB_OK;
     }
     if (plan_smem > 48 * 1024) SSB_CUDA_TRY(cudaFuncSetAttribute(lex_plan<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan_smem));
-    lex_plan<false><<<nq, 128, plan_smem, st>>>(v, ws.qoff, ws.qkeys, q->term_flags ? ws.qflags : nullptr, filtered ? ws.foff : nullptr, fmask_dev, phrase | (result_type == SSB_RESULT_TOPK ? 2u : 0u), qt_eff, ws.plans, ws.recs, ws.item_start, ws.ctr, ws.theta, ws.lock, ws.count, glist, n_pow2,
+    lex_plan<false><<<nq, 128, plan_smem, st>>>(v, ws.qoff, ws.qkeys, q->term_flags ? ws.qflags : nullptr, filtered ? ws.foff : nullptr, fmask_dev, phrase | topk_flag, qt_eff, ws.plans, ws.recs, ws.item_start, ws.ctr, ws.theta, ws.lock, ws.count, glist, n_pow2,
                                                 item_w, first_lim, gmax, SortDev{});
     SSB_CUDA_TRY(cudaGetLastError());
     if (ws.ev0) cudaEventRecord(ws.ev0, st);
@@ -2397,7 +2518,8 @@ int32_t LexIndex::search_keys(LexWorkspace& ws, cudaStream_t st, const ssb_lex_b
         if (launches) *launches += 1;
     }
     // queries with 5..16 live terms (the kernel returns at once when the batch has none)
-    auto generic = (phrase && n_fields_ > 1) ? lex_generic<true, false> : lex_generic<false, false>;
+    auto generic = (phrase && n_fields_ > 1) ? (geo ? lex_generic<true, false, true> : lex_generic<true, false>)
+                                             : (geo ? lex_generic<false, false, true> : lex_generic<false, false>);
     generic<<<n_sms_ * 2, 256, 0, st>>>(v, ws.plans, ws.recs, ws.item_start, nq, qt_eff, result_type, kk, ws.ctr, ws.theta, ws.lock, ws.count, glist, ws.stats, ceil_dev, SortDev{});
     SSB_CUDA_TRY(cudaGetLastError());
     if (need_count) {     // returns at once unless some query of the batch carries NOT terms

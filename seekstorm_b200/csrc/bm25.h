@@ -69,8 +69,11 @@ struct BmSec { uint64_t w[2]; uint32_t meta[2]; uint32_t pad[2]; };
 static_assert(sizeof(BmSec) == 32, "BmSec must be one 32-byte sector");
 
 // One facet filter of one query, bounds already in key space (FilterSparse, search.rs:863-881): RANGE lo <= key < hi;
-// SET key in filt_sets[set_first .. +set_n); NEVER rejects every doc (a NaN bound: Range::contains is false for every value)
-enum { FILT_RANGE = 0, FILT_SET = 1, FILT_NEVER = 2 };
+// SET key in filt_sets[set_first .. +set_n); NEVER rejects every doc (a NaN bound: Range::contains is false for every value);
+// POINT: lo <= Morton code < hi, then the distance test with the staged geo payload filt_sets[set_first .. +GEO_WORDS)
+enum { FILT_RANGE = 0, FILT_SET = 1, FILT_NEVER = 2, FILT_POINT = 3 };
+// payload of a POINT filter in filt_sets, as f64 bits: base lat, base lon, distance start, distance end, earth radius of the unit
+enum { GEO_LAT = 0, GEO_LON = 1, GEO_START = 2, GEO_END = 3, GEO_RADIUS = 4, GEO_WORDS = 5 };
 struct FiltDev { uint32_t facet, kind; uint64_t lo, hi; uint32_t set_first, set_n; };
 
 // device view handed to the kernels (all pointers device)
@@ -146,6 +149,7 @@ struct SortDev {
     uint32_t src[4], facet[4], type[4], desc[4];      // per criterion (type: SSB_FACET_* of a facet criterion)
     const uint32_t* rank[4];                           // String facets: rank_of_id (ssb_set_facet_value_order), else null
     const uint64_t* zones; uint32_t zone_block0, n_zone_blocks;   // FacetSet zones (level bounds)
+    const double* bases;                               // a POINT criterion: [n_queries][2] per-query base (lat, lon), staged by stage_sort_bases
 };
 
 // device-resident delete set shared by the lexical and the vector path
@@ -193,9 +197,12 @@ struct LexWorkspace {
     uint32_t* qoff = nullptr; uint64_t* qkeys = nullptr; uint8_t* qflags = nullptr; LexStats* stats = nullptr;
     uint32_t* foff = nullptr; uint32_t* fmask = nullptr; FiltDev* filt = nullptr; uint64_t* fsets = nullptr; uint32_t cap_filt = 0, cap_fsets = 0;   // facet filters of the batch
     uint64_t* theta2 = nullptr;   // sorted batches: [cap_q][2] 128-bit θ {hi, lo}
+    // sorted batches with a POINT criterion: [n_queries][2] bases, staged before search_keys — kept across release(), which
+    // ensure_workspace calls when the batch outgrows the workspace
+    double* bases = nullptr; uint32_t cap_bases = 0;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;   // recorded around lex_score when set
     void release();
-    ~LexWorkspace() { release(); }
+    ~LexWorkspace() { release(); cudaFree(bases); }
     LexWorkspace() = default;
     LexWorkspace(const LexWorkspace&) = delete;
     LexWorkspace& operator=(const LexWorkspace&) = delete;
@@ -219,8 +226,11 @@ public:
     int32_t search_keys(LexWorkspace& ws, cudaStream_t st, const ssb_lex_batch* q, uint32_t k, uint32_t result_type,
                         uint64_t* keys_out_dev, uint64_t* count_dev, uint64_t* launches, const uint64_t* ceil_dev = nullptr,
                         const SortDev* sort = nullptr) const;
-    // validates ssb_search_lexical_sorted's criteria against the facets and the levels; *sorted = false: they reduce to "_score desc"
-    int32_t prepare_sort(const ssb_sort_criterion* crit, uint32_t n, SortDev* out, bool* sorted) const;
+    // validates ssb_search_lexical_sorted's criteria against the facets and the levels; *sorted = false: they reduce to "_score desc".
+    // has_bases: the call carries POINT bases (else a POINT criterion is dropped)
+    int32_t prepare_sort(const ssb_sort_criterion* crit, uint32_t n, bool has_bases, SortDev* out, bool* sorted) const;
+    // a sort with a POINT criterion: copy the host bases [nq][2] into the workspace and point sort->bases at them
+    static int32_t stage_sort_bases(LexWorkspace& ws, cudaStream_t st, const double* bases, uint32_t nq, SortDev* sort);
     bool committed() const { return committed_; }
     void set_stream(cudaStream_t st) { st_ = st; }   // load-time stream (add_level / commit)
     void set_deleted(const DeleteSet* d) { del_ = d; }
@@ -233,7 +243,7 @@ public:
 
 private:
     int32_t ensure_workspace(LexWorkspace& ws, uint32_t nq, uint32_t total_terms) const;
-    int32_t stage_filters(LexWorkspace& ws, cudaStream_t st, const ssb_lex_batch* q, LexView& v, bool* any) const;
+    int32_t stage_filters(LexWorkspace& ws, cudaStream_t st, const ssb_lex_batch* q, LexView& v, bool* any, bool* geo_any) const;
     cudaStream_t st_;
     int n_sms_;
     uint32_t max_batch_;

@@ -91,15 +91,24 @@ class SearchMode:
         return SearchMode("Hybrid", similarity_threshold, ann_mode)
 
 
+class DistanceUnit(enum.IntEnum):
+    """`DistanceUnit` (index.rs) of a geo filter."""
+    Kilometers = 0
+    Miles = 1
+
+
 @dataclass(frozen=True)
 class FacetFilter:
     """`FacetFilter` (search.rs:735-860): a range filter `start <= value < end` (Rust `Range<T>`) on a numeric / timestamp facet field, or a
-    value-id set on a String16 / String32 facet (values = the ids the reference resolves the filter strings to, FilterSparse::String16/32).
+    value-id set on a String16 / String32 facet (values = the ids the reference resolves the filter strings to, FilterSparse::String16/32),
+    or on a Point facet (`FacetFilter::Point`, base = (lat, lon)) the docs whose distance to base lies in start..end, in unit.
     field: the facet's name (Index.set_facets) or its index."""
     field: object
     start: object = None
     end: object = None
     values: Optional[Sequence[int]] = None
+    base: Optional[Sequence[float]] = None
+    unit: DistanceUnit = DistanceUnit.Kilometers
 
 
 class SortOrder(enum.IntEnum):
@@ -111,8 +120,9 @@ class SortOrder(enum.IntEnum):
 @dataclass(frozen=True)
 class ResultSort:
     """`ResultSort` (search.rs:893-901): sort the hits by a facet field (name given to set_facets), "_id" or "_score".  base: the
-    `FacetValue` of geo proximity sorting — only a Point facet reads it, and Point facets are not built: any base other than None
-    raises NotImplementedError."""
+    `FacetValue::Point` (lat, lon) of geo proximity sorting on a Point facet: the hits are ordered by their distance to it (ascending =
+    nearest first); a Point facet without a base is skipped like the reference does.  A base on any other field raises
+    NotImplementedError."""
     field: str
     order: SortOrder = SortOrder.Descending
     base: object = None
@@ -152,6 +162,48 @@ def synthetic_term_key(term: str) -> int:
     if len(term) > 1 and term[0] == "t" and term[1:].isdigit():
         return splitmix64(int(term[1:])) & ~7
     return fnv1a64(term)
+
+
+def _morton_spread(v):
+    x = v.astype(np.uint64)
+    for sh, m in ((16, 0x0000FFFF0000FFFF), (8, 0x00FF00FF00FF00FF), (4, 0x0F0F0F0F0F0F0F0F), (2, 0x3333333333333333), (1, 0x5555555555555555)):
+        x = (x | (x << np.uint64(sh))) & np.uint64(m)
+    return x
+
+
+def _rust_as_i32(v):
+    """Rust `f64 as i32` on an array: truncation toward zero, saturating at the i32 limits, NaN -> 0"""
+    v = np.asarray(v, dtype=np.float64)
+    out = np.trunc(np.clip(np.where(np.isnan(v), 0.0, v), -2147483648.0, 2147483647.0))
+    return out.astype(np.int64).astype(np.int32)
+
+
+def encode_morton_2d(lat, lon):
+    """encode_morton_2_d (geo_search.rs:27-42) on arrays: x = ((lat * 1e7) as i32) as u32 in the even bits, y = the same of lon in the odd
+    bits -> uint64 codes"""
+    x = _rust_as_i32(np.asarray(lat, dtype=np.float64) * 10000000.0).view(np.uint32)
+    y = _rust_as_i32(np.asarray(lon, dtype=np.float64) * 10000000.0).view(np.uint32)
+    return _morton_spread(x) | (_morton_spread(y) << np.uint64(1))
+
+
+def decode_morton_2d(codes):
+    """decode_morton_2_d (geo_search.rs:58-79) on an array of codes: (x_u32 as i32) as f64 / 1e7 of the even (lat) and odd (lon) bits"""
+    def compact(c):
+        x = c & np.uint64(0x5555555555555555)
+        for sh, m in ((1, 0x3333333333333333), (2, 0x0F0F0F0F0F0F0F0F), (4, 0x00FF00FF00FF00FF), (8, 0x0000FFFF0000FFFF), (16, 0xFFFFFFFF)):
+            x = (x ^ (x >> np.uint64(sh))) & np.uint64(m)
+        return x.astype(np.uint32).view(np.int32).astype(np.float64) / 10000000.0
+    c = np.asarray(codes, dtype=np.uint64)
+    return compact(c), compact(c >> np.uint64(1))
+
+
+def point_column(points):
+    """a Point facet's column as the reference writes it (index.rs:5803-5819): [n, 2] (lat, lon) -> the Morton codes; a coordinate outside
+    [-90, 90] x [-180, 180] (or NaN) is not written, its row stays 0"""
+    p = np.asarray(points, dtype=np.float64).reshape(-1, 2)
+    lat, lon = p[:, 0], p[:, 1]
+    ok = (lat >= -90.0) & (lat <= 90.0) & (lon >= -180.0) & (lon <= 180.0)
+    return np.where(ok, encode_morton_2d(np.where(ok, lat, 0.0), np.where(ok, lon, 0.0)), np.uint64(0)).astype(np.uint64)
 
 
 def _addr(x):
@@ -296,15 +348,21 @@ class Index:
         check(lib().ssb_set_deleted(self._h, a.ctypes.data if a.size else None, a.size))
 
     def set_facets(self, columns: dict, first_doc_id: int = 0, string_facets: Sequence[str] = (), timestamp_facets: Sequence[str] = (),
-                   string_values: Optional[dict] = None):
+                   string_values: Optional[dict] = None, point_facets: Sequence[str] = ()):
         """The shard's facet file (`facets_file_mmap`, add_result.rs:343-347): one typed value per doc and facet field.  columns: name ->
         numpy array [n_docs] (dtype = the facet's FieldType; names in string_facets are String16 / String32 value ids, names in
         timestamp_facets Timestamp); rows are packed field after field like the reference's facet file and handed to ssb_set_facets.
         string_values: name -> the String facet's value strings by id (`facet.values`); sorting by that facet orders by the strings
-        (result_ordering_shard, min_heap.rs:861-898), so their byte-wise order is sent along (ssb_set_facet_value_order)."""
+        (result_ordering_shard, min_heap.rs:861-898), so their byte-wise order is sent along (ssb_set_facet_value_order).
+        point_facets: names whose column is an [n_docs, 2] float64 array of (lat, lon): Point facets, stored as their Morton codes
+        (point_column: invalid coordinates are stored as 0)."""
         from ._lib import SsbFacetField
         kinds = {"uint8": _lib.FACET_U8, "uint16": _lib.FACET_U16, "uint32": _lib.FACET_U32, "uint64": _lib.FACET_U64, "int8": _lib.FACET_I8,
                  "int16": _lib.FACET_I16, "int32": _lib.FACET_I32, "int64": _lib.FACET_I64, "float32": _lib.FACET_F32, "float64": _lib.FACET_F64}
+        for name in point_facets:
+            if name not in columns:
+                raise ValueError(f"point_facets: {name!r} is not a column")
+        columns = {name: (point_column(c) if name in point_facets else c) for name, c in columns.items()}
         names = list(columns)
         n = len(next(iter(columns.values()))) if names else 0
         fields, off, self._facet_schema = (SsbFacetField * max(len(names), 1))(), 0, {}
@@ -315,6 +373,8 @@ class Index:
                 t = {"uint16": _lib.FACET_STRING16, "uint32": _lib.FACET_STRING32}[a.dtype.name]
             if name in timestamp_facets:
                 t = {"int64": _lib.FACET_TIMESTAMP}[a.dtype.name]
+            if name in point_facets:
+                t = _lib.FACET_POINT
             fields[i] = SsbFacetField(t, off)
             self._facet_schema[name] = (i, t)
             off += a.dtype.itemsize
@@ -336,12 +396,13 @@ class Index:
 
     def _sort_criteria(self, result_sort):
         """ResultSort list -> ssb_sort_criterion array (ResultSortIndex, search.rs:2497-2525): "_id" / "_score", facet names resolved to
-        their index; unknown names are dropped like the reference does (facets_map.get, :2517)."""
+        their index; unknown names are dropped like the reference does (facets_map.get, :2517).  A base is accepted on a Point facet
+        only (the bases themselves travel separately, _sort_bases)."""
         from ._lib import SsbSortCriterion
         out = []
         for rs in result_sort:
-            if rs.base is not None:
-                raise NotImplementedError("geo proximity sorting (FacetValue::Point base) is not built")
+            if rs.base is not None and getattr(self, "_facet_schema", {}).get(rs.field, (None, None))[1] != _lib.FACET_POINT:
+                raise NotImplementedError("a ResultSort base (FacetValue::Point) is only read on a Point facet; other bases are not built")
             order = _lib.SORT_DESCENDING if SortOrder(rs.order) == SortOrder.Descending else _lib.SORT_ASCENDING
             if rs.field == "_id":
                 out.append(SsbSortCriterion(_lib.SORT_ID, 0, order, 0))
@@ -350,6 +411,19 @@ class Index:
             elif rs.field in getattr(self, "_facet_schema", {}):
                 out.append(SsbSortCriterion(_lib.SORT_FACET, self._facet_schema[rs.field][0], order, 0))
         return (SsbSortCriterion * max(len(out), 1))(*out), len(out)
+
+    def _sort_bases(self, result_sort, nq, sort_bases=None):
+        """the bases array of ssb_search_lexical_sorted_ex: sort_bases ([nq] (lat, lon) per query) or else the base of the sort's Point
+        criterion for every query; None when neither exists (a Point criterion is then dropped)"""
+        if sort_bases is None:
+            base = next((rs.base for rs in result_sort if rs.base is not None), None)
+            if base is None:
+                return None
+            sort_bases = [base] * nq
+        b = np.ascontiguousarray(np.asarray(sort_bases, dtype=np.float64).reshape(-1, 2))
+        if len(b) != nq:
+            raise ValueError(f"sort_bases: {len(b)} bases for {nq} queries")
+        return b
 
     def _encode_filters(self, filters):
         """filters: per query a list of FacetFilter -> (filter_offsets, ssb_facet_filter array, set values)"""
@@ -361,7 +435,11 @@ class Index:
                 idx, t = self._facet_schema[f.field] if isinstance(f.field, str) else (int(f.field), None)
                 if t is None:
                     t = next((v[1] for v in getattr(self, "_facet_schema", {}).values() if v[0] == idx), _lib.FACET_U64)
-                if f.values is not None:
+                if f.base is not None:                                        # FacetFilter::Point: (base, start..end, unit)
+                    f64 = lambda x: int(np.float64(x).view(np.uint64))
+                    flat.append(SsbFacetFilter(idx, _lib.FILTER_POINT, f64(f.start), f64(f.end), len(sets), 3))
+                    sets.extend([f64(f.base[0]), f64(f.base[1]), int(DistanceUnit(f.unit))])
+                elif f.values is not None:
                     flat.append(SsbFacetFilter(idx, _lib.FILTER_SET, 0, 0, len(sets), len(f.values)))
                     sets.extend(int(v) for v in f.values)
                 else:
@@ -450,9 +528,11 @@ class Index:
         return b, tuple(keep)
 
     def search_lexical_batch(self, queries_keys, query_type: QueryType, k: int,
-                             result_type: ResultType = ResultType.TopkCount, not_keys=None, filters=None, field_masks=None, sort=None):
+                             result_type: ResultType = ResultType.TopkCount, not_keys=None, filters=None, field_masks=None, sort=None,
+                             sort_bases=None):
         """Batched search_lexical_shard.  Returns (list of [(doc_id, score)...], counts ndarray).  not_keys: '-' terms per query;
-        filters: FacetFilter list per query (needs set_facets); sort: ResultSort list for the whole batch (ssb_search_lexical_sorted)."""
+        filters: FacetFilter list per query (needs set_facets); sort: ResultSort list for the whole batch (ssb_search_lexical_sorted_ex);
+        sort_bases: per query the (lat, lon) base of the sort's Point criterion (default: that criterion's ResultSort.base)."""
         nq = len(queries_keys)
         b, keep = self._lex_batch(queries_keys, query_type, not_keys, filters, field_masks)
         hits = _hits_array(max(nq * max(k, 1), 1))
@@ -460,8 +540,9 @@ class Index:
         counts = np.zeros(max(nq, 1), dtype=np.uint64)
         if sort is not None:
             crit, n_crit = self._sort_criteria(sort)
-            check(lib().ssb_search_lexical_sorted(self._h, C.byref(b), C.addressof(crit), n_crit, k, int(result_type), hits.ctypes.data,
-                                                  n_hits.ctypes.data, counts.ctypes.data))
+            bases = self._sort_bases(sort, nq, sort_bases)
+            check(lib().ssb_search_lexical_sorted_ex(self._h, C.byref(b), C.addressof(crit), n_crit, bases.ctypes.data if bases is not None else None,
+                                                     k, int(result_type), hits.ctypes.data, n_hits.ctypes.data, counts.ctypes.data))
         else:
             check(lib().ssb_search_lexical(self._h, C.byref(b), k, int(result_type), hits.ctypes.data, n_hits.ctypes.data,
                                            counts.ctypes.data))
@@ -586,18 +667,19 @@ class Index:
                result_sort: Sequence = (), query_rewriting=None) -> ResultObject:
         """`Search::search` (search.rs:1134-1150) for committed data, 1-shard semantics.
 
-        facet_filter: FacetFilter objects (range / value-set filters on the facet fields given to set_facets) — applied to the lexical
-        search like the reference does (the vector search takes no facet filter, vector.rs:1105-1115).
-        result_sort: ResultSort objects — lexical search only (the hits in sort order, ssb_search_lexical_sorted).
-        Unsupported reference features (facet counting, sorting vector / hybrid results or by geo distance, uncommitted, rewriting) raise
-        NotImplementedError rather than being silently ignored."""
+        facet_filter: FacetFilter objects (range / value-set / geo distance filters on the facet fields given to set_facets) — applied to
+        the lexical search like the reference does (the vector search takes no facet filter, vector.rs:1105-1115).
+        result_sort: ResultSort objects — lexical search only (the hits in sort order, ssb_search_lexical_sorted_ex; a Point facet's
+        ResultSort.base sorts by the distance to it).
+        Unsupported reference features (facet counting, sorting vector / hybrid results, a base on a non-Point facet, uncommitted,
+        rewriting) raise NotImplementedError rather than being silently ignored."""
         if query_facets or include_uncommitted:
             raise NotImplementedError("facet counts / uncommitted search are outside the GPU hot path")
         search_mode = search_mode or SearchMode.Lexical()
         if result_sort and search_mode.kind != "Lexical":
             raise NotImplementedError("result_sort on vector / hybrid search is not built")
         if result_sort:
-            self._sort_criteria(result_sort)                     # a FacetValue::Point base raises before any search runs
+            self._sort_criteria(result_sort)                     # a base on a non-Point facet raises before any search runs
         # field_filter: names of indexed fields (self.field_names, in schema order) or their indices -> one bitmask
         fmask = 0
         for f in field_filter:
