@@ -876,8 +876,6 @@ int32_t ssb_set_deleted(ssb_index* ix, const uint64_t* doc_ids, uint64_t n) {
     SSB_API_END
 }
 
-// facets_file_mmap (is_facet_filter, add_result.rs:340-478, reads `facets_size_sum * docid + facet.offset`): every value becomes an
-// order-preserving 64-bit key, one column per facet, so the kernels test any FilterSparse range with two unsigned compares.
 int32_t ssb_set_facets(ssb_index* ix, const void* rows, uint64_t first_doc_id, uint64_t n_docs, uint32_t row_bytes,
                        const ssb_facet_field* fields, uint32_t n_fields) {
     SSB_API_BEGIN
@@ -885,34 +883,7 @@ int32_t ssb_set_facets(ssb_index* ix, const void* rows, uint64_t first_doc_id, u
     std::unique_lock<std::shared_mutex> g(ix->rw);
     SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
     SSB_CUDA_TRY(cudaDeviceSynchronize());        // searches may run on a caller-owned stream (ssb_set_stream): nothing may still read the old columns
-    ix->facets.release();
-    if (n_docs == 0 || n_fields == 0) return SSB_OK;
-    if (!rows || !fields) { set_error("ssb_set_facets: null argument"); return SSB_E_INVALID; }
-    if (n_fields > SSB_MAX_FACETS) { set_error("ssb_set_facets: more than %u facets", SSB_MAX_FACETS); return SSB_E_UNSUPPORTED; }
-    if (first_doc_id + n_docs > (1ull << 32)) { set_error("ssb_set_facets: doc ids must be < 2^32"); return SSB_E_INVALID; }
-    for (uint32_t f = 0; f < n_fields; f++) {
-        const uint32_t w = facet_type_bytes(fields[f].type);
-        if (!w) { set_error("ssb_set_facets: field %u has unsupported type %u", f, fields[f].type); return SSB_E_UNSUPPORTED; }
-        if ((uint64_t)fields[f].offset + w > row_bytes) { set_error("ssb_set_facets: field %u does not fit a %u-byte row", f, row_bytes); return SSB_E_INVALID; }
-    }
-    std::vector<uint64_t> keys((size_t)n_fields * n_docs);
-    const uint8_t* base = (const uint8_t*)rows;
-    for (uint32_t f = 0; f < n_fields; f++) {
-        uint64_t* col = keys.data() + (size_t)f * n_docs;
-        const uint32_t type = fields[f].type, off = fields[f].offset;
-        for (uint64_t d = 0; d < n_docs; d++) col[d] = facet_value_key(type, base + d * row_bytes + off);
-    }
-    SSB_CUDA_TRY(cudaMalloc(&ix->facets.d_keys, keys.size() * 8));
-    SSB_CUDA_TRY(cudaMemcpy(ix->facets.d_keys, keys.data(), keys.size() * 8, cudaMemcpyHostToDevice));
-    ix->facets.n_rows = n_docs; ix->facets.first_doc = (uint32_t)first_doc_id; ix->facets.n_facets = n_fields;
-    for (uint32_t f = 0; f < n_fields; f++) {
-        ix->facets.types[f] = (uint8_t)fields[f].type;
-        const uint64_t* col = keys.data() + (size_t)f * n_docs;
-        ix->facets.max_key[f] = *std::max_element(col, col + n_docs);
-        SSB_TRY(facet_zones(ix->facets, f, ix->load_st));           // per-level bounds of sorted searches
-    }
-    SSB_CUDA_TRY(cudaStreamSynchronize(ix->load_st));
-    return SSB_OK;
+    return ix->facets.set_columns(rows, first_doc_id, n_docs, row_bytes, fields, n_fields, ix->load_st);
     SSB_API_END
 }
 
@@ -925,18 +896,12 @@ int32_t ssb_set_facet_value_order(ssb_index* ix, uint32_t facet, const uint32_t*
     if (!fs.n_facets) { set_error("ssb_set_facet_value_order: no facets (ssb_set_facets)"); return SSB_E_STATE; }
     if (facet >= fs.n_facets) { set_error("ssb_set_facet_value_order: facet %u of %u", facet, fs.n_facets); return SSB_E_INVALID; }
     const uint32_t type = fs.types[facet];
-    if (type != SSB_FACET_STRING16 && type != SSB_FACET_STRING32) { set_error("ssb_set_facet_value_order: facet %u is not a String16 / String32 facet", facet); return SSB_E_INVALID; }
+    if (!facet_is_string(type)) { set_error("ssb_set_facet_value_order: facet %u is not a String16 / String32 facet", facet); return SSB_E_INVALID; }
     const uint64_t lim = type == SSB_FACET_STRING16 ? 65536ull : (1ull << 32);
     if (n_ids == 0 || n_ids > lim) { set_error("ssb_set_facet_value_order: n_ids must be in 1..%llu", (unsigned long long)lim); return SSB_E_INVALID; }
     for (uint32_t i = 0; i < n_ids; i++) if (rank_of_id[i] >= n_ids) { set_error("ssb_set_facet_value_order: rank %u of id %u is not below n_ids", rank_of_id[i], i); return SSB_E_INVALID; }
     SSB_CUDA_TRY(cudaDeviceSynchronize());        // searches on a caller-owned stream may still read the old order
-    cudaFree(fs.d_rank[facet]); fs.d_rank[facet] = nullptr; fs.n_rank[facet] = 0;
-    SSB_CUDA_TRY(cudaMalloc(&fs.d_rank[facet], (size_t)n_ids * 4));
-    SSB_CUDA_TRY(cudaMemcpy(fs.d_rank[facet], rank_of_id, (size_t)n_ids * 4, cudaMemcpyHostToDevice));
-    fs.n_rank[facet] = n_ids;
-    SSB_TRY(facet_zones(fs, facet, ix->load_st));                   // the level bounds of this facet are ranks from now on
-    SSB_CUDA_TRY(cudaStreamSynchronize(ix->load_st));
-    return SSB_OK;
+    return fs.set_value_order(facet, rank_of_id, n_ids, ix->load_st);
     SSB_API_END
 }
 

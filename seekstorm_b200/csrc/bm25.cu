@@ -35,6 +35,7 @@
 // (__fmul_rn/__fdiv_rn/__fadd_rn), summed in query order from 0.0 (add_result.rs:1450-1452), idf and the 256-entry
 // cache computed on the host.
 #include "bm25.h"
+#include "facets.cuh"
 
 #include <cuda_fp16.h>
 #include <math.h>
@@ -266,7 +267,6 @@ __device__ __forceinline__ uint32_t meta_cperm(uint32_t m, uint32_t c) { return 
 // SORTED (ssb_search_lexical_sorted): every query takes lex_generic, theta / glist are the 128-bit θ and lists, and the levels are ordered
 // by the upper bound of the sort key instead of the score bound (its top 32 bits: the order only decides how early θ rises; the exact
 // bound goes into the record, rec_sort_bound, for the skip test).
-__device__ __forceinline__ uint64_t level_sort_bound(const SortDev& s, uint32_t level_id);
 __device__ __forceinline__ void rec_set_sort_bound(LvRec& r, uint64_t b) { r.S[0] = __uint_as_float((uint32_t)b); r.S[1] = __uint_as_float((uint32_t)(b >> 32)); }
 __device__ __forceinline__ uint64_t rec_sort_bound(const LvRec& r) { return ((uint64_t)__float_as_uint(r.S[1]) << 32) | __float_as_uint(r.S[0]); }
 template <bool SORTED>
@@ -583,78 +583,6 @@ __device__ __forceinline__ bool in_not_lists(const LexView& v, const QueryPlan* 
     return in_not_lists_impl(list_view(v), pl, n_not, lv, d);
 }
 
-// is_facet_filter (add_result.rs:340-478): true = the doc is filtered OUT.  The typed range / set tests of the reference run on the
-// order-preserving 64-bit keys ssb_set_facets stored per doc and facet (bounds converted the same way by the host), so one unsigned
-// compare pair covers every FilterSparse range type.  Out of line, by value, on the rare candidate / count path of lex_generic only.
-struct FacetArgs { const uint64_t* keys; uint64_t rows; const FiltDev* filt; const uint64_t* sets; uint32_t first_doc; };
-
-// ---- geo (Point facets, geo_search.rs): Morton decode and the two distances, every f64 operation individually rounded in the reference's
-// order (Rust does not contract into FMA); cos is CUDA's double cos (documented within 2 ulp of the exact value, not bit-equal to glibc's)
-#define SSB_DEG2RAD 0.017453292519943295
-// decode_morton_64_bit (geo_search.rs:44-52): the even bits of code, compacted
-__device__ __forceinline__ uint32_t morton_even_bits(uint64_t code) {
-    uint64_t x = code & 0x5555555555555555ull;
-    x = (x ^ (x >> 1)) & 0x3333333333333333ull;
-    x = (x ^ (x >> 2)) & 0x0F0F0F0F0F0F0F0Full;
-    x = (x ^ (x >> 4)) & 0x00FF00FF00FF00FFull;
-    x = (x ^ (x >> 8)) & 0x0000FFFF0000FFFFull;
-    x = (x ^ (x >> 16)) & 0x00000000FFFFFFFFull;
-    return (uint32_t)x;
-}
-// decode_morton_2_d (geo_search.rs:58-79): (x_u32 as i32) as f64 / 1e7 — lat from the even bits, lon from the odd bits
-__device__ __forceinline__ double morton_lat(uint64_t code) { return __ddiv_rn((double)(int32_t)morton_even_bits(code), 10000000.0); }
-__device__ __forceinline__ double morton_lon(uint64_t code) { return __ddiv_rn((double)(int32_t)morton_even_bits(code >> 1), 10000000.0); }
-// FilterSparse::Point (add_result.rs:462-478): true = the doc is filtered OUT.  range.contains(code) on the Morton interval staged in
-// [lo, hi), then distance_range.contains(euclidian_distance(base, decode(code), unit)) (geo_search.rs:95-107).  g: the staged payload
-// (GEO_* words, f64 bits).  Out of line: only POINT filters reach it.
-__device__ __noinline__ bool geo_rejects_impl(uint64_t code, uint64_t lo, uint64_t hi, const uint64_t* g) {
-    if (!(code >= lo && code < hi)) return true;
-    const double blat = __longlong_as_double((long long)__ldg(&g[GEO_LAT])), blon = __longlong_as_double((long long)__ldg(&g[GEO_LON]));
-    const double plat = morton_lat(code), plon = morton_lon(code);
-    const double c = cos(__ddiv_rn(__dmul_rn(SSB_DEG2RAD, __dadd_rn(blat, plat)), 2.0));
-    const double x = __dmul_rn(__dmul_rn(SSB_DEG2RAD, __dsub_rn(plon, blon)), c);
-    const double y = __dmul_rn(SSB_DEG2RAD, __dsub_rn(plat, blat));
-    const double d = __dmul_rn(__longlong_as_double((long long)__ldg(&g[GEO_RADIUS])), __dsqrt_rn(__dadd_rn(__dmul_rn(x, x), __dmul_rn(y, y))));
-    const double start = __longlong_as_double((long long)__ldg(&g[GEO_START])), end = __longlong_as_double((long long)__ldg(&g[GEO_END]));
-    return !(start <= d && d < end);
-}
-// the sort key of a POINT criterion (morton_ordering, geo_search.rs:82-93): the order key of simplified_distance(decode(code), base) — the
-// F64 column key (key_of_f64: NaN = all ones, above +inf).  base: the query's (lat, lon).  Out of line: only POINT criteria reach it.
-__device__ __noinline__ uint64_t point_sort_key(uint64_t code, const double* base) {
-    const double blat = __ldg(&base[0]), blon = __ldg(&base[1]);
-    const double plat = morton_lat(code), plon = morton_lon(code);
-    const double x = __dmul_rn(__dsub_rn(blon, plon), cos(__ddiv_rn(__dmul_rn(SSB_DEG2RAD, __dadd_rn(plat, blat)), 2.0)));
-    const double y = __dsub_rn(blat, plat);
-    double d = __dadd_rn(__dmul_rn(x, x), __dmul_rn(y, y));
-    if (d != d) return ~0ull;
-    if (d == 0.0) d = 0.0;                                               // -0.0 == +0.0
-    const uint64_t b = (uint64_t)__double_as_longlong(d);
-    return (b >> 63) ? ~b : (b | 0x8000000000000000ull);
-}
-
-// GEO: the batch holds a POINT filter — its own instantiation, so that the common one keeps its code and its callers their registers
-template <bool GEO>
-__device__ __noinline__ bool facet_rejects_impl(FacetArgs a, uint32_t f0, uint32_t nf, uint32_t doc) {
-    const uint64_t row = (uint64_t)doc - a.first_doc;
-    if (doc < a.first_doc || row >= a.rows) return true;             // no facet row for this doc
-    for (uint32_t i = 0; i < nf; i++) {
-        const FiltDev f = a.filt[f0 + i];
-        const uint64_t key = __ldg(&a.keys[(size_t)f.facet * a.rows + row]);
-        if (f.kind == FILT_RANGE) { if (!(key >= f.lo && key < f.hi)) return true; }
-        else if (f.kind == FILT_SET) {
-            bool in = false;
-            for (uint32_t s = 0; s < f.set_n; s++) in = in || __ldg(&a.sets[f.set_first + s]) == key;
-            if (!in) return true;
-        } else if (GEO && f.kind == FILT_POINT) { if (geo_rejects_impl(key, f.lo, f.hi, a.sets + f.set_first)) return true; }
-        else return true;
-    }
-    return false;
-}
-template <bool GEO = false>
-__device__ __forceinline__ bool facet_rejects(const LexView& v, uint32_t f0, uint32_t nf, uint32_t doc) {
-    return facet_rejects_impl<GEO>(FacetArgs{v.facet_keys, v.facet_rows, v.filt, v.filt_sets, v.facet_first_doc}, f0, nf, doc);
-}
-
 // field_filter (`field_filter_set`, add_result.rs:3124-3137, 3558-3571): every query term the doc contains must occur in at least one
 // field of the filter — tested only when (fields the term occurs in) + (fields of the filter) <= indexed fields, otherwise they overlap for
 // certain.  The score still sums every field.  true = the doc is filtered OUT.  Out of line, on the filtered path of lex_generic only.
@@ -790,24 +718,6 @@ __device__ __forceinline__ void wl_merge128(uint64_t& Ah, uint64_t& Al, uint64_t
 }
 // the warp's list of one sorted item; thr = a lower bound of θ.hi (global θ.hi, or the local list's k-th hi once it is full)
 struct SortTop { uint64_t h, l, thr; };
-// doc's packed sort key for query q: the facet column keys of its row (a String facet's id through its value order, a Point facet's code
-// through its distance to the query's base), or its id
-__device__ __forceinline__ uint64_t sort_pack_hi(const SortDev& s, const uint64_t* v);
-template <bool GEO>
-__device__ __forceinline__ uint64_t doc_sort_hi(const LexView& v, const SortDev& s, uint32_t doc, uint32_t q) {
-    const uint64_t row = (uint64_t)(doc - v.facet_first_doc);          // prepare_sort: the facet rows cover every doc of the levels
-    uint64_t val[SSB_MAX_SORT_CRITERIA];
-#pragma unroll
-    for (uint32_t i = 0; i < SSB_MAX_SORT_CRITERIA; i++) {
-        val[i] = doc;
-        if (i < s.n && s.src[i] == SORT_SRC_FACET) {
-            val[i] = __ldg(&v.facet_keys[(size_t)s.facet[i] * v.facet_rows + row]);
-            if (s.rank[i]) val[i] = __ldg(&s.rank[i][val[i]]);          // prepare_sort: every id of the column has a rank
-            else if (GEO && s.type[i] == SSB_FACET_POINT) val[i] = point_sort_key(val[i], s.bases + 2 * (size_t)q);
-        }
-    }
-    return sort_pack_hi(s, val);
-}
 // insert the lanes' candidates (cand) below the paging ceiling (ch, cl) into the warp list; raise thr from the k-th entry
 __device__ __forceinline__ void insert_sorted(SortTop& T, bool cand, uint64_t hi, float score, uint32_t doc, bool score_asc,
                                               uint32_t k, int lane, bool& dirty, uint64_t ch, uint64_t cl) {
@@ -2117,183 +2027,12 @@ int32_t LexIndex::ensure_workspace(LexWorkspace& ws, uint32_t nq, uint32_t total
     return SSB_OK;
 }
 
-// ---- facet filters: FilterSparse bounds -> the key space of the facet columns ----
-// Keys: unsigned types as they are; signed types and Timestamp with the sign bit flipped; F32 / F64 through the f64 value's bits
-// (negative: all bits flipped, else sign bit set; -0.0 counts as +0.0, PartialOrd) — NaN has no key: a NaN VALUE gets ~0, which
-// no range contains (every finite / infinite bound maps below it), a NaN BOUND makes the filter reject everything.
-static inline uint64_t key_of_f64(double x) {
-    if (x == 0.0) x = 0.0;                                           // -0.0 == +0.0
-    uint64_t b; memcpy(&b, &x, 8);
-    return (b >> 63) ? ~b : (b | 0x8000000000000000ull);
-}
-static inline bool facet_is_signed(uint32_t t) { return t == SSB_FACET_I8 || t == SSB_FACET_I16 || t == SSB_FACET_I32 || t == SSB_FACET_I64 || t == SSB_FACET_TIMESTAMP; }
-static inline bool facet_is_float(uint32_t t) { return t == SSB_FACET_F32 || t == SSB_FACET_F64; }
-uint64_t facet_value_key(uint32_t type, const uint8_t* p) {
-    switch (type) {
-        case SSB_FACET_U8: return p[0];
-        case SSB_FACET_U16: case SSB_FACET_STRING16: { uint16_t x; memcpy(&x, p, 2); return x; }
-        case SSB_FACET_U32: case SSB_FACET_STRING32: { uint32_t x; memcpy(&x, p, 4); return x; }
-        case SSB_FACET_U64: case SSB_FACET_POINT: { uint64_t x; memcpy(&x, p, 8); return x; }   // Point: the Morton code itself
-        case SSB_FACET_I8: { int8_t x; memcpy(&x, p, 1); return (uint64_t)(int64_t)x ^ 0x8000000000000000ull; }
-        case SSB_FACET_I16: { int16_t x; memcpy(&x, p, 2); return (uint64_t)(int64_t)x ^ 0x8000000000000000ull; }
-        case SSB_FACET_I32: { int32_t x; memcpy(&x, p, 4); return (uint64_t)(int64_t)x ^ 0x8000000000000000ull; }
-        case SSB_FACET_I64: case SSB_FACET_TIMESTAMP: { int64_t x; memcpy(&x, p, 8); return (uint64_t)x ^ 0x8000000000000000ull; }
-        case SSB_FACET_F32: { float x; memcpy(&x, p, 4); return x != x ? ~0ull : key_of_f64((double)x); }
-        case SSB_FACET_F64: { double x; memcpy(&x, p, 8); return x != x ? ~0ull : key_of_f64(x); }
-    }
-    return ~0ull;
-}
-uint32_t facet_type_bytes(uint32_t type) {
-    switch (type) {
-        case SSB_FACET_U8: case SSB_FACET_I8: return 1;
-        case SSB_FACET_U16: case SSB_FACET_I16: case SSB_FACET_STRING16: return 2;
-        case SSB_FACET_U32: case SSB_FACET_I32: case SSB_FACET_F32: case SSB_FACET_STRING32: return 4;
-        case SSB_FACET_U64: case SSB_FACET_I64: case SSB_FACET_TIMESTAMP: case SSB_FACET_F64: case SSB_FACET_POINT: return 8;
-    }
-    return 0;
-}
-
-// ---- geo on the host: encode_morton_2_d and point_distance_to_morton_range (geo_search.rs:27-42, 109-144) for the filter interval.  The
-// host code is compiled without FMA contraction (-ffp-contract=off); the expressions hold no multiply-add anyway.
-static inline int32_t rust_as_i32(double v) {                      // Rust `f64 as i32`: truncation, saturating, NaN -> 0
-    if (v != v) return 0;
-    if (v >= 2147483648.0) return INT32_MAX;
-    if (v <= -2147483648.0) return INT32_MIN;
-    return (int32_t)v;
-}
-static inline uint64_t morton_spread(uint32_t v) {                  // encode_morton_64_bit (geo_search.rs:11-20)
-    uint64_t x = v;
-    x = (x | (x << 16)) & 0x0000FFFF0000FFFFull;
-    x = (x | (x << 8)) & 0x00FF00FF00FF00FFull;
-    x = (x | (x << 4)) & 0x0F0F0F0F0F0F0F0Full;
-    x = (x | (x << 2)) & 0x3333333333333333ull;
-    x = (x | (x << 1)) & 0x5555555555555555ull;
-    return x;
-}
-static inline uint64_t encode_morton_2d(double lat, double lon) {
-    return morton_spread((uint32_t)rust_as_i32(lat * 10000000.0)) | (morton_spread((uint32_t)rust_as_i32(lon * 10000000.0)) << 1);
-}
-static inline double earth_radius(uint64_t unit) { return unit == SSB_UNIT_MILES ? 3958.761315801475 : 6371.0087714; }
-
-// ---- sort keys (ssb_search_lexical_sorted; result_ordering_shard, min_heap.rs:574-1051) ----
-// The packed sort key `hi` — the one place that knows its layout.  v[i] is criterion i's value: the facet's column key (facet_value_key;
-// for a String facet already replaced by the rank of its id in the value order) or the doc id (_id).  Each is narrowed to its natural
-// width (sort_width) keeping its order: unsigned values and ranks as they are, signed ones with the sign bit flipped within the width,
-// F32 by the IEEE order trick on 32 bits (-0.0 already folded into +0.0, NaN = all ones: above +inf), 64-bit keys as they are; inverted
-// within the width when ascending; concatenated with the first criterion most significant, left-aligned at bit 63.  Compared as one
-// unsigned word, hi orders docs like the criteria compared left to right.  The 128-bit top-k key is (hi, lo), lo = pack_key(score, doc)
-// with its score half inverted for `_score` ascending: ties on every criterion fall back to score desc (min_heap.rs:1043-1050), then
-// doc id asc.  hi is monotone in every v[i]: packing per-criterion upper bounds bounds the key of every doc (level_sort_bound).
-__host__ __device__ __forceinline__ uint32_t sort_width(uint32_t src, uint32_t type) {
-    if (src == SORT_SRC_ID) return 32;
-    switch (type) {
-        case SSB_FACET_U8: case SSB_FACET_I8: return 8;
-        case SSB_FACET_U16: case SSB_FACET_I16: case SSB_FACET_STRING16: return 16;
-        case SSB_FACET_U32: case SSB_FACET_I32: case SSB_FACET_F32: case SSB_FACET_STRING32: return 32;
-    }
-    return 64;
-}
-__device__ __forceinline__ uint64_t sort_pack_hi(const SortDev& s, const uint64_t* v) {
-    uint64_t hi = 0; uint32_t used = 0;
-#pragma unroll
-    for (uint32_t i = 0; i < SSB_MAX_SORT_CRITERIA; i++) {
-        if (i >= s.n) break;
-        const uint32_t w = sort_width(s.src[i], s.type[i]);
-        const uint64_t mask = w == 64 ? ~0ull : (1ull << w) - 1ull;
-        uint64_t x = v[i];
-        if (s.src[i] == SORT_SRC_FACET) {
-            const uint32_t t = s.type[i];
-            if (t == SSB_FACET_I8 || t == SSB_FACET_I16 || t == SSB_FACET_I32) x = (x & mask) ^ (1ull << (w - 1));
-            else if (t == SSB_FACET_F32) {        // column key = the f64 order key of the value (key_of_f64): back to the float, 32-bit order key
-                if (x == ~0ull) x = 0xFFFFFFFFull;
-                else x = ord_f32(__double2float_rn(__longlong_as_double((long long)((x >> 63) ? (x & 0x7FFFFFFFFFFFFFFFull) : ~x))));
-            }
-        }
-        x &= mask;
-        if (!s.desc[i]) x ^= mask;
-        used += w;
-        hi |= x << (64 - used);
-    }
-    return hi;
-}
-// upper bound of hi over the docs of a level: per criterion the level's largest value (descending) or smallest (ascending, inverted by
-// the packing) — the block's zone for a facet, level << 16 | 0xFFFF or level << 16 for _id.  A Point criterion takes the trivial bound
-// (the largest key after packing): its zones hold Morton codes, not distances, and no level is skipped.
-__device__ __forceinline__ uint64_t level_sort_bound(const SortDev& s, uint32_t level_id) {
-    uint64_t val[SSB_MAX_SORT_CRITERIA];
-    const uint32_t b = level_id - s.zone_block0;                       // prepare_sort: the zones cover every level
-#pragma unroll
-    for (uint32_t i = 0; i < SSB_MAX_SORT_CRITERIA; i++) {
-        val[i] = s.desc[i] ? ((uint64_t)level_id << 16 | 0xFFFFu) : ((uint64_t)level_id << 16);
-        if (i < s.n && s.src[i] == SORT_SRC_FACET)
-            val[i] = s.type[i] == SSB_FACET_POINT ? (s.desc[i] ? ~0ull : 0ull) : s.zones[((size_t)s.facet[i] * s.n_zone_blocks + b) * 2 + (s.desc[i] ? 1 : 0)];
-    }
-    return sort_pack_hi(s, val);
-}
-
-// one CTA per zone block: min / max of the block's column keys (or ranks) -> zone[2 * block]
-__global__ void __launch_bounds__(256) facet_zone_minmax(const uint64_t* __restrict__ col, uint64_t rows, uint32_t first_doc, uint32_t block0,
-                                                         const uint32_t* __restrict__ rank, uint32_t n_rank, uint64_t* __restrict__ zone) {
-    __shared__ uint64_t smin[8], smax[8];
-    const uint64_t d0 = (uint64_t)(block0 + blockIdx.x) << 16;
-    const uint64_t lo = d0 > first_doc ? d0 - first_doc : 0, hi = (d0 + 65536 - first_doc) < rows ? d0 + 65536 - first_doc : rows;
-    uint64_t mn = ~0ull, mx = 0;
-    for (uint64_t r = lo + threadIdx.x; r < hi; r += blockDim.x) {
-        uint64_t x = col[r];
-        if (rank) x = x < n_rank ? rank[x] : ~0ull;
-        mn = x < mn ? x : mn; mx = x > mx ? x : mx;
-    }
-    for (int s = 16; s; s >>= 1) {
-        const uint64_t a = shfl64_xor(mn, s), b = shfl64_xor(mx, s);
-        mn = a < mn ? a : mn; mx = b > mx ? b : mx;
-    }
-    if ((threadIdx.x & 31) == 0) { smin[threadIdx.x >> 5] = mn; smax[threadIdx.x >> 5] = mx; }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        for (int i = 1; i < 8; i++) { mn = smin[i] < mn ? smin[i] : mn; mx = smax[i] > mx ? smax[i] : mx; }
-        zone[2 * blockIdx.x] = mn; zone[2 * blockIdx.x + 1] = mx;
-    }
-}
-int32_t facet_zones(FacetSet& fs, uint32_t f, cudaStream_t st) {
-    if (!fs.n_facets || !fs.n_rows) return SSB_OK;
-    if (!fs.d_zones) {
-        fs.zone_block0 = fs.first_doc >> 16;
-        fs.n_zone_blocks = (uint32_t)(((uint64_t)fs.first_doc + fs.n_rows - 1) >> 16) - fs.zone_block0 + 1;
-        SSB_CUDA_TRY(cudaMalloc(&fs.d_zones, (size_t)fs.n_facets * fs.n_zone_blocks * 16));
-    }
-    facet_zone_minmax<<<fs.n_zone_blocks, 256, 0, st>>>(fs.d_keys + (size_t)f * fs.n_rows, fs.n_rows, fs.first_doc, fs.zone_block0, fs.d_rank[f], fs.n_rank[f],
-                                                        fs.d_zones + (size_t)f * fs.n_zone_blocks * 2);
-    SSB_CUDA_TRY(cudaGetLastError());
-    return SSB_OK;
-}
-
 int32_t LexIndex::prepare_sort(const ssb_sort_criterion* crit, uint32_t n, bool has_bases, SortDev* out, bool* sorted) const {
-    if (n && !crit) { set_error("search_lexical_sorted: null criteria"); return SSB_E_INVALID; }
-    if (n > SSB_MAX_SORT_CRITERIA) { set_error("search_lexical_sorted: more than %u criteria", SSB_MAX_SORT_CRITERIA); return SSB_E_UNSUPPORTED; }
-    const uint32_t nf = facets_ ? facets_->n_facets : 0;
-    for (uint32_t i = 0; i < n; i++) {
-        if (crit[i].source > SSB_SORT_SCORE || crit[i].order > SSB_SORT_DESCENDING) { set_error("sort criterion %u: bad source / order", i); return SSB_E_INVALID; }
-        if (crit[i].source == SSB_SORT_FACET && nf && crit[i].facet >= nf) { set_error("sort criterion %u: facet %u of %u", i, crit[i].facet, nf); return SSB_E_INVALID; }
-    }
     SortDev s{};
-    uint32_t bits = 0;
-    bool any_facet = false, ended = false;
-    for (uint32_t i = 0; i < n && !ended; i++) {                   // _id / _score end the comparison (min_heap.rs:580-604)
-        const ssb_sort_criterion& c = crit[i];
-        if (c.source == SSB_SORT_SCORE) { s.score_asc = c.order == SSB_SORT_ASCENDING; ended = true; continue; }
-        // a Point facet without a FacetValue::Point base is skipped (min_heap.rs:510-529: `if let FacetValue::Point(base)`)
-        if (c.source == SSB_SORT_FACET && nf && facets_->types[c.facet] == SSB_FACET_POINT && !has_bases) continue;
-        ended = c.source == SSB_SORT_ID;
-        const uint32_t j = s.n++;
-        s.src[j] = c.source == SSB_SORT_ID ? SORT_SRC_ID : SORT_SRC_FACET; s.desc[j] = c.order == SSB_SORT_DESCENDING;
-        if (s.src[j] == SORT_SRC_FACET) { s.facet[j] = c.facet; any_facet = true; }
-        s.type[j] = s.src[j] == SORT_SRC_FACET && nf ? facets_->types[c.facet] : 0u;
-        bits += sort_width(s.src[j], s.type[j]);
-    }
-    *sorted = s.n > 0 || s.score_asc;
+    SSB_TRY(sort_of_criteria(facets_, crit, n, has_bases, &s, sorted));
     if (!*sorted) return SSB_OK;
-    if (any_facet && !nf) { set_error("search_lexical_sorted: sorting by a facet needs ssb_set_facets"); return SSB_E_STATE; }
-    if (bits > 64) { set_error("search_lexical_sorted: the criteria take %u bits (at most 64)", bits); return SSB_E_UNSUPPORTED; }
+    bool any_facet = false;
+    for (uint32_t j = 0; j < s.n; j++) any_facet = any_facet || s.src[j] == SORT_SRC_FACET;
     if (any_facet) {
         for (const LexLevel& l : levels_) {                           // a sorted doc must have a facet value
             const uint64_t d0 = (uint64_t)l.level_id << 16;
@@ -2301,26 +2040,13 @@ int32_t LexIndex::prepare_sort(const ssb_sort_criterion* crit, uint32_t n, bool 
                 set_error("search_lexical_sorted: the facet rows do not cover level %u", l.level_id); return SSB_E_STATE;
             }
         }
-        for (uint32_t j = 0; j < s.n; j++) {
-            if (s.src[j] != SORT_SRC_FACET) continue;
-            const uint32_t f = s.facet[j];
-            if (s.type[j] == SSB_FACET_STRING16 || s.type[j] == SSB_FACET_STRING32) {
-                if (!facets_->d_rank[f] || facets_->max_key[f] >= facets_->n_rank[f]) {
-                    set_error("search_lexical_sorted: String facet %u needs a value order covering its ids (ssb_set_facet_value_order)", f); return SSB_E_STATE;
-                }
-                s.rank[j] = facets_->d_rank[f];
-            }
-        }
-        s.zones = facets_->d_zones; s.zone_block0 = facets_->zone_block0; s.n_zone_blocks = facets_->n_zone_blocks;
     }
     *out = s;
     return SSB_OK;
 }
 
 int32_t LexIndex::stage_sort_bases(LexWorkspace& ws, cudaStream_t st, const double* bases, uint32_t nq, SortDev* sort) {
-    bool point = false;
-    for (uint32_t j = 0; j < sort->n; j++) point = point || (sort->src[j] == SORT_SRC_FACET && sort->type[j] == SSB_FACET_POINT);
-    if (!point || nq == 0) return SSB_OK;
+    if (!sort_has_point(*sort) || nq == 0) return SSB_OK;
     if (is_device_ptr(bases)) { set_error("search_lexical_sorted: bases must be a host array"); return SSB_E_INVALID; }
     if (nq > ws.cap_bases) {
         cudaFree(ws.bases); ws.bases = nullptr; ws.cap_bases = 0;
@@ -2349,42 +2075,9 @@ int32_t LexIndex::stage_filters(LexWorkspace& ws, cudaStream_t st, const ssb_lex
     for (uint32_t i = 0; i < nf; i++) {
         const ssb_facet_filter& f = q->filters[i];
         if (f.facet >= facets_->n_facets) { set_error("facet filter %u: facet %u of %u", i, f.facet, facets_->n_facets); return SSB_E_INVALID; }
-        const uint32_t type = facets_->types[f.facet];
-        FiltDev d{}; d.facet = f.facet;
-        if ((f.kind == SSB_FILTER_POINT) != (type == SSB_FACET_POINT)) { set_error("facet filter %u: a Point facet takes SSB_FILTER_POINT and only it", i); return SSB_E_INVALID; }
-        if (f.kind == SSB_FILTER_POINT) {
-            // FilterSparse::Point(base, start..end, unit, point_distance_to_morton_range(base, end, unit)) (search.rs:2712-2723)
-            if (f.set_count != 3) { set_error("facet filter %u: SSB_FILTER_POINT takes 3 filter_set_values (lat, lon, unit), not %u", i, f.set_count); return SSB_E_INVALID; }
-            if (!q->filter_set_values) { set_error("facet filter %u: null filter_set_values", i); return SSB_E_INVALID; }
-            const uint64_t* p = q->filter_set_values + f.set_first;
-            if (p[2] > SSB_UNIT_MILES) { set_error("facet filter %u: bad distance unit %llu", i, (unsigned long long)p[2]); return SSB_E_INVALID; }
-            double lat, lon, start, end; memcpy(&lat, &p[0], 8); memcpy(&lon, &p[1], 8); memcpy(&start, &f.start, 8); memcpy(&end, &f.end, 8);
-            const double r = earth_radius(p[2]);
-            const double lat_delta = end / (SSB_DEG2RAD * r);
-            const double lon_delta = end / (SSB_DEG2RAD * r * cos(SSB_DEG2RAD * lat));
-            d.lo = encode_morton_2d(lat - lat_delta, lon - lon_delta);
-            d.hi = encode_morton_2d(lat + lat_delta, lon + lon_delta);
-            // an empty interval (a box across latitude / longitude 0, a NaN anywhere) or a NaN start: no doc passes
-            d.kind = d.lo < d.hi && start == start ? FILT_POINT : FILT_NEVER;
-            *geo_any = *geo_any || d.kind == FILT_POINT;
-            d.set_first = (uint32_t)geo.size();                     // relative to the payloads; rebased behind the SET values below
-            uint64_t rb; memcpy(&rb, &r, 8);
-            for (uint64_t w : {p[0], p[1], f.start, f.end, rb}) geo.push_back(w);
-        } else if (f.kind == SSB_FILTER_RANGE) {
-            if (type == SSB_FACET_STRING16 || type == SSB_FACET_STRING32) { set_error("facet filter %u: a String facet takes SSB_FILTER_SET", i); return SSB_E_INVALID; }
-            d.kind = FILT_RANGE;
-            if (facet_is_float(type)) {
-                double a, b; memcpy(&a, &f.start, 8); memcpy(&b, &f.end, 8);
-                if (a != a || b != b) d.kind = FILT_NEVER; else { d.lo = key_of_f64(a); d.hi = key_of_f64(b); }
-            } else if (facet_is_signed(type)) { d.lo = f.start ^ 0x8000000000000000ull; d.hi = f.end ^ 0x8000000000000000ull; }
-            else { d.lo = f.start; d.hi = f.end; }
-        } else if (f.kind == SSB_FILTER_SET) {
-            if (type != SSB_FACET_STRING16 && type != SSB_FACET_STRING32) { set_error("facet filter %u: SSB_FILTER_SET needs a String16 / String32 facet", i); return SSB_E_INVALID; }
-            if (f.set_count && !q->filter_set_values) { set_error("facet filter %u: null filter_set_values", i); return SSB_E_INVALID; }
-            d.kind = FILT_SET; d.set_first = f.set_first; d.set_n = f.set_count;
-            if ((uint64_t)f.set_first + f.set_count > n_sets) n_sets = f.set_first + f.set_count;
-        } else { set_error("facet filter %u: bad kind %u", i, f.kind); return SSB_E_INVALID; }
-        fd[i] = d;
+        SSB_TRY(encode_filter(f, i, facets_->types[f.facet], q->filter_set_values, &fd[i], geo));
+        *geo_any = *geo_any || fd[i].kind == FILT_POINT;
+        if (f.kind == SSB_FILTER_SET && (uint64_t)f.set_first + f.set_count > n_sets) n_sets = f.set_first + f.set_count;
     }
     for (uint32_t i = 0; i < nf; i++) if (q->filters[i].kind == SSB_FILTER_POINT) fd[i].set_first += n_sets;
     const uint32_t n_staged = n_sets + (uint32_t)geo.size();
@@ -2439,7 +2132,7 @@ int32_t LexIndex::search_keys(LexWorkspace& ws, cudaStream_t st, const ssb_lex_b
     LexView v = view();
     bool filtered = false, geo = false;
     if (q->filter_offsets) SSB_TRY(stage_filters(ws, st, q, v, &filtered, &geo));
-    for (uint32_t j = 0; sort && j < sort->n; j++) geo = geo || (sort->src[j] == SORT_SRC_FACET && sort->type[j] == SSB_FACET_POINT);
+    geo = geo || (sort && sort_has_point(*sort));
     // a batch with a POINT filter plans without flag bit 1: EVERY filtered query of that batch (its range / set filters too) leaves the
     // lex_score record path for lex_generic<.., GEO>, so that lex_score keeps its code and registers; unfiltered queries stay on it
     const uint32_t topk_flag = result_type == SSB_RESULT_TOPK && !geo ? 2u : 0u;

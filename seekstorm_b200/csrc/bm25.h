@@ -5,6 +5,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "facets.h"
 
 namespace ssb {
 
@@ -68,14 +69,6 @@ struct LexLevel {
 struct BmSec { uint64_t w[2]; uint32_t meta[2]; uint32_t pad[2]; };
 static_assert(sizeof(BmSec) == 32, "BmSec must be one 32-byte sector");
 
-// One facet filter of one query, bounds already in key space (FilterSparse, search.rs:863-881): RANGE lo <= key < hi;
-// SET key in filt_sets[set_first .. +set_n); NEVER rejects every doc (a NaN bound: Range::contains is false for every value);
-// POINT: lo <= Morton code < hi, then the distance test with the staged geo payload filt_sets[set_first .. +GEO_WORDS)
-enum { FILT_RANGE = 0, FILT_SET = 1, FILT_NEVER = 2, FILT_POINT = 3 };
-// payload of a POINT filter in filt_sets, as f64 bits: base lat, base lon, distance start, distance end, earth radius of the unit
-enum { GEO_LAT = 0, GEO_LON = 1, GEO_START = 2, GEO_END = 3, GEO_RADIUS = 4, GEO_WORDS = 5 };
-struct FiltDev { uint32_t facet, kind; uint64_t lo, hi; uint32_t set_first, set_n; };
-
 // device view handed to the kernels (all pointers device)
 struct LexView {
     const uint64_t* dict_keys; uint32_t n_terms;
@@ -122,34 +115,6 @@ struct LexView {
     // per batch (filled by search_keys): the queries' facet filters, QueryPlan.filt_first / n_filt index into them
     const FiltDev* filt;
     const uint64_t* filt_sets;
-};
-
-// device-resident facet columns of an index (api.cu owns it, the lexical view borrows it)
-// zones: per facet and 65536-doc block of doc ids (block b = doc ids (zone_block0 + b) << 16 ..), the min and the max key of the block's rows
-// — the column key, or for a String facet with a value order the rank of the id; sorted searches bound a level's sort key with them.
-// rank / n_rank: the value order of a String facet (ssb_set_facet_value_order); max_key: the largest column key (host copy)
-struct FacetSet {
-    uint64_t* d_keys = nullptr; uint64_t n_rows = 0; uint32_t first_doc = 0; uint32_t n_facets = 0; uint8_t types[16] = {0};
-    uint64_t* d_zones = nullptr; uint32_t zone_block0 = 0, n_zone_blocks = 0;   // [n_facets][n_zone_blocks][2] {min, max}
-    uint32_t* d_rank[16] = {}; uint32_t n_rank[16] = {}; uint64_t max_key[16] = {};
-    void release() {
-        cudaFree(d_keys); d_keys = nullptr; n_rows = 0; n_facets = 0;
-        cudaFree(d_zones); d_zones = nullptr; n_zone_blocks = 0;
-        for (int f = 0; f < 16; f++) { cudaFree(d_rank[f]); d_rank[f] = nullptr; n_rank[f] = 0; }
-    }
-};
-// per-block min / max of facet f's column (through its value order when it has one) -> d_zones; asynchronous on st
-int32_t facet_zones(FacetSet& fs, uint32_t f, cudaStream_t st);
-
-// The sort of one sorted batch (ssb_search_lexical_sorted), validated and reduced by LexIndex::prepare_sort.  Criteria 0..n-1 are the
-// facet / _id criteria that make up the packed key `hi` (sort_pack_hi in bm25.cu); a `_score` criterion ends the list and only sets score_asc.
-enum { SORT_SRC_FACET = 0, SORT_SRC_ID = 1 };
-struct SortDev {
-    uint32_t n; uint32_t score_asc;                    // score_asc: `_score` ascending — the score half of the 128-bit top-k key is inverted
-    uint32_t src[4], facet[4], type[4], desc[4];      // per criterion (type: SSB_FACET_* of a facet criterion)
-    const uint32_t* rank[4];                           // String facets: rank_of_id (ssb_set_facet_value_order), else null
-    const uint64_t* zones; uint32_t zone_block0, n_zone_blocks;   // FacetSet zones (level bounds)
-    const double* bases;                               // a POINT criterion: [n_queries][2] per-query base (lat, lon), staged by stage_sort_bases
 };
 
 // device-resident delete set shared by the lexical and the vector path
@@ -226,8 +191,7 @@ public:
     int32_t search_keys(LexWorkspace& ws, cudaStream_t st, const ssb_lex_batch* q, uint32_t k, uint32_t result_type,
                         uint64_t* keys_out_dev, uint64_t* count_dev, uint64_t* launches, const uint64_t* ceil_dev = nullptr,
                         const SortDev* sort = nullptr) const;
-    // validates ssb_search_lexical_sorted's criteria against the facets and the levels; *sorted = false: they reduce to "_score desc".
-    // has_bases: the call carries POINT bases (else a POINT criterion is dropped)
+    // sort_of_criteria against the index's facets, then the check that the facet rows cover every level
     int32_t prepare_sort(const ssb_sort_criterion* crit, uint32_t n, bool has_bases, SortDev* out, bool* sorted) const;
     // a sort with a POINT criterion: copy the host bases [nq][2] into the workspace and point sort->bases at them
     static int32_t stage_sort_bases(LexWorkspace& ws, cudaStream_t st, const double* bases, uint32_t nq, SortDev* sort);
@@ -270,10 +234,6 @@ private:
     void free_committed();
     LexView view() const;
 };
-
-// facet value (as stored in the reference's facet file) -> order-preserving key; byte width of a facet type (0 = unknown type)
-uint64_t facet_value_key(uint32_t type, const uint8_t* p);
-uint32_t facet_type_bytes(uint32_t type);
 
 // loader.cu: the reference's on-disk files -> index
 struct VectorLevel { uint32_t level_id; std::vector<uint16_t> ids; std::vector<float> rows; std::vector<uint32_t> cluster_counts; };
