@@ -316,6 +316,45 @@ int32_t ssb_search_lexical_sorted(ssb_index* ix, const ssb_lex_batch* q, const s
 int32_t ssb_search_lexical_sorted_ex(ssb_index* ix, const ssb_lex_batch* q, const ssb_sort_criterion* sort, uint32_t n_sort,
                                      const double* bases, uint32_t k, uint32_t result_type, ssb_hit* hits, uint32_t* n_hits,
                                      uint64_t* count_total);
+/* Facet counts of a lexical batch (`query_facets` of Search::search, QueryFacet search.rs:234-…, facet_count add_result.rs:487-640): per
+ * query and request, how many of the query's matches fall on each value (VALUES) or into each range (RANGES).  The docs counted are
+ * exactly those result_count_total counts under Count / TopkCount for the same batch (delete set, NOT terms, facet filters, field filter
+ * and phrase check applied).  The call computes the counts only: a caller runs it next to whichever search it makes on the batch.
+ * One request set for the whole batch (as one sort is); a RANGES request on a POINT facet reads one base per query.
+ *   VALUES (String16 / String32 facets): the `length` value ids with the most matches, count descending, then id ascending (the reference
+ *     orders ties by hash-map arrival); ids with count 0 are left out.  has_prefix: only ids whose rank in the facet's value order
+ *     (ssb_set_facet_value_order, else SSB_E_STATE) lies in [rank_lo, rank_hi) — the ids whose string starts with a prefix form one such
+ *     interval.  length = 0: the facet is not collected (n_out 0).  length <= SSB_MAX_FACET_LENGTH.
+ *   RANGES (numeric, Timestamp, F32 / F64 facets; POINT facets by the distance to the query's base in `unit`): bin i holds the docs whose
+ *     value v has range_starts[i] <= v < range_starts[i + 1] (the last range is open above): the reference's binary search over the
+ *     starts.  range_starts: n_ranges strictly ascending starts widened like SSB_FILTER_RANGE bounds (unsigned as u64, signed and
+ *     Timestamp as i64, F32 / F64 and POINT distances as f64 bits); a NaN start or a list that does not ascend is SSB_E_INVALID.  All
+ *     n_ranges raw counts are written, zeros included; RangeType (CountAboveRange / CountBelowRange), labels and the label prefix belong
+ *     to the caller.  A value below the first start, a NaN value or distance and a doc without a facet row are not counted (the
+ *     reference panics or reads out of bounds on them).
+ * Counts are over every match: the reference counts only the docs it visits under Topk pruning and, for multi-term Union queries, only
+ * the docs of blocks with one valid term.  out: HOST [n_queries][sum of caps], cap = length (VALUES) or n_ranges (RANGES), requests in
+ * order; n_out: HOST [n_queries][n_req] entries written per request.  bases: HOST [n_queries][number of POINT requests][2] (lat, lon), or
+ * NULL when no request is on a POINT facet.  The value histograms take n_queries x (sum over VALUES requests of the facet's largest id
+ * + 1) x 4 bytes; the batch runs in query chunks within a 256 MiB workspace per search context (one query above it: SSB_E_UNSUPPORTED).
+ * Not on a handle with a communicator (SSB_E_UNSUPPORTED). */
+enum { SSB_FACET_COUNT_VALUES = 0, SSB_FACET_COUNT_RANGES = 1 };
+#define SSB_MAX_FACET_RANGES 256u
+#define SSB_MAX_FACET_LENGTH 1024u
+#define SSB_MAX_FACET_REQUESTS 16u
+typedef struct {
+    uint32_t facet;                  /* index into ssb_set_facets' fields                                                */
+    uint32_t kind;                   /* SSB_FACET_COUNT_*                                                                */
+    uint32_t length;                 /* VALUES: at most this many (id, count); 0 = not collected                         */
+    uint32_t has_prefix;             /* VALUES: restrict to value-order ranks in [rank_lo, rank_hi)                      */
+    uint32_t rank_lo, rank_hi;
+    uint32_t n_ranges;               /* RANGES: 1 .. SSB_MAX_FACET_RANGES                                                */
+    uint32_t unit;                   /* RANGES on a POINT facet: SSB_UNIT_*                                              */
+    const uint64_t* range_starts;    /* RANGES: HOST [n_ranges]                                                          */
+} ssb_facet_request;
+typedef struct { uint32_t value; uint32_t pad; uint64_t count; } ssb_facet_count;   /* value: id (VALUES) or range index (RANGES) */
+int32_t ssb_search_lexical_facets(ssb_index* ix, const ssb_lex_batch* q, const ssb_facet_request* req, uint32_t n_req,
+                                  const double* bases, ssb_facet_count* out, uint32_t* n_out);
 /* queries: [n_queries, dims] f32; Cosine: normalised by the callee (search.rs:1464-1475).  score = dot
  * (Dot/Cosine) or -Σ(q-x)² (Euclidean) exactly as Result.score in vector.rs:1489. */
 int32_t ssb_search_vector(ssb_index* ix, const float* queries, uint32_t n_queries, uint32_t k,

@@ -150,6 +150,25 @@ public:
     void set_field_names(std::vector<std::string> names) { field_names_ = std::move(names); }
     // TurboQuantI8 indexes: the index's +-1 sign mask (TurboQuant.seed_mask)
     void set_turboquant_mask(const std::vector<float>& seed_mask) { check(ssb_vector_set_turboquant_mask(h_, seed_mask.data(), static_cast<uint32_t>(seed_mask.size()))); }
+    // facet counts of a lexical batch (query_facets; ssb_search_lexical_facets), to run next to the batch's search: per query and request,
+    // in request order, the (value, count) entries the call wrote.  bases: [n_queries][number of POINT requests][2] (lat, lon), or empty.
+    std::vector<std::vector<std::vector<ssb_facet_count>>> facet_counts(const ssb_lex_batch& batch, const std::vector<ssb_facet_request>& req,
+                                                                        const std::vector<double>& bases = {}) const {
+        std::vector<size_t> cap(req.size());
+        size_t stride = 0;
+        for (size_t r = 0; r < req.size(); r++) stride += cap[r] = req[r].kind == SSB_FACET_COUNT_VALUES ? req[r].length : req[r].n_ranges;
+        const size_t nq = batch.n_queries;
+        std::vector<ssb_facet_count> out(nq * stride + 1);
+        std::vector<uint32_t> n_out(nq * req.size() + 1);
+        check(ssb_search_lexical_facets(h_, &batch, req.data(), static_cast<uint32_t>(req.size()), bases.empty() ? nullptr : bases.data(),
+                                        out.data(), n_out.data()));
+        std::vector<std::vector<std::vector<ssb_facet_count>>> res(nq, std::vector<std::vector<ssb_facet_count>>(req.size()));
+        for (size_t q = 0; q < nq; q++) {
+            const ssb_facet_count* p = out.data() + q * stride;
+            for (size_t r = 0; r < req.size(); r++) { res[q][r].assign(p, p + n_out[q * req.size() + r]); p += cap[r]; }
+        }
+        return res;
+    }
     uint64_t indexed_doc_count() const { return indexed_doc_count_; }
     uint64_t vector_count() const { uint64_t n = 0; check(ssb_vector_count(h_, &n)); return n; }
 

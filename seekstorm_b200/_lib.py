@@ -80,6 +80,21 @@ class SsbSortCriterion(C.Structure):
     _fields_ = [("source", C.c_uint32), ("facet", C.c_uint32), ("order", C.c_uint32), ("pad", C.c_uint32)]
 
 
+class SsbFacetRequest(C.Structure):
+    _fields_ = [("facet", C.c_uint32), ("kind", C.c_uint32), ("length", C.c_uint32), ("has_prefix", C.c_uint32),
+                ("rank_lo", C.c_uint32), ("rank_hi", C.c_uint32), ("n_ranges", C.c_uint32), ("unit", C.c_uint32),
+                ("range_starts", C.c_void_p)]
+
+
+class SsbFacetCount(C.Structure):
+    _fields_ = [("value", C.c_uint32), ("pad", C.c_uint32), ("count", C.c_uint64)]
+
+
+# SSB_FACET_COUNT_* (kind of a facet request) and the request limits
+FACET_COUNT_VALUES, FACET_COUNT_RANGES = 0, 1
+MAX_FACET_RANGES, MAX_FACET_LENGTH, MAX_FACET_REQUESTS = 256, 1024, 16
+
+
 # SSB_SORT_* (source of a sort criterion) and SSB_SORT_ASCENDING / DESCENDING
 SORT_FACET, SORT_ID, SORT_SCORE = 0, 1, 2
 SORT_ASCENDING, SORT_DESCENDING = 0, 1
@@ -96,7 +111,7 @@ class SsbStats(C.Structure):
 EXPORTS = [
     "ssb_abi_version", "ssb_last_error", "ssb_create", "ssb_destroy", "ssb_lexical_add_level",
     "ssb_vector_add_level_clustered", "ssb_lexical_set_field_boosts", "ssb_lexical_commit", "ssb_lexical_dict_size", "ssb_lexical_dict_export", "ssb_lexical_set_global_df",
-    "ssb_load_index_bin", "ssb_load_vector_bin", "ssb_index_bin_inspect", "ssb_set_deleted", "ssb_set_facets", "ssb_set_facet_value_order", "ssb_vector_set_turboquant_mask", "ssb_vector_add_level", "ssb_vector_count", "ssb_vector_reserve", "ssb_set_vector_kernel", "ssb_search_lexical", "ssb_search_lexical_sorted", "ssb_search_lexical_sorted_ex", "ssb_search_vector", "ssb_search_vector_ex", "ssb_search_hybrid",
+    "ssb_load_index_bin", "ssb_load_vector_bin", "ssb_index_bin_inspect", "ssb_set_deleted", "ssb_set_facets", "ssb_set_facet_value_order", "ssb_vector_set_turboquant_mask", "ssb_vector_add_level", "ssb_vector_count", "ssb_vector_reserve", "ssb_set_vector_kernel", "ssb_search_lexical", "ssb_search_lexical_sorted", "ssb_search_lexical_sorted_ex", "ssb_search_lexical_facets", "ssb_search_vector", "ssb_search_vector_ex", "ssb_search_hybrid",
     "ssb_rrf_fuse", "ssb_comm_unique_id", "ssb_comm_init", "ssb_comm_attach", "ssb_comm_destroy", "ssb_lexical_sync_df",
     "ssb_search_vector_keys", "ssb_search_lexical_keys", "ssb_merge_keys", "ssb_sync",
     "ssb_stream", "ssb_set_stream", "ssb_last_stats",
@@ -144,6 +159,7 @@ def lib():
         "ssb_search_lexical": [vp, C.POINTER(SsbLexBatch), u32, u32, vp, vp, vp],
         "ssb_search_lexical_sorted": [vp, C.POINTER(SsbLexBatch), vp, u32, u32, u32, vp, vp, vp],
         "ssb_search_lexical_sorted_ex": [vp, C.POINTER(SsbLexBatch), vp, u32, vp, u32, u32, vp, vp, vp],
+        "ssb_search_lexical_facets": [vp, C.POINTER(SsbLexBatch), vp, u32, vp, vp, vp],
         "ssb_search_vector": [vp, vp, u32, u32, vp, vp],
         "ssb_search_vector_ex": [vp, C.POINTER(SsbVecQuery), vp, vp, vp, vp],
         "ssb_search_hybrid": [vp, C.POINTER(SsbLexBatch), vp, u32, vp, vp],

@@ -1064,6 +1064,21 @@ int32_t ssb_search_lexical_sorted_ex(ssb_index* ix, const ssb_lex_batch* q, cons
     SSB_API_END
 }
 
+// query_facets of Search::search (facet_count, add_result.rs:487-640): the facet counts of a lexical batch, next to its search
+int32_t ssb_search_lexical_facets(ssb_index* ix, const ssb_lex_batch* q, const ssb_facet_request* req, uint32_t n_req,
+                                  const double* bases, ssb_facet_count* out, uint32_t* n_out) {
+    SSB_API_BEGIN
+    if (!ix || !q) { set_error("ssb_search_lexical_facets: null argument"); return SSB_E_INVALID; }
+    std::shared_lock<std::shared_mutex> g(ix->rw);
+    SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
+    if (ix->comm.active()) { set_error("ssb_search_lexical_facets: facet counts across shards are not built"); return SSB_E_UNSUPPORTED; }
+    CtxLease l(ix); SSB_TRY(l.acquire());
+    SearchCtx& c = *l.c;
+    return ix->lex->facet_counts(c.lex, c.st, q, req, n_req, bases, out, n_out, &c.stats.kernel_launches, &c.stats.dominant_kernel_ns,
+                                 &c.stats.algorithmic_bytes);
+    SSB_API_END
+}
+
 int32_t ssb_rrf_fuse(const ssb_hit* lex, uint32_t n_lex, const ssb_hit* vec, uint32_t n_vec, ssb_hit* out, uint32_t* n_out) {
     SSB_API_BEGIN
     // search.rs:1962-2035: k = 0.6, rank from 0 over each list sorted by score desc; then :2097-2106 sort desc.

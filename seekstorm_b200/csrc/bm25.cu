@@ -37,6 +37,7 @@
 #include "bm25.h"
 #include "facets.cuh"
 
+#include <algorithm>
 #include <cuda_fp16.h>
 #include <math.h>
 #include <stdlib.h>
@@ -1654,6 +1655,252 @@ __global__ void copy_out(const uint64_t* __restrict__ glist, const uint64_t* __r
     if (count_out && i < nq) count_out[i] = count[i];
 }
 
+// ================================================================= facet counts (ssb_search_lexical_facets; facet_count, add_result.rs:487-640)
+// A pass of its own after lex_plan<false> (Count): every scoring and counting kernel above keeps its code.  One warp per (query, record):
+// the level's matches as a bitmap of its 65536 doc ids in shared memory (as CountSm), then the set bits in doc order through the same
+// predicates the count path runs, then one bin per doc and request.  Range bins go to a warp-private shared histogram flushed with one
+// global atomic per nonzero bin at the end of the record; value bins (ids) go to the query's dense histogram in global memory.
+constexpr uint32_t FACET_WARPS = 4;
+struct FacetCall {
+    const FacetReqDev* req; uint32_t n_req;
+    const uint64_t* starts; uint32_t n_starts;      // RANGES / POINT starts in key space
+    const double* bases; uint32_t n_point;          // [n_queries][n_point][2]
+    uint32_t* hist; uint32_t hist_words, range_words;   // [chunk][hist_words]: the range bins first, then the value bins
+    uint64_t* stats;                                // {postings read, dense words read, counted docs}
+};
+struct FacetWarpSm { uint32_t bm[2048]; uint16_t list[1024]; };
+
+template <bool FIELD_RUNS, bool GEO>
+__global__ void __launch_bounds__(FACET_WARPS * 32) lex_facets(LexView v, const QueryPlan* __restrict__ plans, const LvRec* __restrict__ recs,
+                                                                uint32_t q0, uint32_t nqc, uint32_t query_type, FacetCall fc) {
+    extern __shared__ __align__(16) uint8_t fsm_raw[];
+    uint64_t* sstart = reinterpret_cast<uint64_t*>(fsm_raw);                                   // [n_starts]
+    FacetReqDev* sreq = reinterpret_cast<FacetReqDev*>(sstart + fc.n_starts);                  // [n_req]
+    FacetWarpSm* wsm = reinterpret_cast<FacetWarpSm*>(sreq + fc.n_req);                        // [FACET_WARPS]
+    uint32_t* rhist_all = reinterpret_cast<uint32_t*>(wsm + FACET_WARPS);                      // [FACET_WARPS][range_words]
+    for (uint32_t i = threadIdx.x; i < fc.n_starts; i += blockDim.x) sstart[i] = fc.starts[i];
+    for (uint32_t i = threadIdx.x; i < fc.n_req; i += blockDim.x) sreq[i] = fc.req[i];
+    for (uint32_t i = threadIdx.x; i < FACET_WARPS * fc.range_words; i += blockDim.x) rhist_all[i] = 0;
+    __syncthreads();
+    const uint32_t wi = threadIdx.x >> 5;
+    const int lane = threadIdx.x & 31;
+    uint32_t* bm = wsm[wi].bm;
+    uint64_t* bm64 = reinterpret_cast<uint64_t*>(bm);
+    uint16_t* list = wsm[wi].list;
+    uint32_t* rhist = rhist_all + (size_t)wi * fc.range_words;
+    const uint32_t nlv = v.n_levels;
+    const bool is_and = query_type == SSB_QUERY_INTERSECTION;
+    uint64_t st_post = 0, st_words = 0, st_docs = 0;
+    const uint64_t n_warps = (uint64_t)gridDim.x * FACET_WARPS;
+    for (uint64_t it = (uint64_t)blockIdx.x * FACET_WARPS + wi; it < (uint64_t)nqc * nlv; it += n_warps) {
+        const uint32_t ql = (uint32_t)(it / nlv), j = (uint32_t)(it % nlv), q = q0 + ql;
+        const QueryPlan* pl = &plans[q];
+        if (j >= __ldg(&pl->n_recs)) continue;
+        const uint32_t lv = __ldg(&recs[(size_t)q * nlv + j].lv);
+        const uint32_t docbase = __ldg(&recs[(size_t)q * nlv + j].docbase);
+        const uint32_t n = __ldg(&pl->n_live);
+        // lane t: the list of query term t at this level (a record exists: OR some list, AND every list is there)
+        uint32_t cnt = 0, bmi = NONE; uint64_t off = 0;
+        if ((uint32_t)lane < n) {
+            uint32_t e;
+            if (find_entry(v, pl->t[lane], lv, e)) { cnt = __ldg(&v.e_count[e]); off = __ldg(&v.e_off[e]); bmi = __ldg(&v.e_bitmap[e]); }
+        }
+        // ---- 1. the match bitmap ----
+        if (!is_and) {
+            for (uint32_t i = lane; i < 2048u; i += 32u) bm[i] = 0u;
+            __syncwarp();
+            for (uint32_t t = 0; t < n; t++) {
+                const uint32_t tc = __shfl_sync(FULL, cnt, t), tb = __shfl_sync(FULL, bmi, t); const uint64_t to = shfl64(off, t);
+                if (tc == 0) continue;
+                if (tb != NONE) {
+                    for (uint32_t i = lane; i < 1024u; i += 32u) bm64[i] |= __ldg(&v.bm_words[(size_t)tb * 1024 + i]);
+                    st_words += 32;
+                } else {
+                    for_each_posting(v, to, tc, lane, [&](uint32_t d, bool valid) { if (valid) atomicOr(&bm[d >> 5], 1u << (d & 31u)); });
+                    st_post += tc;
+                }
+                __syncwarp();
+            }
+        } else {
+            // the shortest list drives; all lists dense (the shortest has a bitmap): word AND, else its postings probe the others
+            uint32_t key = (uint32_t)lane < n ? cnt : 0xFFFFFFFFu; int drv = lane;
+            for (int s = 16; s; s >>= 1) {
+                const uint32_t ok = __shfl_xor_sync(FULL, key, s); const int od = __shfl_xor_sync(FULL, drv, s);
+                if (ok < key || (ok == key && od < drv)) { key = ok; drv = od; }
+            }
+            const uint32_t dcnt = __shfl_sync(FULL, cnt, drv), dbmi = __shfl_sync(FULL, bmi, drv); const uint64_t doff = shfl64(off, drv);
+            if (dcnt == 0) continue;
+            if (dbmi != NONE) {
+                for (uint32_t i = lane; i < 1024u; i += 32u) {
+                    uint64_t a = ~0ull;
+                    for (uint32_t t = 0; t < n; t++) a &= __ldg(&v.bm_words[(size_t)__shfl_sync(FULL, bmi, t) * 1024 + i]);
+                    bm64[i] = a;
+                }
+                st_words += 32u * n;
+            } else {
+                for (uint32_t i = lane; i < 2048u; i += 32u) bm[i] = 0u;
+                __syncwarp();
+                for_each_posting(v, doff, dcnt, lane, [&](uint32_t d, bool valid) {
+                    bool ok = valid;
+                    for (uint32_t t = 0; t < n; t++) {
+                        const uint32_t tc = __shfl_sync(FULL, cnt, t), tb = __shfl_sync(FULL, bmi, t); const uint64_t to = shfl64(off, t);
+                        if ((int)t != drv && ok) ok = present_in(v, tc, to, tb, d);
+                    }
+                    if (ok) atomicOr(&bm[d >> 5], 1u << (d & 31u));
+                });
+                st_post += dcnt;
+            }
+        }
+        __syncwarp();
+        // NOT lists and the delete set clear their bits
+        const uint32_t n_not = __ldg(&pl->n_not);
+        for (uint32_t i = 0; i < n_not; i++) {
+            uint32_t e;
+            if (!find_entry(v, pl->tn[i], lv, e)) continue;
+            const uint32_t tc = __ldg(&v.e_count[e]), tb = __ldg(&v.e_bitmap[e]); const uint64_t to = __ldg(&v.e_off[e]);
+            if (tb != NONE) { for (uint32_t w = lane; w < 1024u; w += 32u) bm64[w] &= ~__ldg(&v.bm_words[(size_t)tb * 1024 + w]); st_words += 32; }
+            else { for_each_posting(v, to, tc, lane, [&](uint32_t d, bool valid) { if (valid) atomicAnd(&bm[d >> 5], ~(1u << (d & 31u))); }); st_post += tc; }
+            __syncwarp();
+        }
+        if (v.del_slot) {
+            const uint32_t slot = __ldg(&v.del_slot[docbase >> 16]);
+            if (slot != NONE) for (uint32_t w = lane; w < 1024u; w += 32u) bm64[w] &= ~__ldg(&v.del_words[(size_t)slot * 1024 + w]);
+            __syncwarp();
+        }
+        // ---- 2. the set bits in doc order, 1024 doc ids at a time: the per-doc predicates, then 3. the bins ----
+        const uint32_t nf = __ldg(&pl->n_filt), f0 = __ldg(&pl->filt_first), fmask = __ldg(&pl->field_mask), n_phr = __ldg(&pl->n_phr);
+        const bool filtered = nf || fmask || n_phr;
+        uint32_t* qhist = fc.hist + (size_t)ql * fc.hist_words;
+        for (uint32_t w0 = 0; w0 < 2048u; w0 += 32u) {
+            uint32_t word = bm[w0 + lane];
+            const uint32_t c = __popc(word);
+            uint32_t incl = c;
+            for (int s = 1; s < 32; s <<= 1) { const uint32_t y = __shfl_up_sync(FULL, incl, s); if (lane >= s) incl += y; }
+            const uint32_t total = __shfl_sync(FULL, incl, 31);
+            if (total == 0) continue;
+            uint32_t pos = incl - c;
+            while (word) { const uint32_t b = __ffs(word) - 1; word &= word - 1; list[pos++] = (uint16_t)(((w0 + lane) << 5) | b); }
+            __syncwarp();
+            for (uint32_t i0 = 0; i0 < total; i0 += 32u) {
+                const bool act = i0 + lane < total;
+                const uint32_t d = act ? list[i0 + lane] : 0u, doc = docbase | d;
+                bool ok = act;
+                if (filtered && ok) ok = !filters_reject<FIELD_RUNS, GEO>(v, pl, f0, nf, fmask, n, lv, d, doc);
+                const uint64_t row = (uint64_t)doc - v.facet_first_doc;
+                ok = ok && doc >= v.facet_first_doc && row < v.facet_rows;          // no facet row: not counted
+                const uint32_t n_ok = __popc(__ballot_sync(FULL, ok));
+                if (lane == 0) st_docs += n_ok;
+                for (uint32_t r = 0; r < fc.n_req; r++) {
+                    const FacetReqDev& R = sreq[r];
+                    if (R.kind == FREQ_VALUES && R.length == 0) continue;
+                    const uint64_t key = ok ? __ldg(&v.facet_keys[(size_t)R.facet * v.facet_rows + row]) : 0ull;
+                    if (R.kind == FREQ_VALUES) {                               // warp-aggregated: one atomic per distinct id
+                        const unsigned grp = __match_any_sync(FULL, ok ? key : ~0ull);
+                        if (ok && lane == __ffs(grp) - 1) atomicAdd(&qhist[R.hist_off + key], (uint32_t)__popc(grp));
+                        continue;
+                    }
+                    bool c2 = ok; uint64_t kk = key;
+                    if (R.kind == FREQ_POINT) {
+                        if (c2) {
+                            const double* b = fc.bases + ((size_t)q * fc.n_point + R.point_idx) * 2;
+                            const double dist = geo_distance(key, __ldg(&b[0]), __ldg(&b[1]), [&] { return R.radius; });
+                            c2 = dist == dist;                                   // a NaN distance is not counted
+                            kk = f64_order_key(dist);
+                        }
+                    } else if (R.is_float) c2 = c2 && key != ~0ull;             // NaN value
+                    uint32_t lo = 0, hi = R.n_bins;                              // the first start above the key
+                    while (lo < hi) { const uint32_t m = (lo + hi) >> 1; if (sstart[R.start_first + m] <= kk) lo = m + 1; else hi = m; }
+                    if (c2 && lo > 0) atomicAdd(&rhist[R.hist_off + lo - 1], 1u);
+                }
+            }
+            __syncwarp();
+        }
+        for (uint32_t i = lane; i < fc.range_words; i += 32u)
+            if (rhist[i]) { atomicAdd(&qhist[i], rhist[i]); rhist[i] = 0; }
+        __syncwarp();
+    }
+    if (lane == 0) {
+        atomicAdd((unsigned long long*)&fc.stats[0], (unsigned long long)st_post);
+        atomicAdd((unsigned long long*)&fc.stats[1], (unsigned long long)st_words);
+        atomicAdd((unsigned long long*)&fc.stats[2], (unsigned long long)st_docs);
+    }
+}
+
+// One CTA per (query of the chunk, request).  RANGES: the bins as they are.  VALUES: the `length` ids with count > 0 (and, with a prefix,
+// a value-order rank in [rank_lo, rank_hi)) of largest key (count << 32 | ~id): count descending, id ascending.  A radix select over the
+// keys' bytes finds the length-th largest key, the ids at or above it are sorted in shared memory.  Deterministic.
+struct RankPtrs { const uint32_t* p[SSB_MAX_FACETS]; };
+__global__ void __launch_bounds__(256) facet_select(const FacetReqDev* __restrict__ req, uint32_t n_req, const uint32_t* __restrict__ hist,
+                                                    uint32_t hist_words, RankPtrs rank, ssb_facet_count* out, uint32_t out_stride, uint32_t* n_out) {
+    __shared__ uint32_t h[256];
+    __shared__ uint64_t sel[SSB_MAX_FACET_LENGTH];
+    __shared__ uint64_t s_prefix; __shared__ uint32_t s_need, s_all, s_n;
+    const uint32_t r = blockIdx.x, ql = blockIdx.y;
+    const FacetReqDev R = req[r];
+    const uint32_t* qh = hist + (size_t)ql * hist_words + R.hist_off;
+    ssb_facet_count* o = out + (size_t)ql * out_stride + R.out_off;
+    if (R.kind != FREQ_VALUES) {
+        for (uint32_t i = threadIdx.x; i < R.n_bins; i += blockDim.x) { ssb_facet_count c; c.value = i; c.pad = 0; c.count = qh[i]; o[i] = c; }
+        if (threadIdx.x == 0) n_out[(size_t)ql * n_req + r] = R.n_bins;
+        return;
+    }
+    if (R.length == 0) { if (threadIdx.x == 0) n_out[(size_t)ql * n_req + r] = 0; return; }
+    const uint32_t* rk = rank.p[R.facet];
+    auto key_of = [&](uint32_t id) -> uint64_t {                      // 0 = not eligible
+        const uint32_t c = qh[id];
+        if (c == 0) return 0ull;
+        if (R.has_prefix) { const uint32_t x = __ldg(&rk[id]); if (x < R.rank_lo || x >= R.rank_hi) return 0ull; }
+        return ((uint64_t)c << 32) | (0xFFFFFFFFu - id);
+    };
+    if (threadIdx.x == 0) { s_prefix = 0; s_need = R.length; s_all = 0; s_n = 0; }
+    for (int shift = 56; shift >= 0; shift -= 8) {
+        for (uint32_t i = threadIdx.x; i < 256; i += blockDim.x) h[i] = 0;
+        __syncthreads();
+        const uint64_t pre = s_prefix;
+        for (uint32_t id = threadIdx.x; id < R.n_bins; id += blockDim.x) {
+            const uint64_t k = key_of(id);
+            if (k && (shift == 56 || (k >> (shift + 8)) == (pre >> (shift + 8)))) atomicAdd(&h[(k >> shift) & 255u], 1u);
+        }
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            if (shift == 56) { uint32_t tot = 0; for (int b = 0; b < 256; b++) tot += h[b]; if (tot <= s_need) s_all = 1; }
+            if (!s_all) {
+                uint32_t acc = 0;
+                for (int b = 255; b >= 0; b--) {
+                    if (acc + h[b] >= s_need) { s_prefix |= (uint64_t)b << shift; s_need -= acc; break; }
+                    acc += h[b];
+                }
+            }
+        }
+        __syncthreads();
+        if (s_all) break;
+    }
+    const uint64_t thr = s_all ? 1ull : s_prefix;                    // the smallest key taken
+    for (uint32_t id = threadIdx.x; id < R.n_bins; id += blockDim.x) {
+        const uint64_t k = key_of(id);
+        if (k && k >= thr) sel[atomicAdd(&s_n, 1u)] = k;
+    }
+    __syncthreads();
+    const uint32_t m = s_n;
+    uint32_t p2 = 1; while (p2 < m) p2 <<= 1;
+    for (uint32_t i = m + threadIdx.x; i < p2; i += blockDim.x) sel[i] = 0;
+    __syncthreads();
+    for (uint32_t size = 2; size <= p2; size <<= 1)                  // bitonic sort, descending
+        for (uint32_t stride = size >> 1; stride > 0; stride >>= 1) {
+            for (uint32_t i = threadIdx.x; i < p2 / 2; i += blockDim.x) {
+                const uint32_t lo = 2 * i - (i & (stride - 1)), hi = lo + stride;
+                const bool desc = (lo & size) == 0;
+                const uint64_t a = sel[lo], b = sel[hi];
+                if (desc ? (a < b) : (a > b)) { sel[lo] = b; sel[hi] = a; }
+            }
+            __syncthreads();
+        }
+    for (uint32_t i = threadIdx.x; i < m; i += blockDim.x) {
+        ssb_facet_count c; c.value = 0xFFFFFFFFu - (uint32_t)sel[i]; c.pad = 0; c.count = sel[i] >> 32; o[i] = c;
+    }
+    if (threadIdx.x == 0) n_out[(size_t)ql * n_req + r] = m;
+}
+
 // ================================================================= host side
 LexIndex::~LexIndex() {
     for (auto& l : levels_) { cudaFree(l.d_term_keys); cudaFree(l.d_posting_offsets); }
@@ -1678,6 +1925,11 @@ void LexWorkspace::release() {
     cudaFree(theta2); theta2 = nullptr;
     qflags = nullptr; plans = nullptr; recs = nullptr; item_start = nullptr; theta = nullptr; lock = nullptr; count = nullptr; ctr = nullptr;
     qoff = nullptr; qkeys = nullptr; stats = nullptr; cap_q = cap_terms = cap_levels = 0;
+}
+void LexWorkspace::release_facets() {
+    cudaFree(fhist); cudaFree(freq); cudaFree(fstarts); cudaFree(fstats); cudaFree(fbases); cudaFree(fout); cudaFree(fnout); cudaFree(fglist);
+    fhist = nullptr; freq = nullptr; fstarts = nullptr; fstats = nullptr; fbases = nullptr; fout = nullptr; fnout = nullptr; fglist = nullptr;
+    cap_fbases = cap_fout = cap_fnout = 0; cap_fglist = 0;
 }
 
 static uint32_t env_u32(const char* name, uint32_t dflt, uint32_t lo, uint32_t hi) {
@@ -2094,19 +2346,9 @@ int32_t LexIndex::stage_filters(LexWorkspace& ws, cudaStream_t st, const ssb_lex
     return SSB_OK;
 }
 
-int32_t LexIndex::search_keys(LexWorkspace& ws, cudaStream_t st, const ssb_lex_batch* q, uint32_t k, uint32_t result_type,
-                              uint64_t* keys_out_dev, uint64_t* count_dev, uint64_t* launches, const uint64_t* ceil_dev, const SortDev* sort) const {
-    if (!committed_) { set_error("search before ssb_lexical_commit"); return SSB_E_STATE; }
-    if (!q || (q->n_queries && (!q->term_offsets || !keys_out_dev))) { set_error("search_lexical: null argument"); return SSB_E_INVALID; }
-    if (k > SSB_K_MAX) { set_error("k=%u exceeds SSB_K_MAX=%u", k, SSB_K_MAX); return SSB_E_UNSUPPORTED; }
-    if (result_type > SSB_RESULT_TOPKCOUNT || q->query_type > SSB_QUERY_PHRASE) { set_error("bad result_type/query_type"); return SSB_E_INVALID; }
-    const uint32_t phrase = q->query_type == SSB_QUERY_PHRASE ? 1u : 0u;
-    if (phrase && has_positions_ != 1) { set_error("phrase query: the index holds no term positions (ssb_level_desc.positions)"); return SSB_E_STATE; }
-    if (phrase && q->term_flags) { set_error("phrase query: NOT terms are not accepted inside a phrase batch"); return SSB_E_UNSUPPORTED; }
-    const uint32_t qt_eff = phrase ? (uint32_t)SSB_QUERY_INTERSECTION : q->query_type;   // a phrase is an intersection + the position check
-    if (result_type != SSB_RESULT_COUNT && k == 0) result_type = SSB_RESULT_COUNT;   // search.rs:2472-2478
+int32_t LexIndex::stage_batch(LexWorkspace& ws, cudaStream_t st, const ssb_lex_batch* q, LexView& v, bool* filtered, bool* geo,
+                              const uint32_t** fmask_dev) const {
     const uint32_t nq = q->n_queries;
-    if (nq == 0) return SSB_OK;
     uint32_t total_terms = 0;
     const bool off_dev = is_device_ptr(q->term_offsets);
     if (off_dev) SSB_CUDA_TRY(cudaMemcpy(&total_terms, q->term_offsets + nq, 4, cudaMemcpyDeviceToHost));
@@ -2129,20 +2371,39 @@ int32_t LexIndex::search_keys(LexWorkspace& ws, cudaStream_t st, const ssb_lex_b
     SSB_CUDA_TRY(to_device(ws.qoff, q->term_offsets, ((size_t)nq + 1) * 4, st));
     SSB_CUDA_TRY(to_device(ws.qkeys, q->term_keys, (size_t)total_terms * 8, st));
     if (q->term_flags) SSB_CUDA_TRY(to_device(ws.qflags, q->term_flags, (size_t)total_terms, st));
-    LexView v = view();
-    bool filtered = false, geo = false;
-    if (q->filter_offsets) SSB_TRY(stage_filters(ws, st, q, v, &filtered, &geo));
-    geo = geo || (sort && sort_has_point(*sort));
-    // a batch with a POINT filter plans without flag bit 1: EVERY filtered query of that batch (its range / set filters too) leaves the
-    // lex_score record path for lex_generic<.., GEO>, so that lex_score keeps its code and registers; unfiltered queries stay on it
-    const uint32_t topk_flag = result_type == SSB_RESULT_TOPK && !geo ? 2u : 0u;
-    const uint32_t* fmask_dev = nullptr;
+    v = view();
+    *filtered = false; *geo = false; *fmask_dev = nullptr;
+    if (q->filter_offsets) SSB_TRY(stage_filters(ws, st, q, v, filtered, geo));
     if (q->field_masks && n_fields_ > 1) {                   // field_filter: one bitmask of indexed fields per query (host array)
         if (is_device_ptr(q->field_masks)) { set_error("search_lexical: field_masks must be a host array"); return SSB_E_INVALID; }
         if (!ws.fmask) SSB_CUDA_TRY(cudaMalloc(&ws.fmask, (size_t)ws.cap_q * 4));
         SSB_CUDA_TRY(cudaMemcpyAsync(ws.fmask, q->field_masks, (size_t)nq * 4, cudaMemcpyHostToDevice, st));
-        fmask_dev = ws.fmask;
+        *fmask_dev = ws.fmask;
     }
+    return SSB_OK;
+}
+
+int32_t LexIndex::search_keys(LexWorkspace& ws, cudaStream_t st, const ssb_lex_batch* q, uint32_t k, uint32_t result_type,
+                              uint64_t* keys_out_dev, uint64_t* count_dev, uint64_t* launches, const uint64_t* ceil_dev, const SortDev* sort) const {
+    if (!committed_) { set_error("search before ssb_lexical_commit"); return SSB_E_STATE; }
+    if (!q || (q->n_queries && (!q->term_offsets || !keys_out_dev))) { set_error("search_lexical: null argument"); return SSB_E_INVALID; }
+    if (k > SSB_K_MAX) { set_error("k=%u exceeds SSB_K_MAX=%u", k, SSB_K_MAX); return SSB_E_UNSUPPORTED; }
+    if (result_type > SSB_RESULT_TOPKCOUNT || q->query_type > SSB_QUERY_PHRASE) { set_error("bad result_type/query_type"); return SSB_E_INVALID; }
+    const uint32_t phrase = q->query_type == SSB_QUERY_PHRASE ? 1u : 0u;
+    if (phrase && has_positions_ != 1) { set_error("phrase query: the index holds no term positions (ssb_level_desc.positions)"); return SSB_E_STATE; }
+    if (phrase && q->term_flags) { set_error("phrase query: NOT terms are not accepted inside a phrase batch"); return SSB_E_UNSUPPORTED; }
+    const uint32_t qt_eff = phrase ? (uint32_t)SSB_QUERY_INTERSECTION : q->query_type;   // a phrase is an intersection + the position check
+    if (result_type != SSB_RESULT_COUNT && k == 0) result_type = SSB_RESULT_COUNT;   // search.rs:2472-2478
+    const uint32_t nq = q->n_queries;
+    if (nq == 0) return SSB_OK;
+    LexView v;
+    bool filtered = false, geo = false;
+    const uint32_t* fmask_dev = nullptr;
+    SSB_TRY(stage_batch(ws, st, q, v, &filtered, &geo, &fmask_dev));
+    geo = geo || (sort && sort_has_point(*sort));
+    // a batch with a POINT filter plans without flag bit 1: EVERY filtered query of that batch (its range / set filters too) leaves the
+    // lex_score record path for lex_generic<.., GEO>, so that lex_score keeps its code and registers; unfiltered queries stay on it
+    const uint32_t topk_flag = result_type == SSB_RESULT_TOPK && !geo ? 2u : 0u;
     SSB_CUDA_TRY(cudaMemsetAsync(ws.ctr, 0, 32, st));
     SSB_CUDA_TRY(cudaMemsetAsync(ws.stats, 0, sizeof(LexStats), st));
 
@@ -2230,6 +2491,120 @@ int32_t LexIndex::search_keys(LexWorkspace& ws, cudaStream_t st, const ssb_lex_b
     copy_out<<<(nq * LIST + 255) / 256, 256, 0, st>>>(glist, ws.count, nq, result_type == SSB_RESULT_COUNT ? 0 : k, keys_out_dev, count_dev);
     SSB_CUDA_TRY(cudaGetLastError());
     if (launches) *launches += 3;   // plan + generic + copy_out
+    return SSB_OK;
+}
+
+// (re)allocate a device buffer of at least n elements (contents are not kept)
+template <typename T>
+static cudaError_t grow(T*& p, size_t& cap, size_t n) {
+    if (n <= cap) return cudaSuccess;
+    cudaFree(p); p = nullptr; cap = 0;
+    const cudaError_t e = cudaMalloc(&p, n * sizeof(T));
+    if (e == cudaSuccess) cap = n;
+    return e;
+}
+
+constexpr size_t FACET_HIST_BYTES = 256ull << 20;   // per search context: the histograms of one query chunk
+
+int32_t LexIndex::facet_counts(LexWorkspace& ws, cudaStream_t st, const ssb_lex_batch* q, const ssb_facet_request* req, uint32_t n_req,
+                               const double* bases, ssb_facet_count* out, uint32_t* n_out, uint64_t* launches, uint64_t* kernel_ns,
+                               uint64_t* alg_bytes) const {
+    if (!committed_) { set_error("search before ssb_lexical_commit"); return SSB_E_STATE; }
+    if (!q || (n_req && !req) || (q->n_queries && (!q->term_offsets || (n_req && (!out || !n_out))))) { set_error("search_lexical_facets: null argument"); return SSB_E_INVALID; }
+    if (n_req > SSB_MAX_FACET_REQUESTS) { set_error("search_lexical_facets: %u requests, at most %u", n_req, SSB_MAX_FACET_REQUESTS); return SSB_E_UNSUPPORTED; }
+    if (q->query_type > SSB_QUERY_PHRASE) { set_error("bad query_type"); return SSB_E_INVALID; }
+    const uint32_t phrase = q->query_type == SSB_QUERY_PHRASE ? 1u : 0u;
+    if (phrase && has_positions_ != 1) { set_error("phrase query: the index holds no term positions (ssb_level_desc.positions)"); return SSB_E_STATE; }
+    if (phrase && q->term_flags) { set_error("phrase query: NOT terms are not accepted inside a phrase batch"); return SSB_E_UNSUPPORTED; }
+    const uint32_t qt_eff = phrase ? (uint32_t)SSB_QUERY_INTERSECTION : q->query_type;
+    const uint32_t nq = q->n_queries;
+    if (nq == 0 || n_req == 0) return SSB_OK;
+    if (!facets_ || !facets_->n_facets) { set_error("search_lexical_facets: facet counts need ssb_set_facets"); return SSB_E_STATE; }
+    if (bases && is_device_ptr(bases)) { set_error("search_lexical_facets: bases must be a host array"); return SSB_E_INVALID; }
+    // ---- the requests: keys, and the layout of a query's histogram (range bins, then value bins) and output (request order) ----
+    const FacetSet& fs = *facets_;
+    std::vector<FacetReqDev> rd(n_req);
+    std::vector<uint64_t> starts;
+    uint32_t range_words = 0, n_point = 0; uint64_t value_words = 0, out_stride = 0;
+    for (uint32_t i = 0; i < n_req; i++) {
+        const uint32_t f = req[i].facet;
+        if (f >= fs.n_facets) { set_error("facet request %u: facet %u of %u", i, f, fs.n_facets); return SSB_E_INVALID; }
+        if (req[i].kind == SSB_FACET_COUNT_VALUES && req[i].length && (fs.max_key[f] + 1) * 4 > FACET_HIST_BYTES) {
+            set_error("facet request %u: %llu value ids, above the %zu MiB facet workspace", i, (unsigned long long)fs.max_key[f] + 1, FACET_HIST_BYTES >> 20);
+            return SSB_E_UNSUPPORTED;
+        }
+        const bool has_order = fs.d_rank[f] && fs.max_key[f] < fs.n_rank[f];
+        SSB_TRY(encode_facet_request(req[i], i, fs.types[f], has_order, fs.max_key[f], bases != nullptr, &rd[i], starts));
+        if (rd[i].kind != FREQ_VALUES) { rd[i].hist_off = range_words; range_words += rd[i].n_bins; }
+        if (rd[i].kind == FREQ_POINT) rd[i].point_idx = n_point++;
+        rd[i].out_off = (uint32_t)out_stride;
+        out_stride += rd[i].kind == FREQ_VALUES ? rd[i].length : rd[i].n_bins;
+    }
+    for (uint32_t i = 0; i < n_req; i++)
+        if (rd[i].kind == FREQ_VALUES && rd[i].length) { rd[i].hist_off = (uint32_t)(range_words + value_words); value_words += rd[i].n_bins; }
+    const uint64_t hist_words = range_words + value_words;
+    if (hist_words * 4 > FACET_HIST_BYTES) {
+        set_error("search_lexical_facets: one query's histograms take %llu bytes, above the %zu MiB facet workspace", (unsigned long long)hist_words * 4, FACET_HIST_BYTES >> 20);
+        return SSB_E_UNSUPPORTED;
+    }
+    const uint32_t chunk = (uint32_t)std::min<uint64_t>(nq, FACET_HIST_BYTES / 4 / (hist_words ? hist_words : 1));
+    // ---- the batch and its plans (Count: every match, no top-k) ----
+    LexView v;
+    bool filtered = false, geo = false;
+    const uint32_t* fmask_dev = nullptr;
+    SSB_TRY(stage_batch(ws, st, q, v, &filtered, &geo, &fmask_dev));
+    if (!ws.fhist) SSB_CUDA_TRY(cudaMalloc(&ws.fhist, FACET_HIST_BYTES));
+    if (!ws.freq) SSB_CUDA_TRY(cudaMalloc(&ws.freq, SSB_MAX_FACET_REQUESTS * sizeof(FacetReqDev)));
+    if (!ws.fstarts) SSB_CUDA_TRY(cudaMalloc(&ws.fstarts, (size_t)SSB_MAX_FACET_REQUESTS * SSB_MAX_FACET_RANGES * 8));
+    if (!ws.fstats) SSB_CUDA_TRY(cudaMalloc(&ws.fstats, 4 * 8));
+    SSB_CUDA_TRY(grow(ws.fout, ws.cap_fout, (size_t)chunk * (out_stride ? out_stride : 1)));
+    SSB_CUDA_TRY(grow(ws.fnout, ws.cap_fnout, (size_t)chunk * n_req));
+    SSB_CUDA_TRY(grow(ws.fglist, ws.cap_fglist, (size_t)nq * LIST));
+    SSB_CUDA_TRY(cudaMemcpyAsync(ws.freq, rd.data(), n_req * sizeof(FacetReqDev), cudaMemcpyHostToDevice, st));
+    if (!starts.empty()) SSB_CUDA_TRY(cudaMemcpyAsync(ws.fstarts, starts.data(), starts.size() * 8, cudaMemcpyHostToDevice, st));
+    if (n_point) {
+        SSB_CUDA_TRY(grow(ws.fbases, ws.cap_fbases, (size_t)nq * n_point * 2));
+        SSB_CUDA_TRY(cudaMemcpyAsync(ws.fbases, bases, (size_t)nq * n_point * 16, cudaMemcpyHostToDevice, st));
+    }
+    SSB_CUDA_TRY(cudaMemsetAsync(ws.fstats, 0, 4 * 8, st));
+    SSB_CUDA_TRY(cudaMemsetAsync(ws.ctr, 0, 32, st));
+    uint32_t n_pow2 = 1; while (n_pow2 < v.n_levels) n_pow2 <<= 1;
+    if (n_pow2 < 2) n_pow2 = 2;
+    const size_t plan_smem = (size_t)v.n_levels * (8 + 2 * FAST_T) + 16 + (size_t)n_pow2 * 8;
+    if (plan_smem > 48 * 1024) SSB_CUDA_TRY(cudaFuncSetAttribute(lex_plan<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan_smem));
+    lex_plan<false><<<nq, 128, plan_smem, st>>>(v, ws.qoff, ws.qkeys, q->term_flags ? ws.qflags : nullptr, filtered ? ws.foff : nullptr, fmask_dev, phrase, qt_eff, ws.plans, ws.recs, ws.item_start, ws.ctr, ws.theta, ws.lock, ws.count, ws.fglist, n_pow2,
+                                                ITEM_W, 2, GMAX, SortDev{});
+    SSB_CUDA_TRY(cudaGetLastError());
+    if (launches) *launches += 1;
+    // ---- per query chunk: the counts, the selection, the copy out ----
+    auto kern = (phrase && n_fields_ > 1) ? (geo ? lex_facets<true, true> : lex_facets<true, false>) : (geo ? lex_facets<false, true> : lex_facets<false, false>);
+    const size_t smem = starts.size() * 8 + n_req * sizeof(FacetReqDev) + FACET_WARPS * (sizeof(FacetWarpSm) + (size_t)range_words * 4);
+    if (smem > 48 * 1024) SSB_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    FacetCall fc{ws.freq, n_req, ws.fstarts, (uint32_t)starts.size(), ws.fbases, n_point, ws.fhist, (uint32_t)hist_words, range_words, ws.fstats};
+    RankPtrs rk{};
+    for (uint32_t f = 0; f < fs.n_facets && f < SSB_MAX_FACETS; f++) rk.p[f] = fs.d_rank[f];
+    cudaEvent_t e0 = ws.ev0, e1 = ws.ev1;
+    float ms_sum = 0.f;
+    for (uint32_t q0 = 0; q0 < nq; q0 += chunk) {
+        const uint32_t nqc = std::min(chunk, nq - q0);
+        SSB_CUDA_TRY(cudaMemsetAsync(ws.fhist, 0, (size_t)nqc * hist_words * 4, st));
+        if (e0) cudaEventRecord(e0, st);
+        kern<<<n_sms_ * 4, FACET_WARPS * 32, smem, st>>>(v, ws.plans, ws.recs, q0, nqc, qt_eff, fc);
+        SSB_CUDA_TRY(cudaGetLastError());
+        if (e1) cudaEventRecord(e1, st);
+        facet_select<<<dim3(n_req, nqc), 256, 0, st>>>(ws.freq, n_req, ws.fhist, (uint32_t)hist_words, rk, ws.fout, (uint32_t)out_stride, ws.fnout);
+        SSB_CUDA_TRY(cudaGetLastError());
+        if (launches) *launches += 2;
+        if (out_stride) SSB_CUDA_TRY(cudaMemcpyAsync(out + (size_t)q0 * out_stride, ws.fout, (size_t)nqc * out_stride * sizeof(ssb_facet_count), cudaMemcpyDeviceToHost, st));
+        SSB_CUDA_TRY(cudaMemcpyAsync(n_out + (size_t)q0 * n_req, ws.fnout, (size_t)nqc * n_req * 4, cudaMemcpyDeviceToHost, st));
+        SSB_CUDA_TRY(cudaStreamSynchronize(st));
+        float ms = 0.f;
+        if (e0 && e1 && cudaEventElapsedTime(&ms, e0, e1) == cudaSuccess) ms_sum += ms; else cudaGetLastError();
+    }
+    uint64_t fst[4] = {0, 0, 0, 0};
+    SSB_CUDA_TRY(cudaMemcpy(fst, ws.fstats, 4 * 8, cudaMemcpyDeviceToHost));
+    if (kernel_ns) *kernel_ns = (uint64_t)((double)ms_sum * 1e6);
+    if (alg_bytes) *alg_bytes = fst[0] * 4 + fst[1] * 8 + fst[2] * n_req * 8;
     return SSB_OK;
 }
 

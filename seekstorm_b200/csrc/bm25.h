@@ -165,9 +165,17 @@ struct LexWorkspace {
     // sorted batches with a POINT criterion: [n_queries][2] bases, staged before search_keys — kept across release(), which
     // ensure_workspace calls when the batch outgrows the workspace
     double* bases = nullptr; uint32_t cap_bases = 0;
+    // facet count calls (facet_counts), kept across release() like `bases`: the value / range histograms of one query chunk (allocated on
+    // the first call, FACET_HIST_BYTES), the call's requests, range starts and Point bases, the selected counts of the chunk, the plan's
+    // scratch list and the call's work counters {postings, dense words, counted docs}
+    uint32_t* fhist = nullptr; FacetReqDev* freq = nullptr; uint64_t* fstarts = nullptr; uint64_t* fstats = nullptr;
+    double* fbases = nullptr; size_t cap_fbases = 0;
+    ssb_facet_count* fout = nullptr; uint32_t* fnout = nullptr; size_t cap_fout = 0, cap_fnout = 0;
+    uint64_t* fglist = nullptr; size_t cap_fglist = 0;
+    void release_facets();
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;   // recorded around lex_score when set
     void release();
-    ~LexWorkspace() { release(); cudaFree(bases); }
+    ~LexWorkspace() { release(); cudaFree(bases); release_facets(); }
     LexWorkspace() = default;
     LexWorkspace(const LexWorkspace&) = delete;
     LexWorkspace& operator=(const LexWorkspace&) = delete;
@@ -195,6 +203,11 @@ public:
     int32_t prepare_sort(const ssb_sort_criterion* crit, uint32_t n, bool has_bases, SortDev* out, bool* sorted) const;
     // a sort with a POINT criterion: copy the host bases [nq][2] into the workspace and point sort->bases at them
     static int32_t stage_sort_bases(LexWorkspace& ws, cudaStream_t st, const double* bases, uint32_t nq, SortDev* sort);
+    // ssb_search_lexical_facets: the batch's facet counts into the host arrays out / n_out (synchronous).  *kernel_ns: the CUDA-event time
+    // of lex_facets summed over the query chunks; *alg_bytes: list bytes + 8 B of column key per counted doc and request
+    int32_t facet_counts(LexWorkspace& ws, cudaStream_t st, const ssb_lex_batch* q, const ssb_facet_request* req, uint32_t n_req,
+                         const double* bases, ssb_facet_count* out, uint32_t* n_out, uint64_t* launches, uint64_t* kernel_ns,
+                         uint64_t* alg_bytes) const;
     bool committed() const { return committed_; }
     void set_stream(cudaStream_t st) { st_ = st; }   // load-time stream (add_level / commit)
     void set_deleted(const DeleteSet* d) { del_ = d; }
@@ -208,6 +221,10 @@ public:
 private:
     int32_t ensure_workspace(LexWorkspace& ws, uint32_t nq, uint32_t total_terms) const;
     int32_t stage_filters(LexWorkspace& ws, cudaStream_t st, const ssb_lex_batch* q, LexView& v, bool* any, bool* geo_any) const;
+    // what every lexical batch starts with: the per-query term checks, the workspace, the terms, the facet filters (*filtered, *geo: a
+    // POINT filter) and the field masks (*fmask_dev, null = none) on the device; v: the view with the batch's filters
+    int32_t stage_batch(LexWorkspace& ws, cudaStream_t st, const ssb_lex_batch* q, LexView& v, bool* filtered, bool* geo,
+                        const uint32_t** fmask_dev) const;
     cudaStream_t st_;
     int n_sms_;
     uint32_t max_batch_;

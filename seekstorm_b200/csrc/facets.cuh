@@ -20,17 +20,24 @@ __device__ __forceinline__ uint32_t morton_even_bits(uint64_t code) {
 // decode_morton_2_d (geo_search.rs:58-79): (x_u32 as i32) as f64 / 1e7 — lat from the even bits, lon from the odd bits
 __device__ __forceinline__ double morton_lat(uint64_t code) { return __ddiv_rn((double)(int32_t)morton_even_bits(code), 10000000.0); }
 __device__ __forceinline__ double morton_lon(uint64_t code) { return __ddiv_rn((double)(int32_t)morton_even_bits(code >> 1), 10000000.0); }
+// euclidian_distance(base, decode(code), unit) (geo_search.rs:95-107): the equirectangular distance of the doc at Morton code `code` from
+// (blat, blon); radius() returns the unit's earth radius.  The distance filter and the Point facet counts share it.  radius is read where
+// the product needs it: the filter loads it from its payload there, and with it geo_rejects_impl keeps the code it had as one expression.
+template <class Radius>
+__device__ __forceinline__ double geo_distance(uint64_t code, double blat, double blon, Radius radius) {
+    const double plat = morton_lat(code), plon = morton_lon(code);
+    const double c = cos(__ddiv_rn(__dmul_rn(SSB_DEG2RAD, __dadd_rn(blat, plat)), 2.0));
+    const double x = __dmul_rn(__dmul_rn(SSB_DEG2RAD, __dsub_rn(plon, blon)), c);
+    const double y = __dmul_rn(SSB_DEG2RAD, __dsub_rn(plat, blat));
+    return __dmul_rn(radius(), __dsqrt_rn(__dadd_rn(__dmul_rn(x, x), __dmul_rn(y, y))));
+}
 // FilterSparse::Point (add_result.rs:462-478): true = the doc is filtered OUT.  range.contains(code) on the Morton interval staged in
 // [lo, hi), then distance_range.contains(euclidian_distance(base, decode(code), unit)) (geo_search.rs:95-107).  g: the staged payload
 // (GEO_* words, f64 bits).  Out of line: only POINT filters reach it.
 __device__ __noinline__ bool geo_rejects_impl(uint64_t code, uint64_t lo, uint64_t hi, const uint64_t* g) {
     if (!(code >= lo && code < hi)) return true;
     const double blat = __longlong_as_double((long long)__ldg(&g[GEO_LAT])), blon = __longlong_as_double((long long)__ldg(&g[GEO_LON]));
-    const double plat = morton_lat(code), plon = morton_lon(code);
-    const double c = cos(__ddiv_rn(__dmul_rn(SSB_DEG2RAD, __dadd_rn(blat, plat)), 2.0));
-    const double x = __dmul_rn(__dmul_rn(SSB_DEG2RAD, __dsub_rn(plon, blon)), c);
-    const double y = __dmul_rn(SSB_DEG2RAD, __dsub_rn(plat, blat));
-    const double d = __dmul_rn(__longlong_as_double((long long)__ldg(&g[GEO_RADIUS])), __dsqrt_rn(__dadd_rn(__dmul_rn(x, x), __dmul_rn(y, y))));
+    const double d = geo_distance(code, blat, blon, [&] { return __longlong_as_double((long long)__ldg(&g[GEO_RADIUS])); });
     const double start = __longlong_as_double((long long)__ldg(&g[GEO_START])), end = __longlong_as_double((long long)__ldg(&g[GEO_END]));
     return !(start <= d && d < end);
 }

@@ -176,6 +176,59 @@ inline int32_t encode_filter(const ssb_facet_filter& f, uint32_t i, uint32_t typ
     return SSB_OK;
 }
 
+// ---- facet counts (ssb_search_lexical_facets; facet_count, add_result.rs:487-640) ----
+// One request of a facet count call in key space.  VALUES: n_bins = the facet's largest id + 1, one histogram bin per id.  RANGES: n_bins =
+// n_ranges; the starts' keys are staged at start_first of the call's start array, a doc's bin is the last start <= its key.  POINT: a RANGES
+// request on a POINT facet, binned by f64_order_key of the distance to base point_idx of the query (radius: earth_radius(unit)).
+// is_float: F32 / F64 (a NaN value, key ~0, is not counted).  hist_off / out_off / point_idx are set by the caller once it knows the layout.
+enum { FREQ_VALUES = 0, FREQ_RANGES = 1, FREQ_POINT = 2 };
+struct FacetReqDev {
+    uint32_t facet, kind, n_bins, is_float;
+    uint32_t start_first, point_idx, hist_off, out_off;
+    uint32_t length, has_prefix, rank_lo, rank_hi;
+    double radius;
+};
+// Request i of a call on a facet of type `type` -> *out, its starts' keys appended to `starts`.  has_order: the facet has a value order
+// (ssb_set_facet_value_order); max_key: its largest column key; has_bases: the call carries POINT bases.  Returns SSB_OK or an SSB_E_* code
+// with set_error called.
+inline int32_t encode_facet_request(const ssb_facet_request& r, uint32_t i, uint32_t type, bool has_order, uint64_t max_key, bool has_bases,
+                                    FacetReqDev* out, std::vector<uint64_t>& starts) {
+    FacetReqDev d{}; d.facet = r.facet;
+    if (r.kind == SSB_FACET_COUNT_VALUES) {
+        if (!facet_is_string(type)) { set_error("facet request %u: SSB_FACET_COUNT_VALUES needs a String16 / String32 facet", i); return SSB_E_INVALID; }
+        if (r.length > SSB_MAX_FACET_LENGTH) { set_error("facet request %u: length %u above %u", i, r.length, SSB_MAX_FACET_LENGTH); return SSB_E_UNSUPPORTED; }
+        if (r.has_prefix && !has_order) { set_error("facet request %u: a prefix needs the facet's value order (ssb_set_facet_value_order)", i); return SSB_E_STATE; }
+        if (r.has_prefix && r.rank_lo > r.rank_hi) { set_error("facet request %u: rank_lo %u above rank_hi %u", i, r.rank_lo, r.rank_hi); return SSB_E_INVALID; }
+        d.kind = FREQ_VALUES; d.n_bins = (uint32_t)(max_key + 1); d.length = r.length;
+        d.has_prefix = r.has_prefix ? 1u : 0u; d.rank_lo = r.rank_lo; d.rank_hi = r.rank_hi;
+    } else if (r.kind == SSB_FACET_COUNT_RANGES) {
+        if (facet_is_string(type)) { set_error("facet request %u: a String facet takes SSB_FACET_COUNT_VALUES", i); return SSB_E_INVALID; }
+        if (r.n_ranges == 0) { set_error("facet request %u: no ranges", i); return SSB_E_INVALID; }
+        if (r.n_ranges > SSB_MAX_FACET_RANGES) { set_error("facet request %u: %u ranges, at most %u", i, r.n_ranges, SSB_MAX_FACET_RANGES); return SSB_E_UNSUPPORTED; }
+        if (!r.range_starts) { set_error("facet request %u: null range_starts", i); return SSB_E_INVALID; }
+        const bool point = type == SSB_FACET_POINT;
+        if (point) {
+            if (r.unit > SSB_UNIT_MILES) { set_error("facet request %u: bad distance unit %u", i, r.unit); return SSB_E_INVALID; }
+            if (!has_bases) { set_error("facet request %u: a Point facet needs the queries' bases", i); return SSB_E_INVALID; }
+            d.radius = earth_radius(r.unit);
+        }
+        d.kind = point ? FREQ_POINT : FREQ_RANGES; d.n_bins = r.n_ranges; d.is_float = facet_is_float(type) ? 1u : 0u;
+        d.start_first = (uint32_t)starts.size();
+        for (uint32_t j = 0; j < r.n_ranges; j++) {
+            uint64_t key = r.range_starts[j];
+            if (point || facet_is_float(type)) {
+                double x; memcpy(&x, &key, 8);
+                if (x != x) { set_error("facet request %u: range start %u is NaN", i, j); return SSB_E_INVALID; }
+                key = f64_order_key(x);
+            } else if (facet_is_signed(type)) key ^= 0x8000000000000000ull;
+            if (j && key <= starts.back()) { set_error("facet request %u: range starts must ascend strictly (start %u)", i, j); return SSB_E_INVALID; }
+            starts.push_back(key);
+        }
+    } else { set_error("facet request %u: bad kind %u", i, r.kind); return SSB_E_INVALID; }
+    *out = d;
+    return SSB_OK;
+}
+
 }  // namespace ssb
 
 // The rest owns device memory: nvcc translation units only.

@@ -16,6 +16,7 @@ mandatory term (tokenizer.rs:546-563); terms are mapped to 64-bit keys by `term_
 """
 from __future__ import annotations
 
+import bisect
 import ctypes as C
 import enum
 from dataclasses import dataclass, field
@@ -111,6 +112,64 @@ class FacetFilter:
     unit: DistanceUnit = DistanceUnit.Kilometers
 
 
+class RangeType(enum.IntEnum):
+    """`RangeType` (search.rs:216-228) of a range facet: the count within each range, or the running sum from the top / the bottom."""
+    CountWithinRange = 0
+    CountAboveRange = 1
+    CountBelowRange = 2
+
+
+@dataclass(frozen=True)
+class QueryFacet:
+    """`QueryFacet` (search.rs:234-…): facet counts of the query's matches on one facet field.  A String16 / String32 field takes `prefix`
+    and `length` (the `length` values with the most matches whose string starts with prefix; 0 = not collected); a numeric / Timestamp /
+    F32 / F64 field takes `range_type` and `ranges` = [(label, start), ...] (start ascending; a range runs up to the next start); a Point
+    field also takes `base` (lat, lon) and `unit`, and ranges over the distance to base.  A request whose shape does not fit the field's
+    type, or an unknown field, is ignored as the reference does."""
+    field: str
+    prefix: str = ""
+    length: int = 0
+    range_type: RangeType = RangeType.CountWithinRange
+    ranges: Sequence = ()
+    base: Optional[Sequence[float]] = None
+    unit: DistanceUnit = DistanceUnit.Kilometers
+
+
+def prefix_rank_interval(order, prefix: bytes):
+    """[lo, hi) of the ranks (positions in `order`, the sorted distinct strings as bytes) of the strings that start with prefix"""
+    lo = bisect.bisect_left(order, prefix)
+    succ = prefix.rstrip(b"\xff")
+    if not succ:
+        return lo, len(order)
+    succ = succ[:-1] + bytes([succ[-1] + 1])
+    return lo, bisect.bisect_left(order, succ)
+
+
+def assemble_range_facet(counts, labels, range_type, prefix=""):
+    """One range facet of one shard (search.rs:3660-3745): the bins with a nonzero count, RangeType applied (the running sum over those
+    bins from the top or the bottom), in range order, labels attached, filtered by the label prefix."""
+    vals = {i: int(c) for i, c in enumerate(counts) if c}
+    rt = RangeType(range_type)
+    if rt != RangeType.CountWithinRange:
+        s = 0
+        for i in sorted(vals, reverse=rt == RangeType.CountAboveRange):
+            s += vals[i]
+            vals[i] = s
+    return [(labels[i], vals[i]) for i in sorted(vals) if not prefix or labels[i].startswith(prefix)]
+
+
+def merge_facets(per_field, lengths):
+    """Search::search's final step (search.rs:1932-1936, 2038-2048): per field, the counts of equal labels summed, then the (label, count)
+    pairs by count descending (stable: ties keep their order), at most `length` of them"""
+    out = {}
+    for f, v in per_field.items():
+        acc = {}
+        for label, c in v:
+            acc[label] = acc.get(label, 0) + c
+        out[f] = sorted(acc.items(), key=lambda x: -x[1])[:lengths[f]]
+    return out
+
+
 class SortOrder(enum.IntEnum):
     """search.rs:885-890."""
     Ascending = 0
@@ -137,7 +196,7 @@ class Result:
 
 @dataclass
 class ResultObject:
-    """search.rs:186-213 (facets / suggestions are outside the hot path)."""
+    """search.rs:186-213 (suggestions are outside the hot path).  facets: {field: [(string or range label, count), ...]}."""
     original_query: str = ""
     query: str = ""
     query_terms: list = field(default_factory=list)
@@ -146,6 +205,7 @@ class ResultObject:
     results: list = field(default_factory=list)
     observed_vector_count: int = 0
     observed_cluster_count: int = 0
+    facets: dict = field(default_factory=dict)
 
 
 def fnv1a64(term: str) -> int:
@@ -383,6 +443,7 @@ class Index:
             a = np.ascontiguousarray(columns[name])
             rows[:n, fields[i].offset:fields[i].offset + a.dtype.itemsize] = a.view(np.uint8).reshape(n, a.dtype.itemsize)
         self._facet_rows = (rows, fields, int(first_doc_id), n, off)      # also what the tests hand to the oracle
+        self._string_values, self._string_order = {}, {}
         check(lib().ssb_set_facets(self._h, rows.ctypes.data, int(first_doc_id), n, off, fields, len(names)))
         for name, values in (string_values or {}).items():
             t = self._facet_schema.get(name, (None, None))[1]
@@ -393,6 +454,7 @@ class Index:
             pos = {b: i for i, b in enumerate(order)}
             rank = np.ascontiguousarray([pos[b] for b in enc], dtype=np.uint32)
             check(lib().ssb_set_facet_value_order(self._h, self._facet_schema[name][0], rank.ctypes.data, rank.size))
+            self._string_values[name], self._string_order[name] = [str(v) for v in values], order
 
     def _sort_criteria(self, result_sort):
         """ResultSort list -> ssb_sort_criterion array (ResultSortIndex, search.rs:2497-2525): "_id" / "_score", facet names resolved to
@@ -454,6 +516,97 @@ class Index:
         arr = (SsbFacetFilter * max(len(flat), 1))(*flat)
         sv = np.asarray(sets if sets else [0], dtype=np.uint64)
         return offs, arr, sv
+
+    def _facet_requests(self, query_facets):
+        """QueryFacet list -> (ssb_facet_request array, kept buffers, [(field, kind, QueryFacet)] per request).  The reference keeps one
+        request per facet field (the last one wins) and ignores requests whose shape does not fit the field's type (search.rs:2729-3012)."""
+        from ._lib import SsbFacetRequest
+        by_field = {}
+        for qf in query_facets:
+            idx, t = getattr(self, "_facet_schema", {}).get(qf.field, (None, None))
+            if idx is None:
+                continue
+            string = t in (_lib.FACET_STRING16, _lib.FACET_STRING32)
+            if string == bool(qf.ranges):
+                continue
+            by_field[qf.field] = (idx, t, qf)
+        reqs, keep, meta = [], [], []
+        for name, (idx, t, qf) in by_field.items():
+            if t in (_lib.FACET_STRING16, _lib.FACET_STRING32):
+                lo = hi = has = 0
+                if qf.prefix:
+                    if name not in self._string_order:
+                        raise ValueError(f"query facet {name!r}: a prefix needs the facet's string_values (set_facets)")
+                    lo, hi = prefix_rank_interval(self._string_order[name], qf.prefix.encode("utf-8"))
+                    has = 1
+                reqs.append(SsbFacetRequest(idx, _lib.FACET_COUNT_VALUES, int(qf.length), has, lo, hi, 0, 0, None))
+            else:
+                starts = [r[1] for r in qf.ranges]
+                if t in (_lib.FACET_F32, _lib.FACET_F64, _lib.FACET_POINT):
+                    a = np.asarray(starts, dtype=np.float64).view(np.uint64)
+                elif t in (_lib.FACET_I8, _lib.FACET_I16, _lib.FACET_I32, _lib.FACET_I64, _lib.FACET_TIMESTAMP):
+                    a = np.asarray(starts, dtype=np.int64).view(np.uint64)
+                else:
+                    a = np.asarray(starts, dtype=np.uint64)
+                a = np.ascontiguousarray(a)
+                keep.append(a)
+                reqs.append(SsbFacetRequest(idx, _lib.FACET_COUNT_RANGES, 0, 0, 0, 0, len(starts), int(DistanceUnit(qf.unit)), a.ctypes.data))
+            meta.append((name, t, qf))
+        arr = (SsbFacetRequest * max(len(reqs), 1))(*reqs)
+        return arr, len(reqs), keep, meta
+
+    def search_lexical_facets(self, queries_keys, query_type: QueryType, query_facets, not_keys=None, filters=None, field_masks=None,
+                              facet_bases=None):
+        """Facet counts of a lexical batch (ssb_search_lexical_facets): the docs result_count_total counts for the same arguments, per query
+        {field: raw} with raw = [(value id, count), ...] (String facets: count desc, id asc, at most `length`) or the counts of every range
+        (zeros included).  facet_bases: per query the (lat, lon) base of each Point request in request order (default: QueryFacet.base)."""
+        nq = len(queries_keys)
+        b, keep = self._lex_batch(queries_keys, query_type, not_keys, filters, field_masks)
+        arr, n_req, keep2, meta = self._facet_requests(query_facets)
+        if n_req == 0 or nq == 0:
+            return [{} for _ in range(nq)]
+        points = [qf for _, t, qf in meta if t == _lib.FACET_POINT]
+        bases = None
+        if points:
+            if facet_bases is None:
+                facet_bases = [[qf.base for qf in points]] * nq
+            bases = np.ascontiguousarray(np.asarray(facet_bases, dtype=np.float64).reshape(nq, len(points), 2))
+        caps = [qf.length if t in (_lib.FACET_STRING16, _lib.FACET_STRING32) else len(qf.ranges) for _, t, qf in meta]
+        stride = sum(caps)
+        out = np.zeros(max(nq * stride, 1), dtype=[("value", np.uint32), ("pad", np.uint32), ("count", np.uint64)])
+        n_out = np.zeros(max(nq * n_req, 1), dtype=np.uint32)
+        check(lib().ssb_search_lexical_facets(self._h, C.byref(b), C.addressof(arr), n_req, bases.ctypes.data if bases is not None else None,
+                                              out.ctypes.data, n_out.ctypes.data))
+        res = []
+        for i in range(nq):
+            d, o = {}, i * stride
+            for r, (name, t, qf) in enumerate(meta):
+                m = int(n_out[i * n_req + r])
+                e = out[o:o + m]
+                d[name] = ([(int(v), int(c)) for v, c in zip(e["value"], e["count"])] if t in (_lib.FACET_STRING16, _lib.FACET_STRING32)
+                           else [int(c) for c in e["count"]])
+                o += caps[r]
+            res.append(d)
+        return res
+
+    def assemble_facets(self, raw, query_facets):
+        """One query's raw counts (search_lexical_facets) -> ResultObject.facets: per field the shard's assembly (search.rs:3598-3750: the
+        strings of the counted ids; for ranges RangeType, labels, the label prefix, no zero bins), then Search::search's ordering by count
+        and truncation to `length` (search.rs:2038-2048).  A field whose list comes out empty is left out."""
+        per_field, lengths = {}, {}
+        reqs = {qf.field: qf for qf in query_facets if qf.field in raw}
+        for name, qf in reqs.items():
+            t = self._facet_schema[name][1]
+            if t in (_lib.FACET_STRING16, _lib.FACET_STRING32):
+                sv = getattr(self, "_string_values", {}).get(name)
+                v = [(sv[i] if sv is not None else i, c) for i, c in raw[name]]
+                lengths[name] = int(qf.length)
+            else:
+                v = assemble_range_facet(raw[name], [r[0] for r in qf.ranges], qf.range_type, qf.prefix)
+                lengths[name] = 65535
+            if v:
+                per_field[name] = v
+        return merge_facets(per_field, lengths)
 
     def add_vector_level(self, level_id: int, rows, local_ids=None, cluster_counts=None):
         """rows: [n, dims] f32 (numpy or torch, host or device), n <= 65536.  cluster_counts: the level's IVF cluster table (rows in
@@ -671,11 +824,17 @@ class Index:
         the lexical search like the reference does (the vector search takes no facet filter, vector.rs:1105-1115).
         result_sort: ResultSort objects — lexical search only (the hits in sort order, ssb_search_lexical_sorted_ex; a Point facet's
         ResultSort.base sorts by the distance to it).
-        Unsupported reference features (facet counting, sorting vector / hybrid results, a base on a non-Point facet, uncommitted,
-        rewriting) raise NotImplementedError rather than being silently ignored."""
-        if query_facets or include_uncommitted:
-            raise NotImplementedError("facet counts / uncommitted search are outside the GPU hot path")
+        query_facets: QueryFacet objects — facet counts of the lexical matches in ResultObject.facets (ssb_search_lexical_facets), unless
+        the result type is Topk (search.rs:1748).
+        Unsupported reference features (facet counts of vector-only or empty queries, sorting vector / hybrid results, a base on a
+        non-Point facet, uncommitted, rewriting) raise NotImplementedError rather than being silently ignored."""
+        if include_uncommitted:
+            raise NotImplementedError("uncommitted search is outside the GPU hot path")
         search_mode = search_mode or SearchMode.Lexical()
+        if query_facets and search_mode.kind == "Vector":
+            raise NotImplementedError("facet counts of a vector search are not built")
+        if any(not isinstance(qf, QueryFacet) for qf in query_facets):
+            raise NotImplementedError("query_facets takes QueryFacet requests; other forms (bare field names) are not built")
         if result_sort and search_mode.kind != "Lexical":
             raise NotImplementedError("result_sort on vector / hybrid search is not built")
         if result_sort:
@@ -726,6 +885,12 @@ class Index:
                                                     [list(facet_filter)] if facet_filter else None, [fmask] if fmask else None,
                                                     list(result_sort) if result_sort else None)
             lex, total = res[0], int(counts[0])
+            if query_facets and rt != ResultType.Topk:
+                raw = self.search_lexical_facets([keys], qt, list(query_facets), [nkeys] if nkeys else None,
+                                                 [list(facet_filter)] if facet_filter else None, [fmask] if fmask else None)
+                ro.facets = self.assemble_facets(raw[0], list(query_facets))
+        elif query_facets and rt != ResultType.Topk and search_mode.kind != "Vector":
+            raise NotImplementedError("facet counts of the empty query (get_index_string_facets_shard) are not built")
         if want_vec:
             qv = np.asarray(query_vector, dtype=np.float32).reshape(1, -1)
             # similarity_threshold (TopK::new, vector.rs:388-399) and observed_vector_count are handled behind the C-ABI
