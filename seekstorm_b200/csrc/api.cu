@@ -56,12 +56,6 @@ int32_t encode_tmap_2d(CUtensorMap* out, const void* base, int elem_bytes, uint6
     return SSB_OK;
 }
 
-static bool dev_ptr(const void* p) {
-    cudaPointerAttributes a;
-    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
-    return a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
-}
-
 }  // namespace ssb
 
 using namespace ssb;
@@ -194,7 +188,7 @@ int32_t vec_keys(ssb_index* ix, SearchCtx& c, const void* queries, bool queries_
     if (scan != vec::Scan::I8_128) SSB_TRY(c.qpad.reserve((size_t)nq_pad * ix->dpad, 0, st));
     const size_t qbytes = (size_t)nq * ix->dims * (queries_i8 ? 1 : 4);
     const void* qsrc = queries;
-    if (!dev_ptr(queries)) {
+    if (!is_device_ptr(queries)) {
         SSB_TRY(c.qstage.reserve(((size_t)nq * ix->dims + 3) / (queries_i8 ? 4 : 1) + 1, 0, st));
         SSB_CUDA_TRY(cudaMemcpyAsync(c.qstage.p, queries, qbytes, cudaMemcpyHostToDevice, st));
         c.stats.h2d_bytes += qbytes;
@@ -567,7 +561,7 @@ int32_t ssb_lexical_add_level(ssb_index* ix, const ssb_level_desc* level) {
     if (!ix) { set_error("null index"); return SSB_E_INVALID; }
     std::unique_lock<std::shared_mutex> g(ix->rw);
     SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
-    if (level && (dev_ptr(level->doc_ids) || dev_ptr(level->term_keys))) SSB_CUDA_TRY(cudaDeviceSynchronize());   // inputs produced on another stream
+    if (level && (is_device_ptr(level->doc_ids) || is_device_ptr(level->term_keys))) SSB_CUDA_TRY(cudaDeviceSynchronize());   // inputs produced on another stream
     return ix->lex->add_level(level);
     SSB_API_END
 }
@@ -575,7 +569,7 @@ int32_t ssb_lexical_add_level(ssb_index* ix, const ssb_level_desc* level) {
 int32_t ssb_lexical_set_field_boosts(ssb_index* ix, uint32_t n_fields, const float* boosts) {
     SSB_API_BEGIN
     if (!ix) { set_error("null index"); return SSB_E_INVALID; }
-    if (boosts && dev_ptr(boosts)) { set_error("boosts must be host memory"); return SSB_E_INVALID; }
+    if (boosts && is_device_ptr(boosts)) { set_error("boosts must be host memory"); return SSB_E_INVALID; }
     std::unique_lock<std::shared_mutex> g(ix->rw);
     return ix->lex->set_fields(n_fields, boosts);
     SSB_API_END
@@ -637,7 +631,7 @@ static int32_t vector_add_level_impl(ssb_index* ix, uint32_t level_id, const flo
     if (!ix || (n && !rows)) { set_error("ssb_vector_add_level: null argument"); return SSB_E_INVALID; }
     if (ix->dims == 0 || dims != ix->dims) { set_error("dims %u != configured vector_dims %u", dims, ix->dims); return SSB_E_INVALID; }
     if (cluster_counts) {
-        if (dev_ptr(cluster_counts)) { set_error("cluster_counts must be host memory"); return SSB_E_INVALID; }
+        if (is_device_ptr(cluster_counts)) { set_error("cluster_counts must be host memory"); return SSB_E_INVALID; }
         uint64_t sum = 0;
         for (uint32_t c = 0; c < n_clusters; c++) { if (cluster_counts[c] == 0) { set_error("empty cluster %u", c); return SSB_E_INVALID; } sum += cluster_counts[c]; }
         if (sum != n || (n && n_clusters == 0)) { set_error("cluster table covers %llu of %u rows", (unsigned long long)sum, n); return SSB_E_INVALID; }
@@ -652,7 +646,7 @@ static int32_t vector_add_level_impl(ssb_index* ix, uint32_t level_id, const flo
     cudaStream_t st = ix->load_st;
     // device-resident inputs may still be in flight on the caller's stream (the load stream is non-blocking): load time is not
     // hot, wait for the device once
-    if (dev_ptr(rows) || (local_ids && dev_ptr(local_ids))) SSB_CUDA_TRY(cudaDeviceSynchronize());
+    if (is_device_ptr(rows) || (local_ids && is_device_ptr(local_ids))) SSB_CUDA_TRY(cudaDeviceSynchronize());
     // multi-chunk documents: several rows may share a local id (one vector per chunk, vector.rs:62-73); the reference's TopK keeps
     // the best chunk per doc id (vector.rs:436-470) — remember that this index needs the de-duplicating result path
     std::vector<uint16_t> h_ids;
@@ -750,7 +744,7 @@ static int32_t vector_add_level_impl(ssb_index* ix, uint32_t level_id, const flo
     }
     DevTmp<uint16_t> tmp;
     const uint16_t* lid = local_ids;
-    if (local_ids && !dev_ptr(local_ids)) {
+    if (local_ids && !is_device_ptr(local_ids)) {
         SSB_CUDA_TRY(tmp.alloc(n));
         SSB_CUDA_TRY(cudaMemcpyAsync(tmp.p, h_ids.data(), (size_t)n * 2, cudaMemcpyHostToDevice, st));
         lid = tmp.p;
@@ -806,7 +800,7 @@ int32_t ssb_vector_add_level_clustered(ssb_index* ix, uint32_t level_id, const f
 int32_t ssb_load_index_bin(ssb_index* ix, const void* bytes, uint64_t len, const ssb_index_bin_params* params, uint64_t* n_docs_out) {
     SSB_API_BEGIN
     if (!ix || !bytes || !params) { set_error("ssb_load_index_bin: null argument"); return SSB_E_INVALID; }
-    if (dev_ptr(bytes)) { set_error("ssb_load_index_bin: bytes must be host memory"); return SSB_E_INVALID; }
+    if (is_device_ptr(bytes)) { set_error("ssb_load_index_bin: bytes must be host memory"); return SSB_E_INVALID; }
     std::unique_lock<std::shared_mutex> g(ix->rw);
     SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
     return load_index_bin(ix->lex, (const uint8_t*)bytes, len, params, n_docs_out);
@@ -823,7 +817,7 @@ int32_t ssb_index_bin_inspect(const void* bytes, uint64_t len, const ssb_index_b
 int32_t ssb_load_vector_bin(ssb_index* ix, const void* bytes, uint64_t len, uint64_t* n_vectors_out) {
     SSB_API_BEGIN
     if (!ix || !bytes) { set_error("ssb_load_vector_bin: null argument"); return SSB_E_INVALID; }
-    if (dev_ptr(bytes)) { set_error("ssb_load_vector_bin: bytes must be host memory"); return SSB_E_INVALID; }
+    if (is_device_ptr(bytes)) { set_error("ssb_load_vector_bin: bytes must be host memory"); return SSB_E_INVALID; }
     if (ix->dims == 0) { set_error("ssb_load_vector_bin: the index has no vector_dims"); return SSB_E_STATE; }
     std::vector<VectorLevel> levels;
     SSB_TRY(parse_vector_bin((const uint8_t*)bytes, len, ix->dims, levels));
@@ -1309,7 +1303,7 @@ int32_t ssb_last_stats(const ssb_index* cix, ssb_stats* out) {
         if (cudaEventSynchronize(c->ev1) == cudaSuccess && cudaEventElapsedTime(&ms, c->ev0, c->ev1) == cudaSuccess)
             out->dominant_kernel_ns = (uint64_t)((double)ms * 1e6);
         else cudaGetLastError();
-        if (c->last_lex && out->postings_visited == 0 && c->lex.stats) {
+        if (c->last_lex && out->postings_visited == 0 && c->lex.stats.p) {
             const LexStats ls = LexIndex::read_stats(c->lex, ix->ext_stream_set ? ix->ext_stream : c->own_st);
             out->postings_visited = ls.postings_visited; out->probes = ls.probes; out->items_processed = ls.items_processed; out->items_skipped = ls.items_skipped;
             if (ls.postings_visited) out->algorithmic_bytes = ls.postings_visited * 4 + ls.probes * 16 + ls.recs_processed * 128 + ls.dense_words * 8;

@@ -1918,33 +1918,6 @@ void LexIndex::free_committed() {
     committed_ = false;
 }
 
-void LexWorkspace::release() {
-    cudaFree(plans); cudaFree(recs); cudaFree(item_start); cudaFree(theta); cudaFree(lock); cudaFree(count); cudaFree(ctr);
-    cudaFree(qoff); cudaFree(qkeys); cudaFree(qflags); cudaFree(stats); cudaFree(foff); cudaFree(filt); cudaFree(fsets); cudaFree(fmask);
-    foff = nullptr; filt = nullptr; fsets = nullptr; fmask = nullptr; cap_filt = cap_fsets = 0;
-    cudaFree(theta2); theta2 = nullptr;
-    qflags = nullptr; plans = nullptr; recs = nullptr; item_start = nullptr; theta = nullptr; lock = nullptr; count = nullptr; ctr = nullptr;
-    qoff = nullptr; qkeys = nullptr; stats = nullptr; cap_q = cap_terms = cap_levels = 0;
-}
-void LexWorkspace::release_facets() {
-    cudaFree(fhist); cudaFree(freq); cudaFree(fstarts); cudaFree(fstats); cudaFree(fbases); cudaFree(fout); cudaFree(fnout); cudaFree(fglist);
-    fhist = nullptr; freq = nullptr; fstarts = nullptr; fstats = nullptr; fbases = nullptr; fout = nullptr; fnout = nullptr; fglist = nullptr;
-    cap_fbases = cap_fout = cap_fnout = 0; cap_fglist = 0;
-}
-
-static uint32_t env_u32(const char* name, uint32_t dflt, uint32_t lo, uint32_t hi) {
-    const char* e = getenv(name);
-    if (!e || !*e) return dflt;
-    long v = strtol(e, nullptr, 10);
-    return v < (long)lo ? lo : (v > (long)hi ? hi : (uint32_t)v);
-}
-
-static bool is_device_ptr(const void* p) {
-    cudaPointerAttributes a;
-    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
-    return a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
-}
-
 // copy n bytes from a host-or-device pointer into device memory
 static cudaError_t to_device(void* dst, const void* src, size_t n, cudaStream_t st) {
     if (n == 0) return cudaSuccess;
@@ -2260,22 +2233,21 @@ int32_t LexIndex::set_global_df(const uint64_t* keys, const uint32_t* dfs, uint6
     return SSB_OK;
 }
 
-int32_t LexIndex::ensure_workspace(LexWorkspace& ws, uint32_t nq, uint32_t total_terms) const {
-    const uint32_t nlv = (uint32_t)levels_.size();
-    if (nq <= ws.cap_q && total_terms <= ws.cap_terms && nlv == ws.cap_levels) return SSB_OK;
-    ws.release();
-    uint32_t cq = nq > max_batch_ ? nq : max_batch_;
-    uint32_t ct = total_terms > cq * 4 ? total_terms : cq * 4;
-    const size_t nl1 = nlv ? nlv : 1;
-    SSB_CUDA_TRY(cudaMalloc(&ws.plans, (size_t)cq * sizeof(QueryPlan)));
-    SSB_CUDA_TRY(cudaMalloc(&ws.recs, (size_t)cq * nl1 * sizeof(LvRec)));
-    SSB_CUDA_TRY(cudaMalloc(&ws.item_start, (size_t)cq * (nl1 + 1) * sizeof(uint16_t)));
-    SSB_CUDA_TRY(cudaMalloc(&ws.theta, (size_t)cq * 8)); SSB_CUDA_TRY(cudaMalloc(&ws.lock, (size_t)cq * 4));
-    SSB_CUDA_TRY(cudaMalloc(&ws.count, (size_t)cq * 8)); SSB_CUDA_TRY(cudaMalloc(&ws.ctr, 32));
-    SSB_CUDA_TRY(cudaMalloc(&ws.qoff, ((size_t)cq + 1) * 4)); SSB_CUDA_TRY(cudaMalloc(&ws.qkeys, (size_t)ct * 8));
-    SSB_CUDA_TRY(cudaMalloc(&ws.qflags, (size_t)ct));
-    SSB_CUDA_TRY(cudaMalloc(&ws.stats, sizeof(LexStats)));
-    ws.cap_q = cq; ws.cap_terms = ct; ws.cap_levels = nlv;
+int32_t LexIndex::ensure_workspace(LexWorkspace& ws, cudaStream_t st, uint32_t nq, uint32_t total_terms) const {
+    const size_t cq = nq > max_batch_ ? nq : max_batch_;
+    const size_t ct = total_terms > cq * 4 ? total_terms : cq * 4;
+    const size_t nl1 = levels_.empty() ? 1 : levels_.size();
+    SSB_TRY(ws.plans.reserve(cq, 0, st, true));
+    SSB_TRY(ws.recs.reserve(cq * nl1, 0, st, true));
+    SSB_TRY(ws.item_start.reserve(cq * (nl1 + 1), 0, st, true));
+    SSB_TRY(ws.theta.reserve(cq * 2, 0, st, true));
+    SSB_TRY(ws.lock.reserve(cq, 0, st, true));
+    SSB_TRY(ws.count.reserve(cq, 0, st, true));
+    SSB_TRY(ws.ctr.reserve(8, 0, st, true));
+    SSB_TRY(ws.qoff.reserve(cq + 1, 0, st, true));
+    SSB_TRY(ws.qkeys.reserve(ct, 0, st, true));
+    SSB_TRY(ws.qflags.reserve(ct, 0, st, true));
+    SSB_TRY(ws.stats.reserve(1, 0, st, true));
     return SSB_OK;
 }
 
@@ -2300,12 +2272,9 @@ int32_t LexIndex::prepare_sort(const ssb_sort_criterion* crit, uint32_t n, bool 
 int32_t LexIndex::stage_sort_bases(LexWorkspace& ws, cudaStream_t st, const double* bases, uint32_t nq, SortDev* sort) {
     if (!sort_has_point(*sort) || nq == 0) return SSB_OK;
     if (is_device_ptr(bases)) { set_error("search_lexical_sorted: bases must be a host array"); return SSB_E_INVALID; }
-    if (nq > ws.cap_bases) {
-        cudaFree(ws.bases); ws.bases = nullptr; ws.cap_bases = 0;
-        SSB_CUDA_TRY(cudaMalloc(&ws.bases, (size_t)nq * 16)); ws.cap_bases = nq;
-    }
-    SSB_CUDA_TRY(cudaMemcpyAsync(ws.bases, bases, (size_t)nq * 16, cudaMemcpyHostToDevice, st));
-    sort->bases = ws.bases;
+    SSB_TRY(ws.bases.reserve((size_t)nq * 2, 0, st, true));
+    SSB_CUDA_TRY(cudaMemcpyAsync(ws.bases.p, bases, (size_t)nq * 16, cudaMemcpyHostToDevice, st));
+    sort->bases = ws.bases.p;
     return SSB_OK;
 }
 
@@ -2333,15 +2302,15 @@ int32_t LexIndex::stage_filters(LexWorkspace& ws, cudaStream_t st, const ssb_lex
     }
     for (uint32_t i = 0; i < nf; i++) if (q->filters[i].kind == SSB_FILTER_POINT) fd[i].set_first += n_sets;
     const uint32_t n_staged = n_sets + (uint32_t)geo.size();
-    if (!ws.foff) SSB_CUDA_TRY(cudaMalloc(&ws.foff, ((size_t)ws.cap_q + 1) * 4));
-    if (nf > ws.cap_filt) { cudaFree(ws.filt); ws.filt = nullptr; ws.cap_filt = 0; const uint32_t c = nf + nf / 2 + 64; SSB_CUDA_TRY(cudaMalloc(&ws.filt, (size_t)c * sizeof(FiltDev))); ws.cap_filt = c; }
-    if (n_staged > ws.cap_fsets) { cudaFree(ws.fsets); ws.fsets = nullptr; ws.cap_fsets = 0; const uint32_t c = n_staged + n_staged / 2 + 64; SSB_CUDA_TRY(cudaMalloc(&ws.fsets, (size_t)c * 8)); ws.cap_fsets = c; }
+    SSB_TRY(ws.foff.reserve((size_t)nq + 1, 0, st, true));
+    SSB_TRY(ws.filt.reserve(nf, 0, st));
+    SSB_TRY(ws.fsets.reserve(n_staged, 0, st));
     // pageable host sources: cudaMemcpyAsync returns after staging them, the vectors may go out of scope
-    SSB_CUDA_TRY(cudaMemcpyAsync(ws.foff, q->filter_offsets, ((size_t)nq + 1) * 4, cudaMemcpyHostToDevice, st));
-    SSB_CUDA_TRY(cudaMemcpyAsync(ws.filt, fd.data(), (size_t)nf * sizeof(FiltDev), cudaMemcpyHostToDevice, st));
-    if (n_sets) SSB_CUDA_TRY(cudaMemcpyAsync(ws.fsets, q->filter_set_values, (size_t)n_sets * 8, cudaMemcpyHostToDevice, st));
-    if (!geo.empty()) SSB_CUDA_TRY(cudaMemcpyAsync(ws.fsets + n_sets, geo.data(), geo.size() * 8, cudaMemcpyHostToDevice, st));
-    v.filt = ws.filt; v.filt_sets = ws.fsets;
+    SSB_CUDA_TRY(cudaMemcpyAsync(ws.foff.p, q->filter_offsets, ((size_t)nq + 1) * 4, cudaMemcpyHostToDevice, st));
+    SSB_CUDA_TRY(cudaMemcpyAsync(ws.filt.p, fd.data(), (size_t)nf * sizeof(FiltDev), cudaMemcpyHostToDevice, st));
+    if (n_sets) SSB_CUDA_TRY(cudaMemcpyAsync(ws.fsets.p, q->filter_set_values, (size_t)n_sets * 8, cudaMemcpyHostToDevice, st));
+    if (!geo.empty()) SSB_CUDA_TRY(cudaMemcpyAsync(ws.fsets.p + n_sets, geo.data(), geo.size() * 8, cudaMemcpyHostToDevice, st));
+    v.filt = ws.filt.p; v.filt_sets = ws.fsets.p;
     *any = true;
     return SSB_OK;
 }
@@ -2367,141 +2336,112 @@ int32_t LexIndex::stage_batch(LexWorkspace& ws, cudaStream_t st, const ssb_lex_b
     }
     if (total_terms && !q->term_keys) { set_error("search_lexical: null term_keys"); return SSB_E_INVALID; }
     if ((uint64_t)nq * (levels_.size() ? levels_.size() : 1) >= 0xFFFFFFFFull) { set_error("batch too large: n_queries * n_levels must be < 2^32"); return SSB_E_UNSUPPORTED; }
-    SSB_TRY(ensure_workspace(ws, nq, total_terms));
-    SSB_CUDA_TRY(to_device(ws.qoff, q->term_offsets, ((size_t)nq + 1) * 4, st));
-    SSB_CUDA_TRY(to_device(ws.qkeys, q->term_keys, (size_t)total_terms * 8, st));
-    if (q->term_flags) SSB_CUDA_TRY(to_device(ws.qflags, q->term_flags, (size_t)total_terms, st));
+    SSB_TRY(ensure_workspace(ws, st, nq, total_terms));
+    SSB_CUDA_TRY(to_device(ws.qoff.p, q->term_offsets, ((size_t)nq + 1) * 4, st));
+    SSB_CUDA_TRY(to_device(ws.qkeys.p, q->term_keys, (size_t)total_terms * 8, st));
+    if (q->term_flags) SSB_CUDA_TRY(to_device(ws.qflags.p, q->term_flags, (size_t)total_terms, st));
     v = view();
     *filtered = false; *geo = false; *fmask_dev = nullptr;
     if (q->filter_offsets) SSB_TRY(stage_filters(ws, st, q, v, filtered, geo));
     if (q->field_masks && n_fields_ > 1) {                   // field_filter: one bitmask of indexed fields per query (host array)
         if (is_device_ptr(q->field_masks)) { set_error("search_lexical: field_masks must be a host array"); return SSB_E_INVALID; }
-        if (!ws.fmask) SSB_CUDA_TRY(cudaMalloc(&ws.fmask, (size_t)ws.cap_q * 4));
-        SSB_CUDA_TRY(cudaMemcpyAsync(ws.fmask, q->field_masks, (size_t)nq * 4, cudaMemcpyHostToDevice, st));
-        *fmask_dev = ws.fmask;
+        SSB_TRY(ws.fmask.reserve(nq, 0, st, true));
+        SSB_CUDA_TRY(cudaMemcpyAsync(ws.fmask.p, q->field_masks, (size_t)nq * 4, cudaMemcpyHostToDevice, st));
+        *fmask_dev = ws.fmask.p;
     }
+    return SSB_OK;
+}
+
+int32_t LexIndex::plan_batch(LexWorkspace& ws, cudaStream_t st, const ssb_lex_batch* q, bool topk_only, const SortDev* sort, uint64_t* glist,
+                            Batch* b, uint64_t* launches) const {
+    if (!committed_) { set_error("search before ssb_lexical_commit"); return SSB_E_STATE; }
+    if (!q || (q->n_queries && (!q->term_offsets || !glist))) { set_error("search_lexical: null argument"); return SSB_E_INVALID; }
+    if (q->query_type > SSB_QUERY_PHRASE) { set_error("bad query_type"); return SSB_E_INVALID; }
+    b->phrase = q->query_type == SSB_QUERY_PHRASE ? 1u : 0u;
+    if (b->phrase && has_positions_ != 1) { set_error("phrase query: the index holds no term positions (ssb_level_desc.positions)"); return SSB_E_STATE; }
+    if (b->phrase && q->term_flags) { set_error("phrase query: NOT terms are not accepted inside a phrase batch"); return SSB_E_UNSUPPORTED; }
+    b->qt_eff = b->phrase ? (uint32_t)SSB_QUERY_INTERSECTION : q->query_type;   // a phrase is an intersection + the position check
+    b->nq = q->n_queries;
+    if (b->nq == 0) return SSB_OK;
+    const uint32_t* fmask_dev = nullptr;
+    SSB_TRY(stage_batch(ws, st, q, b->v, &b->filtered, &b->geo, &fmask_dev));
+    b->geo = b->geo || (sort && sort_has_point(*sort));
+    // a batch with a POINT filter plans without flag bit 1: EVERY filtered query of that batch (its range / set filters too) leaves the
+    // lex_score record path for lex_generic<.., GEO>, so that lex_score keeps its code and registers; unfiltered queries stay on it
+    const uint32_t topk_flag = topk_only && !b->geo ? 2u : 0u;
+    SSB_CUDA_TRY(cudaMemsetAsync(ws.ctr.p, 0, 32, st));
+    uint32_t n_pow2 = 2; while (n_pow2 < b->v.n_levels) n_pow2 <<= 1;
+    const size_t plan_smem = (size_t)b->v.n_levels * (8 + 2 * FAST_T) + 16 + (size_t)n_pow2 * 8;
+    auto plan = sort ? lex_plan<true> : lex_plan<false>;
+    if (plan_smem > 48 * 1024) SSB_CUDA_TRY(cudaFuncSetAttribute(plan, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan_smem));
+    plan<<<b->nq, 128, plan_smem, st>>>(b->v, ws.qoff.p, ws.qkeys.p, q->term_flags ? ws.qflags.p : nullptr, b->filtered ? ws.foff.p : nullptr, fmask_dev,
+                                        b->phrase | topk_flag, b->qt_eff, ws.plans.p, ws.recs.p, ws.item_start.p, ws.ctr.p, ws.theta.p, ws.lock.p,
+                                        ws.count.p, glist, n_pow2, ITEM_W, 2, GMAX, sort ? *sort : SortDev{});
+    SSB_CUDA_TRY(cudaGetLastError());
+    if (launches) *launches += 1;
     return SSB_OK;
 }
 
 int32_t LexIndex::search_keys(LexWorkspace& ws, cudaStream_t st, const ssb_lex_batch* q, uint32_t k, uint32_t result_type,
                               uint64_t* keys_out_dev, uint64_t* count_dev, uint64_t* launches, const uint64_t* ceil_dev, const SortDev* sort) const {
-    if (!committed_) { set_error("search before ssb_lexical_commit"); return SSB_E_STATE; }
-    if (!q || (q->n_queries && (!q->term_offsets || !keys_out_dev))) { set_error("search_lexical: null argument"); return SSB_E_INVALID; }
     if (k > SSB_K_MAX) { set_error("k=%u exceeds SSB_K_MAX=%u", k, SSB_K_MAX); return SSB_E_UNSUPPORTED; }
-    if (result_type > SSB_RESULT_TOPKCOUNT || q->query_type > SSB_QUERY_PHRASE) { set_error("bad result_type/query_type"); return SSB_E_INVALID; }
-    const uint32_t phrase = q->query_type == SSB_QUERY_PHRASE ? 1u : 0u;
-    if (phrase && has_positions_ != 1) { set_error("phrase query: the index holds no term positions (ssb_level_desc.positions)"); return SSB_E_STATE; }
-    if (phrase && q->term_flags) { set_error("phrase query: NOT terms are not accepted inside a phrase batch"); return SSB_E_UNSUPPORTED; }
-    const uint32_t qt_eff = phrase ? (uint32_t)SSB_QUERY_INTERSECTION : q->query_type;   // a phrase is an intersection + the position check
+    if (result_type > SSB_RESULT_TOPKCOUNT) { set_error("bad result_type"); return SSB_E_INVALID; }
     if (result_type != SSB_RESULT_COUNT && k == 0) result_type = SSB_RESULT_COUNT;   // search.rs:2472-2478
-    const uint32_t nq = q->n_queries;
-    if (nq == 0) return SSB_OK;
-    LexView v;
-    bool filtered = false, geo = false;
-    const uint32_t* fmask_dev = nullptr;
-    SSB_TRY(stage_batch(ws, st, q, v, &filtered, &geo, &fmask_dev));
-    geo = geo || (sort && sort_has_point(*sort));
-    // a batch with a POINT filter plans without flag bit 1: EVERY filtered query of that batch (its range / set filters too) leaves the
-    // lex_score record path for lex_generic<.., GEO>, so that lex_score keeps its code and registers; unfiltered queries stay on it
-    const uint32_t topk_flag = result_type == SSB_RESULT_TOPK && !geo ? 2u : 0u;
-    SSB_CUDA_TRY(cudaMemsetAsync(ws.ctr, 0, 32, st));
-    SSB_CUDA_TRY(cudaMemsetAsync(ws.stats, 0, sizeof(LexStats), st));
-
-    uint32_t n_pow2 = 1; while (n_pow2 < v.n_levels) n_pow2 <<= 1;
-    if (n_pow2 < 2) n_pow2 = 2;
-    size_t plan_smem = (size_t)v.n_levels * (8 + 2 * FAST_T) + 16 + (size_t)n_pow2 * 8;
-    // keys_out_dev doubles as the per-query global list (32 u64 per query); copy_out masks the entries >= k afterwards
+    // keys_out_dev doubles as the per-query global list (32 u64 per query, 32 x 2 sorted); copy_out masks the entries >= k afterwards
     uint64_t* glist = keys_out_dev;
-    // item shape (tunable for experiments; defaults measured on C3): target postings per item, levels of a query's first item, levels per item
-    static const uint32_t item_w = env_u32("SSB_LEX_ITEM_W", ITEM_W, 64, 1u << 20), first_lim = env_u32("SSB_LEX_FIRST", 2, 1, GMAX),
-                          gmax = env_u32("SSB_LEX_GMAX", GMAX, 1, GMAX), grid_mult = env_u32("SSB_LEX_GRID", SSB_LEX_MINB, 1, 16);
-    const bool is_and = qt_eff == SSB_QUERY_INTERSECTION;
-    const bool want_topk = result_type != SSB_RESULT_COUNT && k > 0;
+    Batch b;
+    SSB_TRY(plan_batch(ws, st, q, result_type == SSB_RESULT_TOPK, sort, glist, &b, launches));
+    if (b.nq == 0) return SSB_OK;
+    SSB_CUDA_TRY(cudaMemsetAsync(ws.stats.p, 0, sizeof(LexStats), st));   // lex_plan keeps no stats
+    const uint32_t nq = b.nq, kk = k ? k : 1;
+    const LexView& v = b.v;
+    if (ws.ev0) cudaEventRecord(ws.ev0, st);
     const bool need_count = result_type != SSB_RESULT_TOPK;
-    const uint32_t kk = k ? k : 1;
-    if (sort) {
-        // sorted batch: every query takes lex_generic with 128-bit keys; keys_out_dev is its [nq][32][2] global list, left unmasked (callers
-        // read the first k entries), counted as usual
-        if (!ws.theta2) SSB_CUDA_TRY(cudaMalloc(&ws.theta2, (size_t)ws.cap_q * 16));
-        if (plan_smem > 48 * 1024) SSB_CUDA_TRY(cudaFuncSetAttribute(lex_plan<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan_smem));
-        lex_plan<true><<<nq, 128, plan_smem, st>>>(v, ws.qoff, ws.qkeys, q->term_flags ? ws.qflags : nullptr, filtered ? ws.foff : nullptr, fmask_dev, phrase | topk_flag, qt_eff, ws.plans, ws.recs, ws.item_start, ws.ctr, ws.theta2, ws.lock, ws.count, glist, n_pow2,
-                                                   item_w, first_lim, gmax, *sort);
-        SSB_CUDA_TRY(cudaGetLastError());
-        if (ws.ev0) cudaEventRecord(ws.ev0, st);
-        auto generic = (phrase && n_fields_ > 1) ? (geo ? lex_generic<true, true, true> : lex_generic<true, true>)
-                                                 : (geo ? lex_generic<false, true, true> : lex_generic<false, true>);
-        generic<<<n_sms_ * 2, 256, 0, st>>>(v, ws.plans, ws.recs, ws.item_start, nq, qt_eff, result_type, kk, ws.ctr, ws.theta2, ws.lock, ws.count, glist, ws.stats, ceil_dev, *sort);
-        SSB_CUDA_TRY(cudaGetLastError());
-        if (need_count) {
-            lex_not_count<<<n_sms_ * 4, 256, 0, st>>>(v, ws.plans, nq, qt_eff, ws.ctr, ws.count);
+    // a sorted batch: every query takes lex_generic with 128-bit keys; keys_out_dev is left unmasked (callers read the first k entries)
+    if (!sort) {
+        if (result_type != SSB_RESULT_COUNT) {
+            // batches that carry NOT terms ('-' operator) run their own instantiation: the common kernel stays free of the out-of-line probe
+            const bool hn = q->term_flags != nullptr || b.filtered;
+            auto score = b.qt_eff == SSB_QUERY_INTERSECTION ? (hn ? lex_score<true, true> : lex_score<true, false>)
+                                                            : (hn ? lex_score<false, true> : lex_score<false, false>);
+            score<<<n_sms_ * SSB_LEX_MINB, 256, 0, st>>>(v, ws.plans.p, ws.recs.p, ws.item_start.p, nq, kk, ws.ctr.p, ws.theta.p, ws.lock.p, glist, ws.stats.p, ceil_dev);
             SSB_CUDA_TRY(cudaGetLastError());
-            if (v.n_del) {
-                const uint64_t pairs = (uint64_t)nq * v.n_del;
-                lex_del_count<<<(unsigned)((pairs + 255) / 256), 256, 0, st>>>(v, ws.plans, nq, qt_eff, ws.count);
-                SSB_CUDA_TRY(cudaGetLastError());
-                if (launches) *launches += 1;
-            }
             if (launches) *launches += 1;
         }
-        if (ws.ev1) cudaEventRecord(ws.ev1, st);
-        if (count_dev) SSB_CUDA_TRY(cudaMemcpyAsync(count_dev, ws.count, (size_t)nq * 8, cudaMemcpyDeviceToDevice, st));
-        if (launches) *launches += 2;   // plan + generic
-        return SSB_OK;
+        if (need_count) {
+            lex_count<<<n_sms_ * 6, 128, 0, st>>>(v, ws.plans.p, ws.recs.p, ws.item_start.p, nq, b.qt_eff, ws.ctr.p, ws.count.p, ws.stats.p);
+            SSB_CUDA_TRY(cudaGetLastError());
+            if (launches) *launches += 1;
+        }
     }
-    if (plan_smem > 48 * 1024) SSB_CUDA_TRY(cudaFuncSetAttribute(lex_plan<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan_smem));
-    lex_plan<false><<<nq, 128, plan_smem, st>>>(v, ws.qoff, ws.qkeys, q->term_flags ? ws.qflags : nullptr, filtered ? ws.foff : nullptr, fmask_dev, phrase | topk_flag, qt_eff, ws.plans, ws.recs, ws.item_start, ws.ctr, ws.theta, ws.lock, ws.count, glist, n_pow2,
-                                                item_w, first_lim, gmax, SortDev{});
+    // unsorted: queries with 5..16 live terms (the kernel returns at once when the batch has none)
+    const bool runs = b.phrase && n_fields_ > 1;
+    auto generic = sort ? (runs ? (b.geo ? lex_generic<true, true, true> : lex_generic<true, true>) : (b.geo ? lex_generic<false, true, true> : lex_generic<false, true>))
+                        : (runs ? (b.geo ? lex_generic<true, false, true> : lex_generic<true, false>) : (b.geo ? lex_generic<false, false, true> : lex_generic<false, false>));
+    generic<<<n_sms_ * 2, 256, 0, st>>>(v, ws.plans.p, ws.recs.p, ws.item_start.p, nq, b.qt_eff, result_type, kk, ws.ctr.p, ws.theta.p, ws.lock.p, ws.count.p, glist,
+                                        ws.stats.p, ceil_dev, sort ? *sort : SortDev{});
     SSB_CUDA_TRY(cudaGetLastError());
-    if (ws.ev0) cudaEventRecord(ws.ev0, st);
-    if (want_topk) {
-        const int grid = n_sms_ * (int)grid_mult;
-        // batches that carry NOT terms ('-' operator) run their own instantiation: the common kernel stays free of the out-of-line probe
-        const bool hn = q->term_flags != nullptr || filtered;
-#define SSB_LAUNCH_SCORE(A, N) lex_score<A, N><<<grid, 256, 0, st>>>(v, ws.plans, ws.recs, ws.item_start, nq, kk, ws.ctr, ws.theta, ws.lock, glist, ws.stats, ceil_dev)
-#define SSB_LAUNCH_SCORE_ALL() do { if (is_and) { if (hn) SSB_LAUNCH_SCORE(true, true); else SSB_LAUNCH_SCORE(true, false); } \
-                                    else { if (hn) SSB_LAUNCH_SCORE(false, true); else SSB_LAUNCH_SCORE(false, false); } } while (0)
-        SSB_LAUNCH_SCORE_ALL();
-#undef SSB_LAUNCH_SCORE_ALL
-#undef SSB_LAUNCH_SCORE
-        SSB_CUDA_TRY(cudaGetLastError());
-        if (launches) *launches += 1;
-    }
-    if (need_count) {
-        lex_count<<<n_sms_ * 6, 128, 0, st>>>(v, ws.plans, ws.recs, ws.item_start, nq, qt_eff, ws.ctr, ws.count, ws.stats);
-        SSB_CUDA_TRY(cudaGetLastError());
-        if (launches) *launches += 1;
-    }
-    // queries with 5..16 live terms (the kernel returns at once when the batch has none)
-    auto generic = (phrase && n_fields_ > 1) ? (geo ? lex_generic<true, false, true> : lex_generic<true, false>)
-                                             : (geo ? lex_generic<false, false, true> : lex_generic<false, false>);
-    generic<<<n_sms_ * 2, 256, 0, st>>>(v, ws.plans, ws.recs, ws.item_start, nq, qt_eff, result_type, kk, ws.ctr, ws.theta, ws.lock, ws.count, glist, ws.stats, ceil_dev, SortDev{});
-    SSB_CUDA_TRY(cudaGetLastError());
+    if (launches) *launches += 1;
     if (need_count) {     // returns at once unless some query of the batch carries NOT terms
-        lex_not_count<<<n_sms_ * 4, 256, 0, st>>>(v, ws.plans, nq, qt_eff, ws.ctr, ws.count);
+        lex_not_count<<<n_sms_ * 4, 256, 0, st>>>(v, ws.plans.p, nq, b.qt_eff, ws.ctr.p, ws.count.p);
         SSB_CUDA_TRY(cudaGetLastError());
         if (launches) *launches += 1;
-    }
-    if (need_count && v.n_del) {
-        const uint64_t pairs = (uint64_t)nq * v.n_del;
-        lex_del_count<<<(unsigned)((pairs + 255) / 256), 256, 0, st>>>(v, ws.plans, nq, qt_eff, ws.count);
-        SSB_CUDA_TRY(cudaGetLastError());
-        if (launches) *launches += 1;
+        if (v.n_del) {
+            const uint64_t pairs = (uint64_t)nq * v.n_del;
+            lex_del_count<<<(unsigned)((pairs + 255) / 256), 256, 0, st>>>(v, ws.plans.p, nq, b.qt_eff, ws.count.p);
+            SSB_CUDA_TRY(cudaGetLastError());
+            if (launches) *launches += 1;
+        }
     }
     if (ws.ev1) cudaEventRecord(ws.ev1, st);
-    copy_out<<<(nq * LIST + 255) / 256, 256, 0, st>>>(glist, ws.count, nq, result_type == SSB_RESULT_COUNT ? 0 : k, keys_out_dev, count_dev);
+    if (sort) {
+        if (count_dev) SSB_CUDA_TRY(cudaMemcpyAsync(count_dev, ws.count.p, (size_t)nq * 8, cudaMemcpyDeviceToDevice, st));
+        return SSB_OK;
+    }
+    copy_out<<<(nq * LIST + 255) / 256, 256, 0, st>>>(glist, ws.count.p, nq, result_type == SSB_RESULT_COUNT ? 0 : k, keys_out_dev, count_dev);
     SSB_CUDA_TRY(cudaGetLastError());
-    if (launches) *launches += 3;   // plan + generic + copy_out
+    if (launches) *launches += 1;
     return SSB_OK;
-}
-
-// (re)allocate a device buffer of at least n elements (contents are not kept)
-template <typename T>
-static cudaError_t grow(T*& p, size_t& cap, size_t n) {
-    if (n <= cap) return cudaSuccess;
-    cudaFree(p); p = nullptr; cap = 0;
-    const cudaError_t e = cudaMalloc(&p, n * sizeof(T));
-    if (e == cudaSuccess) cap = n;
-    return e;
 }
 
 constexpr size_t FACET_HIST_BYTES = 256ull << 20;   // per search context: the histograms of one query chunk
@@ -2509,15 +2449,13 @@ constexpr size_t FACET_HIST_BYTES = 256ull << 20;   // per search context: the h
 int32_t LexIndex::facet_counts(LexWorkspace& ws, cudaStream_t st, const ssb_lex_batch* q, const ssb_facet_request* req, uint32_t n_req,
                                const double* bases, ssb_facet_count* out, uint32_t* n_out, uint64_t* launches, uint64_t* kernel_ns,
                                uint64_t* alg_bytes) const {
-    if (!committed_) { set_error("search before ssb_lexical_commit"); return SSB_E_STATE; }
-    if (!q || (n_req && !req) || (q->n_queries && (!q->term_offsets || (n_req && (!out || !n_out))))) { set_error("search_lexical_facets: null argument"); return SSB_E_INVALID; }
+    if (!q || (n_req && !req) || (q->n_queries && n_req && (!out || !n_out))) { set_error("search_lexical_facets: null argument"); return SSB_E_INVALID; }
     if (n_req > SSB_MAX_FACET_REQUESTS) { set_error("search_lexical_facets: %u requests, at most %u", n_req, SSB_MAX_FACET_REQUESTS); return SSB_E_UNSUPPORTED; }
-    if (q->query_type > SSB_QUERY_PHRASE) { set_error("bad query_type"); return SSB_E_INVALID; }
-    const uint32_t phrase = q->query_type == SSB_QUERY_PHRASE ? 1u : 0u;
-    if (phrase && has_positions_ != 1) { set_error("phrase query: the index holds no term positions (ssb_level_desc.positions)"); return SSB_E_STATE; }
-    if (phrase && q->term_flags) { set_error("phrase query: NOT terms are not accepted inside a phrase batch"); return SSB_E_UNSUPPORTED; }
-    const uint32_t qt_eff = phrase ? (uint32_t)SSB_QUERY_INTERSECTION : q->query_type;
-    const uint32_t nq = q->n_queries;
+    // ---- the batch and its plans (Count: every match, no top-k) ----
+    SSB_TRY(ws.fglist.reserve((size_t)q->n_queries * LIST, 0, st, true));
+    Batch b;
+    SSB_TRY(plan_batch(ws, st, q, false, nullptr, ws.fglist.p, &b, launches));
+    const uint32_t nq = b.nq;
     if (nq == 0 || n_req == 0) return SSB_OK;
     if (!facets_ || !facets_->n_facets) { set_error("search_lexical_facets: facet counts need ssb_set_facets"); return SSB_E_STATE; }
     if (bases && is_device_ptr(bases)) { set_error("search_lexical_facets: bases must be a host array"); return SSB_E_INVALID; }
@@ -2548,61 +2486,46 @@ int32_t LexIndex::facet_counts(LexWorkspace& ws, cudaStream_t st, const ssb_lex_
         return SSB_E_UNSUPPORTED;
     }
     const uint32_t chunk = (uint32_t)std::min<uint64_t>(nq, FACET_HIST_BYTES / 4 / (hist_words ? hist_words : 1));
-    // ---- the batch and its plans (Count: every match, no top-k) ----
-    LexView v;
-    bool filtered = false, geo = false;
-    const uint32_t* fmask_dev = nullptr;
-    SSB_TRY(stage_batch(ws, st, q, v, &filtered, &geo, &fmask_dev));
-    if (!ws.fhist) SSB_CUDA_TRY(cudaMalloc(&ws.fhist, FACET_HIST_BYTES));
-    if (!ws.freq) SSB_CUDA_TRY(cudaMalloc(&ws.freq, SSB_MAX_FACET_REQUESTS * sizeof(FacetReqDev)));
-    if (!ws.fstarts) SSB_CUDA_TRY(cudaMalloc(&ws.fstarts, (size_t)SSB_MAX_FACET_REQUESTS * SSB_MAX_FACET_RANGES * 8));
-    if (!ws.fstats) SSB_CUDA_TRY(cudaMalloc(&ws.fstats, 4 * 8));
-    SSB_CUDA_TRY(grow(ws.fout, ws.cap_fout, (size_t)chunk * (out_stride ? out_stride : 1)));
-    SSB_CUDA_TRY(grow(ws.fnout, ws.cap_fnout, (size_t)chunk * n_req));
-    SSB_CUDA_TRY(grow(ws.fglist, ws.cap_fglist, (size_t)nq * LIST));
-    SSB_CUDA_TRY(cudaMemcpyAsync(ws.freq, rd.data(), n_req * sizeof(FacetReqDev), cudaMemcpyHostToDevice, st));
-    if (!starts.empty()) SSB_CUDA_TRY(cudaMemcpyAsync(ws.fstarts, starts.data(), starts.size() * 8, cudaMemcpyHostToDevice, st));
+    SSB_TRY(ws.fhist.reserve(FACET_HIST_BYTES / 4, 0, st, true));
+    SSB_TRY(ws.freq.reserve(SSB_MAX_FACET_REQUESTS, 0, st, true));
+    SSB_TRY(ws.fstarts.reserve((size_t)SSB_MAX_FACET_REQUESTS * SSB_MAX_FACET_RANGES, 0, st, true));
+    SSB_TRY(ws.fstats.reserve(4, 0, st, true));
+    SSB_TRY(ws.fout.reserve((size_t)chunk * (out_stride ? out_stride : 1), 0, st, true));
+    SSB_TRY(ws.fnout.reserve((size_t)chunk * n_req, 0, st, true));
+    SSB_CUDA_TRY(cudaMemcpyAsync(ws.freq.p, rd.data(), n_req * sizeof(FacetReqDev), cudaMemcpyHostToDevice, st));
+    if (!starts.empty()) SSB_CUDA_TRY(cudaMemcpyAsync(ws.fstarts.p, starts.data(), starts.size() * 8, cudaMemcpyHostToDevice, st));
     if (n_point) {
-        SSB_CUDA_TRY(grow(ws.fbases, ws.cap_fbases, (size_t)nq * n_point * 2));
-        SSB_CUDA_TRY(cudaMemcpyAsync(ws.fbases, bases, (size_t)nq * n_point * 16, cudaMemcpyHostToDevice, st));
+        SSB_TRY(ws.fbases.reserve((size_t)nq * n_point * 2, 0, st, true));
+        SSB_CUDA_TRY(cudaMemcpyAsync(ws.fbases.p, bases, (size_t)nq * n_point * 16, cudaMemcpyHostToDevice, st));
     }
-    SSB_CUDA_TRY(cudaMemsetAsync(ws.fstats, 0, 4 * 8, st));
-    SSB_CUDA_TRY(cudaMemsetAsync(ws.ctr, 0, 32, st));
-    uint32_t n_pow2 = 1; while (n_pow2 < v.n_levels) n_pow2 <<= 1;
-    if (n_pow2 < 2) n_pow2 = 2;
-    const size_t plan_smem = (size_t)v.n_levels * (8 + 2 * FAST_T) + 16 + (size_t)n_pow2 * 8;
-    if (plan_smem > 48 * 1024) SSB_CUDA_TRY(cudaFuncSetAttribute(lex_plan<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan_smem));
-    lex_plan<false><<<nq, 128, plan_smem, st>>>(v, ws.qoff, ws.qkeys, q->term_flags ? ws.qflags : nullptr, filtered ? ws.foff : nullptr, fmask_dev, phrase, qt_eff, ws.plans, ws.recs, ws.item_start, ws.ctr, ws.theta, ws.lock, ws.count, ws.fglist, n_pow2,
-                                                ITEM_W, 2, GMAX, SortDev{});
-    SSB_CUDA_TRY(cudaGetLastError());
-    if (launches) *launches += 1;
+    SSB_CUDA_TRY(cudaMemsetAsync(ws.fstats.p, 0, 4 * 8, st));
     // ---- per query chunk: the counts, the selection, the copy out ----
-    auto kern = (phrase && n_fields_ > 1) ? (geo ? lex_facets<true, true> : lex_facets<true, false>) : (geo ? lex_facets<false, true> : lex_facets<false, false>);
+    auto kern = (b.phrase && n_fields_ > 1) ? (b.geo ? lex_facets<true, true> : lex_facets<true, false>) : (b.geo ? lex_facets<false, true> : lex_facets<false, false>);
     const size_t smem = starts.size() * 8 + n_req * sizeof(FacetReqDev) + FACET_WARPS * (sizeof(FacetWarpSm) + (size_t)range_words * 4);
     if (smem > 48 * 1024) SSB_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    FacetCall fc{ws.freq, n_req, ws.fstarts, (uint32_t)starts.size(), ws.fbases, n_point, ws.fhist, (uint32_t)hist_words, range_words, ws.fstats};
+    FacetCall fc{ws.freq.p, n_req, ws.fstarts.p, (uint32_t)starts.size(), ws.fbases.p, n_point, ws.fhist.p, (uint32_t)hist_words, range_words, ws.fstats.p};
     RankPtrs rk{};
     for (uint32_t f = 0; f < fs.n_facets && f < SSB_MAX_FACETS; f++) rk.p[f] = fs.d_rank[f];
     cudaEvent_t e0 = ws.ev0, e1 = ws.ev1;
     float ms_sum = 0.f;
     for (uint32_t q0 = 0; q0 < nq; q0 += chunk) {
         const uint32_t nqc = std::min(chunk, nq - q0);
-        SSB_CUDA_TRY(cudaMemsetAsync(ws.fhist, 0, (size_t)nqc * hist_words * 4, st));
+        SSB_CUDA_TRY(cudaMemsetAsync(ws.fhist.p, 0, (size_t)nqc * hist_words * 4, st));
         if (e0) cudaEventRecord(e0, st);
-        kern<<<n_sms_ * 4, FACET_WARPS * 32, smem, st>>>(v, ws.plans, ws.recs, q0, nqc, qt_eff, fc);
+        kern<<<n_sms_ * 4, FACET_WARPS * 32, smem, st>>>(b.v, ws.plans.p, ws.recs.p, q0, nqc, b.qt_eff, fc);
         SSB_CUDA_TRY(cudaGetLastError());
         if (e1) cudaEventRecord(e1, st);
-        facet_select<<<dim3(n_req, nqc), 256, 0, st>>>(ws.freq, n_req, ws.fhist, (uint32_t)hist_words, rk, ws.fout, (uint32_t)out_stride, ws.fnout);
+        facet_select<<<dim3(n_req, nqc), 256, 0, st>>>(ws.freq.p, n_req, ws.fhist.p, (uint32_t)hist_words, rk, ws.fout.p, (uint32_t)out_stride, ws.fnout.p);
         SSB_CUDA_TRY(cudaGetLastError());
         if (launches) *launches += 2;
-        if (out_stride) SSB_CUDA_TRY(cudaMemcpyAsync(out + (size_t)q0 * out_stride, ws.fout, (size_t)nqc * out_stride * sizeof(ssb_facet_count), cudaMemcpyDeviceToHost, st));
-        SSB_CUDA_TRY(cudaMemcpyAsync(n_out + (size_t)q0 * n_req, ws.fnout, (size_t)nqc * n_req * 4, cudaMemcpyDeviceToHost, st));
+        if (out_stride) SSB_CUDA_TRY(cudaMemcpyAsync(out + (size_t)q0 * out_stride, ws.fout.p, (size_t)nqc * out_stride * sizeof(ssb_facet_count), cudaMemcpyDeviceToHost, st));
+        SSB_CUDA_TRY(cudaMemcpyAsync(n_out + (size_t)q0 * n_req, ws.fnout.p, (size_t)nqc * n_req * 4, cudaMemcpyDeviceToHost, st));
         SSB_CUDA_TRY(cudaStreamSynchronize(st));
         float ms = 0.f;
         if (e0 && e1 && cudaEventElapsedTime(&ms, e0, e1) == cudaSuccess) ms_sum += ms; else cudaGetLastError();
     }
     uint64_t fst[4] = {0, 0, 0, 0};
-    SSB_CUDA_TRY(cudaMemcpy(fst, ws.fstats, 4 * 8, cudaMemcpyDeviceToHost));
+    SSB_CUDA_TRY(cudaMemcpy(fst, ws.fstats.p, 4 * 8, cudaMemcpyDeviceToHost));
     if (kernel_ns) *kernel_ns = (uint64_t)((double)ms_sum * 1e6);
     if (alg_bytes) *alg_bytes = fst[0] * 4 + fst[1] * 8 + fst[2] * n_req * 8;
     return SSB_OK;
@@ -2610,7 +2533,7 @@ int32_t LexIndex::facet_counts(LexWorkspace& ws, cudaStream_t st, const ssb_lex_
 
 LexStats LexIndex::read_stats(const LexWorkspace& ws, cudaStream_t st) {
     LexStats s{};
-    if (ws.stats) { cudaMemcpyAsync(&s, ws.stats, sizeof(s), cudaMemcpyDeviceToHost, st); cudaStreamSynchronize(st); }
+    if (ws.stats.p) { cudaMemcpyAsync(&s, ws.stats.p, sizeof(s), cudaMemcpyDeviceToHost, st); cudaStreamSynchronize(st); }
     return s;
 }
 

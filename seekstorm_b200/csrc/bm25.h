@@ -43,6 +43,12 @@ struct DevBuf {
     }
 };
 
+inline bool is_device_ptr(const void* p) {
+    cudaPointerAttributes a;
+    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
+    return a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
+}
+
 // scoped device temporary (freed on every exit path, including SSB_CUDA_TRY early returns)
 template <typename T>
 struct DevTmp {
@@ -156,29 +162,19 @@ struct LexStats { uint64_t postings_visited, probes, items_processed, items_skip
 
 // Per-call scratch of one search context (api.cu keeps a pool of them: concurrent searches on one index do not share any).
 struct LexWorkspace {
-    uint32_t cap_q = 0, cap_terms = 0, cap_levels = 0;
-    QueryPlan* plans = nullptr; uint64_t* items = nullptr; LvRec* recs = nullptr; uint16_t* item_start = nullptr;
-    uint64_t* theta = nullptr; int* lock = nullptr; uint64_t* count = nullptr; uint32_t* ctr = nullptr; /* [0] score / [2] count / [3] generic work counters, [1] max_items, [4] any query with > 4 live terms */
-    uint32_t* qoff = nullptr; uint64_t* qkeys = nullptr; uint8_t* qflags = nullptr; LexStats* stats = nullptr;
-    uint32_t* foff = nullptr; uint32_t* fmask = nullptr; FiltDev* filt = nullptr; uint64_t* fsets = nullptr; uint32_t cap_filt = 0, cap_fsets = 0;   // facet filters of the batch
-    uint64_t* theta2 = nullptr;   // sorted batches: [cap_q][2] 128-bit θ {hi, lo}
-    // sorted batches with a POINT criterion: [n_queries][2] bases, staged before search_keys — kept across release(), which
-    // ensure_workspace calls when the batch outgrows the workspace
-    double* bases = nullptr; uint32_t cap_bases = 0;
-    // facet count calls (facet_counts), kept across release() like `bases`: the value / range histograms of one query chunk (allocated on
-    // the first call, FACET_HIST_BYTES), the call's requests, range starts and Point bases, the selected counts of the chunk, the plan's
-    // scratch list and the call's work counters {postings, dense words, counted docs}
-    uint32_t* fhist = nullptr; FacetReqDev* freq = nullptr; uint64_t* fstarts = nullptr; uint64_t* fstats = nullptr;
-    double* fbases = nullptr; size_t cap_fbases = 0;
-    ssb_facet_count* fout = nullptr; uint32_t* fnout = nullptr; size_t cap_fout = 0, cap_fnout = 0;
-    uint64_t* fglist = nullptr; size_t cap_fglist = 0;
-    void release_facets();
+    DevBuf<QueryPlan> plans; DevBuf<LvRec> recs; DevBuf<uint16_t> item_start;
+    DevBuf<uint64_t> theta;   // [n][2]: the 64-bit θ of an unsorted batch in the first n words, the 128-bit θ {hi, lo} of a sorted one
+    DevBuf<int> lock; DevBuf<uint64_t> count;
+    DevBuf<uint32_t> ctr;     // [0] score / [2] count / [3] generic work counters, [1] max_items, [4] any query with > 4 live terms
+    DevBuf<uint32_t> qoff; DevBuf<uint64_t> qkeys; DevBuf<uint8_t> qflags; DevBuf<LexStats> stats;
+    DevBuf<uint32_t> foff, fmask; DevBuf<FiltDev> filt; DevBuf<uint64_t> fsets;   // facet filters and field masks of the batch
+    DevBuf<double> bases;     // sorted batches with a POINT criterion: [n_queries][2] bases, staged before search_keys
+    // facet count calls (facet_counts): the value / range histograms of one query chunk (FACET_HIST_BYTES), the call's requests, range
+    // starts and Point bases, the selected counts of the chunk, the plan's scratch list and the call's work counters {postings, dense
+    // words, counted docs}
+    DevBuf<uint32_t> fhist; DevBuf<FacetReqDev> freq; DevBuf<uint64_t> fstarts, fstats;
+    DevBuf<double> fbases; DevBuf<ssb_facet_count> fout; DevBuf<uint32_t> fnout; DevBuf<uint64_t> fglist;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;   // recorded around lex_score when set
-    void release();
-    ~LexWorkspace() { release(); cudaFree(bases); release_facets(); }
-    LexWorkspace() = default;
-    LexWorkspace(const LexWorkspace&) = delete;
-    LexWorkspace& operator=(const LexWorkspace&) = delete;
 };
 
 class LexIndex {
@@ -219,7 +215,13 @@ public:
     uint32_t n_levels() const { return (uint32_t)levels_.size(); }
 
 private:
-    int32_t ensure_workspace(LexWorkspace& ws, uint32_t nq, uint32_t total_terms) const;
+    struct Batch { LexView v; uint32_t nq, phrase, qt_eff; bool filtered, geo; };
+    // the start of search_keys and facet_counts: the batch checks, stage_batch and the one lex_plan launch (lex_plan<true> when `sort` is
+    // set), which zeroes glist ([n_queries][32] keys, [n_queries][32][2] when sorted).  topk_only: a Topk batch, whose queries plan
+    // without counts unless the batch has a POINT filter or sort criterion (b->geo).  b->nq = 0: an empty batch, nothing staged or launched
+    int32_t plan_batch(LexWorkspace& ws, cudaStream_t st, const ssb_lex_batch* q, bool topk_only, const SortDev* sort, uint64_t* glist,
+                       Batch* b, uint64_t* launches) const;
+    int32_t ensure_workspace(LexWorkspace& ws, cudaStream_t st, uint32_t nq, uint32_t total_terms) const;
     int32_t stage_filters(LexWorkspace& ws, cudaStream_t st, const ssb_lex_batch* q, LexView& v, bool* any, bool* geo_any) const;
     // what every lexical batch starts with: the per-query term checks, the workspace, the terms, the facet filters (*filtered, *geo: a
     // POINT filter) and the field masks (*fmask_dev, null = none) on the device; v: the view with the batch's filters
