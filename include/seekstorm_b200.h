@@ -355,6 +355,31 @@ typedef struct {
 typedef struct { uint32_t value; uint32_t pad; uint64_t count; } ssb_facet_count;   /* value: id (VALUES) or range index (RANGES) */
 int32_t ssb_search_lexical_facets(ssb_index* ix, const ssb_lex_batch* q, const ssb_facet_request* req, uint32_t n_req,
                                   const double* bases, ssb_facet_count* out, uint32_t* n_out);
+/* The empty query (Search::search("", enable_empty_query = true, ..): search_iterator_shard iterator.rs:316-358 with add_result.rs:95-338,
+ * and search_iterator_index iterator.rs:360-413): a batch of filter-only queries over every document.
+ *   Batch: q supplies n_queries and the facet filters (filter_offsets / filters / filter_set_values, exactly as for ssb_search_lexical).
+ *     Terms must be absent: term_offsets NULL or all zero (HOST array), else SSB_E_INVALID.  field_masks and query_type are ignored.
+ *   Documents: the doc ids of the added lexical levels (level << 16 | 0 .. n_docs - 1) outside the delete set — the reference's
+ *     0 .. indexed_doc_count when every level but the last is full, which is how the reference writes its levels.  A doc passes when every
+ *     filter of its query accepts it (is_facet_filter); a doc without a facet row fails every filter.
+ *   Order: the criteria are those of ssb_search_lexical_sorted_ex (the same validation, 64-bit budget and Point bases).  A LEADING `_score`
+ *     orders by the doc id in its own direction, as the index route does (deviation: with a filter the reference's shard route keeps the
+ *     first k docs in heap order); a later `_score` compares equal scores and ends the comparison.  Ties on every criterion, and no
+ *     criterion at all, go to the doc id DESCENDING (min_heap.rs:535-536, search.rs:3575-3579).  Hits carry score 0.
+ *   Counts: count_total is exact for Count / TopkCount (unspecified for Topk); Count ignores the sort.  An unfiltered Count costs no kernel.
+ *   k up to SSB_K_LIMIT (paged like ssb_search_lexical).  Not on a handle with a communicator (SSB_E_UNSUPPORTED). */
+int32_t ssb_search_empty(ssb_index* ix, const ssb_lex_batch* q, const ssb_sort_criterion* sort, uint32_t n_sort, const double* bases,
+                         uint32_t k, uint32_t result_type, ssb_hit* hits, uint32_t* n_hits, uint64_t* count_total);
+/* Facet counts of the empty query (get_index_string_facets_shard, index.rs:4441-4569): not counts over matches but the index-wide
+ * per-value counters ingest keeps.  One result set for the call: out HOST [sum of caps] (caps as for ssb_search_lexical_facets),
+ * n_out HOST [n_req].
+ *   VALUES (String16 / String32): the `length` ids with the most facet rows, over EVERY row given to ssb_set_facets (no filter, deleted docs
+ *     included, as the reference's counters are never decremented); count descending, then id ascending; has_prefix restricts to a
+ *     value-order rank interval as in ssb_search_lexical_facets.  Deviation: a row whose id is 0 because its doc had no value is counted
+ *     under id 0.
+ *   RANGES: validated, n_out = 0 (the reference returns no range facets for the empty query).
+ * Not on a handle with a communicator (SSB_E_UNSUPPORTED). */
+int32_t ssb_search_empty_facets(ssb_index* ix, const ssb_facet_request* req, uint32_t n_req, ssb_facet_count* out, uint32_t* n_out);
 /* queries: [n_queries, dims] f32; Cosine: normalised by the callee (search.rs:1464-1475).  score = dot
  * (Dot/Cosine) or -Σ(q-x)² (Euclidean) exactly as Result.score in vector.rs:1489. */
 int32_t ssb_search_vector(ssb_index* ix, const float* queries, uint32_t n_queries, uint32_t k,

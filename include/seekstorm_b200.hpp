@@ -178,11 +178,12 @@ public:
                         size_t length, ResultType result_type, bool include_uncommitted = false,
                         const std::vector<std::string>& field_filter = {}, size_t n_query_facets = 0,
                         const std::vector<FacetFilter>& facet_filter = {}, const std::vector<ResultSort>& result_sort = {}) const {
-        (void)enable_empty_query;
         if (include_uncommitted || n_query_facets)
             throw Error(SSB_E_UNSUPPORTED, "facet counts / uncommitted search are outside the GPU hot path");
         if (!result_sort.empty() && search_mode.kind != SearchMode::Lexical)
             throw Error(SSB_E_UNSUPPORTED, "result_sort on vector / hybrid search is not built");
+        if (enable_empty_query && query_string.empty() && !query_vector && search_mode.kind == SearchMode::Lexical)
+            return search_empty(offset, length, result_type, facet_filter, result_sort);
         // field_filter: names of indexed fields (set_field_names, schema order) -> field_filter_set as a bitmask
         uint32_t field_mask = 0;
         for (auto& name : field_filter) {
@@ -238,33 +239,15 @@ public:
             uint32_t offs[2] = {0, static_cast<uint32_t>(keys.size())};
             ssb_lex_batch b{1, static_cast<uint32_t>(qt), offs, keys.data(), not_terms.empty() ? nullptr : flags.data(), nullptr, nullptr, nullptr, nullptr};
             // facet_filter (search.rs:735-860 -> FilterSparse per facet): applied to every candidate of the lexical search
-            std::vector<ssb_facet_filter> ff; std::vector<uint64_t> set_values;
-            uint32_t foffs[2] = {0, static_cast<uint32_t>(facet_filter.size())};
-            for (auto& f : facet_filter) {
-                ssb_facet_filter c{};
-                c.facet = f.facet; c.kind = f.point ? SSB_FILTER_POINT : f.values.empty() ? SSB_FILTER_RANGE : SSB_FILTER_SET; c.start = f.start; c.end = f.end;
-                c.set_first = static_cast<uint32_t>(set_values.size());
-                if (f.point) {                // payload: base lat / lon as f64 bits, the unit
-                    uint64_t la, lo; std::memcpy(&la, &f.lat, 8); std::memcpy(&lo, &f.lon, 8);
-                    set_values.insert(set_values.end(), {la, lo, static_cast<uint64_t>(f.unit)});
-                    c.set_count = 3;
-                } else {
-                    c.set_count = static_cast<uint32_t>(f.values.size());
-                    set_values.insert(set_values.end(), f.values.begin(), f.values.end());
-                }
-                ff.push_back(c);
-            }
-            if (!ff.empty()) { b.filter_offsets = foffs; b.filters = ff.data(); b.filter_set_values = set_values.data(); }
+            Filters fs(facet_filter);
+            fs.apply(b);
             if (field_mask) b.field_masks = &field_mask;
             const uint32_t k = rt == ResultType::Count ? 0u : static_cast<uint32_t>(heap);
             lex.resize(k ? k : 1);
             uint32_t n = 0;
-            std::vector<ssb_sort_criterion> sc;
-            double base[2] = {0.0, 0.0}; bool has_base = false;   // the Point criterion's FacetValue::Point base (one query: one base)
-            for (auto& r : result_sort) {
-                sc.push_back(ssb_sort_criterion{r.source, r.facet, static_cast<uint32_t>(r.order), 0});
-                if (r.has_base && !has_base) { base[0] = r.lat; base[1] = r.lon; has_base = true; }
-            }
+            Sort so(result_sort);
+            const std::vector<ssb_sort_criterion>& sc = so.sc;
+            const double* base = so.base; const bool has_base = so.has_base;
             if (sc.empty()) check(ssb_search_lexical(h_, &b, k, static_cast<uint32_t>(rt), lex.data(), &n, &total));
             else check(ssb_search_lexical_sorted_ex(h_, &b, sc.data(), static_cast<uint32_t>(sc.size()), has_base ? base : nullptr, k,
                                                     static_cast<uint32_t>(rt), lex.data(), &n, &total));
@@ -302,6 +285,82 @@ public:
     }
 
 private:
+    // one query's facet filters in ABI form (ssb_facet_filter + filter_set_values), kept alive next to the batch that points at them
+    struct Filters {
+        std::vector<ssb_facet_filter> ff; std::vector<uint64_t> set_values; uint32_t foffs[2] = {0, 0};
+        explicit Filters(const std::vector<FacetFilter>& facet_filter) {
+            for (auto& f : facet_filter) {
+                ssb_facet_filter c{};
+                c.facet = f.facet; c.kind = f.point ? SSB_FILTER_POINT : f.values.empty() ? SSB_FILTER_RANGE : SSB_FILTER_SET; c.start = f.start; c.end = f.end;
+                c.set_first = static_cast<uint32_t>(set_values.size());
+                if (f.point) {                // payload: base lat / lon as f64 bits, the unit
+                    uint64_t la, lo; std::memcpy(&la, &f.lat, 8); std::memcpy(&lo, &f.lon, 8);
+                    set_values.insert(set_values.end(), {la, lo, static_cast<uint64_t>(f.unit)});
+                    c.set_count = 3;
+                } else {
+                    c.set_count = static_cast<uint32_t>(f.values.size());
+                    set_values.insert(set_values.end(), f.values.begin(), f.values.end());
+                }
+                ff.push_back(c);
+            }
+            foffs[1] = static_cast<uint32_t>(ff.size());
+        }
+        void apply(ssb_lex_batch& b) { if (!ff.empty()) { b.filter_offsets = foffs; b.filters = ff.data(); b.filter_set_values = set_values.data(); } }
+    };
+    // result_sort in ABI form and the Point criterion's FacetValue::Point base (one query: one base)
+    struct Sort {
+        std::vector<ssb_sort_criterion> sc; double base[2] = {0.0, 0.0}; bool has_base = false;
+        explicit Sort(const std::vector<ResultSort>& result_sort) {
+            for (auto& r : result_sort) {
+                sc.push_back(ssb_sort_criterion{r.source, r.facet, static_cast<uint32_t>(r.order), 0});
+                if (r.has_base && !has_base) { base[0] = r.lat; base[1] = r.lon; has_base = true; }
+            }
+        }
+    };
+    // Search::search("", enable_empty_query = true, ..): the index route (search.rs:1413-1432, iterator.rs:360-413) without facet filter and
+    // with at most one _id / _score criterion — the live doc ids from the largest (ascending when that criterion is Ascending), total = the
+    // live docs for every result type; else the shard route (iterator.rs:316-358) — the filters and the sort through ssb_search_empty,
+    // counted under Count / TopkCount, total 0 under Topk.
+    ResultObject search_empty(size_t offset, size_t length, ResultType result_type, const std::vector<FacetFilter>& facet_filter,
+                              const std::vector<ResultSort>& result_sort) const {
+        ResultObject ro;
+        ResultType rt = result_type;
+        const bool index_route = facet_filter.empty() &&
+                                 (result_sort.empty() || (result_sort.size() == 1 && result_sort[0].source != SSB_SORT_FACET));
+        uint32_t offs[2] = {0, 0};
+        ssb_lex_batch b{1, SSB_QUERY_UNION, offs, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+        std::vector<ssb_hit> hits;
+        uint32_t n = 0;
+        uint64_t total = 0;
+        if (index_route) {
+            check(ssb_search_empty(h_, &b, nullptr, 0, nullptr, 0, SSB_RESULT_COUNT, nullptr, &n, &total));
+            ro.result_count_total = total;
+            if (rt != ResultType::Count && length) {
+                const ssb_sort_criterion asc{SSB_SORT_ID, 0, SSB_SORT_ASCENDING, 0};
+                const bool up = !result_sort.empty() && result_sort[0].order == SortOrder::Ascending;
+                hits.resize(offset + length);
+                check(ssb_search_empty(h_, &b, up ? &asc : nullptr, up ? 1u : 0u, nullptr, static_cast<uint32_t>(offset + length), SSB_RESULT_TOPK,
+                                       hits.data(), &n, &total));
+            }
+        } else {
+            if (length == 0 && rt != ResultType::Count) {              // search.rs:2472-2478
+                if (rt == ResultType::Topk) return ro;
+                rt = ResultType::Count;
+            }
+            Filters fs(facet_filter);
+            fs.apply(b);
+            Sort so(rt == ResultType::Count ? std::vector<ResultSort>{} : result_sort);
+            const uint32_t k = rt == ResultType::Count ? 0u : static_cast<uint32_t>(offset + length);
+            hits.resize(k ? k : 1);
+            check(ssb_search_empty(h_, &b, so.sc.data(), static_cast<uint32_t>(so.sc.size()), so.has_base ? so.base : nullptr, k,
+                                   static_cast<uint32_t>(rt), hits.data(), &n, &total));
+            ro.result_count_total = rt == ResultType::Topk ? 0 : total;
+        }
+        for (size_t i = offset; i < n && ro.results.size() < length; i++) ro.results.push_back({hits[i].doc_id, hits[i].score});
+        ro.result_count = ro.results.size();
+        return ro;
+    }
+
     ssb_index* h_ = nullptr;
     TermKeyFn key_fn_;
     VectorSimilarity sim_;

@@ -339,12 +339,13 @@ int32_t shard_sum_counts(ssb_index* ix, SearchCtx& c, uint64_t* counts_dev, uint
 
 // Paging state of the host-facing search calls (k > SSB_K_MAX, or de-duplication of multi-chunk documents).  W = words per key:
 // 1 = the 64-bit (score, doc) keys, 2 = the 128-bit keys {hi, lo} of a sorted lexical search, lo = pack_key(score, doc) with its score
-// half inverted when score_inv (`_score` ascending).
+// half inverted when score_inv (`_score` ascending).  doc_desc: lo = pack_key(0, 0xFFFFFFFF - doc) of an empty-query search (ties by doc
+// id descending).
 template <int W>
 struct PageState {
-    SearchCtx& c; uint32_t nq, k; ssb_hit* hits; uint32_t* n_hits; std::vector<uint32_t> cnt; std::vector<uint8_t> open; bool dedup, score_inv;
-    PageState(SearchCtx& c_, uint32_t nq_, uint32_t k_, ssb_hit* h, uint32_t* n, bool dedup_ = false, bool score_inv_ = false)
-        : c(c_), nq(nq_), k(k_), hits(h), n_hits(n), cnt(nq_, 0), open(nq_, 1), dedup(dedup_), score_inv(score_inv_) {
+    SearchCtx& c; uint32_t nq, k; ssb_hit* hits; uint32_t* n_hits; std::vector<uint32_t> cnt; std::vector<uint8_t> open; bool dedup, score_inv, doc_desc;
+    PageState(SearchCtx& c_, uint32_t nq_, uint32_t k_, ssb_hit* h, uint32_t* n, bool dedup_ = false, bool score_inv_ = false, bool doc_desc_ = false)
+        : c(c_), nq(nq_), k(k_), hits(h), n_hits(n), cnt(nq_, 0), open(nq_, 1), dedup(dedup_), score_inv(score_inv_), doc_desc(doc_desc_) {
         c.h_ceil.assign(((size_t)nq_ + 256) * W, 0);
     }
     // consume one [nq][32] page that was fetched with `kk` results per query; returns true if any query wants another page
@@ -361,7 +362,7 @@ struct PageState {
                 if (empty) break;
                 seen++; last = key;
                 const uint64_t lo = key[W - 1];
-                const uint64_t doc = key_doc(lo);
+                const uint64_t doc = doc_desc ? (uint32_t)lo : key_doc(lo);
                 if (dedup) {
                     bool dup = false;
                     for (uint32_t i = 0; i < cnt[q]; i++) dup = dup || hits[(size_t)q * k + i].doc_id == doc;
@@ -484,6 +485,43 @@ int32_t search_lexical_host(ssb_index* ix, SearchCtx& c, const ssb_lex_batch* q,
     // the 1-byte coarse-table lookups of the stream filter are not counted
     c.stats.algorithmic_bytes = ls.postings_visited * 4 + ls.probes * 16 + ls.recs_processed * 128 + ls.dense_words * 8;
     c.stats.probes = ls.probes; c.stats.items_processed = ls.items_processed; c.stats.items_skipped = ls.items_skipped;
+    return SSB_OK;
+}
+
+// host-facing empty-query search: the first page of <= SSB_K_MAX hits with the counts, then pages below the previous page's last key
+int32_t search_empty_host(ssb_index* ix, SearchCtx& c, const ssb_lex_batch* q, uint32_t k, uint32_t result_type, ssb_hit* hits, uint32_t* n_hits,
+                          uint64_t* count_total, const SortDev& sort) {
+    const uint32_t nq = q->n_queries;
+    SSB_TRY(c.keys_a.reserve((size_t)nq * LIST * 2, 0, c.st));
+    SSB_TRY(c.counts.reserve(nq, 0, c.st));
+    c.h_keys_a.resize((size_t)nq * LIST * 2); c.h_counts.resize(nq);
+    const bool want_hits = hits && k && result_type != SSB_RESULT_COUNT;
+    const uint32_t k1 = want_hits ? (k < SSB_K_MAX ? k : SSB_K_MAX) : 0;
+    EmptyStats es{};
+    SSB_TRY(ix->lex->search_empty(c.lex, c.st, q, k1, result_type, sort, c.keys_a.p, c.counts.p, nullptr, &es));
+    SSB_CUDA_TRY(cudaMemcpyAsync(c.h_keys_a.data(), c.keys_a.p, (size_t)nq * LIST * 16, cudaMemcpyDeviceToHost, c.st));
+    SSB_CUDA_TRY(cudaMemcpyAsync(c.h_counts.data(), c.counts.p, (size_t)nq * 8, cudaMemcpyDeviceToHost, c.st));
+    SSB_CUDA_TRY(cudaStreamSynchronize(c.st));
+    c.stats.d2h_bytes += (uint64_t)nq * (LIST * 16 + 8);
+    c.ev_used = true;
+    finish_stats(ix, c);                                        // the first page's scan is the one reported
+    if (want_hits) {
+        PageState<2> ps(c, nq, k, hits, n_hits, false, false, true);
+        bool more = ps.append(c.h_keys_a.data(), k1);
+        while (more) {
+            const uint32_t kk = ps.next_page_k();
+            SSB_TRY(ps.upload_ceilings());
+            SSB_TRY(ix->lex->search_empty(c.lex, c.st, q, kk, SSB_RESULT_TOPK, sort, c.keys_a.p, nullptr, c.ceil.p, &es));
+            SSB_CUDA_TRY(cudaMemcpyAsync(c.h_keys_a.data(), c.keys_a.p, (size_t)nq * LIST * 16, cudaMemcpyDeviceToHost, c.st));
+            SSB_CUDA_TRY(cudaStreamSynchronize(c.st));
+            c.stats.d2h_bytes += (uint64_t)nq * LIST * 16;
+            more = ps.append(c.h_keys_a.data(), kk);
+        }
+        ps.finish();
+    } else if (n_hits) for (uint32_t i = 0; i < nq; i++) n_hits[i] = 0;
+    if (count_total) for (uint32_t i = 0; i < nq; i++) count_total[i] = c.h_counts[i];
+    c.stats.kernel_launches += es.launches; c.stats.algorithmic_bytes = es.alg_bytes;
+    c.stats.items_processed = es.items_processed; c.stats.items_skipped = es.items_skipped;
     return SSB_OK;
 }
 
@@ -853,7 +891,7 @@ int32_t ssb_set_deleted(ssb_index* ix, const uint64_t* doc_ids, uint64_t n) {
     docs.erase(std::unique(docs.begin(), docs.end()), docs.end());
     for (auto& c : ix->pool) cudaStreamSynchronize(c->own_st);
     ix->del.release();
-    if (docs.empty()) return SSB_OK;
+    if (docs.empty()) { ix->lex->refresh_live_docs(); return SSB_OK; }
     std::vector<uint32_t> slot(65536, 0xFFFFFFFFu);
     uint32_t n_slots = 0;
     for (uint32_t d : docs) if (slot[d >> 16] == 0xFFFFFFFFu) slot[d >> 16] = n_slots++;
@@ -866,6 +904,8 @@ int32_t ssb_set_deleted(ssb_index* ix, const uint64_t* doc_ids, uint64_t n) {
     SSB_CUDA_TRY(cudaMemcpy(ix->del.d_words, words.data(), words.size() * 8, cudaMemcpyHostToDevice));
     SSB_CUDA_TRY(cudaMemcpy(ix->del.d_docs, docs.data(), docs.size() * 4, cudaMemcpyHostToDevice));
     ix->del.n = (uint32_t)docs.size();
+    ix->del.h_docs = std::move(docs);
+    ix->lex->refresh_live_docs();
     return SSB_OK;
     SSB_API_END
 }
@@ -1070,6 +1110,58 @@ int32_t ssb_search_lexical_facets(ssb_index* ix, const ssb_lex_batch* q, const s
     SearchCtx& c = *l.c;
     return ix->lex->facet_counts(c.lex, c.st, q, req, n_req, bases, out, n_out, &c.stats.kernel_launches, &c.stats.dominant_kernel_ns,
                                  &c.stats.algorithmic_bytes);
+    SSB_API_END
+}
+
+// Search::search("", enable_empty_query = true, ..) on committed data: a batch of filter-only queries over every live doc of the levels
+int32_t ssb_search_empty(ssb_index* ix, const ssb_lex_batch* q, const ssb_sort_criterion* sort, uint32_t n_sort, const double* bases, uint32_t k,
+                         uint32_t result_type, ssb_hit* hits, uint32_t* n_hits, uint64_t* count_total) {
+    SSB_API_BEGIN
+    if (!ix || !q || (n_sort && !sort) || (q->n_queries && k && result_type != SSB_RESULT_COUNT && !hits)) { set_error("ssb_search_empty: null argument"); return SSB_E_INVALID; }
+    if (result_type > SSB_RESULT_TOPKCOUNT) { set_error("ssb_search_empty: bad result_type"); return SSB_E_INVALID; }
+    std::shared_lock<std::shared_mutex> g(ix->rw);
+    SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
+    if (ix->comm.active()) { set_error("ssb_search_empty: the empty query across shards is not built"); return SSB_E_UNSUPPORTED; }
+    if (k > SSB_K_LIMIT) { set_error("k=%u exceeds SSB_K_LIMIT=%u", k, SSB_K_LIMIT); return SSB_E_UNSUPPORTED; }
+    if (n_sort > SSB_MAX_SORT_CRITERIA) { set_error("ssb_search_empty: more than %u criteria", SSB_MAX_SORT_CRITERIA); return SSB_E_UNSUPPORTED; }
+    // a leading `_score` orders by doc id in its own direction (the index route, iterator.rs:360-413); a later one compares the all-zero
+    // scores and ends the comparison, ties then go to the larger doc id (min_heap.rs:535-536)
+    ssb_sort_criterion crit[SSB_MAX_SORT_CRITERIA];
+    for (uint32_t i = 0; i < n_sort; i++) crit[i] = sort[i];
+    if (n_sort && crit[0].source == SSB_SORT_SCORE) crit[0].source = SSB_SORT_ID;
+    SortDev sd{}; bool sorted = false;
+    SSB_TRY(ix->lex->prepare_sort(crit, n_sort, bases != nullptr, &sd, &sorted));
+    if (sd.n == 0) {                                            // no criterion: doc id descending
+        const ssb_sort_criterion id_desc{SSB_SORT_ID, 0, SSB_SORT_DESCENDING, 0};
+        SSB_TRY(ix->lex->prepare_sort(&id_desc, 1, false, &sd, &sorted));
+    }
+    if (q->n_queries == 0) return SSB_OK;
+    CtxLease l(ix); SSB_TRY(l.acquire());
+    if ((result_type == SSB_RESULT_COUNT || k == 0) && !(q->filter_offsets && q->filter_offsets[q->n_queries])) {
+        if (!ix->lex->committed()) { set_error("search before ssb_lexical_commit"); return SSB_E_STATE; }
+        for (uint32_t i = 0; i < q->n_queries; i++) {           // unfiltered counts: the live docs, no kernel
+            if (count_total) count_total[i] = ix->lex->live_docs();
+            if (n_hits) n_hits[i] = 0;
+        }
+        return SSB_OK;
+    }
+    SSB_TRY(LexIndex::stage_sort_bases(l.c->lex, l.c->st, bases, q->n_queries, &sd));
+    return search_empty_host(ix, *l.c, q, k, result_type, hits, n_hits, count_total, sd);
+    SSB_API_END
+}
+
+int32_t ssb_search_empty_facets(ssb_index* ix, const ssb_facet_request* req, uint32_t n_req, ssb_facet_count* out, uint32_t* n_out) {
+    SSB_API_BEGIN
+    if (!ix) { set_error("ssb_search_empty_facets: null argument"); return SSB_E_INVALID; }
+    std::shared_lock<std::shared_mutex> g(ix->rw);
+    SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
+    if (ix->comm.active()) { set_error("ssb_search_empty_facets: facet counts across shards are not built"); return SSB_E_UNSUPPORTED; }
+    CtxLease l(ix); SSB_TRY(l.acquire());
+    SearchCtx& c = *l.c;
+    EmptyStats es{};
+    SSB_TRY(ix->lex->empty_facets(c.lex, c.st, req, n_req, out, n_out, &es));
+    c.stats.kernel_launches = es.launches; c.stats.algorithmic_bytes = es.alg_bytes; c.stats.dominant_kernel_ns = es.kernel_ns;
+    return SSB_OK;
     SSB_API_END
 }
 

@@ -36,6 +36,7 @@
 // cache computed on the host.
 #include "bm25.h"
 #include "facets.cuh"
+#include "sort_list.cuh"
 
 #include <algorithm>
 #include <cuda_fp16.h>
@@ -696,61 +697,6 @@ __device__ __forceinline__ void insert_candidates(uint64_t& L, uint32_t& thr, bo
     dirty = true;
     uint32_t kth = (uint32_t)(shfl64(L, (int)k - 1) >> 32);
     if (kth > thr) thr = kth;
-}
-
-// ---- sorted batches: 128-bit top-k keys (hi = packed sort key, lo = pack_key(score, doc)), warp lists descending like wl_* ----
-__device__ __forceinline__ bool gt128(uint64_t ah, uint64_t al, uint64_t bh, uint64_t bl) { return ah > bh || (ah == bh && al > bl); }
-__device__ __forceinline__ void wl_insert128(uint64_t& Lh, uint64_t& Ll, uint64_t ch, uint64_t cl, int lane) {
-    const int pos = __popc(__ballot_sync(FULL, !gt128(ch, cl, Lh, Ll)));   // entries >= cand stay in front
-    if (__any_sync(FULL, Lh == ch && Ll == cl)) return;
-    const uint64_t uh = shfl64_up1(Lh), ul = shfl64_up1(Ll);
-    if (lane == pos) { Lh = ch; Ll = cl; }
-    else if (lane > pos) { Lh = uh; Ll = ul; }
-}
-__device__ __forceinline__ void wl_merge128(uint64_t& Ah, uint64_t& Al, uint64_t Bh, uint64_t Bl, int lane) {
-    const uint64_t rh = shfl64(Bh, 31 - lane), rl = shfl64(Bl, 31 - lane);
-    if (gt128(rh, rl, Ah, Al)) { Ah = rh; Al = rl; }                   // bitonic, holds the top 32 of the union
-#pragma unroll
-    for (int s = 16; s >= 1; s >>= 1) {
-        const uint64_t ph = shfl64_xor(Ah, s), pl = shfl64_xor(Al, s);
-        const bool keep_max = (lane & s) == 0;
-        if (keep_max == gt128(ph, pl, Ah, Al)) { Ah = ph; Al = pl; }
-    }
-}
-// the warp's list of one sorted item; thr = a lower bound of θ.hi (global θ.hi, or the local list's k-th hi once it is full)
-struct SortTop { uint64_t h, l, thr; };
-// insert the lanes' candidates (cand) below the paging ceiling (ch, cl) into the warp list; raise thr from the k-th entry
-__device__ __forceinline__ void insert_sorted(SortTop& T, bool cand, uint64_t hi, float score, uint32_t doc, bool score_asc,
-                                              uint32_t k, int lane, bool& dirty, uint64_t ch, uint64_t cl) {
-    const uint64_t lo = pack_key(score, doc) ^ (score_asc ? 0xFFFFFFFF00000000ull : 0ull);
-    unsigned m = __ballot_sync(FULL, cand && gt128(ch, cl, hi, lo));
-    if (!m) return;
-    while (m) {
-        const int src = __ffs(m) - 1; m &= m - 1;
-        wl_insert128(T.h, T.l, shfl64(hi, src), shfl64(lo, src), lane);
-    }
-    dirty = true;
-    const uint64_t kth = shfl64(T.h, (int)k - 1);
-    if (kth > T.thr) T.thr = kth;
-}
-// merge the warp's list into the query's global list (glist [q][32][2], theta [q][2]) under the per-query lock.  Readers outside the lock
-// load θ.hi alone — the pair can tear, θ.hi never decreases — and prune only docs with hi < θ.hi.
-__device__ __forceinline__ void publish_sorted(const SortTop& T, uint32_t q, uint32_t k, int lane, uint64_t* theta, int* lock, uint64_t* glist) {
-    if (lane == 0) { while (atomicCAS(&lock[q], 0, 1) != 0) __nanosleep(40); }
-    __syncwarp();
-    __threadfence();
-    uint64_t* g = glist + ((size_t)q * LIST + lane) * 2;
-    uint64_t Mh = T.h, Ml = T.l;
-    wl_merge128(Mh, Ml, __ldcg(&g[0]), __ldcg(&g[1]), lane);
-    __stcg(&g[0], Mh); __stcg(&g[1], Ml);
-    const uint64_t nh = shfl64(Mh, (int)k - 1), nl = shfl64(Ml, (int)k - 1);
-    __threadfence();
-    __syncwarp();
-    if (lane == 0) {
-        if (gt128(nh, nl, __ldcg(&theta[2 * q]), __ldcg(&theta[2 * q + 1]))) { __stcg(&theta[2 * q + 1], nl); __stcg(&theta[2 * q], nh); }
-        __threadfence();
-        atomicExch(&lock[q], 0);
-    }
 }
 
 struct ItemCtx {
@@ -1902,6 +1848,15 @@ __global__ void __launch_bounds__(256) facet_select(const FacetReqDev* __restric
 }
 
 // ================================================================= host side
+int32_t launch_facet_select(const FacetSet& fs, const FacetReqDev* req, uint32_t n_req, const uint32_t* hist, uint32_t hist_words, uint32_t nq,
+                            ssb_facet_count* out, uint32_t out_stride, uint32_t* n_out, cudaStream_t st) {
+    RankPtrs rk{};
+    for (uint32_t f = 0; f < fs.n_facets && f < SSB_MAX_FACETS; f++) rk.p[f] = fs.d_rank[f];
+    facet_select<<<dim3(n_req, nq), 256, 0, st>>>(req, n_req, hist, hist_words, rk, out, out_stride, n_out);
+    SSB_CUDA_TRY(cudaGetLastError());
+    return SSB_OK;
+}
+
 LexIndex::~LexIndex() {
     for (auto& l : levels_) { cudaFree(l.d_term_keys); cudaFree(l.d_posting_offsets); }
     free_committed();
@@ -2207,6 +2162,7 @@ int32_t LexIndex::commit(uint64_t n_docs, uint64_t len_sum) {
     }
     SSB_CUDA_TRY(cudaStreamSynchronize(st_));
     committed_ = true;
+    refresh_live_docs();
     return SSB_OK;
 }
 
@@ -2504,8 +2460,6 @@ int32_t LexIndex::facet_counts(LexWorkspace& ws, cudaStream_t st, const ssb_lex_
     const size_t smem = starts.size() * 8 + n_req * sizeof(FacetReqDev) + FACET_WARPS * (sizeof(FacetWarpSm) + (size_t)range_words * 4);
     if (smem > 48 * 1024) SSB_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     FacetCall fc{ws.freq.p, n_req, ws.fstarts.p, (uint32_t)starts.size(), ws.fbases.p, n_point, ws.fhist.p, (uint32_t)hist_words, range_words, ws.fstats.p};
-    RankPtrs rk{};
-    for (uint32_t f = 0; f < fs.n_facets && f < SSB_MAX_FACETS; f++) rk.p[f] = fs.d_rank[f];
     cudaEvent_t e0 = ws.ev0, e1 = ws.ev1;
     float ms_sum = 0.f;
     for (uint32_t q0 = 0; q0 < nq; q0 += chunk) {
@@ -2515,8 +2469,7 @@ int32_t LexIndex::facet_counts(LexWorkspace& ws, cudaStream_t st, const ssb_lex_
         kern<<<n_sms_ * 4, FACET_WARPS * 32, smem, st>>>(b.v, ws.plans.p, ws.recs.p, q0, nqc, b.qt_eff, fc);
         SSB_CUDA_TRY(cudaGetLastError());
         if (e1) cudaEventRecord(e1, st);
-        facet_select<<<dim3(n_req, nqc), 256, 0, st>>>(ws.freq.p, n_req, ws.fhist.p, (uint32_t)hist_words, rk, ws.fout.p, (uint32_t)out_stride, ws.fnout.p);
-        SSB_CUDA_TRY(cudaGetLastError());
+        SSB_TRY(launch_facet_select(fs, ws.freq.p, n_req, ws.fhist.p, (uint32_t)hist_words, nqc, ws.fout.p, (uint32_t)out_stride, ws.fnout.p, st));
         if (launches) *launches += 2;
         if (out_stride) SSB_CUDA_TRY(cudaMemcpyAsync(out + (size_t)q0 * out_stride, ws.fout.p, (size_t)nqc * out_stride * sizeof(ssb_facet_count), cudaMemcpyDeviceToHost, st));
         SSB_CUDA_TRY(cudaMemcpyAsync(n_out + (size_t)q0 * n_req, ws.fnout.p, (size_t)nqc * n_req * 4, cudaMemcpyDeviceToHost, st));

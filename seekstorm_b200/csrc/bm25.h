@@ -124,9 +124,11 @@ struct LexView {
 };
 
 // device-resident delete set shared by the lexical and the vector path
+// h_docs: the deleted doc ids, ascending, on the host (the live-doc count of the empty query)
 struct DeleteSet {
     uint32_t* d_slot = nullptr; uint64_t* d_words = nullptr; uint32_t* d_docs = nullptr; uint32_t n = 0;
-    void release() { cudaFree(d_slot); cudaFree(d_words); cudaFree(d_docs); d_slot = nullptr; d_words = nullptr; d_docs = nullptr; n = 0; }
+    std::vector<uint32_t> h_docs;
+    void release() { cudaFree(d_slot); cudaFree(d_words); cudaFree(d_docs); d_slot = nullptr; d_words = nullptr; d_docs = nullptr; n = 0; h_docs.clear(); }
 };
 
 struct QTerm { uint32_t first, n; float idf; uint32_t df; };
@@ -159,6 +161,9 @@ static_assert(sizeof(LvRec) == 128, "LvRec must be one 128-byte line");
 //   [29:32) n_live   live terms of the query (== n_pres for AND records)
 
 struct LexStats { uint64_t postings_visited, probes, items_processed, items_skipped, recs_processed, dense_words; };
+// the statistics of an empty-query call (ssb_last_stats): launches, the bytes the scan staged, (query, tile) pairs evaluated / skipped,
+// the CUDA-event time of the scan (or histogram) kernels
+struct EmptyStats { uint64_t launches, alg_bytes, items_processed, items_skipped, kernel_ns; };
 
 // Per-call scratch of one search context (api.cu keeps a pool of them: concurrent searches on one index do not share any).
 struct LexWorkspace {
@@ -174,6 +179,8 @@ struct LexWorkspace {
     // words, counted docs}
     DevBuf<uint32_t> fhist; DevBuf<FacetReqDev> freq; DevBuf<uint64_t> fstarts, fstats;
     DevBuf<double> fbases; DevBuf<ssb_facet_count> fout; DevBuf<uint32_t> fnout; DevBuf<uint64_t> fglist;
+    // empty-query calls (empty_query.cu): the call's tiles in scan order and its work counters (EQ_STAT_*)
+    DevBuf<uint2> etiles; DevBuf<unsigned long long> estats;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;   // recorded around lex_score when set
 };
 
@@ -204,6 +211,19 @@ public:
     int32_t facet_counts(LexWorkspace& ws, cudaStream_t st, const ssb_lex_batch* q, const ssb_facet_request* req, uint32_t n_req,
                          const double* bases, ssb_facet_count* out, uint32_t* n_out, uint64_t* launches, uint64_t* kernel_ns,
                          uint64_t* alg_bytes) const;
+    // ssb_search_empty (empty_query.cu): the filter-only batch q over every live doc of the levels, in the order of `sort` — prepared by
+    // prepare_sort, at least one criterion (the caller puts `_id` descending in place of none).  keys_out_dev: [n_queries][32] 128-bit keys
+    // {hi, lo}, lo = pack_key(0, 0xFFFFFFFF - doc): ties by doc id descending (unmasked: callers read the first k); count_dev: [n_queries]
+    // or null, exact unless Topk; ceil_dev: [n_queries][2] exclusive key ceilings of a further page, or null.  Asynchronous on st except
+    // for the host checks; the scan's time is recorded between ws.ev0 and ws.ev1.
+    int32_t search_empty(LexWorkspace& ws, cudaStream_t st, const ssb_lex_batch* q, uint32_t k, uint32_t result_type, const SortDev& sort,
+                         uint64_t* keys_out_dev, uint64_t* count_dev, const uint64_t* ceil_dev, EmptyStats* stats) const;
+    // ssb_search_empty_facets (synchronous): the top values of String facets over every facet row; RANGES requests give n_out 0
+    int32_t empty_facets(LexWorkspace& ws, cudaStream_t st, const ssb_facet_request* req, uint32_t n_req, ssb_facet_count* out,
+                         uint32_t* n_out, EmptyStats* stats) const;
+    // the docs of the levels outside the delete set: the count of an unfiltered empty query (kept by commit and refresh_live_docs)
+    uint64_t live_docs() const { return live_docs_; }
+    void refresh_live_docs();                    // after the delete set changed
     bool committed() const { return committed_; }
     void set_stream(cudaStream_t st) { st_ = st; }   // load-time stream (add_level / commit)
     void set_deleted(const DeleteSet* d) { del_ = d; }
@@ -250,9 +270,14 @@ private:
     std::vector<uint64_t> h_dict_keys_; std::vector<uint32_t> h_term_df_, h_local_df_;
     const DeleteSet* del_ = nullptr;
     const FacetSet* facets_ = nullptr;
+    uint64_t live_docs_ = 0;
     void free_committed();
     LexView view() const;
 };
+
+// bm25.cu: facet_select over the value / range histograms of nq queries (hist [nq][hist_words]) -> out [nq][out_stride], n_out [nq][n_req]
+int32_t launch_facet_select(const FacetSet& fs, const FacetReqDev* req, uint32_t n_req, const uint32_t* hist, uint32_t hist_words, uint32_t nq,
+                            ssb_facet_count* out, uint32_t out_stride, uint32_t* n_out, cudaStream_t st);
 
 // loader.cu: the reference's on-disk files -> index
 struct VectorLevel { uint32_t level_id; std::vector<uint16_t> ids; std::vector<float> rows; std::vector<uint32_t> cluster_counts; };

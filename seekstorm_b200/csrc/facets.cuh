@@ -1,5 +1,5 @@
 // facets.cuh — the device side of the facet key format (facets.h): the facet filter test, the geo distance test and the packed sort key
-// of sorted batches.  Included by bm25.cu only, after the lexical view (LexView) it reads.
+// of sorted batches.  Included by bm25.cu and empty_query.cu, after the lexical view (LexView) it reads.
 #pragma once
 #include "facets.h"
 
@@ -34,7 +34,7 @@ __device__ __forceinline__ double geo_distance(uint64_t code, double blat, doubl
 // FilterSparse::Point (add_result.rs:462-478): true = the doc is filtered OUT.  range.contains(code) on the Morton interval staged in
 // [lo, hi), then distance_range.contains(euclidian_distance(base, decode(code), unit)) (geo_search.rs:95-107).  g: the staged payload
 // (GEO_* words, f64 bits).  Out of line: only POINT filters reach it.
-__device__ __noinline__ bool geo_rejects_impl(uint64_t code, uint64_t lo, uint64_t hi, const uint64_t* g) {
+static __device__ __noinline__ bool geo_rejects_impl(uint64_t code, uint64_t lo, uint64_t hi, const uint64_t* g) {
     if (!(code >= lo && code < hi)) return true;
     const double blat = __longlong_as_double((long long)__ldg(&g[GEO_LAT])), blon = __longlong_as_double((long long)__ldg(&g[GEO_LON]));
     const double d = geo_distance(code, blat, blon, [&] { return __longlong_as_double((long long)__ldg(&g[GEO_RADIUS])); });
@@ -43,7 +43,7 @@ __device__ __noinline__ bool geo_rejects_impl(uint64_t code, uint64_t lo, uint64
 }
 // the sort key of a POINT criterion (morton_ordering, geo_search.rs:82-93): the order key of simplified_distance(decode(code), base) — the
 // F64 column key (f64_order_key: NaN = all ones, above +inf).  base: the query's (lat, lon).  Out of line: only POINT criteria reach it.
-__device__ __noinline__ uint64_t point_sort_key(uint64_t code, const double* base) {
+static __device__ __noinline__ uint64_t point_sort_key(uint64_t code, const double* base) {
     const double blat = __ldg(&base[0]), blon = __ldg(&base[1]);
     const double plat = morton_lat(code), plon = morton_lon(code);
     const double x = __dmul_rn(__dsub_rn(blon, plon), cos(__ddiv_rn(__dmul_rn(SSB_DEG2RAD, __dadd_rn(plat, blat)), 2.0)));
@@ -53,9 +53,22 @@ __device__ __noinline__ uint64_t point_sort_key(uint64_t code, const double* bas
 
 // is_facet_filter (add_result.rs:340-478): true = the doc is filtered OUT.  The typed range / set tests of the reference run on the
 // order-preserving 64-bit keys ssb_set_facets stored per doc and facet (bounds converted the same way by the host), so one unsigned
-// compare pair covers every FilterSparse range type.  Out of line, by value, on the rare candidate / count path of lex_generic only.
-struct FacetArgs { const uint64_t* keys; uint64_t rows; const FiltDev* filt; const uint64_t* sets; uint32_t first_doc; };
+// compare pair covers every FilterSparse range type.  filter_rejects_key is the test of one filter on one key: the column path below and
+// the staged rows of the empty-query scan (empty_query.cu) share it.  sets: the batch's filter_sets.
 // GEO: the batch holds a POINT filter — its own instantiation, so that the common one keeps its code and its callers their registers
+template <bool GEO>
+__device__ __forceinline__ bool filter_rejects_key(const FiltDev& f, uint64_t key, const uint64_t* sets) {
+    if (f.kind == FILT_RANGE) return !(key >= f.lo && key < f.hi);
+    if (f.kind == FILT_SET) {
+        bool in = false;
+        for (uint32_t s = 0; s < f.set_n; s++) in = in || __ldg(&sets[f.set_first + s]) == key;
+        return !in;
+    }
+    if (GEO && f.kind == FILT_POINT) return geo_rejects_impl(key, f.lo, f.hi, sets + f.set_first);
+    return true;
+}
+// Out of line, by value, on the rare candidate / count path of lex_generic only.
+struct FacetArgs { const uint64_t* keys; uint64_t rows; const FiltDev* filt; const uint64_t* sets; uint32_t first_doc; };
 template <bool GEO>
 __device__ __noinline__ bool facet_rejects_impl(FacetArgs a, uint32_t f0, uint32_t nf, uint32_t doc) {
     const uint64_t row = (uint64_t)doc - a.first_doc;
@@ -63,13 +76,7 @@ __device__ __noinline__ bool facet_rejects_impl(FacetArgs a, uint32_t f0, uint32
     for (uint32_t i = 0; i < nf; i++) {
         const FiltDev f = a.filt[f0 + i];
         const uint64_t key = __ldg(&a.keys[(size_t)f.facet * a.rows + row]);
-        if (f.kind == FILT_RANGE) { if (!(key >= f.lo && key < f.hi)) return true; }
-        else if (f.kind == FILT_SET) {
-            bool in = false;
-            for (uint32_t s = 0; s < f.set_n; s++) in = in || __ldg(&a.sets[f.set_first + s]) == key;
-            if (!in) return true;
-        } else if (GEO && f.kind == FILT_POINT) { if (geo_rejects_impl(key, f.lo, f.hi, a.sets + f.set_first)) return true; }
-        else return true;
+        if (filter_rejects_key<GEO>(f, key, a.sets)) return true;
     }
     return false;
 }
@@ -112,34 +119,39 @@ __device__ __forceinline__ uint64_t sort_pack_hi(const SortDev& s, const uint64_
 }
 // upper bound of hi over the docs of a level: per criterion the level's largest value (descending) or smallest (ascending, inverted by
 // the packing) — the block's zone for a facet, level << 16 | 0xFFFF or level << 16 for _id.  A Point criterion takes the trivial bound
-// (the largest key after packing): its zones hold Morton codes, not distances, and no level is skipped.
-__device__ __forceinline__ uint64_t level_sort_bound(const SortDev& s, uint32_t level_id) {
+// (the largest key after packing): its zones hold Morton codes, not distances, and no level is skipped.  id_lo / id_hi: the smallest and
+// largest doc id of the docs bounded when they are a part of the level (the empty-query scan bounds one tile of a level).
+__device__ __forceinline__ uint64_t level_sort_bound(const SortDev& s, uint32_t level_id, uint32_t id_lo = 0u, uint32_t id_hi = 0xFFFFu) {
     uint64_t val[SSB_MAX_SORT_CRITERIA];
     const uint32_t b = level_id - s.zone_block0;                       // prepare_sort: the zones cover every level
 #pragma unroll
     for (uint32_t i = 0; i < SSB_MAX_SORT_CRITERIA; i++) {
-        val[i] = s.desc[i] ? ((uint64_t)level_id << 16 | 0xFFFFu) : ((uint64_t)level_id << 16);
+        val[i] = s.desc[i] ? ((uint64_t)level_id << 16 | id_hi) : ((uint64_t)level_id << 16 | id_lo);
         if (i < s.n && s.src[i] == SORT_SRC_FACET)
             val[i] = s.type[i] == SSB_FACET_POINT ? (s.desc[i] ? ~0ull : 0ull) : s.zones[((size_t)s.facet[i] * s.n_zone_blocks + b) * 2 + (s.desc[i] ? 1 : 0)];
     }
     return sort_pack_hi(s, val);
 }
-// doc's packed sort key for query q: the facet column keys of its row (a String facet's id through its value order, a Point facet's code
-// through its distance to the query's base), or its id
-template <bool GEO>
-__device__ __forceinline__ uint64_t doc_sort_hi(const LexView& v, const SortDev& s, uint32_t doc, uint32_t q) {
-    const uint64_t row = (uint64_t)(doc - v.facet_first_doc);          // prepare_sort: the facet rows cover every doc of the levels
+// doc's packed sort key for query q: the facet keys of its row (a String facet's id through its value order, a Point facet's code
+// through its distance to the query's base), or its id.  key_of(i): criterion i's column key of the doc.
+template <bool GEO, class KeyOf>
+__device__ __forceinline__ uint64_t sort_hi_of(const SortDev& s, uint32_t doc, uint32_t q, KeyOf key_of) {
     uint64_t val[SSB_MAX_SORT_CRITERIA];
 #pragma unroll
     for (uint32_t i = 0; i < SSB_MAX_SORT_CRITERIA; i++) {
         val[i] = doc;
         if (i < s.n && s.src[i] == SORT_SRC_FACET) {
-            val[i] = __ldg(&v.facet_keys[(size_t)s.facet[i] * v.facet_rows + row]);
+            val[i] = key_of(i);
             if (s.rank[i]) val[i] = __ldg(&s.rank[i][val[i]]);          // sort_of_criteria: every id of the column has a rank
             else if (GEO && s.type[i] == SSB_FACET_POINT) val[i] = point_sort_key(val[i], s.bases + 2 * (size_t)q);
         }
     }
     return sort_pack_hi(s, val);
+}
+template <bool GEO>
+__device__ __forceinline__ uint64_t doc_sort_hi(const LexView& v, const SortDev& s, uint32_t doc, uint32_t q) {
+    const uint64_t row = (uint64_t)(doc - v.facet_first_doc);          // prepare_sort: the facet rows cover every doc of the levels
+    return sort_hi_of<GEO>(s, doc, q, [&](uint32_t i) { return __ldg(&v.facet_keys[(size_t)s.facet[i] * v.facet_rows + row]); });
 }
 
 }  // namespace ssb

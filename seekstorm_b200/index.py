@@ -705,6 +705,77 @@ class Index:
             out.append([(int(d), float(s)) for d, s in zip(h["doc_id"], h["score"])])
         return out, counts[:nq]
 
+    def search_empty_batch(self, n_queries: int, k: int, result_type: ResultType = ResultType.TopkCount, filters=None, sort=None,
+                           sort_bases=None):
+        """The empty query for a batch of n_queries filter-only queries (ssb_search_empty): every live doc of the lexical levels through
+        each query's FacetFilter list (filters: per query a list, or None), in the order of the ResultSort list `sort` (a leading "_score"
+        orders by doc id; ties and no sort: doc id descending).  Returns (list of [(doc_id, 0.0)...], counts ndarray)."""
+        nq = int(n_queries)
+        b, keep = self._lex_batch([[] for _ in range(nq)], QueryType.Union, None, filters)
+        b.term_offsets = None
+        hits = _hits_array(max(nq * max(k, 1), 1))
+        n_hits = np.zeros(max(nq, 1), dtype=np.uint32)
+        counts = np.zeros(max(nq, 1), dtype=np.uint64)
+        crit, n_crit = self._sort_criteria(sort or [])
+        bases = self._sort_bases(sort or [], nq, sort_bases)
+        check(lib().ssb_search_empty(self._h, C.byref(b), C.addressof(crit), n_crit, bases.ctypes.data if bases is not None else None,
+                                     k, int(result_type), hits.ctypes.data, n_hits.ctypes.data, counts.ctypes.data))
+        out = []
+        for i in range(nq):
+            h = hits[i * k: i * k + int(n_hits[i])]
+            out.append([(int(d), float(s)) for d, s in zip(h["doc_id"], h["score"])])
+        return out, counts[:nq]
+
+    def search_empty_facets(self, query_facets):
+        """Facet counts of the empty query (ssb_search_empty_facets, get_index_string_facets_shard index.rs:4441-4569): per String facet
+        of query_facets [(value id, count), ...] over every facet row, count desc, id asc, at most `length`, prefix applied before the
+        cut.  Range facets are left out."""
+        arr, n_req, keep, meta = self._facet_requests(query_facets)
+        if n_req == 0:
+            return {}
+        caps = [qf.length if t in (_lib.FACET_STRING16, _lib.FACET_STRING32) else len(qf.ranges) for _, t, qf in meta]
+        out = np.zeros(max(sum(caps), 1), dtype=[("value", np.uint32), ("pad", np.uint32), ("count", np.uint64)])
+        n_out = np.zeros(n_req, dtype=np.uint32)
+        check(lib().ssb_search_empty_facets(self._h, C.addressof(arr), n_req, out.ctypes.data, n_out.ctypes.data))
+        res, o = {}, 0
+        for r, (name, t, qf) in enumerate(meta):
+            if t in (_lib.FACET_STRING16, _lib.FACET_STRING32):
+                e = out[o:o + int(n_out[r])]
+                res[name] = [(int(v), int(c)) for v, c in zip(e["value"], e["count"])]
+            o += caps[r]
+        return res
+
+    def _search_empty(self, offset, length, result_type, query_facets, facet_filter, result_sort) -> ResultObject:
+        """Search::search("", enable_empty_query = true, ..) on one shard.  Without facet filter and query_facets and with at most one
+        "_id" / "_score" criterion, the index route (search.rs:1413-1432, search_iterator_index iterator.rs:360-413): the live doc ids from
+        the largest (ascending when that criterion is Ascending), result_count_total = the live docs for every result type.  Otherwise the
+        shard route (search_iterator_shard, iterator.rs:316-358): every doc through the facet filters and the sort, counted under Count /
+        TopkCount (Topk counts nothing: total 0), and the index-wide String facet counts (search.rs:3598-3602) for every result type."""
+        ro = ResultObject()
+        rt = ResultType(result_type)
+        index_route = not query_facets and not facet_filter and (not result_sort or (len(result_sort) == 1 and result_sort[0].field in ("_id", "_score")))
+        if index_route:
+            _, counts = self.search_empty_batch(1, 0, ResultType.Count)
+            ro.result_count_total = int(counts[0])
+            if rt != ResultType.Count and length > 0:
+                asc = bool(result_sort) and SortOrder(result_sort[0].order) == SortOrder.Ascending
+                res, _ = self.search_empty_batch(1, offset + length, ResultType.Topk, sort=[ResultSort("_id", SortOrder.Ascending)] if asc else None)
+                ro.results = [Result(d, s) for d, s in res[0][offset:offset + length]]
+        else:
+            if length == 0 and rt != ResultType.Count:           # search.rs:2472-2478
+                if rt == ResultType.Topk:
+                    return ro
+                rt = ResultType.Count
+            heap = offset + length
+            res, counts = self.search_empty_batch(1, heap if rt != ResultType.Count else 0, rt, [list(facet_filter)] if facet_filter else None,
+                                                  list(result_sort) if result_sort and rt != ResultType.Count else None)
+            ro.result_count_total = int(counts[0]) if rt != ResultType.Topk else 0
+            ro.results = [Result(d, s) for d, s in res[0][offset:offset + length]]
+            if query_facets:
+                ro.facets = self.assemble_facets(self.search_empty_facets(list(query_facets)), list(query_facets))
+        ro.result_count = len(ro.results)
+        return ro
+
     def search_vector_batch(self, queries, k: int):
         """Batched search_vector_shard (AnnMode::All).  queries: [nq, dims] f32 numpy/torch."""
         nq = int(queries.shape[0])
@@ -826,8 +897,11 @@ class Index:
         ResultSort.base sorts by the distance to it).
         query_facets: QueryFacet objects — facet counts of the lexical matches in ResultObject.facets (ssb_search_lexical_facets), unless
         the result type is Topk (search.rs:1748).
-        Unsupported reference features (facet counts of vector-only or empty queries, sorting vector / hybrid results, a base on a
-        non-Point facet, uncommitted, rewriting) raise NotImplementedError rather than being silently ignored."""
+        enable_empty_query with query_string "" and no query_vector (Lexical mode): every live doc through facet_filter, result_sort and
+        the paging, the index-wide String facet counts in `facets` (_search_empty).
+        Unsupported reference features (facet counts of vector-only queries or of an empty query without enable_empty_query, sorting
+        vector / hybrid results, a base on a non-Point facet, uncommitted, rewriting) raise NotImplementedError rather than being silently
+        ignored."""
         if include_uncommitted:
             raise NotImplementedError("uncommitted search is outside the GPU hot path")
         search_mode = search_mode or SearchMode.Lexical()
@@ -839,6 +913,8 @@ class Index:
             raise NotImplementedError("result_sort on vector / hybrid search is not built")
         if result_sort:
             self._sort_criteria(result_sort)                     # a base on a non-Point facet raises before any search runs
+        if enable_empty_query and query_string == "" and query_vector is None and search_mode.kind == "Lexical":
+            return self._search_empty(offset, length, result_type, query_facets, facet_filter, result_sort)
         # field_filter: names of indexed fields (self.field_names, in schema order) or their indices -> one bitmask
         fmask = 0
         for f in field_filter:
