@@ -137,10 +137,13 @@ typedef struct {
 /* FieldType of a facet field (index.rs `FieldType`; FilterSparse search.rs:863-881).  POINT (geo, index.rs:5803-5819): the row holds
  * the u64 Morton code encode_morton_2_d([lat, lon]) (geo_search.rs:27-42): x = ((lat * 1e7) as i32) as u32 in the even bits, y = the
  * same of lon in the odd bits, Rust's saturating `as i32` (NaN -> 0).  The reference writes no code for a coordinate outside
- * [-90, 90] x [-180, 180]: that row stays 0, which decodes to (0.0, 0.0).  Decode: (x as i32) as f64 / 1e7 (geo_search.rs:58-79). */
+ * [-90, 90] x [-180, 180]: that row stays 0, which decodes to (0.0, 0.0).  Decode: (x as i32) as f64 / 1e7 (geo_search.rs:58-79).
+ * STRINGSET16 / STRINGSET32 (multi-value string facets, index.rs:5763-5801): the row holds the u16 / u32 id of the doc's COMBINATION —
+ * its strings sorted byte-wise and joined with "_", numbered in first-insertion order; the member lists of the combinations are given
+ * by ssb_set_facet_string_sets. */
 enum { SSB_FACET_U8 = 0, SSB_FACET_U16 = 1, SSB_FACET_U32 = 2, SSB_FACET_U64 = 3, SSB_FACET_I8 = 4, SSB_FACET_I16 = 5,
        SSB_FACET_I32 = 6, SSB_FACET_I64 = 7, SSB_FACET_TIMESTAMP = 8, SSB_FACET_F32 = 9, SSB_FACET_F64 = 10,
-       SSB_FACET_STRING16 = 11, SSB_FACET_STRING32 = 12, SSB_FACET_POINT = 13 };
+       SSB_FACET_STRING16 = 11, SSB_FACET_STRING32 = 12, SSB_FACET_POINT = 13, SSB_FACET_STRINGSET16 = 14, SSB_FACET_STRINGSET32 = 15 };
 /* DistanceUnit (index.rs) of a POINT filter */
 enum { SSB_UNIT_KILOMETERS = 0, SSB_UNIT_MILES = 1 };
 /* one facet field of the shard's facet file: its type and its byte offset inside a doc's row (`facet.offset`, add_result.rs:345) */
@@ -160,8 +163,15 @@ typedef struct { uint32_t type; uint32_t offset; } ssb_facet_field;
  * Precision: the integer decode, /1e7, + - * and sqrt are IEEE round-to-nearest in the reference's operation order without FMA
  * contraction, bit for bit; the Morton interval is computed on the host with the C library's cos.  The device evaluates the distance's
  * cos with CUDA's double cos (within 2 ulp, not guaranteed equal to the host libm): a filter decision can differ from the reference only
- * for a distance within a few ulp of a bound. */
+ * for a distance within a few ulp of a bound.
+ * SET on a STRINGSET facet (FacetFilter::StringSet16 / 32, search.rs:2643-2710): the values are MEMBER ids (ssb_set_facet_string_sets),
+ * or, with bit 63 (SSB_SET_COMBINATION) set, a combination id that must match exactly.  A doc passes when its combination id equals a
+ * flagged id or when one of its combination's members is listed.  The reference accepts, per filter string v, every combination whose
+ * members contain v (string_set_to_single_term_id, index.rs:4282-4297) plus the combination whose joined key equals v: the host sends
+ * v's member id, and the flagged id of that combination when it does not already hold v (["a", "b"] for v = "a_b").  A member id
+ * >= n_values or a flagged id >= n_sets is SSB_E_INVALID; a STRINGSET facet without string sets is SSB_E_STATE. */
 enum { SSB_FILTER_RANGE = 0, SSB_FILTER_SET = 1, SSB_FILTER_POINT = 2 };
+#define SSB_SET_COMBINATION (1ull << 63)
 typedef struct ssb_facet_filter {
     uint32_t facet;                   /* index into the fields given to ssb_set_facets                    */
     uint32_t kind;                    /* SSB_FILTER_*                                                     */
@@ -261,6 +271,16 @@ int32_t ssb_set_facets(ssb_index* ix, const void* rows, uint64_t first_doc_id, u
  * String order = byte-wise lexicographic), which the library does not hold: rank_of_id[id] = position of id's string in that order
  * (equal strings, equal rank), computed by the host.  HOST array [n_ids].  ssb_set_facets clears it.  Needed by sorted searches only. */
 int32_t ssb_set_facet_value_order(ssb_index* ix, uint32_t facet, const uint32_t* rank_of_id, uint32_t n_ids);
+/* The member lists of a STRINGSET facet's combinations (facet.values of index.rs:5763-5801: per combination the FIRST doc's sorted list,
+ * repeats and the empty list included), CSR over MEMBER ids: combination c holds members[set_offsets[c] .. set_offsets[c + 1]).  Member
+ * ids are the ranks of the distinct member strings in byte-wise order (Rust String order), so a string prefix is an id interval and id
+ * order is string order.  HOST arrays set_offsets [n_sets + 1] (ascending, from 0), members [set_offsets[n_sets]].  SSB_E_INVALID when a
+ * member id is >= n_values, the facet's column holds an id >= n_sets, or a STRINGSET16 facet gets more than 65,535 sets (the reference's
+ * ingest bound).  The sort rank of a combination is derived from its first member
+ * (the empty combination below every string), with the facet's zones in those ranks: no ssb_set_facet_value_order for these facets.
+ * ssb_set_facets clears it; filters, counts and sorting on the facet need it (else SSB_E_STATE).  Exclusive. */
+int32_t ssb_set_facet_string_sets(ssb_index* ix, uint32_t facet, const uint64_t* set_offsets, const uint32_t* members, uint32_t n_sets,
+                                  uint32_t n_values);
 
 /* ---- vector index -------------------------------------------------------------------------------- */
 /* rows: [n, dims] row-major f32 (row_stride_floats >= dims, 0 = dims); local_ids: [n] u16 or NULL (= 0..n-1).
@@ -298,7 +318,9 @@ int32_t ssb_search_lexical(ssb_index* ix, const ssb_lex_batch* q, uint32_t k, ui
  * of ssb_search_lexical (Count ignores the sort, search.rs:2498).  One sort for the whole batch; n_sort = 0, or criteria that reduce to
  * "_score desc", is ssb_search_lexical.  The facet criteria with their natural widths (8 bits U8 / I8, 16 bits U16 / I16 / String16,
  * 32 bits U32 / I32 / F32 / String32 / _id, 64 bits U64 / I64 / Timestamp / F64) must fit 64 bits in total (else SSB_E_UNSUPPORTED).
- * Needs ssb_set_facets rows for every doc of the lexical levels.  Not on a handle with a communicator (SSB_E_UNSUPPORTED). */
+ * Needs ssb_set_facets rows for every doc of the lexical levels.  Not on a handle with a communicator (SSB_E_UNSUPPORTED).
+ * STRINGSET16 / 32 (16 / 32 bits) sort by the combination's FIRST member string (min_heap.rs:393-420, 900-925); equal first members
+ * tie.  Deviation: the empty combination, on which the reference panics, sorts below every string. */
 enum { SSB_SORT_FACET = 0, SSB_SORT_ID = 1, SSB_SORT_SCORE = 2 };
 enum { SSB_SORT_ASCENDING = 0, SSB_SORT_DESCENDING = 1 };          /* SortOrder, search.rs:885-890 */
 typedef struct { uint32_t source, facet, order, pad; } ssb_sort_criterion;   /* facet: index into ssb_set_facets' fields (SSB_SORT_FACET) */
@@ -337,7 +359,10 @@ int32_t ssb_search_lexical_sorted_ex(ssb_index* ix, const ssb_lex_batch* q, cons
  * order; n_out: HOST [n_queries][n_req] entries written per request.  bases: HOST [n_queries][number of POINT requests][2] (lat, lon), or
  * NULL when no request is on a POINT facet.  The value histograms take n_queries x (sum over VALUES requests of the facet's largest id
  * + 1) x 4 bytes; the batch runs in query chunks within a 256 MiB workspace per search context (one query above it: SSB_E_UNSUPPORTED).
- * Not on a handle with a communicator (SSB_E_UNSUPPORTED). */
+ * Not on a handle with a communicator (SSB_E_UNSUPPORTED).
+ *   STRINGSET16 / 32 facets take VALUES only (RANGES: SSB_E_INVALID) and need ssb_set_facet_string_sets (else SSB_E_STATE): a doc counts
+ *     once under every member occurrence of its combination (search.rs:3615-3640), `value` is a MEMBER id, [rank_lo, rank_hi) a member-id
+ *     interval, ties go to the smaller id, and the histogram takes n_values words. */
 enum { SSB_FACET_COUNT_VALUES = 0, SSB_FACET_COUNT_RANGES = 1 };
 #define SSB_MAX_FACET_RANGES 256u
 #define SSB_MAX_FACET_LENGTH 1024u
@@ -376,7 +401,8 @@ int32_t ssb_search_empty(ssb_index* ix, const ssb_lex_batch* q, const ssb_sort_c
  *   VALUES (String16 / String32): the `length` ids with the most facet rows, over EVERY row given to ssb_set_facets (no filter, deleted docs
  *     included, as the reference's counters are never decremented); count descending, then id ascending; has_prefix restricts to a
  *     value-order rank interval as in ssb_search_lexical_facets.  Deviation: a row whose id is 0 because its doc had no value is counted
- *     under id 0.
+ *     under id 0.  STRINGSET16 / 32: every row counts under each member occurrence of its combination (index.rs:4531-4550), over rows
+ *     rather than the ingest counters as for String facets.
  *   RANGES: validated, n_out = 0 (the reference returns no range facets for the empty query).
  * Not on a handle with a communicator (SSB_E_UNSUPPORTED). */
 int32_t ssb_search_empty_facets(ssb_index* ix, const ssb_facet_request* req, uint32_t n_req, ssb_facet_count* out, uint32_t* n_out);

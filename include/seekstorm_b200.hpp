@@ -77,16 +77,25 @@ inline uint64_t fnv1a64(const std::string& term) {
 // `FacetFilter` (search.rs:735-860) resolved against the schema: facet = index of the facet field (order of set_facets), a Rust
 // `Range<T>` as start <= value < end with the bounds widened to 8 bytes (u64 / i64 two's complement / f64 bits — see ssb_facet_filter),
 // or the value ids of a String16 / String32 filter, or a geo distance range on a Point facet (`FacetFilter::Point`: base (lat, lon),
-// start <= distance < end in unit — SSB_FILTER_POINT)
+// start <= distance < end in unit — SSB_FILTER_POINT), or a StringSet16 / StringSet32 filter (string_set: the member ids of the filter
+// strings and the combination ids whose joined key equals a filter string without holding it, search.rs:2643-2710; an empty list passes
+// no doc)
 struct FacetFilter {
     uint32_t facet = 0;
     uint64_t start = 0, end = 0;
     std::vector<uint64_t> values;
     bool point = false; double lat = 0.0, lon = 0.0; uint32_t unit = SSB_UNIT_KILOMETERS;
+    bool is_set = false;              // SSB_FILTER_SET even with no values (a StringSet filter none of whose strings resolved)
     static FacetFilter range_u(uint32_t facet, uint64_t a, uint64_t b) { FacetFilter f; f.facet = facet; f.start = a; f.end = b; return f; }
     static FacetFilter range_i(uint32_t facet, int64_t a, int64_t b) { return range_u(facet, static_cast<uint64_t>(a), static_cast<uint64_t>(b)); }
     static FacetFilter range_f(uint32_t facet, double a, double b) { uint64_t x, y; std::memcpy(&x, &a, 8); std::memcpy(&y, &b, 8); return range_u(facet, x, y); }
     static FacetFilter set(uint32_t facet, std::vector<uint64_t> ids) { FacetFilter f; f.facet = facet; f.values = std::move(ids); return f; }
+    static FacetFilter string_set(uint32_t facet, const std::vector<uint32_t>& member_ids, const std::vector<uint32_t>& combination_ids = {}) {
+        FacetFilter f; f.facet = facet; f.is_set = true;
+        f.values.assign(member_ids.begin(), member_ids.end());
+        for (uint32_t c : combination_ids) f.values.push_back(SSB_SET_COMBINATION | c);
+        return f;
+    }
     static FacetFilter geo(uint32_t facet, double lat, double lon, double start, double end, uint32_t unit = SSB_UNIT_KILOMETERS) {
         FacetFilter f = range_f(facet, start, end); f.point = true; f.lat = lat; f.lon = lon; f.unit = unit; return f;
     }
@@ -144,6 +153,10 @@ public:
     // String16 / String32 facet: rank_of_id[id] = position of the id's string in byte-wise order (what sorting by the facet compares)
     void set_facet_value_order(uint32_t facet, const std::vector<uint32_t>& rank_of_id) {
         check(ssb_set_facet_value_order(h_, facet, rank_of_id.data(), static_cast<uint32_t>(rank_of_id.size())));
+    }
+    // StringSet16 / StringSet32 facet: the member ids of every combination as CSR (set_offsets [n_sets + 1]), n_values distinct members
+    void set_facet_string_sets(uint32_t facet, const std::vector<uint64_t>& set_offsets, const std::vector<uint32_t>& members, uint32_t n_values) {
+        check(ssb_set_facet_string_sets(h_, facet, set_offsets.data(), members.data(), set_offsets.empty() ? 0u : static_cast<uint32_t>(set_offsets.size() - 1), n_values));
     }
     // several indexed fields: boosts (before the first level) and the fields' names in schema order (for field_filter)
     void set_field_boosts(const std::vector<float>& boosts) { check(ssb_lexical_set_field_boosts(h_, static_cast<uint32_t>(boosts.size()), boosts.data())); }
@@ -291,7 +304,7 @@ private:
         explicit Filters(const std::vector<FacetFilter>& facet_filter) {
             for (auto& f : facet_filter) {
                 ssb_facet_filter c{};
-                c.facet = f.facet; c.kind = f.point ? SSB_FILTER_POINT : f.values.empty() ? SSB_FILTER_RANGE : SSB_FILTER_SET; c.start = f.start; c.end = f.end;
+                c.facet = f.facet; c.kind = f.point ? SSB_FILTER_POINT : (f.values.empty() && !f.is_set) ? SSB_FILTER_RANGE : SSB_FILTER_SET; c.start = f.start; c.end = f.end;
                 c.set_first = static_cast<uint32_t>(set_values.size());
                 if (f.point) {                // payload: base lat / lon as f64 bits, the unit
                     uint64_t la, lo; std::memcpy(&la, &f.lat, 8); std::memcpy(&lo, &f.lon, 8);

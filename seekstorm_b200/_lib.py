@@ -71,8 +71,9 @@ class SsbFacetFilter(C.Structure):
 
 # SSB_FACET_* (FieldType of a facet field) and SSB_FILTER_*
 FACET_U8, FACET_U16, FACET_U32, FACET_U64, FACET_I8, FACET_I16, FACET_I32, FACET_I64, FACET_TIMESTAMP, FACET_F32, FACET_F64, \
-    FACET_STRING16, FACET_STRING32, FACET_POINT = range(14)
+    FACET_STRING16, FACET_STRING32, FACET_POINT, FACET_STRINGSET16, FACET_STRINGSET32 = range(16)
 FILTER_RANGE, FILTER_SET, FILTER_POINT = 0, 1, 2
+SET_COMBINATION = 1 << 63           # SSB_SET_COMBINATION: a StringSet filter value that is a combination id, not a member id
 UNIT_KILOMETERS, UNIT_MILES = 0, 1
 
 
@@ -111,7 +112,7 @@ class SsbStats(C.Structure):
 EXPORTS = [
     "ssb_abi_version", "ssb_last_error", "ssb_create", "ssb_destroy", "ssb_lexical_add_level",
     "ssb_vector_add_level_clustered", "ssb_lexical_set_field_boosts", "ssb_lexical_commit", "ssb_lexical_dict_size", "ssb_lexical_dict_export", "ssb_lexical_set_global_df",
-    "ssb_load_index_bin", "ssb_load_vector_bin", "ssb_index_bin_inspect", "ssb_set_deleted", "ssb_set_facets", "ssb_set_facet_value_order", "ssb_vector_set_turboquant_mask", "ssb_vector_add_level", "ssb_vector_count", "ssb_vector_reserve", "ssb_set_vector_kernel", "ssb_search_lexical", "ssb_search_lexical_sorted", "ssb_search_lexical_sorted_ex", "ssb_search_lexical_facets", "ssb_search_empty", "ssb_search_empty_facets", "ssb_search_vector", "ssb_search_vector_ex", "ssb_search_hybrid",
+    "ssb_load_index_bin", "ssb_load_vector_bin", "ssb_index_bin_inspect", "ssb_set_deleted", "ssb_set_facets", "ssb_set_facet_value_order", "ssb_set_facet_string_sets", "ssb_vector_set_turboquant_mask", "ssb_vector_add_level", "ssb_vector_count", "ssb_vector_reserve", "ssb_set_vector_kernel", "ssb_search_lexical", "ssb_search_lexical_sorted", "ssb_search_lexical_sorted_ex", "ssb_search_lexical_facets", "ssb_search_empty", "ssb_search_empty_facets", "ssb_search_vector", "ssb_search_vector_ex", "ssb_search_hybrid",
     "ssb_rrf_fuse", "ssb_comm_unique_id", "ssb_comm_init", "ssb_comm_attach", "ssb_comm_destroy", "ssb_lexical_sync_df",
     "ssb_search_vector_keys", "ssb_search_lexical_keys", "ssb_merge_keys", "ssb_sync",
     "ssb_stream", "ssb_set_stream", "ssb_last_stats",
@@ -152,6 +153,7 @@ def lib():
         "ssb_set_deleted": [vp, vp, u64],
         "ssb_set_facets": [vp, vp, u64, u64, u32, vp, u32],
         "ssb_set_facet_value_order": [vp, u32, vp, u32],
+        "ssb_set_facet_string_sets": [vp, u32, vp, vp, u32, u32],
         "ssb_vector_set_turboquant_mask": [vp, vp, u32],
         "ssb_vector_count": [vp, C.POINTER(u64)],
         "ssb_vector_reserve": [vp, u64],

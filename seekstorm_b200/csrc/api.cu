@@ -939,6 +939,31 @@ int32_t ssb_set_facet_value_order(ssb_index* ix, uint32_t facet, const uint32_t*
     SSB_API_END
 }
 
+int32_t ssb_set_facet_string_sets(ssb_index* ix, uint32_t facet, const uint64_t* set_offsets, const uint32_t* members, uint32_t n_sets,
+                                  uint32_t n_values) {
+    SSB_API_BEGIN
+    if (!ix || !set_offsets) { set_error("ssb_set_facet_string_sets: null argument"); return SSB_E_INVALID; }
+    std::unique_lock<std::shared_mutex> g(ix->rw);
+    SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
+    FacetSet& fs = ix->facets;
+    if (!fs.n_facets) { set_error("ssb_set_facet_string_sets: no facets (ssb_set_facets)"); return SSB_E_STATE; }
+    if (facet >= fs.n_facets) { set_error("ssb_set_facet_string_sets: facet %u of %u", facet, fs.n_facets); return SSB_E_INVALID; }
+    if (!facet_is_stringset(fs.types[facet])) { set_error("ssb_set_facet_string_sets: facet %u is not a StringSet16 / StringSet32 facet", facet); return SSB_E_INVALID; }
+    // the reference's ingest writes at most 65,535 combinations to a StringSet16 facet; the first-member ranks take 16 bits there
+    const uint32_t lim = fs.types[facet] == SSB_FACET_STRINGSET16 ? 65535u : 0xFFFFFFFFu;
+    if (n_sets > lim) { set_error("ssb_set_facet_string_sets: %u sets, at most %u on a StringSet16 facet", n_sets, lim); return SSB_E_INVALID; }
+    if (n_sets == 0 || fs.max_key[facet] >= n_sets) { set_error("ssb_set_facet_string_sets: the column holds id %llu, n_sets is %u", (unsigned long long)fs.max_key[facet], n_sets); return SSB_E_INVALID; }
+    if (set_offsets[0] != 0) { set_error("ssb_set_facet_string_sets: set_offsets[0] must be 0"); return SSB_E_INVALID; }
+    for (uint32_t c = 0; c < n_sets; c++)
+        if (set_offsets[c + 1] < set_offsets[c]) { set_error("ssb_set_facet_string_sets: set_offsets must ascend (set %u)", c); return SSB_E_INVALID; }
+    if (set_offsets[n_sets] && !members) { set_error("ssb_set_facet_string_sets: null members"); return SSB_E_INVALID; }
+    for (uint64_t j = 0; j < set_offsets[n_sets]; j++)
+        if (members[j] >= n_values) { set_error("ssb_set_facet_string_sets: member id %u at %llu is not below n_values %u", members[j], (unsigned long long)j, n_values); return SSB_E_INVALID; }
+    SSB_CUDA_TRY(cudaDeviceSynchronize());        // searches on a caller-owned stream may still read the old sets
+    return fs.set_string_sets(facet, set_offsets, members, n_sets, n_values, ix->load_st);
+    SSB_API_END
+}
+
 // TurboQuant.seed_mask (vector_similarity.rs:1845-1859): the reference draws the +-1 mask once per index from ChaCha8Rng::seed_from_u64(1234)
 // (index.rs:2215-2216) — a third-party generator this library does not restate; the host hands over the mask it holds.
 int32_t ssb_vector_set_turboquant_mask(ssb_index* ix, const float* seed_mask, uint32_t dim) {

@@ -1612,13 +1612,17 @@ struct FacetCall {
     const uint64_t* starts; uint32_t n_starts;      // RANGES / POINT starts in key space
     const double* bases; uint32_t n_point;          // [n_queries][n_point][2]
     uint32_t* hist; uint32_t hist_words, range_words;   // [chunk][hist_words]: the range bins first, then the value bins
-    uint64_t* stats;                                // {postings read, dense words read, counted docs}
+    uint64_t* stats;                                // {postings read, dense words read, counted docs, StringSet CSR bytes read}
 };
 struct FacetWarpSm { uint32_t bm[2048]; uint16_t list[1024]; };
 
-template <bool FIELD_RUNS, bool GEO>
+// SETS: the call has a VALUES request on a StringSet facet (search.rs:3615-3640: each doc counts under each member occurrence of its
+// combination); csr [2 * n_req]: per request the facet's set offsets and member ids as addresses (0: not a StringSet facet).  Its own
+// instantiation, and the table an argument of its own, so that the other instantiations keep their code and registers.
+template <bool FIELD_RUNS, bool GEO, bool SETS>
 __global__ void __launch_bounds__(FACET_WARPS * 32) lex_facets(LexView v, const QueryPlan* __restrict__ plans, const LvRec* __restrict__ recs,
-                                                                uint32_t q0, uint32_t nqc, uint32_t query_type, FacetCall fc) {
+                                                                uint32_t q0, uint32_t nqc, uint32_t query_type, FacetCall fc,
+                                                                const uint64_t* __restrict__ csr) {
     extern __shared__ __align__(16) uint8_t fsm_raw[];
     uint64_t* sstart = reinterpret_cast<uint64_t*>(fsm_raw);                                   // [n_starts]
     FacetReqDev* sreq = reinterpret_cast<FacetReqDev*>(sstart + fc.n_starts);                  // [n_req]
@@ -1636,7 +1640,7 @@ __global__ void __launch_bounds__(FACET_WARPS * 32) lex_facets(LexView v, const 
     uint32_t* rhist = rhist_all + (size_t)wi * fc.range_words;
     const uint32_t nlv = v.n_levels;
     const bool is_and = query_type == SSB_QUERY_INTERSECTION;
-    uint64_t st_post = 0, st_words = 0, st_docs = 0;
+    uint64_t st_post = 0, st_words = 0, st_docs = 0, st_csr = 0;
     const uint64_t n_warps = (uint64_t)gridDim.x * FACET_WARPS;
     for (uint64_t it = (uint64_t)blockIdx.x * FACET_WARPS + wi; it < (uint64_t)nqc * nlv; it += n_warps) {
         const uint32_t ql = (uint32_t)(it / nlv), j = (uint32_t)(it % nlv), q = q0 + ql;
@@ -1740,6 +1744,20 @@ __global__ void __launch_bounds__(FACET_WARPS * 32) lex_facets(LexView v, const 
                     const FacetReqDev& R = sreq[r];
                     if (R.kind == FREQ_VALUES && R.length == 0) continue;
                     const uint64_t key = ok ? __ldg(&v.facet_keys[(size_t)R.facet * v.facet_rows + row]) : 0ull;
+                    if (SETS && R.kind == FREQ_VALUES && __ldg(&csr[2 * r])) {
+                        // member j of every lane's combination in one round, warp-aggregated by member id: one atomic per distinct member
+                        const uint64_t* so = reinterpret_cast<const uint64_t*>(__ldg(&csr[2 * r]));
+                        const uint32_t* sm = reinterpret_cast<const uint32_t*>(__ldg(&csr[2 * r + 1]));
+                        const uint64_t b = ok ? __ldg(&so[key]) : 0ull, nm = ok ? __ldg(&so[key + 1]) - b : 0ull;
+                        if (ok) st_csr += 16 + nm * 4;
+                        const uint32_t rounds = __reduce_max_sync(FULL, (uint32_t)nm);
+                        for (uint32_t j = 0; j < rounds; j++) {
+                            const uint32_t m = j < nm ? __ldg(&sm[b + j]) : 0xFFFFFFFFu;
+                            const unsigned grp = __match_any_sync(FULL, m);
+                            if (m != 0xFFFFFFFFu && lane == __ffs(grp) - 1) atomicAdd(&qhist[R.hist_off + m], (uint32_t)__popc(grp));
+                        }
+                        continue;
+                    }
                     if (R.kind == FREQ_VALUES) {                               // warp-aggregated: one atomic per distinct id
                         const unsigned grp = __match_any_sync(FULL, ok ? key : ~0ull);
                         if (ok && lane == __ffs(grp) - 1) atomicAdd(&qhist[R.hist_off + key], (uint32_t)__popc(grp));
@@ -1770,10 +1788,11 @@ __global__ void __launch_bounds__(FACET_WARPS * 32) lex_facets(LexView v, const 
         atomicAdd((unsigned long long*)&fc.stats[1], (unsigned long long)st_words);
         atomicAdd((unsigned long long*)&fc.stats[2], (unsigned long long)st_docs);
     }
+    if (SETS && st_csr) atomicAdd((unsigned long long*)&fc.stats[3], (unsigned long long)st_csr);
 }
 
 // One CTA per (query of the chunk, request).  RANGES: the bins as they are.  VALUES: the `length` ids with count > 0 (and, with a prefix,
-// a value-order rank in [rank_lo, rank_hi)) of largest key (count << 32 | ~id): count descending, id ascending.  A radix select over the
+// a value-order rank in [rank_lo, rank_hi); StringSet member ids: the id itself) of largest key (count << 32 | ~id): count descending, id ascending.  A radix select over the
 // keys' bytes finds the length-th largest key, the ids at or above it are sorted in shared memory.  Deterministic.
 struct RankPtrs { const uint32_t* p[SSB_MAX_FACETS]; };
 __global__ void __launch_bounds__(256) facet_select(const FacetReqDev* __restrict__ req, uint32_t n_req, const uint32_t* __restrict__ hist,
@@ -1795,7 +1814,7 @@ __global__ void __launch_bounds__(256) facet_select(const FacetReqDev* __restric
     auto key_of = [&](uint32_t id) -> uint64_t {                      // 0 = not eligible
         const uint32_t c = qh[id];
         if (c == 0) return 0ull;
-        if (R.has_prefix) { const uint32_t x = __ldg(&rk[id]); if (x < R.rank_lo || x >= R.rank_hi) return 0ull; }
+        if (R.has_prefix) { const uint32_t x = rk ? __ldg(&rk[id]) : id; if (x < R.rank_lo || x >= R.rank_hi) return 0ull; }
         return ((uint64_t)c << 32) | (0xFFFFFFFFu - id);
     };
     if (threadIdx.x == 0) { s_prefix = 0; s_need = R.length; s_all = 0; s_n = 0; }
@@ -1851,7 +1870,7 @@ __global__ void __launch_bounds__(256) facet_select(const FacetReqDev* __restric
 int32_t launch_facet_select(const FacetSet& fs, const FacetReqDev* req, uint32_t n_req, const uint32_t* hist, uint32_t hist_words, uint32_t nq,
                             ssb_facet_count* out, uint32_t out_stride, uint32_t* n_out, cudaStream_t st) {
     RankPtrs rk{};
-    for (uint32_t f = 0; f < fs.n_facets && f < SSB_MAX_FACETS; f++) rk.p[f] = fs.d_rank[f];
+    for (uint32_t f = 0; f < fs.n_facets && f < SSB_MAX_FACETS; f++) rk.p[f] = facet_is_stringset(fs.types[f]) ? nullptr : fs.d_rank[f];
     facet_select<<<dim3(n_req, nq), 256, 0, st>>>(req, n_req, hist, hist_words, rk, out, out_stride, n_out);
     SSB_CUDA_TRY(cudaGetLastError());
     return SSB_OK;
@@ -2243,7 +2262,7 @@ int32_t LexIndex::stage_filters(LexWorkspace& ws, cudaStream_t st, const ssb_lex
     if (!q->filters) { set_error("search_lexical: null filters"); return SSB_E_INVALID; }
     if (!facets_ || !facets_->n_facets) { set_error("search_lexical: facet filters need ssb_set_facets"); return SSB_E_STATE; }
     std::vector<FiltDev> fd(nf);
-    std::vector<uint64_t> geo;                                       // POINT payloads (GEO_WORDS each), staged behind the SET values
+    std::vector<uint64_t> geo;                                       // POINT payloads (GEO_WORDS each) and MEMBERS payloads, staged behind the SET values
     uint32_t n_sets = 0;
     for (uint32_t i = 0; i < nq; i++) {
         if (q->filter_offsets[i + 1] < q->filter_offsets[i] || q->filter_offsets[i + 1] > nf) { set_error("query %u: filter_offsets must ascend", i); return SSB_E_INVALID; }
@@ -2252,11 +2271,12 @@ int32_t LexIndex::stage_filters(LexWorkspace& ws, cudaStream_t st, const ssb_lex
     for (uint32_t i = 0; i < nf; i++) {
         const ssb_facet_filter& f = q->filters[i];
         if (f.facet >= facets_->n_facets) { set_error("facet filter %u: facet %u of %u", i, f.facet, facets_->n_facets); return SSB_E_INVALID; }
-        SSB_TRY(encode_filter(f, i, facets_->types[f.facet], q->filter_set_values, &fd[i], geo));
-        *geo_any = *geo_any || fd[i].kind == FILT_POINT;
+        SSB_TRY(encode_filter(f, i, facets_->types[f.facet], q->filter_set_values, &fd[i], geo, facets_->n_sets[f.facet], facets_->n_values[f.facet]));
+        if (fd[i].kind == FILT_MEMBERS) { fd[i].lo = (uint64_t)facets_->d_set_off[f.facet]; fd[i].hi = (uint64_t)facets_->d_set_mem[f.facet]; }
+        *geo_any = *geo_any || fd[i].kind == FILT_POINT || fd[i].kind == FILT_MEMBERS;   // the out-of-line tests: the GEO instantiations
         if (f.kind == SSB_FILTER_SET && (uint64_t)f.set_first + f.set_count > n_sets) n_sets = f.set_first + f.set_count;
     }
-    for (uint32_t i = 0; i < nf; i++) if (q->filters[i].kind == SSB_FILTER_POINT) fd[i].set_first += n_sets;
+    for (uint32_t i = 0; i < nf; i++) if (fd[i].kind == FILT_POINT || fd[i].kind == FILT_MEMBERS) fd[i].set_first += n_sets;
     const uint32_t n_staged = n_sets + (uint32_t)geo.size();
     SSB_TRY(ws.foff.reserve((size_t)nq + 1, 0, st, true));
     SSB_TRY(ws.filt.reserve(nf, 0, st));
@@ -2419,16 +2439,22 @@ int32_t LexIndex::facet_counts(LexWorkspace& ws, cudaStream_t st, const ssb_lex_
     const FacetSet& fs = *facets_;
     std::vector<FacetReqDev> rd(n_req);
     std::vector<uint64_t> starts;
+    FacetCall fc{};
+    std::vector<uint64_t> csr(2 * (size_t)n_req, 0);                 // per request a StringSet facet's CSR addresses
+    bool any_set = false;                                            // a StringSet request: the lex_facets<.., true> instantiation
     uint32_t range_words = 0, n_point = 0; uint64_t value_words = 0, out_stride = 0;
     for (uint32_t i = 0; i < n_req; i++) {
         const uint32_t f = req[i].facet;
         if (f >= fs.n_facets) { set_error("facet request %u: facet %u of %u", i, f, fs.n_facets); return SSB_E_INVALID; }
-        if (req[i].kind == SSB_FACET_COUNT_VALUES && req[i].length && (fs.max_key[f] + 1) * 4 > FACET_HIST_BYTES) {
-            set_error("facet request %u: %llu value ids, above the %zu MiB facet workspace", i, (unsigned long long)fs.max_key[f] + 1, FACET_HIST_BYTES >> 20);
+        const bool set = facet_is_stringset(fs.types[f]);
+        const uint64_t max_key = set ? (uint64_t)fs.n_values[f] - 1 : fs.max_key[f];   // a StringSet facet bins its member ids
+        if (req[i].kind == SSB_FACET_COUNT_VALUES && req[i].length && (max_key + 1) * 4 > FACET_HIST_BYTES) {
+            set_error("facet request %u: %llu value ids, above the %zu MiB facet workspace", i, (unsigned long long)max_key + 1, FACET_HIST_BYTES >> 20);
             return SSB_E_UNSUPPORTED;
         }
-        const bool has_order = fs.d_rank[f] && fs.max_key[f] < fs.n_rank[f];
-        SSB_TRY(encode_facet_request(req[i], i, fs.types[f], has_order, fs.max_key[f], bases != nullptr, &rd[i], starts));
+        const bool has_order = set ? fs.n_sets[f] != 0 : fs.d_rank[f] && fs.max_key[f] < fs.n_rank[f];
+        SSB_TRY(encode_facet_request(req[i], i, fs.types[f], has_order, max_key, bases != nullptr, &rd[i], starts));
+        if (set) { csr[2 * i] = (uint64_t)fs.d_set_off[f]; csr[2 * i + 1] = (uint64_t)fs.d_set_mem[f]; any_set = true; }
         if (rd[i].kind != FREQ_VALUES) { rd[i].hist_off = range_words; range_words += rd[i].n_bins; }
         if (rd[i].kind == FREQ_POINT) rd[i].point_idx = n_point++;
         rd[i].out_off = (uint32_t)out_stride;
@@ -2446,8 +2472,10 @@ int32_t LexIndex::facet_counts(LexWorkspace& ws, cudaStream_t st, const ssb_lex_
     SSB_TRY(ws.freq.reserve(SSB_MAX_FACET_REQUESTS, 0, st, true));
     SSB_TRY(ws.fstarts.reserve((size_t)SSB_MAX_FACET_REQUESTS * SSB_MAX_FACET_RANGES, 0, st, true));
     SSB_TRY(ws.fstats.reserve(4, 0, st, true));
+    SSB_TRY(ws.fcsr.reserve(2 * SSB_MAX_FACET_REQUESTS, 0, st, true));
     SSB_TRY(ws.fout.reserve((size_t)chunk * (out_stride ? out_stride : 1), 0, st, true));
     SSB_TRY(ws.fnout.reserve((size_t)chunk * n_req, 0, st, true));
+    SSB_CUDA_TRY(cudaMemcpyAsync(ws.fcsr.p, csr.data(), csr.size() * 8, cudaMemcpyHostToDevice, st));
     SSB_CUDA_TRY(cudaMemcpyAsync(ws.freq.p, rd.data(), n_req * sizeof(FacetReqDev), cudaMemcpyHostToDevice, st));
     if (!starts.empty()) SSB_CUDA_TRY(cudaMemcpyAsync(ws.fstarts.p, starts.data(), starts.size() * 8, cudaMemcpyHostToDevice, st));
     if (n_point) {
@@ -2456,17 +2484,20 @@ int32_t LexIndex::facet_counts(LexWorkspace& ws, cudaStream_t st, const ssb_lex_
     }
     SSB_CUDA_TRY(cudaMemsetAsync(ws.fstats.p, 0, 4 * 8, st));
     // ---- per query chunk: the counts, the selection, the copy out ----
-    auto kern = (b.phrase && n_fields_ > 1) ? (b.geo ? lex_facets<true, true> : lex_facets<true, false>) : (b.geo ? lex_facets<false, true> : lex_facets<false, false>);
+    const bool runs = b.phrase && n_fields_ > 1;
+    auto kern = any_set ? (runs ? (b.geo ? lex_facets<true, true, true> : lex_facets<true, false, true>) : (b.geo ? lex_facets<false, true, true> : lex_facets<false, false, true>))
+                        : (runs ? (b.geo ? lex_facets<true, true, false> : lex_facets<true, false, false>) : (b.geo ? lex_facets<false, true, false> : lex_facets<false, false, false>));
     const size_t smem = starts.size() * 8 + n_req * sizeof(FacetReqDev) + FACET_WARPS * (sizeof(FacetWarpSm) + (size_t)range_words * 4);
     if (smem > 48 * 1024) SSB_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    FacetCall fc{ws.freq.p, n_req, ws.fstarts.p, (uint32_t)starts.size(), ws.fbases.p, n_point, ws.fhist.p, (uint32_t)hist_words, range_words, ws.fstats.p};
+    fc.req = ws.freq.p; fc.n_req = n_req; fc.starts = ws.fstarts.p; fc.n_starts = (uint32_t)starts.size(); fc.bases = ws.fbases.p; fc.n_point = n_point;
+    fc.hist = ws.fhist.p; fc.hist_words = (uint32_t)hist_words; fc.range_words = range_words; fc.stats = ws.fstats.p;
     cudaEvent_t e0 = ws.ev0, e1 = ws.ev1;
     float ms_sum = 0.f;
     for (uint32_t q0 = 0; q0 < nq; q0 += chunk) {
         const uint32_t nqc = std::min(chunk, nq - q0);
         SSB_CUDA_TRY(cudaMemsetAsync(ws.fhist.p, 0, (size_t)nqc * hist_words * 4, st));
         if (e0) cudaEventRecord(e0, st);
-        kern<<<n_sms_ * 4, FACET_WARPS * 32, smem, st>>>(b.v, ws.plans.p, ws.recs.p, q0, nqc, b.qt_eff, fc);
+        kern<<<n_sms_ * 4, FACET_WARPS * 32, smem, st>>>(b.v, ws.plans.p, ws.recs.p, q0, nqc, b.qt_eff, fc, ws.fcsr.p);
         SSB_CUDA_TRY(cudaGetLastError());
         if (e1) cudaEventRecord(e1, st);
         SSB_TRY(launch_facet_select(fs, ws.freq.p, n_req, ws.fhist.p, (uint32_t)hist_words, nqc, ws.fout.p, (uint32_t)out_stride, ws.fnout.p, st));
@@ -2480,7 +2511,7 @@ int32_t LexIndex::facet_counts(LexWorkspace& ws, cudaStream_t st, const ssb_lex_
     uint64_t fst[4] = {0, 0, 0, 0};
     SSB_CUDA_TRY(cudaMemcpy(fst, ws.fstats.p, 4 * 8, cudaMemcpyDeviceToHost));
     if (kernel_ns) *kernel_ns = (uint64_t)((double)ms_sum * 1e6);
-    if (alg_bytes) *alg_bytes = fst[0] * 4 + fst[1] * 8 + fst[2] * n_req * 8;
+    if (alg_bytes) *alg_bytes = fst[0] * 4 + fst[1] * 8 + fst[2] * n_req * 8 + fst[3];
     return SSB_OK;
 }
 

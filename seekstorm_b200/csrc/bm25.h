@@ -178,6 +178,7 @@ struct LexWorkspace {
     // starts and Point bases, the selected counts of the chunk, the plan's scratch list and the call's work counters {postings, dense
     // words, counted docs}
     DevBuf<uint32_t> fhist; DevBuf<FacetReqDev> freq; DevBuf<uint64_t> fstarts, fstats;
+    DevBuf<uint64_t> fcsr;    // [2 * n_req]: per request the StringSet facet's CSR (set offsets, member ids) as addresses, 0 = none
     DevBuf<double> fbases; DevBuf<ssb_facet_count> fout; DevBuf<uint32_t> fnout; DevBuf<uint64_t> fglist;
     // empty-query calls (empty_query.cu): the call's tiles in scan order and its work counters (EQ_STAT_*)
     DevBuf<uint2> etiles; DevBuf<unsigned long long> estats;

@@ -161,14 +161,22 @@ __global__ void __launch_bounds__(EQ_WARPS * 32, eq_minb<GEO>()) empty_scan(Empt
 }
 
 // value counts of one String facet over every facet row (index-wide, as the counters ingest keeps): hist[key]++, per-CTA shared
-// histogram when it fits
-__global__ void __launch_bounds__(256) empty_value_hist(const uint64_t* __restrict__ col, uint64_t rows, uint32_t n_bins, uint32_t* __restrict__ hist) {
+// histogram when it fits.  A StringSet facet (set_off / set_mem: its CSR, else null) scatters each row to the member ids of its
+// combination, once per occurrence (index.rs:4531-4550).
+constexpr uint32_t EQ_HIST_LOCAL = 12288;          // bins of a per-CTA shared histogram
+__global__ void __launch_bounds__(256) empty_value_hist(const uint64_t* __restrict__ col, uint64_t rows, uint32_t n_bins, const uint64_t* __restrict__ set_off,
+                                                        const uint32_t* __restrict__ set_mem, uint32_t* __restrict__ hist) {
     extern __shared__ uint32_t eh[];
-    const bool local = n_bins <= 12288;
+    const bool local = n_bins <= EQ_HIST_LOCAL;
     if (local) { for (uint32_t i = threadIdx.x; i < n_bins; i += blockDim.x) eh[i] = 0; __syncthreads(); }
     for (uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; r < rows; r += (uint64_t)gridDim.x * blockDim.x) {
         const uint32_t v = (uint32_t)__ldg(&col[r]);
-        if (local) atomicAdd(&eh[v], 1u); else atomicAdd(&hist[v], 1u);
+        if (!set_off) { if (local) atomicAdd(&eh[v], 1u); else atomicAdd(&hist[v], 1u); continue; }
+        const uint64_t e = __ldg(&set_off[v + 1]);
+        for (uint64_t j = __ldg(&set_off[v]); j < e; j++) {
+            const uint32_t m = __ldg(&set_mem[j]);
+            if (local) atomicAdd(&eh[m], 1u); else atomicAdd(&hist[m], 1u);
+        }
     }
     if (local) {
         __syncthreads();
@@ -268,8 +276,9 @@ int32_t LexIndex::empty_facets(LexWorkspace& ws, cudaStream_t st, const ssb_face
     for (uint32_t i = 0; i < n_req; i++) {
         const uint32_t f = req[i].facet;
         if (f >= fs.n_facets) { set_error("facet request %u: facet %u of %u", i, f, fs.n_facets); return SSB_E_INVALID; }
-        const bool has_order = fs.d_rank[f] && fs.max_key[f] < fs.n_rank[f];
-        SSB_TRY(encode_facet_request(req[i], i, fs.types[f], has_order, fs.max_key[f], true, &rd[i], starts));
+        const bool set = facet_is_stringset(fs.types[f]);
+        const bool has_order = set ? fs.n_sets[f] != 0 : fs.d_rank[f] && fs.max_key[f] < fs.n_rank[f];
+        SSB_TRY(encode_facet_request(req[i], i, fs.types[f], has_order, set ? (uint64_t)fs.n_values[f] - 1 : fs.max_key[f], true, &rd[i], starts));
         rd[i].out_off = (uint32_t)out_stride;
         if (rd[i].kind == FREQ_VALUES) {
             out_stride += rd[i].length;
@@ -286,11 +295,15 @@ int32_t LexIndex::empty_facets(LexWorkspace& ws, cudaStream_t st, const ssb_face
     if (ws.ev0) cudaEventRecord(ws.ev0, st);
     for (uint32_t i = 0; i < n_req; i++) {
         if (rd[i].kind != FREQ_VALUES || !rd[i].length) continue;
-        const size_t smem = rd[i].n_bins <= 12288 ? (size_t)rd[i].n_bins * 4 : 0;
+        const size_t smem = rd[i].n_bins <= EQ_HIST_LOCAL ? (size_t)rd[i].n_bins * 4 : 0;
         const uint32_t grid = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((fs.n_rows + 255) / 256, (uint64_t)n_sms_ * 4));
-        empty_value_hist<<<grid, 256, smem, st>>>(fs.d_keys + (size_t)rd[i].facet * fs.n_rows, fs.n_rows, rd[i].n_bins, ws.fhist.p + rd[i].hist_off);
+        const uint32_t f = rd[i].facet;
+        const bool set = facet_is_stringset(fs.types[f]);
+        empty_value_hist<<<grid, 256, smem, st>>>(fs.d_keys + (size_t)f * fs.n_rows, fs.n_rows, rd[i].n_bins, set ? fs.d_set_off[f] : nullptr,
+                                                  set ? fs.d_set_mem[f] : nullptr, ws.fhist.p + rd[i].hist_off);
         SSB_CUDA_TRY(cudaGetLastError());
-        if (stats) { stats->launches += 1; stats->alg_bytes += fs.n_rows * 8; }
+        // the column, and for a StringSet facet the two offsets of every row and its member ids
+        if (stats) { stats->launches += 1; stats->alg_bytes += fs.n_rows * 8 + (set ? fs.n_rows * 16 + fs.member_rows[f] * 4 : 0); }
     }
     if (ws.ev1) cudaEventRecord(ws.ev1, st);
     SSB_TRY(launch_facet_select(fs, ws.freq.p, n_req, ws.fhist.p, (uint32_t)hist_words, 1, ws.fout.p, (uint32_t)out_stride, ws.fnout.p, st));

@@ -30,6 +30,17 @@ __global__ void __launch_bounds__(256) facet_zone_minmax(const uint64_t* __restr
         zone[2 * blockIdx.x] = mn; zone[2 * blockIdx.x + 1] = mx;
     }
 }
+// the member occurrences of every row of a StringSet column: sum over rows of the size of the row's combination -> *out
+__global__ void __launch_bounds__(256) facet_member_rows(const uint64_t* __restrict__ col, uint64_t rows, const uint64_t* __restrict__ set_off,
+                                                         unsigned long long* out) {
+    unsigned long long s = 0;
+    for (uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; r < rows; r += (uint64_t)gridDim.x * blockDim.x) {
+        const uint64_t c = col[r];
+        s += set_off[c + 1] - set_off[c];
+    }
+    for (int o = 16; o; o >>= 1) s += __shfl_xor_sync(0xFFFFFFFFu, s, o);
+    if ((threadIdx.x & 31) == 0 && s) atomicAdd(out, s);
+}
 // per-block min / max of facet f's column (through its value order when it has one) -> d_zones; asynchronous on st
 static int32_t facet_zones(FacetSet& fs, uint32_t f, cudaStream_t st) {
     if (!fs.n_facets || !fs.n_rows) return SSB_OK;
@@ -88,6 +99,34 @@ int32_t FacetSet::set_value_order(uint32_t facet, const uint32_t* rank_of_id, ui
     return SSB_OK;
 }
 
+int32_t FacetSet::set_string_sets(uint32_t facet, const uint64_t* set_offsets, const uint32_t* members, uint32_t ns, uint32_t nv, cudaStream_t st) {
+    cudaFree(d_set_off[facet]); d_set_off[facet] = nullptr; cudaFree(d_set_mem[facet]); d_set_mem[facet] = nullptr;
+    cudaFree(d_rank[facet]); d_rank[facet] = nullptr; n_rank[facet] = 0; n_sets[facet] = 0; n_values[facet] = 0; member_rows[facet] = 0;
+    const uint64_t n_mem = set_offsets[ns];
+    const std::vector<uint32_t> rank = string_set_sort_ranks(set_offsets, members, ns);
+    SSB_CUDA_TRY(cudaMalloc(&d_set_off[facet], ((size_t)ns + 1) * 8));
+    SSB_CUDA_TRY(cudaMemcpy(d_set_off[facet], set_offsets, ((size_t)ns + 1) * 8, cudaMemcpyHostToDevice));
+    // member occurrences over every row: the members a pass over all rows reads (ssb_last_stats of the empty query's counts)
+    unsigned long long* d_occ = nullptr;
+    SSB_CUDA_TRY(cudaMalloc(&d_occ, 8));
+    cudaMemsetAsync(d_occ, 0, 8, st);
+    facet_member_rows<<<(uint32_t)std::min<uint64_t>((n_rows + 255) / 256, 4096), 256, 0, st>>>(d_keys + (size_t)facet * n_rows, n_rows, d_set_off[facet], d_occ);
+    unsigned long long occ = 0;
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) e = cudaMemcpyAsync(&occ, d_occ, 8, cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    cudaFree(d_occ);
+    if (e != cudaSuccess) { set_error("ssb_set_facet_string_sets: %s", cudaGetErrorString(e)); return SSB_E_CUDA; }
+    SSB_CUDA_TRY(cudaMalloc(&d_set_mem[facet], (size_t)std::max<uint64_t>(n_mem, 1) * 4));
+    if (n_mem) SSB_CUDA_TRY(cudaMemcpy(d_set_mem[facet], members, (size_t)n_mem * 4, cudaMemcpyHostToDevice));
+    SSB_CUDA_TRY(cudaMalloc(&d_rank[facet], (size_t)ns * 4));
+    SSB_CUDA_TRY(cudaMemcpy(d_rank[facet], rank.data(), (size_t)ns * 4, cudaMemcpyHostToDevice));
+    n_rank[facet] = ns; n_sets[facet] = ns; n_values[facet] = nv; member_rows[facet] = occ;
+    SSB_TRY(facet_zones(*this, facet, st));                          // the level bounds of this facet are first-member ranks from now on
+    SSB_CUDA_TRY(cudaStreamSynchronize(st));
+    return SSB_OK;
+}
+
 int32_t sort_of_criteria(const FacetSet* fs, const ssb_sort_criterion* crit, uint32_t n, bool has_bases, SortDev* out, bool* sorted) {
     if (n && !crit) { set_error("search_lexical_sorted: null criteria"); return SSB_E_INVALID; }
     if (n > SSB_MAX_SORT_CRITERIA) { set_error("search_lexical_sorted: more than %u criteria", SSB_MAX_SORT_CRITERIA); return SSB_E_UNSUPPORTED; }
@@ -124,6 +163,9 @@ int32_t sort_of_criteria(const FacetSet* fs, const ssb_sort_criterion* crit, uin
                     set_error("search_lexical_sorted: String facet %u needs a value order covering its ids (ssb_set_facet_value_order)", f); return SSB_E_STATE;
                 }
                 s.rank[j] = fs->d_rank[f];
+            } else if (facet_is_stringset(s.type[j])) {
+                if (!fs->n_sets[f]) { set_error("search_lexical_sorted: StringSet facet %u needs its string sets (ssb_set_facet_string_sets)", f); return SSB_E_STATE; }
+                s.rank[j] = fs->d_rank[f];                           // the first-member ranks of set_string_sets
             }
         }
         s.zones = fs->d_zones; s.zone_block0 = fs->zone_block0; s.n_zone_blocks = fs->n_zone_blocks;

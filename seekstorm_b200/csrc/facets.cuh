@@ -51,11 +51,32 @@ static __device__ __noinline__ uint64_t point_sort_key(uint64_t code, const doub
     return f64_order_key(__dadd_rn(__dmul_rn(x, x), __dmul_rn(y, y)));
 }
 
+// FilterSparse::String16 / 32 on a StringSet facet (add_result.rs:340-478 over the combination ids search.rs:2643-2710 resolves): true =
+// the doc is filtered OUT.  key: the doc's combination id; p: the MEMBERS payload (FILT_MEMBERS); set_off / set_mem: the facet's CSR.  The
+// doc passes on a flagged id equal to its combination or on one of its combination's members found in the sorted member list.  Out of
+// line: only MEMBERS filters reach it.
+static __device__ __noinline__ bool members_rejects_impl(uint64_t key, const uint64_t* p, uint32_t n, const uint64_t* set_off, const uint32_t* set_mem) {
+    const uint32_t nflag = (uint32_t)__ldg(&p[0]);
+    for (uint32_t i = 0; i < nflag; i++) if (__ldg(&p[1 + i]) == key) return false;
+    const uint64_t* m = p + 1 + nflag;
+    const uint32_t nm = n - 1 - nflag;
+    if (nm == 0) return true;
+    const uint64_t e = __ldg(&set_off[key + 1]);
+    for (uint64_t j = __ldg(&set_off[key]); j < e; j++) {
+        const uint64_t x = __ldg(&set_mem[j]);
+        uint32_t lo = 0, hi = nm;                                      // the first listed member >= x
+        while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (__ldg(&m[mid]) < x) lo = mid + 1; else hi = mid; }
+        if (lo < nm && __ldg(&m[lo]) == x) return false;
+    }
+    return true;
+}
+
 // is_facet_filter (add_result.rs:340-478): true = the doc is filtered OUT.  The typed range / set tests of the reference run on the
 // order-preserving 64-bit keys ssb_set_facets stored per doc and facet (bounds converted the same way by the host), so one unsigned
 // compare pair covers every FilterSparse range type.  filter_rejects_key is the test of one filter on one key: the column path below and
 // the staged rows of the empty-query scan (empty_query.cu) share it.  sets: the batch's filter_sets.
-// GEO: the batch holds a POINT filter — its own instantiation, so that the common one keeps its code and its callers their registers
+// GEO: the batch holds a POINT or a MEMBERS filter (the out-of-line tests) — its own instantiation, so that the common one keeps its
+// code and its callers their registers
 template <bool GEO>
 __device__ __forceinline__ bool filter_rejects_key(const FiltDev& f, uint64_t key, const uint64_t* sets) {
     if (f.kind == FILT_RANGE) return !(key >= f.lo && key < f.hi);
@@ -65,6 +86,8 @@ __device__ __forceinline__ bool filter_rejects_key(const FiltDev& f, uint64_t ke
         return !in;
     }
     if (GEO && f.kind == FILT_POINT) return geo_rejects_impl(key, f.lo, f.hi, sets + f.set_first);
+    if (GEO && f.kind == FILT_MEMBERS)
+        return members_rejects_impl(key, sets + f.set_first, f.set_n, reinterpret_cast<const uint64_t*>(f.lo), reinterpret_cast<const uint32_t*>(f.hi));
     return true;
 }
 // Out of line, by value, on the rare candidate / count path of lex_generic only.

@@ -5,6 +5,7 @@
 #include <math.h>
 #include <stdint.h>
 #include <string.h>
+#include <algorithm>
 #include <vector>
 
 #include "../../include/seekstorm_b200.h"
@@ -21,8 +22,10 @@ void set_error(const char* fmt, ...);   // api.cu: the calling thread's last err
 
 // One facet filter of one query, bounds already in key space (FilterSparse, search.rs:863-881): RANGE lo <= key < hi;
 // SET key in filt_sets[set_first .. +set_n); NEVER rejects every doc (a NaN bound: Range::contains is false for every value);
-// POINT: lo <= Morton code < hi, then the distance test with the staged geo payload filt_sets[set_first .. +GEO_WORDS)
-enum { FILT_RANGE = 0, FILT_SET = 1, FILT_NEVER = 2, FILT_POINT = 3 };
+// POINT: lo <= Morton code < hi, then the distance test with the staged geo payload filt_sets[set_first .. +GEO_WORDS);
+// MEMBERS (SET on a StringSet facet): the key is a combination id, lo / hi the device addresses of the facet's CSR (set offsets, member
+// ids), the staged payload filt_sets[set_first .. +set_n) = {F, F flagged combination ids ascending, the member ids ascending, unique}
+enum { FILT_RANGE = 0, FILT_SET = 1, FILT_NEVER = 2, FILT_POINT = 3, FILT_MEMBERS = 4 };
 // payload of a POINT filter in filt_sets, as f64 bits: base lat, base lon, distance start, distance end, earth radius of the unit
 enum { GEO_LAT = 0, GEO_LON = 1, GEO_START = 2, GEO_END = 3, GEO_RADIUS = 4, GEO_WORDS = 5 };
 struct FiltDev { uint32_t facet, kind; uint64_t lo, hi; uint32_t set_first, set_n; };
@@ -65,12 +68,13 @@ SSB_HD double f64_of_order_key(uint64_t k) {
 inline bool facet_is_signed(uint32_t t) { return t == SSB_FACET_I8 || t == SSB_FACET_I16 || t == SSB_FACET_I32 || t == SSB_FACET_I64 || t == SSB_FACET_TIMESTAMP; }
 inline bool facet_is_float(uint32_t t) { return t == SSB_FACET_F32 || t == SSB_FACET_F64; }
 inline bool facet_is_string(uint32_t t) { return t == SSB_FACET_STRING16 || t == SSB_FACET_STRING32; }
+inline bool facet_is_stringset(uint32_t t) { return t == SSB_FACET_STRINGSET16 || t == SSB_FACET_STRINGSET32; }
 // facet value (as stored in the reference's facet file) -> order-preserving key
 inline uint64_t facet_value_key(uint32_t type, const uint8_t* p) {
     switch (type) {
         case SSB_FACET_U8: return p[0];
-        case SSB_FACET_U16: case SSB_FACET_STRING16: { uint16_t x; memcpy(&x, p, 2); return x; }
-        case SSB_FACET_U32: case SSB_FACET_STRING32: { uint32_t x; memcpy(&x, p, 4); return x; }
+        case SSB_FACET_U16: case SSB_FACET_STRING16: case SSB_FACET_STRINGSET16: { uint16_t x; memcpy(&x, p, 2); return x; }
+        case SSB_FACET_U32: case SSB_FACET_STRING32: case SSB_FACET_STRINGSET32: { uint32_t x; memcpy(&x, p, 4); return x; }
         case SSB_FACET_U64: case SSB_FACET_POINT: { uint64_t x; memcpy(&x, p, 8); return x; }   // Point: the Morton code itself
         case SSB_FACET_I8: { int8_t x; memcpy(&x, p, 1); return (uint64_t)(int64_t)x ^ 0x8000000000000000ull; }
         case SSB_FACET_I16: { int16_t x; memcpy(&x, p, 2); return (uint64_t)(int64_t)x ^ 0x8000000000000000ull; }
@@ -85,8 +89,8 @@ inline uint64_t facet_value_key(uint32_t type, const uint8_t* p) {
 inline uint32_t facet_type_bytes(uint32_t type) {
     switch (type) {
         case SSB_FACET_U8: case SSB_FACET_I8: return 1;
-        case SSB_FACET_U16: case SSB_FACET_I16: case SSB_FACET_STRING16: return 2;
-        case SSB_FACET_U32: case SSB_FACET_I32: case SSB_FACET_F32: case SSB_FACET_STRING32: return 4;
+        case SSB_FACET_U16: case SSB_FACET_I16: case SSB_FACET_STRING16: case SSB_FACET_STRINGSET16: return 2;
+        case SSB_FACET_U32: case SSB_FACET_I32: case SSB_FACET_F32: case SSB_FACET_STRING32: case SSB_FACET_STRINGSET32: return 4;
         case SSB_FACET_U64: case SSB_FACET_I64: case SSB_FACET_TIMESTAMP: case SSB_FACET_F64: case SSB_FACET_POINT: return 8;
     }
     return 0;
@@ -100,10 +104,23 @@ SSB_HD uint32_t sort_width(uint32_t src, uint32_t type) {
     if (src == SORT_SRC_ID) return 32;
     switch (type) {
         case SSB_FACET_U8: case SSB_FACET_I8: return 8;
-        case SSB_FACET_U16: case SSB_FACET_I16: case SSB_FACET_STRING16: return 16;
-        case SSB_FACET_U32: case SSB_FACET_I32: case SSB_FACET_F32: case SSB_FACET_STRING32: return 32;
+        case SSB_FACET_U16: case SSB_FACET_I16: case SSB_FACET_STRING16: case SSB_FACET_STRINGSET16: return 16;
+        case SSB_FACET_U32: case SSB_FACET_I32: case SSB_FACET_F32: case SSB_FACET_STRING32: case SSB_FACET_STRINGSET32: return 32;
     }
     return 64;
+}
+// The sort rank of every combination of a StringSet facet (CSR set_offsets [n_sets + 1] / members): the reference sorts by the FIRST
+// member string of the doc's combination (min_heap.rs:393-420, 900-925), member ids are in string order, so the rank is the dense rank
+// of the first member id among the combinations' first members, + 1, and 0 for the empty combination (the reference panics on it; here
+// it sorts below every string).  Dense, so that the ranks of a StringSet16 facet (at most 65,535 combinations) fit its 16 bits.
+inline std::vector<uint32_t> string_set_sort_ranks(const uint64_t* set_offsets, const uint32_t* members, uint32_t n_sets) {
+    std::vector<uint32_t> first;
+    for (uint32_t c = 0; c < n_sets; c++) if (set_offsets[c + 1] > set_offsets[c]) first.push_back(members[set_offsets[c]]);
+    std::sort(first.begin(), first.end()); first.erase(std::unique(first.begin(), first.end()), first.end());
+    std::vector<uint32_t> rank(n_sets);
+    for (uint32_t c = 0; c < n_sets; c++)
+        rank[c] = set_offsets[c + 1] > set_offsets[c] ? (uint32_t)(std::lower_bound(first.begin(), first.end(), members[set_offsets[c]]) - first.begin()) + 1u : 0u;
+    return rank;
 }
 // a sort with a POINT criterion: it needs the per-query bases and the GEO instantiation of the kernels
 inline bool sort_has_point(const SortDev& s) {
@@ -136,10 +153,11 @@ inline double earth_radius(uint64_t unit) { return unit == SSB_UNIT_MILES ? 3958
 
 // Facet filter i of a batch, on a facet of type `type` -> *out in key space.  set_values: the batch's filter_set_values.  A SET filter keeps
 // its values where they are (out->set_first = f.set_first); a POINT filter appends its payload (GEO_WORDS f64 words) to geo and
-// out->set_first is its index there — the caller rebases it once it knows where the payloads go.  Returns SSB_OK or an SSB_E_* code
-// with set_error called.
+// out->set_first is its index there — the caller rebases it once it knows where the payloads go.  A SET filter on a StringSet facet
+// (n_sets / n_values: its string sets, n_sets = 0: none given) appends its MEMBERS payload to geo the same way; the caller sets lo / hi.
+// Returns SSB_OK or an SSB_E_* code with set_error called.
 inline int32_t encode_filter(const ssb_facet_filter& f, uint32_t i, uint32_t type, const uint64_t* set_values, FiltDev* out,
-                             std::vector<uint64_t>& geo) {
+                             std::vector<uint64_t>& geo, uint32_t n_sets = 0, uint32_t n_values = 0) {
     FiltDev d{}; d.facet = f.facet;
     if ((f.kind == SSB_FILTER_POINT) != (type == SSB_FACET_POINT)) { set_error("facet filter %u: a Point facet takes SSB_FILTER_POINT and only it", i); return SSB_E_INVALID; }
     if (f.kind == SSB_FILTER_POINT) {
@@ -160,13 +178,35 @@ inline int32_t encode_filter(const ssb_facet_filter& f, uint32_t i, uint32_t typ
         uint64_t rb; memcpy(&rb, &r, 8);
         for (uint64_t w : {p[0], p[1], f.start, f.end, rb}) geo.push_back(w);
     } else if (f.kind == SSB_FILTER_RANGE) {
-        if (facet_is_string(type)) { set_error("facet filter %u: a String facet takes SSB_FILTER_SET", i); return SSB_E_INVALID; }
+        if (facet_is_string(type) || facet_is_stringset(type)) { set_error("facet filter %u: a String facet takes SSB_FILTER_SET", i); return SSB_E_INVALID; }
         d.kind = FILT_RANGE;
         if (facet_is_float(type)) {
             double a, b; memcpy(&a, &f.start, 8); memcpy(&b, &f.end, 8);
             if (a != a || b != b) d.kind = FILT_NEVER; else { d.lo = f64_order_key(a); d.hi = f64_order_key(b); }
         } else if (facet_is_signed(type)) { d.lo = f.start ^ 0x8000000000000000ull; d.hi = f.end ^ 0x8000000000000000ull; }
         else { d.lo = f.start; d.hi = f.end; }
+    } else if (f.kind == SSB_FILTER_SET && facet_is_stringset(type)) {
+        // FilterSparse::String16 / 32 of combination ids (search.rs:2643-2710), kept as the member ids and flagged combination ids the
+        // host resolved the strings to: sorted and unique, so that the device test is one binary search per member of the doc
+        if (f.set_count && !set_values) { set_error("facet filter %u: null filter_set_values", i); return SSB_E_INVALID; }
+        if (!n_sets) { set_error("facet filter %u: a StringSet facet needs its string sets (ssb_set_facet_string_sets)", i); return SSB_E_STATE; }
+        std::vector<uint64_t> flagged, members;
+        for (uint32_t j = 0; j < f.set_count; j++) {
+            const uint64_t x = set_values[f.set_first + j];
+            if (x & SSB_SET_COMBINATION) {
+                if ((x & ~SSB_SET_COMBINATION) >= n_sets) { set_error("facet filter %u: combination id %llu of %u", i, (unsigned long long)(x & ~SSB_SET_COMBINATION), n_sets); return SSB_E_INVALID; }
+                flagged.push_back(x & ~SSB_SET_COMBINATION);
+            } else {
+                if (x >= n_values) { set_error("facet filter %u: member id %llu of %u", i, (unsigned long long)x, n_values); return SSB_E_INVALID; }
+                members.push_back(x);
+            }
+        }
+        for (auto* v : {&flagged, &members}) { std::sort(v->begin(), v->end()); v->erase(std::unique(v->begin(), v->end()), v->end()); }
+        d.kind = FILT_MEMBERS;
+        d.set_first = (uint32_t)geo.size(); d.set_n = (uint32_t)(1 + flagged.size() + members.size());
+        geo.push_back(flagged.size());
+        geo.insert(geo.end(), flagged.begin(), flagged.end());
+        geo.insert(geo.end(), members.begin(), members.end());
     } else if (f.kind == SSB_FILTER_SET) {
         if (!facet_is_string(type)) { set_error("facet filter %u: SSB_FILTER_SET needs a String16 / String32 facet", i); return SSB_E_INVALID; }
         if (f.set_count && !set_values) { set_error("facet filter %u: null filter_set_values", i); return SSB_E_INVALID; }
@@ -182,6 +222,8 @@ inline int32_t encode_filter(const ssb_facet_filter& f, uint32_t i, uint32_t typ
 // request on a POINT facet, binned by f64_order_key of the distance to base point_idx of the query (radius: earth_radius(unit)).
 // is_float: F32 / F64 (a NaN value, key ~0, is not counted).  hist_off / out_off / point_idx are set by the caller once it knows the layout.
 enum { FREQ_VALUES = 0, FREQ_RANGES = 1, FREQ_POINT = 2 };
+// A VALUES request on a StringSet facet bins under member ids: n_bins = n_values, and the prefix interval is one of member ids; a doc adds
+// one to the bin of every member occurrence of its combination (the kernels take the facet's CSR next to the request).
 struct FacetReqDev {
     uint32_t facet, kind, n_bins, is_float;
     uint32_t start_first, point_idx, hist_off, out_off;
@@ -189,13 +231,18 @@ struct FacetReqDev {
     double radius;
 };
 // Request i of a call on a facet of type `type` -> *out, its starts' keys appended to `starts`.  has_order: the facet has a value order
-// (ssb_set_facet_value_order); max_key: its largest column key; has_bases: the call carries POINT bases.  Returns SSB_OK or an SSB_E_* code
+// (ssb_set_facet_value_order; a StringSet facet: its string sets); max_key: its largest column key (a StringSet facet: n_values - 1, the
+// largest member id); has_bases: the call carries POINT bases.  Returns SSB_OK or an SSB_E_* code
 // with set_error called.
 inline int32_t encode_facet_request(const ssb_facet_request& r, uint32_t i, uint32_t type, bool has_order, uint64_t max_key, bool has_bases,
                                     FacetReqDev* out, std::vector<uint64_t>& starts) {
     FacetReqDev d{}; d.facet = r.facet;
+    if (facet_is_stringset(type)) {
+        if (r.kind == SSB_FACET_COUNT_RANGES) { set_error("facet request %u: a StringSet facet takes SSB_FACET_COUNT_VALUES", i); return SSB_E_INVALID; }
+        if (r.kind == SSB_FACET_COUNT_VALUES && !has_order) { set_error("facet request %u: a StringSet facet needs its string sets (ssb_set_facet_string_sets)", i); return SSB_E_STATE; }
+    }
     if (r.kind == SSB_FACET_COUNT_VALUES) {
-        if (!facet_is_string(type)) { set_error("facet request %u: SSB_FACET_COUNT_VALUES needs a String16 / String32 facet", i); return SSB_E_INVALID; }
+        if (!facet_is_string(type) && !facet_is_stringset(type)) { set_error("facet request %u: SSB_FACET_COUNT_VALUES needs a String16 / String32 facet", i); return SSB_E_INVALID; }
         if (r.length > SSB_MAX_FACET_LENGTH) { set_error("facet request %u: length %u above %u", i, r.length, SSB_MAX_FACET_LENGTH); return SSB_E_UNSUPPORTED; }
         if (r.has_prefix && !has_order) { set_error("facet request %u: a prefix needs the facet's value order (ssb_set_facet_value_order)", i); return SSB_E_STATE; }
         if (r.has_prefix && r.rank_lo > r.rank_hi) { set_error("facet request %u: rank_lo %u above rank_hi %u", i, r.rank_lo, r.rank_hi); return SSB_E_INVALID; }
@@ -245,15 +292,24 @@ struct FacetSet {
     uint64_t* d_keys = nullptr; uint64_t n_rows = 0; uint32_t first_doc = 0; uint32_t n_facets = 0; uint8_t types[16] = {0};
     uint64_t* d_zones = nullptr; uint32_t zone_block0 = 0, n_zone_blocks = 0;   // [n_facets][n_zone_blocks][2] {min, max}
     uint32_t* d_rank[16] = {}; uint32_t n_rank[16] = {}; uint64_t max_key[16] = {};
+    // StringSet facets (ssb_set_facet_string_sets): the CSR of the combinations' member ids, n_sets / n_values (0: not given), and the
+    // member occurrences over every row (the members a pass over all rows reads); d_rank holds the combinations' first-member ranks
+    uint64_t* d_set_off[16] = {}; uint32_t* d_set_mem[16] = {}; uint32_t n_sets[16] = {}, n_values[16] = {}; uint64_t member_rows[16] = {};
     // ssb_set_facets after the caller's synchronisation: drops the old columns, validates and keys the rows, computes max_key and the zones
     int32_t set_columns(const void* rows, uint64_t first_doc_id, uint64_t n_docs, uint32_t row_bytes, const ssb_facet_field* fields,
                         uint32_t n_fields, cudaStream_t st);
     // ssb_set_facet_value_order after its checks: the rank of every id of String facet `facet`, and that facet's zones in ranks
     int32_t set_value_order(uint32_t facet, const uint32_t* rank_of_id, uint32_t n_ids, cudaStream_t st);
+    // ssb_set_facet_string_sets after its argument checks: validates the ids, uploads the CSR, derives the sort ranks and the zones
+    int32_t set_string_sets(uint32_t facet, const uint64_t* set_offsets, const uint32_t* members, uint32_t n_sets, uint32_t n_values, cudaStream_t st);
     void release() {
         cudaFree(d_keys); d_keys = nullptr; n_rows = 0; n_facets = 0;
         cudaFree(d_zones); d_zones = nullptr; n_zone_blocks = 0;
-        for (int f = 0; f < 16; f++) { cudaFree(d_rank[f]); d_rank[f] = nullptr; n_rank[f] = 0; }
+        for (int f = 0; f < 16; f++) {
+            cudaFree(d_rank[f]); d_rank[f] = nullptr; n_rank[f] = 0;
+            cudaFree(d_set_off[f]); d_set_off[f] = nullptr; cudaFree(d_set_mem[f]); d_set_mem[f] = nullptr;
+            n_sets[f] = 0; n_values[f] = 0; member_rows[f] = 0;
+        }
     }
 };
 

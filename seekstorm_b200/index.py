@@ -102,7 +102,9 @@ class DistanceUnit(enum.IntEnum):
 class FacetFilter:
     """`FacetFilter` (search.rs:735-860): a range filter `start <= value < end` (Rust `Range<T>`) on a numeric / timestamp facet field, or a
     value-id set on a String16 / String32 facet (values = the ids the reference resolves the filter strings to, FilterSparse::String16/32),
-    or on a Point facet (`FacetFilter::Point`, base = (lat, lon)) the docs whose distance to base lies in start..end, in unit.
+    or the strings of a StringSet16 / StringSet32 facet (values = [str, ...]: a doc passes when its set holds one of them, resolved like
+    search.rs:2643-2710), or on a Point facet (`FacetFilter::Point`, base = (lat, lon)) the docs whose distance to base lies in start..end,
+    in unit.
     field: the facet's name (Index.set_facets) or its index."""
     field: object
     start: object = None
@@ -133,6 +135,62 @@ class QueryFacet:
     ranges: Sequence = ()
     base: Optional[Sequence[float]] = None
     unit: DistanceUnit = DistanceUnit.Kilometers
+
+
+_VALUE_FACETS = (_lib.FACET_STRING16, _lib.FACET_STRING32, _lib.FACET_STRINGSET16, _lib.FACET_STRINGSET32)   # counted per value id
+_SET_FACETS = (_lib.FACET_STRINGSET16, _lib.FACET_STRINGSET32)
+
+
+@dataclass
+class StringSetFacet:
+    """A multi-value string facet as the reference ingests it (index.rs:5763-5801).  combos[i]: the sorted member list stored for
+    combination i (the FIRST doc's list of its joined key, repeats kept); by_key: joined key -> combination id; members: the distinct
+    member strings as bytes in byte-wise order (member id = position); offsets / member_ids: the CSR of ssb_set_facet_string_sets."""
+    ids: np.ndarray
+    combos: list
+    by_key: dict
+    members: list
+    offsets: np.ndarray
+    member_ids: np.ndarray
+
+    def filter_values(self, strings):
+        """FacetFilter::StringSet16 / 32 (search.rs:2643-2710) -> filter_set_values: per string v its member id, and the id of the
+        combination whose joined key is v, flagged (SET_COMBINATION), when that combination does not hold v itself (["a", "b"] for "a_b")"""
+        pos = {m: i for i, m in enumerate(self.members)}
+        out = []
+        for v in strings:
+            m = pos.get(v.encode("utf-8"))
+            if m is not None:
+                out.append(m)
+            c = self.by_key.get(v)
+            if c is not None and v not in self.combos[c]:
+                out.append(c | _lib.SET_COMBINATION)
+        return out
+
+
+def string_set_facet(docs, bits: int = 16) -> StringSetFacet:
+    """Ingest of a StringSet16 / StringSet32 column (index.rs:5763-5801): each doc's list sorted byte-wise (Rust Vec<String>::sort) and
+    joined with "_"; the joined key gets the next id on first sight and keeps that first list.  Past 65,535 (StringSet16) / 2^32 - 1
+    combinations the reference writes no id for the remaining docs; this raises ValueError instead."""
+    limit = 65535 if bits == 16 else (1 << 32) - 1
+    by_key, combos = {}, []
+    ids = np.zeros(len(docs), dtype=np.uint16 if bits == 16 else np.uint32)
+    for d, lst in enumerate(docs):
+        if len(combos) >= limit:
+            raise ValueError(f"StringSet{bits}: more than {limit} combinations (the reference stops writing ids there)")
+        key = sorted((str(x) for x in lst), key=lambda x: x.encode("utf-8"))
+        c = by_key.setdefault("_".join(key), len(combos))
+        if c == len(combos):
+            combos.append(key)
+        ids[d] = c
+    members = sorted({m.encode("utf-8") for k in combos for m in k})
+    pos = {m: i for i, m in enumerate(members)}
+    offsets = np.zeros(len(combos) + 1, dtype=np.uint64)
+    flat = []
+    for c, k in enumerate(combos):
+        flat.extend(pos[m.encode("utf-8")] for m in k)
+        offsets[c + 1] = len(flat)
+    return StringSetFacet(ids, combos, by_key, members, offsets, np.asarray(flat, dtype=np.uint32))
 
 
 def prefix_rank_interval(order, prefix: bytes):
@@ -408,21 +466,26 @@ class Index:
         check(lib().ssb_set_deleted(self._h, a.ctypes.data if a.size else None, a.size))
 
     def set_facets(self, columns: dict, first_doc_id: int = 0, string_facets: Sequence[str] = (), timestamp_facets: Sequence[str] = (),
-                   string_values: Optional[dict] = None, point_facets: Sequence[str] = ()):
+                   string_values: Optional[dict] = None, point_facets: Sequence[str] = (), string_set_facets: Sequence[str] = (),
+                   string_set32_facets: Sequence[str] = ()):
         """The shard's facet file (`facets_file_mmap`, add_result.rs:343-347): one typed value per doc and facet field.  columns: name ->
         numpy array [n_docs] (dtype = the facet's FieldType; names in string_facets are String16 / String32 value ids, names in
         timestamp_facets Timestamp); rows are packed field after field like the reference's facet file and handed to ssb_set_facets.
         string_values: name -> the String facet's value strings by id (`facet.values`); sorting by that facet orders by the strings
         (result_ordering_shard, min_heap.rs:861-898), so their byte-wise order is sent along (ssb_set_facet_value_order).
         point_facets: names whose column is an [n_docs, 2] float64 array of (lat, lon): Point facets, stored as their Morton codes
-        (point_column: invalid coordinates are stored as 0)."""
+        (point_column: invalid coordinates are stored as 0).
+        string_set_facets / string_set32_facets: names whose column is a per-doc list of strings: StringSet16 / StringSet32 facets, ingested
+        like the reference (string_set_facet) and sent with their member lists (ssb_set_facet_string_sets)."""
         from ._lib import SsbFacetField
         kinds = {"uint8": _lib.FACET_U8, "uint16": _lib.FACET_U16, "uint32": _lib.FACET_U32, "uint64": _lib.FACET_U64, "int8": _lib.FACET_I8,
                  "int16": _lib.FACET_I16, "int32": _lib.FACET_I32, "int64": _lib.FACET_I64, "float32": _lib.FACET_F32, "float64": _lib.FACET_F64}
-        for name in point_facets:
+        for name in (*point_facets, *string_set_facets, *string_set32_facets):
             if name not in columns:
-                raise ValueError(f"point_facets: {name!r} is not a column")
-        columns = {name: (point_column(c) if name in point_facets else c) for name, c in columns.items()}
+                raise ValueError(f"point_facets / string_set_facets: {name!r} is not a column")
+        sets = {name: string_set_facet(columns[name], 16 if name in string_set_facets else 32)
+                for name in (*string_set_facets, *string_set32_facets)}
+        columns = {name: (point_column(c) if name in point_facets else sets[name].ids if name in sets else c) for name, c in columns.items()}
         names = list(columns)
         n = len(next(iter(columns.values()))) if names else 0
         fields, off, self._facet_schema = (SsbFacetField * max(len(names), 1))(), 0, {}
@@ -435,6 +498,8 @@ class Index:
                 t = {"int64": _lib.FACET_TIMESTAMP}[a.dtype.name]
             if name in point_facets:
                 t = _lib.FACET_POINT
+            if name in sets:
+                t = _lib.FACET_STRINGSET16 if name in string_set_facets else _lib.FACET_STRINGSET32
             fields[i] = SsbFacetField(t, off)
             self._facet_schema[name] = (i, t)
             off += a.dtype.itemsize
@@ -445,6 +510,13 @@ class Index:
         self._facet_rows = (rows, fields, int(first_doc_id), n, off)      # also what the tests hand to the oracle
         self._string_values, self._string_order = {}, {}
         check(lib().ssb_set_facets(self._h, rows.ctypes.data, int(first_doc_id), n, off, fields, len(names)))
+        self._string_sets = sets
+        for name, ss in sets.items():
+            if n:
+                check(lib().ssb_set_facet_string_sets(self._h, self._facet_schema[name][0], ss.offsets.ctypes.data, ss.member_ids.ctypes.data,
+                                                      len(ss.combos), len(ss.members)))
+            self._string_values[name] = [m.decode("utf-8") for m in ss.members]      # facet counts name member ids
+            self._string_order[name] = ss.members                                   # prefixes are member-id intervals
         for name, values in (string_values or {}).items():
             t = self._facet_schema.get(name, (None, None))[1]
             if t not in (_lib.FACET_STRING16, _lib.FACET_STRING32):
@@ -501,6 +573,11 @@ class Index:
                     f64 = lambda x: int(np.float64(x).view(np.uint64))
                     flat.append(SsbFacetFilter(idx, _lib.FILTER_POINT, f64(f.start), f64(f.end), len(sets), 3))
                     sets.extend([f64(f.base[0]), f64(f.base[1]), int(DistanceUnit(f.unit))])
+                elif f.values is not None and t in _SET_FACETS:            # strings -> member ids and flagged combination ids
+                    ss = self._string_sets[next(n for n, v in self._facet_schema.items() if v[0] == idx)]
+                    vals = ss.filter_values([v for v in f.values if isinstance(v, str)]) + [int(v) for v in f.values if not isinstance(v, str)]
+                    flat.append(SsbFacetFilter(idx, _lib.FILTER_SET, 0, 0, len(sets), len(vals)))
+                    sets.extend(vals)
                 elif f.values is not None:
                     flat.append(SsbFacetFilter(idx, _lib.FILTER_SET, 0, 0, len(sets), len(f.values)))
                     sets.extend(int(v) for v in f.values)
@@ -526,13 +603,13 @@ class Index:
             idx, t = getattr(self, "_facet_schema", {}).get(qf.field, (None, None))
             if idx is None:
                 continue
-            string = t in (_lib.FACET_STRING16, _lib.FACET_STRING32)
+            string = t in _VALUE_FACETS
             if string == bool(qf.ranges):
                 continue
             by_field[qf.field] = (idx, t, qf)
         reqs, keep, meta = [], [], []
         for name, (idx, t, qf) in by_field.items():
-            if t in (_lib.FACET_STRING16, _lib.FACET_STRING32):
+            if t in _VALUE_FACETS:
                 lo = hi = has = 0
                 if qf.prefix:
                     if name not in self._string_order:
@@ -571,7 +648,7 @@ class Index:
             if facet_bases is None:
                 facet_bases = [[qf.base for qf in points]] * nq
             bases = np.ascontiguousarray(np.asarray(facet_bases, dtype=np.float64).reshape(nq, len(points), 2))
-        caps = [qf.length if t in (_lib.FACET_STRING16, _lib.FACET_STRING32) else len(qf.ranges) for _, t, qf in meta]
+        caps = [qf.length if t in _VALUE_FACETS else len(qf.ranges) for _, t, qf in meta]
         stride = sum(caps)
         out = np.zeros(max(nq * stride, 1), dtype=[("value", np.uint32), ("pad", np.uint32), ("count", np.uint64)])
         n_out = np.zeros(max(nq * n_req, 1), dtype=np.uint32)
@@ -583,7 +660,7 @@ class Index:
             for r, (name, t, qf) in enumerate(meta):
                 m = int(n_out[i * n_req + r])
                 e = out[o:o + m]
-                d[name] = ([(int(v), int(c)) for v, c in zip(e["value"], e["count"])] if t in (_lib.FACET_STRING16, _lib.FACET_STRING32)
+                d[name] = ([(int(v), int(c)) for v, c in zip(e["value"], e["count"])] if t in _VALUE_FACETS
                            else [int(c) for c in e["count"]])
                 o += caps[r]
             res.append(d)
@@ -597,7 +674,7 @@ class Index:
         reqs = {qf.field: qf for qf in query_facets if qf.field in raw}
         for name, qf in reqs.items():
             t = self._facet_schema[name][1]
-            if t in (_lib.FACET_STRING16, _lib.FACET_STRING32):
+            if t in _VALUE_FACETS:
                 sv = getattr(self, "_string_values", {}).get(name)
                 v = [(sv[i] if sv is not None else i, c) for i, c in raw[name]]
                 lengths[name] = int(qf.length)
@@ -733,13 +810,13 @@ class Index:
         arr, n_req, keep, meta = self._facet_requests(query_facets)
         if n_req == 0:
             return {}
-        caps = [qf.length if t in (_lib.FACET_STRING16, _lib.FACET_STRING32) else len(qf.ranges) for _, t, qf in meta]
+        caps = [qf.length if t in _VALUE_FACETS else len(qf.ranges) for _, t, qf in meta]
         out = np.zeros(max(sum(caps), 1), dtype=[("value", np.uint32), ("pad", np.uint32), ("count", np.uint64)])
         n_out = np.zeros(n_req, dtype=np.uint32)
         check(lib().ssb_search_empty_facets(self._h, C.addressof(arr), n_req, out.ctypes.data, n_out.ctypes.data))
         res, o = {}, 0
         for r, (name, t, qf) in enumerate(meta):
-            if t in (_lib.FACET_STRING16, _lib.FACET_STRING32):
+            if t in _VALUE_FACETS:
                 e = out[o:o + int(n_out[r])]
                 res[name] = [(int(v), int(c)) for v, c in zip(e["value"], e["count"])]
             o += caps[r]
