@@ -247,6 +247,8 @@ int32_t vec_keys(ssb_index* ix, SearchCtx& c, const void* queries, bool queries_
     a.ceil_keys = ceil_dev;
     if (ix->del.n) { a.del_slot = ix->del.d_slot; a.del_words = ix->del.d_words; }
     a.launches = &c.stats.kernel_launches;
+    uint32_t unmerged = 0;
+    if (filter) a.unmerged_lists = &unmerged;
     if (ivf) {
         // cluster probe: medoid scores, per-(query, level) selection -> one bit per (query, cluster); the scans test it per candidate
         vec::IvfArgs v{};
@@ -280,6 +282,7 @@ int32_t vec_keys(ssb_index* ix, SearchCtx& c, const void* queries, bool queries_
         vec::RefineArgs r{};
         r.rows = ix->rows.p; r.doc_ids = ix->doc_ids.p; r.n_rows = ix->n_rows; r.dpad = ix->dpad; r.queries_padded = c.qpad.p; r.margin = c.q_scale.p;
         r.keys = merged; r.keys_out = keys_out_dev;   // the refine step writes the caller's buffer directly
+        if (unmerged) { r.lists = a.scratch; r.n_lists = unmerged; r.qt = vec::queries_per_pass(scan); }   // seeded 256-query pass: merged in the refine step
         r.nq = nq; r.nq_pad = nq_pad; r.k = k;
         r.fb_lists = c.scratch.p + head_words;
         r.fb_state = reinterpret_cast<uint32_t*>(r.fb_lists + (size_t)nq_pad * ix->n_sms * LIST);

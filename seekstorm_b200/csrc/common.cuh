@@ -106,6 +106,50 @@ __device__ __forceinline__ uint64_t wl_merge(uint64_t A, uint64_t B, int lane) {
     return M;
 }
 
+// Block-wide merge of the descending lists of ONE query (256 threads = 8 warps): list l at base[l * stride].  Every warp returns the
+// top 32 of their union.  merge_lists (one CTA per query after a scan) and refine_candidates (the lists a seeded 256-query filter pass
+// left per CTA) both run it.
+constexpr uint32_t MERGE_MAX_LISTS = 2048;   // heads-first path (more lists: plain walk)
+struct MergeSmem {
+    uint64_t part[8][LIST];                  // per-warp partial merges
+    uint16_t ne[MERGE_MAX_LISTS];            // indices of the non-empty lists
+    uint32_t n_ne;
+};
+__device__ __forceinline__ uint64_t merge_lists_block(const uint64_t* __restrict__ base, uint32_t n_lists, size_t stride, MergeSmem& sm) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (threadIdx.x == 0) sm.n_ne = 0;
+    __syncthreads();
+    // Phase 1: the lists are sorted best-first, so a list is empty iff its head is 0 — all heads are probed at once (2-3 independent loads
+    // per thread for the 592 lists of a tensor-core scan) and only the non-empty lists are fetched in phase 2.  Measured on the 256-query
+    // filter batch: 27.9 -> 23.9 us per launch under ncu — a modest gain, because with sample-seeded thresholds nearly every list of a scan
+    // still receives 1-3 entries (~k * rows / sample_rows inserts per query in total); exact scans with tight thresholds and the multi-GPU
+    // merge profit more.  (A block-wide selection over the first 4 entries of every list would be the next step.)
+    const bool small = n_lists <= MERGE_MAX_LISTS;
+    if (small) {
+        for (uint32_t l = threadIdx.x; l < n_lists; l += 256)
+            if (__ldg(&base[(size_t)l * stride]) != 0ull) sm.ne[atomicAdd(&sm.n_ne, 1u)] = (uint16_t)l;
+        __syncthreads();
+    }
+    const uint32_t cnt = small ? sm.n_ne : n_lists;
+    uint64_t L = 0;
+    // Phase 2: four independent loads in flight per warp; the merge order does not matter (the result is the top 32 of the union)
+    for (uint32_t i = warp; i < cnt; i += 32) {
+        uint64_t B[4];
+#pragma unroll
+        for (int u = 0; u < 4; u++) {
+            const uint32_t k = i + 8 * u;
+            B[u] = k < cnt ? __ldg(&base[(size_t)(small ? (uint32_t)sm.ne[k] : k) * stride + lane]) : 0ull;
+        }
+#pragma unroll
+        for (int u = 0; u < 4; u++) if (__any_sync(FULL, B[u] != 0)) L = wl_merge(L, B[u], lane);
+    }
+    sm.part[warp][lane] = L;
+    __syncthreads();
+    L = sm.part[0][lane];
+    for (int w = 1; w < 8; w++) L = wl_merge(L, sm.part[w][lane], lane);
+    return L;
+}
+
 // delete set probe (shard.delete_hashset, vector.rs:1450-1451 / add_result.rs:3435): level table + one bitmap word; only on the
 // rare candidate-insert paths
 __device__ __forceinline__ bool doc_deleted(const uint32_t* __restrict__ del_slot, const uint64_t* __restrict__ del_words, uint32_t doc) {

@@ -18,7 +18,8 @@ namespace ssb {
 namespace vec {
 namespace rf {
 
-constexpr int RTHREADS = 128;   // refine: 4 warps x 8 candidates
+constexpr int RTHREADS = 256;   // refine: 8 warps x 4 candidates
+constexpr int RCAND = LIST / (RTHREADS / 32);
 constexpr int QF = 4;           // fallback: queries per corpus pass
 constexpr int FTHREADS = 256;
 
@@ -26,19 +27,24 @@ __device__ __forceinline__ float dot4(const float4 a, const float4 b, float s) {
     s = fmaf(a.x, b.x, s); s = fmaf(a.y, b.y, s); s = fmaf(a.z, b.z, s); return fmaf(a.w, b.w, s);
 }
 
-// one CTA per query
+// one CTA per query.  The approximate list is keys[q] (merged by merge_lists), or, when `lists` is set, the merge of the n_lists per-CTA
+// lists a seeded 256-query filter pass leaves in its scratch ([nq_pad / qt][n_lists][qt][32]): merged here, with no launch in between
 __global__ void __launch_bounds__(RTHREADS)
 refine_candidates(const float* __restrict__ rows, const uint32_t* __restrict__ doc_ids, uint32_t dpad, const float* __restrict__ queries,
-                  const float* __restrict__ margin, const uint64_t* keys, uint64_t* keys_out, uint32_t k, uint32_t* __restrict__ fb_state) {
+                  const float* __restrict__ margin, const uint64_t* keys, const uint64_t* __restrict__ lists, uint32_t n_lists, uint32_t qt,
+                  uint64_t* keys_out, uint32_t k, uint32_t* __restrict__ fb_state) {
     __shared__ uint64_t ex[LIST];
+    __shared__ MergeSmem msm;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const uint32_t q = blockIdx.x;
-    const uint64_t mine = keys[(size_t)q * LIST + lane];          // approximate keys, descending; low word = 0xFFFFFFFF - row
+    // approximate keys, descending; low word = 0xFFFFFFFF - row
+    const uint64_t mine = lists ? merge_lists_block(lists + (size_t)(q / qt) * n_lists * qt * LIST + (size_t)(q % qt) * LIST, n_lists, (size_t)qt * LIST, msm)
+                                : keys[(size_t)q * LIST + lane];
     const float* qv = queries + (size_t)q * dpad;
-    uint64_t ck[8]; const float* rp[8]; float s[8];
+    uint64_t ck[RCAND]; const float* rp[RCAND]; float s[RCAND];
 #pragma unroll
-    for (int c = 0; c < 8; c++) {
-        ck[c] = shfl64(mine, warp * 8 + c);
+    for (int c = 0; c < RCAND; c++) {
+        ck[c] = shfl64(mine, warp * RCAND + c);
         rp[c] = rows + (size_t)(ck[c] ? key_doc(ck[c]) : 0u) * dpad;   // empty slot: row 0, result discarded
         s[c] = 0.f;
     }
@@ -46,17 +52,17 @@ refine_candidates(const float* __restrict__ rows, const uint32_t* __restrict__ d
         for (uint32_t i = lane * 4; i < dpad; i += 128) {
             const float4 b = *reinterpret_cast<const float4*>(qv + i);
 #pragma unroll
-            for (int c = 0; c < 8; c++) s[c] = dot4(__ldg(reinterpret_cast<const float4*>(rp[c] + i)), b, s[c]);
+            for (int c = 0; c < RCAND; c++) s[c] = dot4(__ldg(reinterpret_cast<const float4*>(rp[c] + i)), b, s[c]);
         }
     }
 #pragma unroll
-    for (int c = 0; c < 8; c++) {
+    for (int c = 0; c < RCAND; c++) {
         float v = s[c];
         for (int m = 16; m; m >>= 1) v += __shfl_xor_sync(FULL, v, m);
         if (lane == 0) {
             uint64_t key = 0;
             if (ck[c] && v == v) { const uint32_t row = key_doc(ck[c]); key = pack_key(v, doc_ids ? __ldg(&doc_ids[row]) : row); }
-            ex[warp * 8 + c] = key;
+            ex[warp * RCAND + c] = key;
         }
     }
     __syncthreads();
@@ -147,7 +153,8 @@ size_t refine_scratch_words(int n_sms, uint32_t nq_pad) { return (size_t)nq_pad 
 int32_t launch_refine(const RefineArgs& a, cudaStream_t st) {
     if (a.nq == 0) return SSB_OK;
     SSB_CUDA_TRY(cudaMemsetAsync(a.fb_state, 0, 4, st));
-    rf::refine_candidates<<<a.nq, rf::RTHREADS, 0, st>>>(a.rows, a.doc_ids, a.dpad, a.queries_padded, a.margin, a.keys, a.keys_out, a.k, a.fb_state);
+    rf::refine_candidates<<<a.nq, rf::RTHREADS, 0, st>>>(a.rows, a.doc_ids, a.dpad, a.queries_padded, a.margin, a.keys, a.lists, a.n_lists, a.qt,
+                                                         a.keys_out, a.k, a.fb_state);
     SSB_CUDA_TRY(cudaGetLastError());
     const int smem = rf::QF * (int)a.dpad * 4;
     if (smem > 200 * 1024) { set_error("filter scan: vector_dims too large for the fallback scan"); return SSB_E_UNSUPPORTED; }

@@ -210,49 +210,14 @@ scan_ffma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
     }
 }
 
-constexpr uint32_t MERGE_MAX_LISTS = 2048;   // heads-first path of merge_lists (more lists: plain walk)
 // Merge `n_lists` descending 32-lists per query into one.  in: [n_groups][n_lists][qt][32] when
 // qt_major==0 ... generic form: list l of query q lives at in[(q / qt) * n_lists * qt * 32 + l * qt * 32 + (q % qt) * 32].
 __global__ void __launch_bounds__(256)
 merge_lists(const uint64_t* __restrict__ in, uint32_t n_lists, uint32_t qt, uint64_t* __restrict__ out /*[nq][32]*/) {
-    __shared__ uint64_t sm[8][LIST];
-    __shared__ uint16_t ne[MERGE_MAX_LISTS];          // indices of the non-empty lists
-    __shared__ uint32_t n_ne;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    __shared__ MergeSmem sm;
     const uint32_t q = blockIdx.x;
-    const uint64_t* base = in + (size_t)(q / qt) * n_lists * qt * LIST + (size_t)(q % qt) * LIST;
-    if (threadIdx.x == 0) n_ne = 0;
-    __syncthreads();
-    // Phase 1: the lists are sorted best-first, so a list is empty iff its head is 0 — all heads are probed at once (2-3 independent loads
-    // per thread for the 592 lists of a tensor-core scan) and only the non-empty lists are fetched in phase 2.  Measured on the 256-query
-    // filter batch: 27.9 -> 23.9 us per launch under ncu — a modest gain, because with sample-seeded thresholds nearly every list of a scan
-    // still receives 1-3 entries (~k * rows / sample_rows inserts per query in total); exact scans with tight thresholds and the multi-GPU
-    // merge profit more.  (A block-wide selection over the first 4 entries of every list would be the next step.)
-    const bool small = n_lists <= MERGE_MAX_LISTS;
-    if (small) {
-        for (uint32_t l = threadIdx.x; l < n_lists; l += 256)
-            if (__ldg(&base[(size_t)l * qt * LIST]) != 0ull) ne[atomicAdd(&n_ne, 1u)] = (uint16_t)l;
-        __syncthreads();
-    }
-    const uint32_t cnt = small ? n_ne : n_lists;
-    uint64_t L = 0;
-    // Phase 2: four independent loads in flight per warp; the merge order does not matter (the result is the top 32 of the union)
-    for (uint32_t i = warp; i < cnt; i += 32) {
-        uint64_t B[4];
-#pragma unroll
-        for (int u = 0; u < 4; u++) {
-            const uint32_t k = i + 8 * u;
-            B[u] = k < cnt ? __ldg(&base[(size_t)(small ? (uint32_t)ne[k] : k) * qt * LIST + lane]) : 0ull;
-        }
-#pragma unroll
-        for (int u = 0; u < 4; u++) if (__any_sync(FULL, B[u] != 0)) L = wl_merge(L, B[u], lane);
-    }
-    sm[warp][lane] = L;
-    __syncthreads();
-    if (warp == 0) {
-        for (int w = 1; w < 8; w++) L = wl_merge(L, sm[w][lane], lane);
-        out[(size_t)q * LIST + lane] = L;
-    }
+    const uint64_t L = merge_lists_block(in + (size_t)(q / qt) * n_lists * qt * LIST + (size_t)(q % qt) * LIST, n_lists, (size_t)qt * LIST, sm);
+    if (threadIdx.x < 32) out[(size_t)q * LIST + threadIdx.x] = L;
 }
 
 // queries [nq][dims] (row stride qstride) -> padded [nq_pad][dpad], optionally L2-normalised

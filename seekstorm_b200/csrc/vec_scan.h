@@ -43,6 +43,9 @@ struct ScanArgs {
     // IVF probe (vec_ivf.cu): selection mask [nq_pad][ivf_words] (bit per (query, cluster)) and each row's cluster id; null = AnnMode::All.
     // f32 scans only.  Like the delete set it disables the threshold-seeding sample pass (an unselected row must never seed a threshold).
     const uint32_t* ivf_sel = nullptr; uint32_t ivf_words = 0; const uint32_t* row_cluster = nullptr;
+    // filter scan: receives the number of lists per query the scan left unmerged in `scratch` ([nq_pad / NQ][n][NQ][32]) for the refine
+    // step to merge (the seeded 256-query pass, one list per query per CTA), or 0 when keys_out holds the merged lists.  Null: always merge.
+    uint32_t* unmerged_lists = nullptr;
 };
 
 // Threshold seeding: `launch` first scans the first `sample_rows` rows keeping only each 32-row group's best score per query (no
@@ -78,7 +81,9 @@ struct RefineArgs {
     const float* rows; const uint32_t* doc_ids; uint64_t n_rows; uint32_t dpad;
     const float* queries_padded;      // [nq_pad][dpad] f32 (normalised for Cosine)
     const float* margin;              // [nq_pad] 2 eps_q
-    const uint64_t* keys;             // in: merged approximate keys [nq_pad][32] (low word = 0xFFFFFFFF - row)
+    const uint64_t* keys;             // in: merged approximate keys [nq_pad][32] (low word = 0xFFFFFFFF - row), unless `lists` is set
+    const uint64_t* lists = nullptr;  // in: the scan's unmerged lists [nq_pad / qt][n_lists][qt][32] (ScanArgs::unmerged_lists), or null
+    uint32_t n_lists = 0, qt = 0;
     uint64_t* keys_out;               // out: exact keys [nq][32] (low word = 0xFFFFFFFF - doc id); may alias `keys`
     uint32_t nq, nq_pad, k;
     uint32_t* fb_state;               // [1 + nq_pad]: count of flagged queries + their indices (zeroed by the refine launch)

@@ -33,8 +33,9 @@
 // record into a shared-memory queue, and warps 1-3 of warpgroup 0 (idle otherwise: one thread issues the TMA loads) run the exact test
 // and the inserts into one list per query per CTA ([NQ][32]), each warp for a fixed third of the 8-query chunks.  An insert is ~1 us of
 // latency-bound work; in the consumer warps it held both warpgroups, and with them the tensor pipe, at the end of every tile.
-// Threshold seeding: the same kernel runs first in sample mode over one tile per SM and writes per-(32-row group, query) score
-// maxima; kth_from_groupmax turns them into valid lower bounds of the k-th best score.
+// Threshold seeding: the same kernel runs first in sample mode over a few tiles per SM and writes per-(32-row group, query) score
+// maxima (256 queries: reduced on the accumulator fragment by shuffles, without the transposition); kth_from_groupmax turns them into
+// valid lower bounds of the k-th best score.  A seeded 256-query filter scan leaves its lists unmerged: refine_candidates merges them.
 #include <cuda_bf16.h>
 #include <stdlib.h>
 #include <type_traits>
@@ -570,6 +571,34 @@ scan_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtenso
 #pragma unroll
                 for (int jb = 0; jb < NQH / CHUNK; jb++) {
                     const int c = q0 / CHUNK + jb;                    // 8-query chunk of the block
+                    if constexpr (FRAG_VOTE && !QUEUE) if (sample_mode) {   // (QUEUE kernels never run the sample pass)
+                        // sample pass, in the fragment layout: per column the best of the lane's 4 rows (2 sub-tiles x 2 rows), then
+                        // of the 8 lanes that share lane % 4 -> the group maximum over the same 32 rows as the transposed path below
+                        // stores, bit for bit (a max of ordered-uint values does not depend on the order it is taken in)
+                        uint32_t mx[2] = {0u, 0u};
+#pragma unroll
+                        for (int hm = 0; hm < 2; hm++)
+#pragma unroll
+                            for (int h = 0; h < 2; h++)
+#pragma unroll
+                                for (int b = 0; b < 2; b++) {
+                                    const uint32_t r = tile * TROWS + (uint32_t)(64 * (2 * p + hm) + 16 * w + (lane >> 2) + 8 * h);
+                                    const float sc = acc[2 * p + hm][4 * jb + 2 * h + b];
+                                    uint32_t so = (r < n_rows && sc == sc) ? ord_f32(sc) : 0u;
+                                    if (ceil_keys && so) {   // paging: rows already returned by an earlier page do not count
+                                        const uint64_t key = ((uint64_t)so << 32) | (uint64_t)(0xFFFFFFFFu - (doc_ids ? __ldg(&doc_ids[r]) : r));
+                                        if (key >= __ldg(&ceil_keys[blockIdx.y * NQ + c * CHUNK + 2 * (lane & 3) + b])) so = 0u;
+                                    }
+                                    mx[b] = max(mx[b], so);
+                                }
+#pragma unroll
+                        for (int m = 4; m < 32; m <<= 1) { mx[0] = max(mx[0], __shfl_xor_sync(FULL, mx[0], m)); mx[1] = max(mx[1], __shfl_xor_sync(FULL, mx[1], m)); }
+                        if (lane < 4) {
+                            uint32_t* g = gmaxu + (size_t)(blockIdx.y * NQ + c * CHUNK + 2 * lane) * n_rg + (tile * (TROWS / 32) + p * 4 + w);
+                            g[0] = mx[0]; g[n_rg] = mx[1];
+                        }
+                        continue;
+                    }
                     if (FRAG_VOTE && !sample_mode) {
                         // common case, in the fragment layout: the lane's 8 scores of the chunk (2 sub-tiles x 2 rows x its 2 columns)
                         // against the thresholds of its 2 columns, one vote.  A superset of the exact per-column test below: float
@@ -915,6 +944,11 @@ static int32_t launch_tc_n(const ScanArgs& a, cudaStream_t st) {
                                                         0, PREC == tc::PREC_F16F ? a.q_scale : nullptr);
         SSB_CUDA_TRY(cudaGetLastError());
         if (a.launches) *a.launches += PREC == tc::PREC_TF32 ? 3 : 2;   // (tf32 query split +) scan + kth
+        return SSB_OK;
+    }
+    if (PREC == tc::PREC_F16F && queue && a.unmerged_lists) {   // refine_candidates merges the per-CTA lists of its query itself
+        *a.unmerged_lists = gx;
+        if (a.launches) *a.launches += 1;   // scan
         return SSB_OK;
     }
     // scratch layout [group][list][q in NQ][32] -> generic merge with qt = NQ
