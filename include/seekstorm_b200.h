@@ -225,6 +225,38 @@ int32_t ssb_lexical_add_level(ssb_index* ix, const ssb_level_desc* level);
  * accumulated left to right like the reference.  Pruning bounds use an upper bound of the boost-weighted per-posting sum; such an
  * index is searched by the general (one term per lane) kernel. */
 int32_t ssb_lexical_set_field_boosts(ssb_index* ix, uint32_t n_fields, const float* boosts);
+/* ---- n-gram posting lists (NGRAM_SEARCH.md; keys tokenizer.rs:678-685) ---------------------------------------------------------
+ * An n-gram key is hash64("a b" / "a b c") | NgramType: the low 3 bits name the type (index.rs:1854-1872).  Its postings are the docs
+ * holding the n-gram, its tf the n-gram's own count, its positions the n-gram's start positions.  A PHRASE batch may list n-gram keys
+ * between single-term keys: token i must then sit at p + i + (1 per earlier bigram) + (2 per earlier trigram) (search.rs:3305-3330).
+ * LexicalSimilarity (index.rs:559-566): BM25F scores an n-gram list as the sum of its components, component c = the c-th word of the
+ * n-gram: idf_c * tf_c*(K+1)/(tf_c + cache[len]), idf_c from the component's df decoded from the key head's byte4 code
+ * (add_result.rs:1448-1478, search.rs:3231-3269).  BM25F_PROXIMITY (the reference's default) leaves the component idfs at 0 on a
+ * single-field index: an n-gram list then adds 0 to a doc's score (it still selects the docs).  With single-term keys only the two
+ * similarities score identically. */
+enum { SSB_LEXSIM_BM25F = 0, SSB_LEXSIM_BM25F_PROXIMITY = 1 };
+/* which level's key-head df bytes an n-gram list takes when it occurs in several levels: the FIRST level's (open_shard with
+ * AccessType::Ram, index.rs:3633-3664) or the LAST level's (AccessType::Mmap, decode_posting_list_counts, search.rs:2224-2277) */
+enum { SSB_NGRAM_DF_FIRST_LEVEL = 0, SSB_NGRAM_DF_LAST_LEVEL = 1 };
+/* NgramType: the low 3 bits of an n-gram key (F = frequent term, R = rare term) */
+enum { SSB_NGRAM_FF = 1, SSB_NGRAM_FR = 2, SSB_NGRAM_RF = 3, SSB_NGRAM_FFF = 4, SSB_NGRAM_RFF = 5, SSB_NGRAM_FFR = 6, SSB_NGRAM_FRF = 7 };
+/* before the first level (else SSB_E_STATE); without it an index scores n-gram lists with BM25F_PROXIMITY and the first level's df bytes */
+int32_t ssb_lexical_set_ngram_config(ssb_index* ix, uint32_t lexical_similarity, uint32_t df_level_rule);
+/* the n-gram data of one level: HOST or DEVICE arrays.  component_tfs [n_postings][3]: per posting the tfs of the n-gram's components in
+ * word order (tf_ngram1..3, add_result.rs:2076-2089; the third is ignored for bigrams, all three for single-term lists);
+ * component_df_bytes [n_terms][3]: per term the key head's posting_count_ngram_{1,2,3}_compressed bytes (compress_postinglist.rs:28-230),
+ * byte4 codes decoded like the document lengths (ignored for single-term keys). */
+typedef struct {
+    const uint16_t* component_tfs;
+    const uint8_t*  component_df_bytes;
+} ssb_level_ngrams;
+/* ssb_lexical_add_level, where every key whose low 3 bits are not 0 is an n-gram list.  ngrams NULL = ssb_lexical_add_level.  One indexed
+ * field only (several: SSB_E_UNSUPPORTED); not on a handle with a communicator, and ssb_comm_init / ssb_comm_attach / ssb_lexical_sync_df
+ * refuse an index holding n-gram lists (SSB_E_UNSUPPORTED): which level's df bytes an n-gram takes is not defined once its levels are
+ * split across GPUs.  ssb_lexical_set_global_df leaves n-gram keys alone: their dictionary idf is 1.0, the components carry the idfs.
+ * Once the index holds n-gram lists, every level must come through this call: ssb_lexical_add_level refuses a level whose keys have low
+ * bits set (SSB_E_INVALID), and this call refuses such keys when an earlier plain level carried them. */
+int32_t ssb_lexical_add_level_ngrams(ssb_index* ix, const ssb_level_desc* level, const ssb_level_ngrams* ngrams);
 int32_t ssb_lexical_commit(ssb_index* ix, uint64_t n_docs, uint64_t len_sum_normalized);
 /* dictionary export / global document-frequency override (multi-GPU block-range sharding: idf uses the
  * global df, search.rs:3225).  keys/dfs are host pointers. */
@@ -250,6 +282,15 @@ int32_t ssb_load_index_bin(ssb_index* ix, const void* bytes, uint64_t len, const
  * positions_sum_normalized, FNV checksum over every (key, level, doc id, tf) in file order, FNV checksum over every decoded
  * position (decode_positions) or 0} */
 int32_t ssb_index_bin_inspect(const void* bytes, uint64_t len, const ssb_index_bin_params* params, uint64_t out[8]);
+/* ssb_load_index_bin that also loads the n-gram posting lists of a shard built with n-gram indexing (key_head_size 22 / 23): the key heads'
+ * df bytes 14..16, the component tfs ahead of positions_count in every n-gram posting's blob (add_result.rs:2076-2089), its tf and (with
+ * decode_positions) its start positions, fed through ssb_lexical_add_level_ngrams (ssb_lexical_set_ngram_config first, if at all).
+ * ssb_load_index_bin keeps skipping n-gram keys. */
+int32_t ssb_load_index_bin_ngrams(ssb_index* ix, const void* bytes, uint64_t len, const ssb_index_bin_params* params, uint64_t* n_docs_out);
+/* host-only walk of the n-gram keys of an index.bin: out = {levels, n-gram keys, n-gram postings, sum of their tfs, FNV checksum over every
+ * n-gram key, level and df bytes and every posting's (doc id, tf, component tfs) in file order, FNV checksum over their positions
+ * (decode_positions) or 0, 0, 0} */
+int32_t ssb_index_bin_inspect_ngrams(const void* bytes, uint64_t len, const ssb_index_bin_params* params, uint64_t out[8]);
 /* vector.bin of one shard (vector.rs:1066-1094; Precision::F32 records of 24 + 4*dims bytes); dims = the index's vector_dims */
 int32_t ssb_load_vector_bin(ssb_index* ix, const void* bytes, uint64_t len, uint64_t* n_vectors_out);
 

@@ -161,6 +161,15 @@ public:
     // several indexed fields: boosts (before the first level) and the fields' names in schema order (for field_filter)
     void set_field_boosts(const std::vector<float>& boosts) { check(ssb_lexical_set_field_boosts(h_, static_cast<uint32_t>(boosts.size()), boosts.data())); }
     void set_field_names(std::vector<std::string> names) { field_names_ = std::move(names); }
+    // n-gram lists: the similarity (SSB_LEXSIM_*) and df-level rule (SSB_NGRAM_DF_*) before the first level, then levels with their
+    // component tfs [n_postings][3] and key-head df bytes [n_terms][3]
+    void set_ngram_config(uint32_t similarity, uint32_t df_rule) { check(ssb_lexical_set_ngram_config(h_, similarity, df_rule)); }
+    void add_level_ngrams(const ssb_level_desc& level, const uint16_t* component_tfs, const uint8_t* component_df_bytes) {
+        const ssb_level_ngrams ng{component_tfs, component_df_bytes};
+        check(ssb_lexical_add_level_ngrams(h_, &level, &ng));
+    }
+    // the key of an n-gram: the hash of its words joined by one space, low 3 bits replaced by its NgramType (SSB_NGRAM_*)
+    static uint64_t ngram_key(uint64_t phrase_hash, uint32_t ngram_type) { return (phrase_hash & ~7ull) | (ngram_type & 7u); }
     // TurboQuantI8 indexes: the index's +-1 sign mask (TurboQuant.seed_mask)
     void set_turboquant_mask(const std::vector<float>& seed_mask) { check(ssb_vector_set_turboquant_mask(h_, seed_mask.data(), static_cast<uint32_t>(seed_mask.size()))); }
     // facet counts of a lexical batch (query_facets; ssb_search_lexical_facets), to run next to the batch's search: per query and request,

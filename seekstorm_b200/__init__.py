@@ -4,9 +4,9 @@ Index::search(): BM25 AND/OR top-k and the brute-force f32 vector scan (+ RRF hy
 The compute lives in libseekstorm_b200.so (hand-written CUDA, C-ABI in include/seekstorm_b200.h);
 this package is the host-side mirror of the reference's search interface.  No CPU fallback.
 """
-from .index import (AnnMode, DistanceUnit, FacetFilter, Index, QueryFacet, QueryType, RangeType, Result, ResultObject, ResultSort, ResultType, SearchMode, SortOrder,
-                    VectorSimilarity, synthetic_term_key)
+from .index import (AnnMode, DistanceUnit, FacetFilter, Index, LexicalSimilarity, NgramSet, NgramType, QueryFacet, QueryType, RangeType, Result, ResultObject, ResultSort, ResultType, SearchMode, SortOrder,
+                    VectorSimilarity, ngram_key, ngram_rewrite, synthetic_term_key)
 from ._lib import SsbError, lib, LIB_PATH
 
-__all__ = ["AnnMode", "DistanceUnit", "FacetFilter", "Index", "QueryFacet", "QueryType", "RangeType", "Result", "ResultObject", "ResultSort", "ResultType", "SearchMode", "SortOrder",
-           "VectorSimilarity", "SsbError", "lib", "LIB_PATH", "synthetic_term_key"]
+__all__ = ["AnnMode", "DistanceUnit", "FacetFilter", "Index", "LexicalSimilarity", "NgramSet", "NgramType", "QueryFacet", "QueryType", "RangeType", "Result", "ResultObject", "ResultSort", "ResultType", "SearchMode", "SortOrder",
+           "VectorSimilarity", "SsbError", "lib", "LIB_PATH", "ngram_key", "ngram_rewrite", "synthetic_term_key"]

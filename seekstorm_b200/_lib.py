@@ -53,6 +53,16 @@ class SsbLevelDesc(C.Structure):
                 ("tfs", C.c_void_p), ("doc_len_bytes", C.c_void_p), ("positions", C.c_void_p)]
 
 
+class SsbLevelNgrams(C.Structure):
+    _fields_ = [("component_tfs", C.c_void_p), ("component_df_bytes", C.c_void_p)]
+
+
+# SSB_LEXSIM_* (LexicalSimilarity), SSB_NGRAM_DF_* (which level's df bytes an n-gram list keeps), SSB_NGRAM_* (NgramType, key low bits)
+LEXSIM_BM25F, LEXSIM_BM25F_PROXIMITY = 0, 1
+NGRAM_DF_FIRST_LEVEL, NGRAM_DF_LAST_LEVEL = 0, 1
+NGRAM_FF, NGRAM_FR, NGRAM_RF, NGRAM_FFF, NGRAM_RFF, NGRAM_FFR, NGRAM_FRF = 1, 2, 3, 4, 5, 6, 7
+
+
 class SsbLexBatch(C.Structure):
     _fields_ = [("n_queries", C.c_uint32), ("query_type", C.c_uint32), ("term_offsets", C.c_void_p),
                 ("term_keys", C.c_void_p), ("term_flags", C.c_void_p),
@@ -111,8 +121,8 @@ class SsbStats(C.Structure):
 # every symbol include/seekstorm_b200.h declares
 EXPORTS = [
     "ssb_abi_version", "ssb_last_error", "ssb_create", "ssb_destroy", "ssb_lexical_add_level",
-    "ssb_vector_add_level_clustered", "ssb_lexical_set_field_boosts", "ssb_lexical_commit", "ssb_lexical_dict_size", "ssb_lexical_dict_export", "ssb_lexical_set_global_df",
-    "ssb_load_index_bin", "ssb_load_vector_bin", "ssb_index_bin_inspect", "ssb_set_deleted", "ssb_set_facets", "ssb_set_facet_value_order", "ssb_set_facet_string_sets", "ssb_vector_set_turboquant_mask", "ssb_vector_add_level", "ssb_vector_count", "ssb_vector_reserve", "ssb_set_vector_kernel", "ssb_search_lexical", "ssb_search_lexical_sorted", "ssb_search_lexical_sorted_ex", "ssb_search_lexical_facets", "ssb_search_empty", "ssb_search_empty_facets", "ssb_search_vector", "ssb_search_vector_ex", "ssb_search_hybrid",
+    "ssb_vector_add_level_clustered", "ssb_lexical_set_field_boosts", "ssb_lexical_set_ngram_config", "ssb_lexical_add_level_ngrams", "ssb_lexical_commit", "ssb_lexical_dict_size", "ssb_lexical_dict_export", "ssb_lexical_set_global_df",
+    "ssb_load_index_bin", "ssb_load_index_bin_ngrams", "ssb_load_vector_bin", "ssb_index_bin_inspect", "ssb_index_bin_inspect_ngrams", "ssb_set_deleted", "ssb_set_facets", "ssb_set_facet_value_order", "ssb_set_facet_string_sets", "ssb_vector_set_turboquant_mask", "ssb_vector_add_level", "ssb_vector_count", "ssb_vector_reserve", "ssb_set_vector_kernel", "ssb_search_lexical", "ssb_search_lexical_sorted", "ssb_search_lexical_sorted_ex", "ssb_search_lexical_facets", "ssb_search_empty", "ssb_search_empty_facets", "ssb_search_vector", "ssb_search_vector_ex", "ssb_search_hybrid",
     "ssb_rrf_fuse", "ssb_comm_unique_id", "ssb_comm_init", "ssb_comm_attach", "ssb_comm_destroy", "ssb_lexical_sync_df",
     "ssb_search_vector_keys", "ssb_search_lexical_keys", "ssb_merge_keys", "ssb_sync",
     "ssb_stream", "ssb_set_stream", "ssb_last_stats",
@@ -142,6 +152,8 @@ def lib():
         "ssb_lexical_add_level": [vp, C.POINTER(SsbLevelDesc)],
         "ssb_lexical_commit": [vp, u64, u64],
         "ssb_lexical_set_field_boosts": [vp, u32, vp],
+        "ssb_lexical_set_ngram_config": [vp, u32, u32],
+        "ssb_lexical_add_level_ngrams": [vp, C.POINTER(SsbLevelDesc), C.POINTER(SsbLevelNgrams)],
         "ssb_lexical_dict_size": [vp, C.POINTER(u64)],
         "ssb_lexical_dict_export": [vp, vp, vp, u64],
         "ssb_lexical_set_global_df": [vp, vp, vp, u64],
@@ -150,6 +162,8 @@ def lib():
         "ssb_load_index_bin": [vp, vp, u64, C.POINTER(SsbIndexBinParams), C.POINTER(u64)],
         "ssb_load_vector_bin": [vp, vp, u64, C.POINTER(u64)],
         "ssb_index_bin_inspect": [vp, u64, C.POINTER(SsbIndexBinParams), vp],
+        "ssb_load_index_bin_ngrams": [vp, vp, u64, C.POINTER(SsbIndexBinParams), C.POINTER(u64)],
+        "ssb_index_bin_inspect_ngrams": [vp, u64, C.POINTER(SsbIndexBinParams), vp],
         "ssb_set_deleted": [vp, vp, u64],
         "ssb_set_facets": [vp, vp, u64, u64, u32, vp, u32],
         "ssb_set_facet_value_order": [vp, u32, vp, u32],

@@ -603,7 +603,7 @@ int32_t ssb_lexical_add_level(ssb_index* ix, const ssb_level_desc* level) {
     std::unique_lock<std::shared_mutex> g(ix->rw);
     SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
     if (level && (is_device_ptr(level->doc_ids) || is_device_ptr(level->term_keys))) SSB_CUDA_TRY(cudaDeviceSynchronize());   // inputs produced on another stream
-    return ix->lex->add_level(level);
+    return ix->lex->add_level_plain(level);
     SSB_API_END
 }
 
@@ -613,6 +613,25 @@ int32_t ssb_lexical_set_field_boosts(ssb_index* ix, uint32_t n_fields, const flo
     if (boosts && is_device_ptr(boosts)) { set_error("boosts must be host memory"); return SSB_E_INVALID; }
     std::unique_lock<std::shared_mutex> g(ix->rw);
     return ix->lex->set_fields(n_fields, boosts);
+    SSB_API_END
+}
+
+int32_t ssb_lexical_set_ngram_config(ssb_index* ix, uint32_t lexical_similarity, uint32_t df_level_rule) {
+    SSB_API_BEGIN
+    if (!ix) { set_error("null index"); return SSB_E_INVALID; }
+    std::unique_lock<std::shared_mutex> g(ix->rw);
+    return ix->lex->set_ngram_config(lexical_similarity, df_level_rule);
+    SSB_API_END
+}
+
+int32_t ssb_lexical_add_level_ngrams(ssb_index* ix, const ssb_level_desc* level, const ssb_level_ngrams* ngrams) {
+    SSB_API_BEGIN
+    if (!ix) { set_error("null index"); return SSB_E_INVALID; }
+    std::unique_lock<std::shared_mutex> g(ix->rw);
+    SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
+    if (ngrams && ix->comm.active()) { set_error("ssb_lexical_add_level_ngrams: n-gram lists on a sharded index are not supported"); return SSB_E_UNSUPPORTED; }
+    if (level && (is_device_ptr(level->doc_ids) || is_device_ptr(level->term_keys))) SSB_CUDA_TRY(cudaDeviceSynchronize());   // inputs produced on another stream
+    return ix->lex->add_level_ngrams(level, ngrams);
     SSB_API_END
 }
 
@@ -852,6 +871,24 @@ int32_t ssb_index_bin_inspect(const void* bytes, uint64_t len, const ssb_index_b
     SSB_API_BEGIN
     if (!bytes || !params || !out) { set_error("ssb_index_bin_inspect: null argument"); return SSB_E_INVALID; }
     return inspect_index_bin((const uint8_t*)bytes, len, params, out);
+    SSB_API_END
+}
+
+int32_t ssb_load_index_bin_ngrams(ssb_index* ix, const void* bytes, uint64_t len, const ssb_index_bin_params* params, uint64_t* n_docs_out) {
+    SSB_API_BEGIN
+    if (!ix || !bytes || !params) { set_error("ssb_load_index_bin_ngrams: null argument"); return SSB_E_INVALID; }
+    if (is_device_ptr(bytes)) { set_error("ssb_load_index_bin_ngrams: bytes must be host memory"); return SSB_E_INVALID; }
+    std::unique_lock<std::shared_mutex> g(ix->rw);
+    SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
+    if (ix->comm.active()) { set_error("ssb_load_index_bin_ngrams: n-gram lists on a sharded index are not supported"); return SSB_E_UNSUPPORTED; }
+    return load_index_bin(ix->lex, (const uint8_t*)bytes, len, params, n_docs_out, true);
+    SSB_API_END
+}
+
+int32_t ssb_index_bin_inspect_ngrams(const void* bytes, uint64_t len, const ssb_index_bin_params* params, uint64_t out[8]) {
+    SSB_API_BEGIN
+    if (!bytes || !params || !out) { set_error("ssb_index_bin_inspect_ngrams: null argument"); return SSB_E_INVALID; }
+    return inspect_index_bin_ngrams((const uint8_t*)bytes, len, params, out);
     SSB_API_END
 }
 
@@ -1296,6 +1333,7 @@ int32_t ssb_comm_init(ssb_index* ix, const uint8_t* id128, uint32_t rank, uint32
     std::unique_lock<std::shared_mutex> g(ix->rw);
     SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
     if (ix->comm.comm) { set_error("ssb_comm_init: the index already has a communicator"); return SSB_E_STATE; }
+    if (ix->lex->has_ngrams() && world > 1) { set_error("ssb_comm_init: n-gram lists on a sharded index are not supported"); return SSB_E_UNSUPPORTED; }
     SSB_TRY(comm_init(ix->comm, id128, rank, world));
     std::lock_guard<std::mutex> g2(ix->pool_mu);
     if (ix->pool.size() > 1) { ix->pool.resize(1); ix->free_ctx.clear(); ix->free_ctx.push_back(ix->pool[0].get()); ix->last_ctx = nullptr; }
@@ -1308,6 +1346,7 @@ int32_t ssb_comm_attach(ssb_index* ix, void* nccl_comm, uint32_t rank, uint32_t 
     if (!ix || !nccl_comm || world == 0 || rank >= world) { set_error("ssb_comm_attach: bad argument"); return SSB_E_INVALID; }
     std::unique_lock<std::shared_mutex> g(ix->rw);
     if (ix->comm.comm) { set_error("ssb_comm_attach: the index already has a communicator"); return SSB_E_STATE; }
+    if (ix->lex->has_ngrams() && world > 1) { set_error("ssb_comm_attach: n-gram lists on a sharded index are not supported"); return SSB_E_UNSUPPORTED; }
     ix->comm.comm = nccl_comm; ix->comm.rank = rank; ix->comm.world = world; ix->comm.owned = false;
     std::lock_guard<std::mutex> g2(ix->pool_mu);
     if (ix->pool.size() > 1) { ix->pool.resize(1); ix->free_ctx.clear(); ix->free_ctx.push_back(ix->pool[0].get()); ix->last_ctx = nullptr; }
@@ -1333,6 +1372,7 @@ int32_t ssb_lexical_sync_df(ssb_index* ix) {
     std::unique_lock<std::shared_mutex> g(ix->rw);
     SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
     if (!ix->comm.active()) return SSB_OK;
+    if (ix->lex->has_ngrams()) { set_error("ssb_lexical_sync_df: n-gram lists on a sharded index are not supported"); return SSB_E_UNSUPPORTED; }
     if (!ix->lex->committed()) { set_error("ssb_lexical_sync_df before ssb_lexical_commit"); return SSB_E_STATE; }
     cudaStream_t st = ix->load_st;
     const std::vector<uint64_t>& keys = ix->lex->host_keys();

@@ -154,6 +154,39 @@ __global__ void fill_bounds(LexView v, uint32_t* __restrict__ post, float* __res
     post[i] = (post[i] & 0xFFFFu) | ((uint32_t)__half_as_ushort(h) << 16);
 }
 
+// n-gram lists (ssb_lexical_add_level_ngrams).  One (n-gram key, level) segment at commit: its postings in the arenas, the first of its
+// component tfs in the commit's tf array (segments in tf order), the resolved component idfs (n_comp = 0: BM25F_PROXIMITY, the list adds 0)
+struct NgSegDev { uint64_t post_off, tf_off; uint32_t cnt, n_comp; float idf[3]; uint32_t pad; };
+__device__ __forceinline__ float ngram_part(const LexView& v, uint32_t tf, float bc) {
+    const float t = (float)tf;
+    return __fdiv_rn(__fmul_rn(t, v.k1p), __fadd_rn(t, bc));       // tf_c*(K+1)/(tf_c + cache[len]) (+ SIGMA = 0)
+}
+// BM25F of an n-gram posting (add_result.rs:1448-1478): idf1*part(tf1) + idf2*part(tf2) [+ idf3*part(tf3)], summed left to right.  It
+// replaces the posting's component and fp16 bound (the list's dictionary idf is 1.0, so idf * comp is that sum bit for bit); maxbits
+// collects the largest component (positive floats order like their bits) for the coarse bound step.  One thread per n-gram posting (the
+// segment by binary search over the segments' first tf slots), one atomic per warp.
+__global__ void fill_ngram_bounds(LexView v, const NgSegDev* __restrict__ segs, uint32_t n_segs, const uint16_t* __restrict__ tfs, uint64_t n,
+                                  uint32_t* __restrict__ post, float* __restrict__ comp, uint32_t* maxbits) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    float c = 0.f;
+    if (i < n) {
+        uint32_t lo = 0, hi = n_segs;                                  // the last segment whose first slot is <= i
+        while (hi - lo > 1) { const uint32_t m = (lo + hi) >> 1; if (segs[m].tf_off <= i) lo = m; else hi = m; }
+        const NgSegDev sg = segs[lo];
+        const uint64_t p = sg.post_off + (i - sg.tf_off);
+        const uint16_t* t = tfs + 3 * i;
+        const float bc = __ldg(&v.cache[(v.pay[p] >> 16) & 255u]);
+        if (sg.n_comp) {
+            c = __fadd_rn(__fmul_rn(sg.idf[0], ngram_part(v, t[0], bc)), __fmul_rn(sg.idf[1], ngram_part(v, t[1], bc)));
+            if (sg.n_comp == 3) c = __fadd_rn(c, __fmul_rn(sg.idf[2], ngram_part(v, t[2], bc)));
+        }
+        comp[p] = c;
+        post[p] = (post[p] & 0xFFFFu) | ((uint32_t)__half_as_ushort(__float2half_ru(c)) << 16);
+    }
+    for (int s = 16; s; s >>= 1) c = fmaxf(c, __shfl_xor_sync(FULL, c, s));
+    if ((threadIdx.x & 31) == 0) atomicMax(maxbits, __float_as_uint(c));
+}
+
 __global__ void gather_dict(const uint64_t* __restrict__ term_keys, uint32_t n_terms, uint32_t level_idx,
                             uint64_t* __restrict__ keys_out, uint64_t* __restrict__ vals_out) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -273,7 +306,7 @@ __device__ __forceinline__ void rec_set_sort_bound(LvRec& r, uint64_t b) { r.S[0
 __device__ __forceinline__ uint64_t rec_sort_bound(const LvRec& r) { return ((uint64_t)__float_as_uint(r.S[1]) << 32) | __float_as_uint(r.S[0]); }
 template <bool SORTED>
 __global__ void __launch_bounds__(128) lex_plan(LexView v, const uint32_t* __restrict__ q_off, const uint64_t* __restrict__ q_keys,
-                                                const uint8_t* __restrict__ q_flags /*or null*/, const uint32_t* __restrict__ f_off /*or null*/, const uint32_t* __restrict__ f_mask /*or null*/, uint32_t flags /* bit 0 phrase batch, bit 1 no counts wanted */, uint32_t query_type, QueryPlan* plans, LvRec* recs, uint16_t* item_start, uint32_t* ctr,
+                                                const uint8_t* __restrict__ q_flags /*or null*/, const uint32_t* __restrict__ f_off /*or null*/, const uint32_t* __restrict__ f_mask /*or null*/, uint32_t flags /* bit 0 phrase batch, bit 1 no counts wanted, bit 2 the index holds n-gram lists */, uint32_t query_type, QueryPlan* plans, LvRec* recs, uint16_t* item_start, uint32_t* ctr,
                                                 uint64_t* theta, int* lock, uint64_t* count, uint64_t* glist, uint32_t n_pow2,
                                                 uint32_t item_w, uint32_t first_lim, uint32_t gmax, SortDev sort) {
     extern __shared__ __align__(16) uint8_t sm_raw[];
@@ -311,7 +344,7 @@ __global__ void __launch_bounds__(128) lex_plan(LexView v, const uint32_t* __res
     __syncthreads();
     if (threadIdx.x == 0) {
         uint32_t nl = 0, nn = 0; bool missing = false;
-        uint32_t n_phr = 0;
+        uint32_t n_phr = 0, phr_off = 0;
         for (uint32_t t = 0; t < nt; t++) {
             if (sflag[t] & SSB_TERM_NOT) {                  // '-' terms: exclusion lists, never scored (an unknown NOT term excludes nothing)
                 bool dup = false;
@@ -326,7 +359,13 @@ __global__ void __launch_bounds__(128) lex_plan(LexView v, const uint32_t* __res
             for (uint32_t u = 0; u < nl; u++) if (pl.t[u].first == st[t].first) { dup = true; uidx = u; }
             if (!dup) pl.t[nl++] = st[t];
             // phrase: token n_phr of the phrase (term_index_nonunique) is unique term uidx (non_unique_query_list, add_result.rs:3594-3607)
-            if ((flags & 1u) && n_phr < SSB_MAX_QUERY_TERMS) pl.phr[n_phr++] = (uint8_t)uidx;
+            // an n-gram token spans 2 (bigram) or 3 (trigram) positions: the tokens after it sit 1 or 2 further on (preceding_ngram_count,
+            // search.rs:3305-3330).  The offsets stay below 32 + 2 * 31.
+            if ((flags & 1u) && n_phr < SSB_MAX_QUERY_TERMS) {
+                pl.phr[n_phr] = (uint8_t)uidx; pl.phr_off[n_phr] = (uint8_t)phr_off; n_phr++;
+                const uint32_t ty = (flags & 4u) ? (uint32_t)(q_keys[t0 + t] & 7u) : 0u;
+                phr_off += ty == 0 ? 1u : (ty <= SSB_NGRAM_RF ? 2u : 3u);
+            }
         }
         if ((flags & 1u) && (missing || nl == 0)) n_phr = 0;
         pl.n_phr = ((flags & 1u) && n_phr >= 2 && nl) ? n_phr : 0u;      // a one-token phrase is a plain term query
@@ -603,9 +642,11 @@ __device__ __noinline__ bool field_rejects_impl(ListView v, const uint32_t* payf
 // Phrase check (add_result.rs:3586-3684): the doc (already known to contain every term) matches iff some start position p has token i of
 // the phrase at p + i for every i — the reference finds it by a k-way merge of the tokens' position lists aligned by their index in the
 // phrase (term_index_nonunique); the same merge here, one thread per candidate doc (rare path, out of line).  Unique term u's positions
-// are positions[ubase[u] .. + utf[u]); true = some start s has token i at s + i for every i (phrasematch_count >= 1).  The cursors `cur`
+// are positions[ubase[u] .. + utf[u]); true = some start s has token i at s + phr_off[i] for every i (phrasematch_count >= 1); phr_off[i]
+// is i unless an earlier token is an n-gram.  OFFS = false (several indexed fields, which hold no n-gram lists): the offsets are i.  The cursors `cur`
 // (one per token) are an array of the calling check, on the thread's stack: declared there, after its own arrays, they keep that
 // function's frame layout and with it the register allocation of lex_generic<true>.
+template <bool OFFS>
 __device__ __forceinline__ bool phrase_in_runs(const uint16_t* positions, const QueryPlan* pl, const uint64_t* ubase, const uint32_t* utf, uint32_t* cur) {
     const uint32_t m = pl->n_phr, u0 = pl->phr[0];
     for (uint32_t i = 0; i < m; i++) cur[i] = 0;
@@ -614,10 +655,11 @@ __device__ __forceinline__ bool phrase_in_runs(const uint16_t* positions, const 
         bool all = true; uint32_t next_s = s;
         for (uint32_t i = 1; i < m; i++) {
             const uint32_t u = pl->phr[i];
-            while (cur[i] < utf[u] && (uint32_t)__ldg(&positions[ubase[u] + cur[i]]) < s + i) cur[i]++;
+            const uint32_t o = OFFS ? (uint32_t)pl->phr_off[i] : i;
+            while (cur[i] < utf[u] && (uint32_t)__ldg(&positions[ubase[u] + cur[i]]) < s + o) cur[i]++;
             if (cur[i] >= utf[u]) return false;                             // a token's positions are exhausted: no (further) match
             const uint32_t p = __ldg(&positions[ubase[u] + cur[i]]);
-            if (p != s + i) { all = false; next_s = p - i; break; }          // p > s + i: the start must move up to at least p - i
+            if (p != s + o) { all = false; next_s = p - o; break; }          // p > s + o: the start must move up to at least p - o
         }
         if (all) return true;
         while (cur[0] < utf[u0] && (uint32_t)__ldg(&positions[ubase[u0] + cur[0]]) < next_s) cur[0]++;
@@ -635,7 +677,7 @@ __device__ __noinline__ bool phrase_rejects_impl(ListView v, PhraseArgs a, const
         utf[t] = __ldg(&a.pay[pos]) & 0xFFFFu;
     }
     uint32_t cur[SSB_MAX_QUERY_TERMS];
-    return !phrase_in_runs(a.positions, pl, ubase, utf, cur);
+    return !phrase_in_runs<true>(a.positions, pl, ubase, utf, cur);
 }
 // Several indexed fields (add_result.rs:3247-3389): a posting's positions are one run per field, field 0 first, each restarting from 0, of
 // the posting's per-field tfs (a.pay = payf here).  The same merge as above runs field by field on those runs only — a phrase never spans two
@@ -665,7 +707,7 @@ __device__ __noinline__ bool phrase_rejects_fields_impl(ListView v, PhraseArgs a
             in_all = in_all && utf[t] != 0;
         }
         if (!in_all || (field_mask && !((field_mask >> f) & 1u))) continue;
-        if (phrase_in_runs(a.positions, pl, ubase, utf, cur)) return false;
+        if (phrase_in_runs<false>(a.positions, pl, ubase, utf, cur)) return false;
     }
     return true;
 }
@@ -1907,6 +1949,67 @@ int32_t LexIndex::set_fields(uint32_t n_fields, const float* boosts) {
     return SSB_OK;
 }
 
+int32_t LexIndex::set_ngram_config(uint32_t similarity, uint32_t df_rule) {
+    if (similarity > SSB_LEXSIM_BM25F_PROXIMITY || df_rule > SSB_NGRAM_DF_LAST_LEVEL) { set_error("set_ngram_config: unknown similarity / df rule"); return SSB_E_INVALID; }
+    if (!levels_.empty()) { set_error("set_ngram_config: call it before the first level is added"); return SSB_E_STATE; }
+    lex_sim_ = similarity; ng_rule_ = df_rule;
+    return SSB_OK;
+}
+
+int32_t LexIndex::add_level_ngrams(const ssb_level_desc* d, const ssb_level_ngrams* ng) {
+    if (!ng) return add_level(d);
+    if (!d) { set_error("add_level: null level"); return SSB_E_INVALID; }
+    if (n_fields_ > 1 || d->n_fields > 1) { set_error("add_level_ngrams: n-gram lists need an index with one indexed field"); return SSB_E_UNSUPPORTED; }
+    // the level's n-gram keys: the terms whose key has low bits set
+    std::vector<uint64_t> keys(d->n_terms); std::vector<uint32_t> offs((size_t)d->n_terms + 1, 0u);
+    if (d->n_terms && d->term_keys && d->posting_offsets) {
+        SSB_CUDA_TRY(cudaMemcpy(keys.data(), d->term_keys, (size_t)d->n_terms * 8, cudaMemcpyDefault));
+        SSB_CUDA_TRY(cudaMemcpy(offs.data(), d->posting_offsets, ((size_t)d->n_terms + 1) * 4, cudaMemcpyDefault));
+    }
+    std::vector<uint32_t> ng_terms;
+    for (uint32_t t = 0; t < d->n_terms; t++) if (keys[t] & 7u) ng_terms.push_back(t);
+    if (ng_terms.empty()) return add_level(d);
+    if (plain_lowbit_) { set_error("add_level_ngrams: an earlier level added without n-gram data carried keys with low bits set"); return SSB_E_INVALID; }
+    if (!ng->component_tfs || !ng->component_df_bytes) { set_error("add_level_ngrams: null component_tfs / component_df_bytes"); return SSB_E_INVALID; }
+    std::vector<uint8_t> dfb((size_t)d->n_terms * 3);
+    SSB_CUDA_TRY(cudaMemcpy(dfb.data(), ng->component_df_bytes, dfb.size(), cudaMemcpyDefault));
+    const uint64_t base = n_post_;
+    SSB_TRY(add_level(d));                                                 // validates the level (offsets ascend) and appends it
+    const uint32_t np = offs[d->n_terms];
+    std::vector<uint64_t> seg; seg.reserve(ng_terms.size() * 3);
+    uint64_t n_tf = 0;
+    for (uint32_t t : ng_terms) {
+        const uint32_t cnt = offs[t + 1] - offs[t];
+        if (!cnt) continue;
+        NgSeg g{}; g.key = keys[t]; g.post_off = base + offs[t]; g.tf_off = n_ng_tf_ + n_tf; g.cnt = cnt;
+        for (int c = 0; c < 3; c++) g.dfb[c] = dfb[(size_t)t * 3 + c];
+        ng_segs_.push_back(g);
+        seg.push_back(offs[t]); seg.push_back(n_tf); seg.push_back(cnt);
+        n_tf += cnt;
+    }
+    if (!n_tf) return SSB_OK;
+    // the component tfs stay on the host (a re-commit recomputes the components from them); only commit uploads them, for its kernel
+    std::vector<uint16_t> all((size_t)np * 3);
+    SSB_CUDA_TRY(cudaMemcpy(all.data(), ng->component_tfs, all.size() * 2, cudaMemcpyDefault));
+    h_ng_tf_.reserve(h_ng_tf_.size() + n_tf * 3);
+    for (size_t j = 0; j < seg.size(); j += 3) h_ng_tf_.insert(h_ng_tf_.end(), all.begin() + 3 * seg[j], all.begin() + 3 * (seg[j] + seg[j + 2]));
+    n_ng_tf_ += n_tf;
+    return SSB_OK;
+}
+
+int32_t LexIndex::add_level_plain(const ssb_level_desc* d) {
+    bool low = false;
+    if (d && d->n_terms && d->term_keys) {
+        std::vector<uint64_t> keys(d->n_terms);
+        SSB_CUDA_TRY(cudaMemcpy(keys.data(), d->term_keys, (size_t)d->n_terms * 8, cudaMemcpyDefault));
+        for (uint64_t k : keys) low = low || (k & 7u) != 0;
+    }
+    if (low && has_ngrams()) { set_error("add_level: keys with low bits set on an index with n-gram lists (ssb_lexical_add_level_ngrams)"); return SSB_E_INVALID; }
+    SSB_TRY(add_level(d));
+    plain_lowbit_ = plain_lowbit_ || low;
+    return SSB_OK;
+}
+
 int32_t LexIndex::add_level(const ssb_level_desc* d) {
     const uint32_t nf = n_fields_;
     if (d && (d->n_fields > 1 ? d->n_fields : 1u) != nf) { set_error("add_level: the level carries %u field(s), the index %u", d->n_fields > 1 ? d->n_fields : 1u, nf); return SSB_E_INVALID; }
@@ -2012,15 +2115,20 @@ int32_t LexIndex::add_level(const ssb_level_desc* d) {
     return SSB_OK;
 }
 
+// DOCUMENT_LENGTH_COMPRESSION (byte4_to_int, index.rs:4255-4279)
+static uint32_t byte4_to_int(uint32_t b) {
+    if (b < 24) return b;
+    const uint32_t x = b - 24, bits = x & 7, shift = x >> 3;
+    return shift == 0 ? 24 + bits : 24 + ((bits | 8) << (shift - 1));
+}
+
 static void host_bm25_cache(uint64_t n_docs, uint64_t len_sum, float* cache) {
     // commit.rs:318-325; DOCUMENT_LENGTH_COMPRESSION = byte4_to_int (index.rs:4255-4279).  volatile keeps every
     // f32 operation individually rounded regardless of host compiler contraction settings.
     volatile float avgdl = (float)len_sum / (float)n_docs;
     const float K = 1.2f, B = 0.75f;
     for (int i = 0; i < 256; i++) {
-        uint32_t b = (uint32_t)i, v;
-        if (b < 24) v = b;
-        else { uint32_t x = b - 24, bits = x & 7, shift = x >> 3; v = shift == 0 ? 24 + bits : 24 + ((bits | 8) << (shift - 1)); }
+        const uint32_t v = byte4_to_int((uint32_t)i);
         volatile float quot = (float)v / avgdl;
         volatile float bq = B * quot;
         volatile float omb = 1.0f - B;
@@ -2043,7 +2151,7 @@ LexView LexIndex::view() const {
     LexView v{};
     v.dict_keys = d_dict_keys_; v.n_terms = n_terms_; v.term_first = d_term_first_; v.term_idf = d_term_idf_; v.term_df = d_term_df_;
     v.e_level = d_e_level_; v.e_off = d_e_off_; v.e_count = d_e_count_; v.e_maxcomp = d_e_maxcomp_; v.e_bitmap = d_e_bitmap_;
-    v.post = post_.p; v.pay = pay_.p; v.comp = comp_.p; v.bm_words = d_bm_words_; v.bm = d_bm_; v.bm_q8 = d_bm_q8_; v.q8_step = Q8_STEP; v.level_ids = d_level_ids_;
+    v.post = post_.p; v.pay = pay_.p; v.comp = comp_.p; v.bm_words = d_bm_words_; v.bm = d_bm_; v.bm_q8 = d_bm_q8_; v.q8_step = q8_step_ > 0.f ? q8_step_ : Q8_STEP; v.level_ids = d_level_ids_;
     v.n_levels = (uint32_t)levels_.size(); v.cache = d_cache_;
     v.k1p = 1.2f + 1.0f;
     v.payf = payf_.p; v.compf = compf_.p; v.n_fields = n_fields_; v.fast_t = n_fields_ > 1 ? 0u : FAST_T;
@@ -2052,6 +2160,58 @@ LexView LexIndex::view() const {
     if (has_positions_ == 1 && d_lvl_pos_base_) { v.positions = positions_.p; v.pos_off = pos_off_.p; v.lvl_pos_base = d_lvl_pos_base_; }
     if (facets_ && facets_->n_facets) { v.facet_keys = facets_->d_keys; v.facet_rows = facets_->n_rows; v.facet_first_doc = facets_->first_doc; v.n_facets = facets_->n_facets; }
     return v;
+}
+
+// the n-gram lists at commit: each key's component dfs from the df bytes of its first or last level (ng_rule_), the component idfs over
+// n_docs (search.rs:3231-3269), then fill_ngram_bounds on every segment; the coarse bound step grows with the largest component
+int32_t LexIndex::commit_ngrams(uint64_t n_docs) {
+    h_ng_keys_.clear();
+    if (ng_segs_.empty()) return SSB_OK;
+    std::vector<uint32_t> order(ng_segs_.size());
+    for (uint32_t i = 0; i < order.size(); i++) order[i] = i;
+    std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return ng_segs_[a].key < ng_segs_[b].key; });   // levels ascend in a key
+    std::vector<NgSegDev> segs(ng_segs_.size());
+    for (size_t a = 0; a < order.size();) {
+        size_t b = a;
+        while (b < order.size() && ng_segs_[order[b]].key == ng_segs_[order[a]].key) b++;
+        const NgSeg& src = ng_segs_[order[ng_rule_ == SSB_NGRAM_DF_LAST_LEVEL ? b - 1 : a]];
+        const uint32_t ty = (uint32_t)(src.key & 7u);
+        const uint32_t n_comp = lex_sim_ == SSB_LEXSIM_BM25F ? (ty <= SSB_NGRAM_RF ? 2u : 3u) : 0u;
+        float idf[3] = {0.f, 0.f, 0.f};
+        for (uint32_t c = 0; c < n_comp; c++) idf[c] = host_idf(n_docs, byte4_to_int(src.dfb[c]));
+        for (size_t j = a; j < b; j++) {
+            const NgSeg& g = ng_segs_[order[j]];
+            NgSegDev& o = segs[order[j]];
+            o.post_off = g.post_off; o.tf_off = g.tf_off; o.cnt = g.cnt; o.n_comp = n_comp; o.pad = 0;
+            for (int c = 0; c < 3; c++) o.idf[c] = idf[c];
+        }
+        h_ng_keys_.push_back(src.key);
+        a = b;
+    }
+    DevTmp<NgSegDev> t_segs; DevTmp<uint32_t> t_max; DevTmp<uint16_t> t_tf;
+    SSB_CUDA_TRY(t_segs.alloc(segs.size())); SSB_CUDA_TRY(t_max.alloc(1)); SSB_CUDA_TRY(t_tf.alloc(h_ng_tf_.size()));
+    SSB_CUDA_TRY(to_device(t_segs.p, segs.data(), segs.size() * sizeof(NgSegDev), st_));
+    SSB_CUDA_TRY(to_device(t_tf.p, h_ng_tf_.data(), h_ng_tf_.size() * 2, st_));
+    SSB_CUDA_TRY(cudaMemsetAsync(t_max.p, 0, 4, st_));
+    LexView v{};
+    v.pay = pay_.p; v.cache = d_cache_; v.k1p = 1.2f + 1.0f;
+    fill_ngram_bounds<<<(unsigned)((n_ng_tf_ + 255) / 256), 256, 0, st_>>>(v, t_segs.p, (uint32_t)segs.size(), t_tf.p, n_ng_tf_, post_.p, comp_.p, t_max.p);
+    SSB_CUDA_TRY(cudaGetLastError());
+    uint32_t maxbits = 0;
+    SSB_CUDA_TRY(cudaMemcpyAsync(&maxbits, t_max.p, 4, cudaMemcpyDeviceToHost, st_));
+    SSB_CUDA_TRY(cudaStreamSynchronize(st_));
+    float maxc; memcpy(&maxc, &maxbits, 4);
+    // build_bitmaps clamps a word's coarse bound to 255 steps: the step must reach the largest fp16 bound (1 % covers the round-up)
+    if (maxc * 1.01f / 255.0f > q8_step_) q8_step_ = maxc * 1.01f / 255.0f;
+    return SSB_OK;
+}
+
+// the dictionary idf of every n-gram key is 1.0 (score = 1.0 * component sum)
+void LexIndex::ngram_idf_one(std::vector<float>& idf) const {
+    for (uint64_t key : h_ng_keys_) {
+        const auto it = std::lower_bound(h_dict_keys_.begin(), h_dict_keys_.end(), key);
+        if (it != h_dict_keys_.end() && *it == key) idf[it - h_dict_keys_.begin()] = 1.0f;
+    }
 }
 
 int32_t LexIndex::commit(uint64_t n_docs, uint64_t len_sum) {
@@ -2090,6 +2250,8 @@ int32_t LexIndex::commit(uint64_t n_docs, uint64_t len_sum) {
         fill_bounds<<<(unsigned)((n_post_ + 255) / 256), 256, 0, st_>>>(v, post_.p, comp_.p, n_post_);
         SSB_CUDA_TRY(cudaGetLastError());
     }
+    q8_step_ = Q8_STEP;
+    SSB_TRY(commit_ngrams(n_docs));
     if (post_.p) SSB_CUDA_TRY(cudaMemsetAsync(post_.p + n_post_, 0, 160 * 4, st_));   // tail read by the vector loads
 
     size_t alloc_n = total ? total : 1;
@@ -2141,6 +2303,7 @@ int32_t LexIndex::commit(uint64_t n_docs, uint64_t len_sum) {
     {   // idf on the host (same libm as the oracle)
         std::vector<float> idf(nt_alloc);
         for (uint32_t t = 0; t < nt; t++) idf[t] = host_idf(n_docs, h_term_df_[t]);
+        ngram_idf_one(idf);
         SSB_CUDA_TRY(cudaMemcpyAsync(d_term_idf_, idf.data(), (size_t)nt * 4, cudaMemcpyHostToDevice, st_));
         SSB_CUDA_TRY(cudaStreamSynchronize(st_));
     }
@@ -2167,7 +2330,7 @@ int32_t LexIndex::commit(uint64_t n_docs, uint64_t len_sum) {
             SSB_CUDA_TRY(t_dense.alloc(n_bitmaps_));
             uint32_t* d_dense = t_dense.p;
             compact_dense<<<(total + 255) / 256, 256, 0, st_>>>(d_e_bitmap_, total, d_dense);
-            build_bitmaps<<<n_bitmaps_, 256, 0, st_>>>(d_e_bitmap_, d_e_off_, d_e_count_, total, post_.p, d_bm_words_, d_bm_, d_bm_q8_, Q8_STEP, d_dense);
+            build_bitmaps<<<n_bitmaps_, 256, 0, st_>>>(d_e_bitmap_, d_e_off_, d_e_count_, total, post_.p, d_bm_words_, d_bm_, d_bm_q8_, q8_step_, d_dense);
             SSB_CUDA_TRY(cudaGetLastError());
             SSB_CUDA_TRY(cudaStreamSynchronize(st_));
         }
@@ -2202,6 +2365,7 @@ int32_t LexIndex::set_global_df(const uint64_t* keys, const uint32_t* dfs, uint6
         if (lo < n_terms_ && h_dict_keys_[lo] == keys[i]) h_term_df_[lo] = dfs[i];
     }
     for (uint32_t t = 0; t < n_terms_; t++) idf[t] = host_idf(n_docs_, h_term_df_[t]);
+    ngram_idf_one(idf);                                                    // n-gram keys: the components carry the idfs
     SSB_CUDA_TRY(cudaMemcpyAsync(d_term_idf_, idf.data(), (size_t)n_terms_ * 4, cudaMemcpyHostToDevice, st_));
     SSB_CUDA_TRY(cudaMemcpyAsync(d_term_df_, h_term_df_.data(), (size_t)n_terms_ * 4, cudaMemcpyHostToDevice, st_));
     SSB_CUDA_TRY(cudaStreamSynchronize(st_));
@@ -2351,7 +2515,7 @@ int32_t LexIndex::plan_batch(LexWorkspace& ws, cudaStream_t st, const ssb_lex_ba
     auto plan = sort ? lex_plan<true> : lex_plan<false>;
     if (plan_smem > 48 * 1024) SSB_CUDA_TRY(cudaFuncSetAttribute(plan, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan_smem));
     plan<<<b->nq, 128, plan_smem, st>>>(b->v, ws.qoff.p, ws.qkeys.p, q->term_flags ? ws.qflags.p : nullptr, b->filtered ? ws.foff.p : nullptr, fmask_dev,
-                                        b->phrase | topk_flag, b->qt_eff, ws.plans.p, ws.recs.p, ws.item_start.p, ws.ctr.p, ws.theta.p, ws.lock.p,
+                                        b->phrase | topk_flag | (has_ngrams() ? 4u : 0u), b->qt_eff, ws.plans.p, ws.recs.p, ws.item_start.p, ws.ctr.p, ws.theta.p, ws.lock.p,
                                         ws.count.p, glist, n_pow2, ITEM_W, 2, GMAX, sort ? *sort : SortDev{});
     SSB_CUDA_TRY(cudaGetLastError());
     if (launches) *launches += 1;

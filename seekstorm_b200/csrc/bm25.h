@@ -134,8 +134,9 @@ struct DeleteSet {
 struct QTerm { uint32_t first, n; float idf; uint32_t df; };
 // fast: the query takes the record path (lex_score / lex_count): <= fast_t live terms and no facet filter; otherwise lex_generic
 struct QueryPlan { QTerm t[SSB_MAX_QUERY_TERMS]; QTerm tn[SSB_MAX_NOT_TERMS]; uint32_t n_live, n_items, n_recs, n_not; uint32_t filt_first, n_filt, fast, field_mask /* field_filter: bit f = indexed field f, 0 = none */;
-                   // phrase query: token i of the phrase is unique term phr[i] (index into t[]); n_phr = 0: not a phrase
-                   uint8_t phr[SSB_MAX_QUERY_TERMS]; uint32_t n_phr, pad[3]; };
+                   // phrase query: token i of the phrase is unique term phr[i] (index into t[]) and sits at start + phr_off[i] (i, plus 1 per
+                   // earlier bigram and 2 per earlier trigram key on an index with n-gram lists); n_phr = 0: not a phrase
+                   uint8_t phr[SSB_MAX_QUERY_TERMS]; uint8_t phr_off[SSB_MAX_QUERY_TERMS]; uint32_t n_phr, pad[3]; };
 
 // One (query, level) record, built by lex_plan for queries with <= 4 live terms; 128 bytes = one cache line.
 // Slots are in QUERY order (scores are summed in query order, add_result.rs:1450-1452); cnt == 0 marks a term
@@ -191,6 +192,14 @@ public:
     ~LexIndex();
     int32_t add_level(const ssb_level_desc* d);
     int32_t set_fields(uint32_t n_fields, const float* boosts);   // before the first level
+    int32_t set_ngram_config(uint32_t similarity, uint32_t df_rule);   // before the first level
+    // add_level + the level's n-gram data (ssb_lexical_add_level_ngrams): component tfs of the n-gram postings and the df bytes of the
+    // n-gram keys, kept until commit computes their components
+    int32_t add_level_ngrams(const ssb_level_desc* d, const ssb_level_ngrams* ng);
+    bool has_ngrams() const { return !ng_segs_.empty(); }
+    // ssb_lexical_add_level: add_level, refusing keys with low bits set once the index holds n-gram lists (they would be scored with the
+    // n-gram keys' dictionary idf 1.0)
+    int32_t add_level_plain(const ssb_level_desc* d);
     int32_t commit(uint64_t n_docs, uint64_t len_sum);
     int32_t dict_size(uint64_t* n) const { *n = n_terms_; return SSB_OK; }
     int32_t dict_export(uint64_t* keys, uint32_t* dfs, uint64_t cap) const;
@@ -260,6 +269,14 @@ private:
     std::vector<uint64_t> h_lvl_pos_base_; uint64_t* d_lvl_pos_base_ = nullptr;
     uint32_t n_fields_ = 1; float boosts_[4] = {1.f, 1.f, 1.f, 1.f};
     DevBuf<uint32_t> payf_; DevBuf<float> compf_;   // several indexed fields: [n_post][n_fields]
+    // n-gram lists (add_level_ngrams): one segment per (n-gram key, level) with its postings' range in the arenas and its component tfs
+    // in h_ng_tf_ ([n][3], host memory: only commit needs them); the df bytes of every level, resolved at commit by ng_rule_
+    struct NgSeg { uint64_t key; uint64_t post_off; uint64_t tf_off; uint32_t cnt; uint8_t dfb[3]; };
+    std::vector<NgSeg> ng_segs_; std::vector<uint16_t> h_ng_tf_; uint64_t n_ng_tf_ = 0;
+    bool plain_lowbit_ = false;                     // a level added without n-gram data carried keys with low bits set
+    uint32_t lex_sim_ = SSB_LEXSIM_BM25F_PROXIMITY, ng_rule_ = SSB_NGRAM_DF_FIRST_LEVEL;
+    std::vector<uint64_t> h_ng_keys_;               // sorted unique n-gram keys (their dictionary idf stays 1.0)
+    float q8_step_ = 0.f;                           // coarse bound step set by commit: Q8_STEP, larger when n-gram components exceed K + 1
     uint64_t n_post_ = 0;
     // committed structures
     uint64_t n_docs_ = 0, len_sum_ = 0;
@@ -273,6 +290,8 @@ private:
     const FacetSet* facets_ = nullptr;
     uint64_t live_docs_ = 0;
     void free_committed();
+    int32_t commit_ngrams(uint64_t n_docs);
+    void ngram_idf_one(std::vector<float>& idf) const;
     LexView view() const;
 };
 
@@ -282,8 +301,9 @@ int32_t launch_facet_select(const FacetSet& fs, const FacetReqDev* req, uint32_t
 
 // loader.cu: the reference's on-disk files -> index
 struct VectorLevel { uint32_t level_id; std::vector<uint16_t> ids; std::vector<float> rows; std::vector<uint32_t> cluster_counts; };
-int32_t load_index_bin(LexIndex* lex, const uint8_t* bytes, uint64_t len, const ssb_index_bin_params* prm, uint64_t* n_docs_out);
+int32_t load_index_bin(LexIndex* lex, const uint8_t* bytes, uint64_t len, const ssb_index_bin_params* prm, uint64_t* n_docs_out, bool ngrams = false);
 int32_t inspect_index_bin(const uint8_t* bytes, uint64_t len, const ssb_index_bin_params* prm, uint64_t out[8]);
+int32_t inspect_index_bin_ngrams(const uint8_t* bytes, uint64_t len, const ssb_index_bin_params* prm, uint64_t out[8]);
 int32_t parse_vector_bin(const uint8_t* bytes, uint64_t len, uint32_t dims, std::vector<VectorLevel>& out);
 
 }  // namespace ssb

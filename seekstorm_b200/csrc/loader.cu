@@ -20,7 +20,9 @@
 //   vector.bin (vector.rs:1066-1094): per level [u32 clusters][u32 child_count x clusters][records], record = packed VectorHeader
 //       {u16 doc_id, u32 field_id, u32 chunk_id, f32 scale, f32 norm, i16 zero_point, i32 sum_q} (24 B, vector.rs:62-73) + f32[dims].
 //
-// Supported: one indexed field (the C1-C5 configs), single-term keys (n-gram keys are skipped), Array / Bitmap / RLE containers
+// Supported: one indexed field (the C1-C5 configs), single-term keys (n-gram keys are skipped unless the caller asks for them with
+// ssb_load_index_bin_ngrams: their heads carry the components' df bytes at 14..16, their postings are never embedded and their blobs
+// start with the component tfs, add_result.rs:2076-2089), Array / Bitmap / RLE containers
 // (the writer's Delta container is disabled, compress_postinglist.rs:242), f32 vectors.  Term hashing (hash64 / hash32 = gxhash /
 // ahash of the term bytes, index.rs:4165-4225) stays on the host side of the boundary: the file carries the 64-bit keys, queries
 // arrive as keys.  No Rust toolchain exists in this environment, so no file written by the reference itself could be tested:
@@ -95,8 +97,10 @@ static bool push_positions(const uint32_t* deltas, uint32_t n, std::vector<uint1
     return true;
 }
 
+// n_comp (n-gram keys: 2 / 3): the blob holds n_comp VINT component tfs ahead of positions_count; they go to ctf_out, 3 per posting
 bool decode_key(const uint8_t* body, uint64_t blen, uint32_t count, uint32_t pivot, uint32_t ctp, std::vector<uint16_t>& ids,
-                std::vector<uint16_t>& tfs, const char*& why, std::vector<uint16_t>* pos_out = nullptr) {
+                std::vector<uint16_t>& tfs, const char*& why, std::vector<uint16_t>* pos_out = nullptr, uint32_t n_comp = 0,
+                std::vector<uint16_t>* ctf_out = nullptr) {
     const uint32_t type = ctp >> 30, range = ctp & 0x3FFFFFFFu;
     // intersection.rs:221-227: pivot*2 + (count - pivot)*3 pointer bytes precede the doc-id container
     const uint64_t psum = (uint64_t)pivot * 2 + (pivot <= count - 1 ? (uint64_t)(count - pivot) * 3 : 0);
@@ -126,6 +130,18 @@ bool decode_key(const uint8_t* body, uint64_t blen, uint32_t count, uint32_t piv
         }
         if (n != count) { why = "rle run lengths != posting_count"; return false; }
     } else { why = "delta container (disabled in the reference writer, compress_postinglist.rs:242) is not supported"; return false; }
+    // component tfs of an n-gram posting, read at the start of its blob; `at` moves past them to positions_count
+    auto components = [&](uint64_t& at) -> bool {
+        if (!n_comp) return true;
+        uint16_t c3[3] = {0, 0, 0};
+        for (uint32_t c = 0; c < n_comp; c++) {
+            uint32_t v = 0, used = 0;
+            if (!vint_len(body, blen, at, v, used)) { why = "n-gram component tf out of range"; return false; }
+            c3[c] = (uint16_t)(v > 65535u ? 65535u : v); at += used;
+        }
+        ctf_out->insert(ctf_out->end(), c3, c3 + 3);
+        return true;
+    };
     // tf from the rank-position pointers
     for (uint32_t p = 0; p < count; p++) {
         uint32_t tf = 0;
@@ -134,6 +150,7 @@ bool decode_key(const uint8_t* body, uint64_t blen, uint32_t count, uint32_t piv
             if (at + 2 > blen) { why = "pointer past the segment body"; return false; }
             const uint32_t rp = rd16(body + at);
             if (rp & 0x8000u) {
+                if (n_comp) { why = "embedded n-gram posting (the writer never embeds them, index_posting.rs:445)"; return false; }
                 tf = (rp >> 14) == 2u ? 1u : 2u;                                     // embedded: 10 -> 1 position, 11 -> 2
                 if (pos_out) {                                                       // 14 payload bits: one 14-bit delta or 7 + 7 (index_posting.rs:590-640)
                     uint32_t dl[2];
@@ -142,14 +159,16 @@ bool decode_key(const uint8_t* body, uint64_t blen, uint32_t count, uint32_t piv
                 }
             } else {
                 const uint32_t back = rp & 0x7FFFu;
-                if (back > range || !vint(body, blen, (uint64_t)range - back, tf)) { why = "position blob out of range"; return false; }
-                if (pos_out && !blob_positions(body, blen, (uint64_t)range - back, tf, *pos_out, why)) return false;
+                uint64_t at = (uint64_t)range - back;
+                if (back > range || !components(at) || !vint(body, blen, at, tf)) { if (!*why) why = "position blob out of range"; return false; }
+                if (pos_out && !blob_positions(body, blen, at, tf, *pos_out, why)) return false;
             }
         } else {
             const uint64_t at = (uint64_t)range + 3ull * p - pivot;
             if (at + 3 > blen) { why = "pointer past the segment body"; return false; }
             const uint32_t rp = (uint32_t)body[at] | ((uint32_t)body[at + 1] << 8) | ((uint32_t)body[at + 2] << 16);
             if (rp & 0x800000u) {
+                if (n_comp) { why = "embedded n-gram posting (the writer never embeds them, index_posting.rs:445)"; return false; }
                 tf = ((rp >> 21) & 3u) + 1u;                                         // embedded: 100 -> 1 ... 111 -> 4
                 if (pos_out) {                                                       // 21 payload bits: 21 | 10 + 11 | 7 + 7 + 7 | 5 + 5 + 5 + 6
                     uint32_t dl[4];
@@ -161,8 +180,9 @@ bool decode_key(const uint8_t* body, uint64_t blen, uint32_t count, uint32_t piv
                 }
             } else {
                 const uint32_t back = rp & 0x7FFFFFu;
-                if (back > range || !vint(body, blen, (uint64_t)range - back, tf)) { why = "position blob out of range"; return false; }
-                if (pos_out && !blob_positions(body, blen, (uint64_t)range - back, tf, *pos_out, why)) return false;
+                uint64_t at = (uint64_t)range - back;
+                if (back > range || !components(at) || !vint(body, blen, at, tf)) { if (!*why) why = "position blob out of range"; return false; }
+                if (pos_out && !blob_positions(body, blen, at, tf, *pos_out, why)) return false;
             }
         }
         if (tf == 0) { why = "positions_count 0"; return false; }
@@ -173,9 +193,12 @@ bool decode_key(const uint8_t* body, uint64_t blen, uint32_t count, uint32_t piv
 }
 }  // namespace
 
-// walk the file; on_level receives every decoded level in the neutral layout (valid during the call only)
+// walk the file; on_level receives every decoded level in the neutral layout (valid during the call only).  ngrams: also decode the n-gram
+// keys (key low bits != 0) and hand their component tfs / df bytes over (single-term postings and keys: zeros); otherwise they are
+// skipped and the second argument of on_level is null.
 static int32_t walk_index_bin(const uint8_t* bytes, uint64_t len, const ssb_index_bin_params* prm,
-                              const std::function<int32_t(const ssb_level_desc&)>& on_level, uint64_t* doc_count_out, uint64_t* pos_sum_out) {
+                              const std::function<int32_t(const ssb_level_desc&, const ssb_level_ngrams*)>& on_level, uint64_t* doc_count_out,
+                              uint64_t* pos_sum_out, bool ngrams = false) {
     if (!bytes || !prm) { set_error("load_index_bin: null argument"); return SSB_E_INVALID; }
     if (prm->indexed_field_count != 1) { set_error("load_index_bin: %u indexed fields (only single-field indexes are supported)", prm->indexed_field_count); return SSB_E_UNSUPPORTED; }
     const uint32_t khs = prm->key_head_size;
@@ -188,6 +211,8 @@ static int32_t walk_index_bin(const uint8_t* bytes, uint64_t len, const ssb_inde
     uint64_t doc_count = 0, pos_sum = 0;
     uint32_t level = 0;
     std::vector<uint64_t> keys; std::vector<uint32_t> offs; std::vector<uint16_t> ids, tfs, poss; std::vector<std::pair<uint32_t, uint32_t>> seg;
+    std::vector<uint16_t> ctf; std::vector<uint8_t> dfb;                // n-gram mode: [n_postings][3] component tfs, [n_terms][3] df bytes
+    if (ngrams && khs == 20) { set_error("load_index_bin_ngrams: key_head_size 20 carries no n-gram df bytes (22 / 23)"); return SSB_E_INVALID; }
     const bool want_pos = prm->decode_positions != 0;   // term positions for phrase queries (off: tf only, as before)
     while (r.pos < len) {
         if (level == 0) r.u16();                                   // longest_field_id
@@ -200,7 +225,7 @@ static int32_t walk_index_bin(const uint8_t* bytes, uint64_t len, const ssb_inde
         if (doc_count <= (uint64_t)level * 65536) { set_error("load_index_bin: level %u: indexed_doc_count %llu", level, (unsigned long long)doc_count); return SSB_E_INVALID; }
         const uint64_t rest = doc_count - (uint64_t)level * 65536;
         const uint32_t n_docs = (uint32_t)(rest < 65536 ? rest : 65536);
-        keys.clear(); offs.assign(1, 0); ids.clear(); tfs.clear(); poss.clear();
+        keys.clear(); offs.assign(1, 0); ids.clear(); tfs.clear(); poss.clear(); ctf.clear(); dfb.clear();
         for (uint32_t s = 0; s < nseg; s++) {
             const uint64_t head_bytes = (uint64_t)seg[s].second * khs;
             if (seg[s].first < head_bytes || !r.need(seg[s].first)) { set_error("load_index_bin: level %u segment %u: block_length %u < key heads / past the end", level, s, seg[s].first); return SSB_E_INVALID; }
@@ -211,11 +236,17 @@ static int32_t walk_index_bin(const uint8_t* bytes, uint64_t len, const ssb_inde
             for (uint32_t k = 0; k < seg[s].second; k++) {
                 const uint8_t* h = heads + (uint64_t)k * khs;
                 const uint64_t key = rd64(h);
-                if (key & 7ull) continue;                          // n-gram posting lists (frequent-term bigrams / trigrams): not on this path
+                const uint32_t ty = (uint32_t)(key & 7ull);
+                if (ty && !ngrams) continue;                       // n-gram posting lists (frequent-term bigrams / trigrams): opt-in
                 const uint32_t count = (uint32_t)rd16(h + 8) + 1u;
                 const uint32_t pivot = rd16(h + khs - 6), ctp = rd32(h + khs - 4);
+                const uint32_t n_comp = ty == 0 ? 0u : (ty <= SSB_NGRAM_RF ? 2u : 3u);
+                if (ngrams) {
+                    for (uint32_t c = 0; c < 3; c++) dfb.push_back(ty && 14 + c < khs - 6 ? h[14 + c] : (uint8_t)0);
+                    if (!ty) ctf.resize(ctf.size() + 3ull * count, 0);
+                }
                 const char* why = "";
-                if (!decode_key(body, blen, count, pivot, ctp, ids, tfs, why, want_pos ? &poss : nullptr)) {
+                if (!decode_key(body, blen, count, pivot, ctp, ids, tfs, why, want_pos ? &poss : nullptr, n_comp, &ctf)) {
                     set_error("load_index_bin: level %u segment %u key %016llx: %s", level, s, (unsigned long long)key, why);
                     return SSB_E_INVALID;
                 }
@@ -226,7 +257,9 @@ static int32_t walk_index_bin(const uint8_t* bytes, uint64_t len, const ssb_inde
         d.level_id = level; d.n_docs = n_docs; d.n_terms = (uint32_t)keys.size();
         d.term_keys = keys.data(); d.posting_offsets = offs.data(); d.doc_ids = ids.data(); d.tfs = tfs.data(); d.doc_len_bytes = doclen;
         if (want_pos) { poss.push_back(0); d.positions = poss.data(); }      // (never null, even for a level without postings)
-        SSB_TRY(on_level(d));
+        ctf.resize(ctf.size() + 3, 0); dfb.resize(dfb.size() + 3, 0);       // (never null either)
+        const ssb_level_ngrams ng{ctf.data(), dfb.data()};
+        SSB_TRY(on_level(d, ngrams ? &ng : nullptr));
         level++;
     }
     if (!r.ok) { set_error("load_index_bin: truncated file (level %u)", level); return SSB_E_INVALID; }
@@ -236,11 +269,12 @@ static int32_t walk_index_bin(const uint8_t* bytes, uint64_t len, const ssb_inde
     return SSB_OK;
 }
 
-int32_t load_index_bin(LexIndex* lex, const uint8_t* bytes, uint64_t len, const ssb_index_bin_params* prm, uint64_t* n_docs_out) {
+int32_t load_index_bin(LexIndex* lex, const uint8_t* bytes, uint64_t len, const ssb_index_bin_params* prm, uint64_t* n_docs_out, bool ngrams) {
     if (!lex) { set_error("load_index_bin: null argument"); return SSB_E_INVALID; }
     if (lex->n_levels() != 0) { set_error("load_index_bin: the index already holds levels"); return SSB_E_STATE; }
     uint64_t doc_count = 0, pos_sum = 0;
-    SSB_TRY(walk_index_bin(bytes, len, prm, [&](const ssb_level_desc& d) { return lex->add_level(&d); }, &doc_count, &pos_sum));
+    SSB_TRY(walk_index_bin(bytes, len, prm, [&](const ssb_level_desc& d, const ssb_level_ngrams* ng) { return lex->add_level_ngrams(&d, ng); },
+                           &doc_count, &pos_sum, ngrams));
     SSB_TRY(lex->commit(doc_count, pos_sum));     // indexed_doc_count / positions_sum_normalized of the last level = the shard's totals
     if (n_docs_out) *n_docs_out = doc_count;
     return SSB_OK;
@@ -252,7 +286,7 @@ int32_t inspect_index_bin(const uint8_t* bytes, uint64_t len, const ssb_index_bi
     uint64_t levels = 0, terms = 0, postings = 0, tf_sum = 0, h = 1469598103934665603ull, hp = 1469598103934665603ull;
     auto mix = [&](uint64_t x) { h = (h ^ x) * 1099511628211ull; };
     uint64_t doc_count = 0, pos_sum = 0;
-    SSB_TRY(walk_index_bin(bytes, len, prm, [&](const ssb_level_desc& d) {
+    SSB_TRY(walk_index_bin(bytes, len, prm, [&](const ssb_level_desc& d, const ssb_level_ngrams*) {
         levels++; terms += d.n_terms; postings += d.posting_offsets[d.n_terms];
         for (uint32_t t = 0; t < d.n_terms; t++) {
             mix(d.term_keys[t]);
@@ -266,6 +300,37 @@ int32_t inspect_index_bin(const uint8_t* bytes, uint64_t len, const ssb_index_bi
         return (int32_t)SSB_OK;
     }, &doc_count, &pos_sum));
     out[0] = levels; out[1] = terms; out[2] = postings; out[3] = tf_sum; out[4] = doc_count; out[5] = pos_sum; out[6] = h; out[7] = prm->decode_positions ? hp : 0;
+    return SSB_OK;
+}
+
+// host-only walk in n-gram mode: out = {levels, n-gram keys, n-gram postings, sum of their tfs, FNV checksum over every n-gram (key, level,
+// df bytes) and (doc id, tf, component tfs) in file order, FNV checksum over the n-gram postings' positions (decode_positions) or 0, 0, 0}
+int32_t inspect_index_bin_ngrams(const uint8_t* bytes, uint64_t len, const ssb_index_bin_params* prm, uint64_t out[8]) {
+    uint64_t levels = 0, terms = 0, postings = 0, tf_sum = 0, h = 1469598103934665603ull, hp = 1469598103934665603ull;
+    auto mix = [&](uint64_t x) { h = (h ^ x) * 1099511628211ull; };
+    SSB_TRY(walk_index_bin(bytes, len, prm, [&](const ssb_level_desc& d, const ssb_level_ngrams* ng) {
+        levels++;
+        uint64_t pbase = 0;
+        for (uint32_t t = 0; t < d.n_terms; t++) {
+            const uint32_t a = d.posting_offsets[t], b = d.posting_offsets[t + 1];
+            uint64_t np = 0;
+            for (uint32_t i = a; i < b; i++) np += d.tfs[i];
+            if (d.term_keys[t] & 7u) {
+                terms++; postings += b - a;
+                const uint8_t* f = ng->component_df_bytes + 3ull * t;
+                mix(d.term_keys[t]); mix(((uint64_t)d.level_id << 32) | ((uint64_t)f[0] << 16) | ((uint64_t)f[1] << 8) | f[2]);
+                for (uint32_t i = a; i < b; i++) {
+                    const uint16_t* c = ng->component_tfs + 3ull * i;
+                    mix(((uint64_t)d.doc_ids[i] << 48) | ((uint64_t)d.tfs[i] << 32) | ((uint64_t)c[0] << 16) | c[1]); mix(c[2]);
+                    tf_sum += d.tfs[i];
+                }
+                if (d.positions) for (uint64_t j = 0; j < np; j++) hp = (hp ^ d.positions[pbase + j]) * 1099511628211ull;
+            }
+            pbase += np;
+        }
+        return (int32_t)SSB_OK;
+    }, nullptr, nullptr, true));
+    out[0] = levels; out[1] = terms; out[2] = postings; out[3] = tf_sum; out[4] = h; out[5] = prm->decode_positions ? hp : 0; out[6] = 0; out[7] = 0;
     return SSB_OK;
 }
 

@@ -25,7 +25,7 @@ from typing import Callable, Optional, Sequence
 import numpy as np
 
 from . import _lib
-from ._lib import SsbConfig, SsbHit, SsbLevelDesc, SsbLexBatch, SsbStats, check, lib
+from ._lib import SsbConfig, SsbHit, SsbLevelDesc, SsbLevelNgrams, SsbLexBatch, SsbStats, check, lib
 
 
 class QueryType(enum.IntEnum):
@@ -282,6 +282,73 @@ def synthetic_term_key(term: str) -> int:
     return fnv1a64(term)
 
 
+class LexicalSimilarity(enum.IntEnum):
+    """index.rs:559-566 (the reference's default is Bm25fProximity).  The two score identically unless the index holds n-gram lists."""
+    Bm25f = 0
+    Bm25fProximity = 1
+
+
+class NgramSet(enum.IntFlag):
+    """index.rs:1834-1851: the n-gram types an index is built with (F = frequent term, R = rare term)"""
+    SingleTerm = 0
+    NgramFF = 1
+    NgramFR = 2
+    NgramRF = 4
+    NgramFFF = 8
+    NgramRFF = 16
+    NgramFFR = 32
+    NgramFRF = 64
+
+
+class NgramType(enum.IntEnum):
+    """index.rs:1854-1872: the low 3 bits of an n-gram key"""
+    SingleTerm = 0
+    NgramFF = 1
+    NgramFR = 2
+    NgramRF = 3
+    NgramFFF = 4
+    NgramRFF = 5
+    NgramFFR = 6
+    NgramFRF = 7
+
+
+def ngram_key(words: Sequence[str], ngram_type: int, term_key_fn: Callable[[str], int] = synthetic_term_key) -> int:
+    """hash64("a b" / "a b c") | NgramType (tokenizer.rs:678-685), with the index's term hash; a single word is its term key"""
+    if int(ngram_type) == 0:
+        return term_key_fn(words[0])
+    return (term_key_fn(" ".join(words)) & ~7 & ((1 << 64) - 1)) | int(ngram_type)
+
+
+def ngram_rewrite(terms: Sequence[str], frequent, ngram_set: int):
+    """The query-time rewrite of a phrase (tokenizer.rs:898-1387): greedy, left to right, each position tries FFF, RFF, FFR, FRF, then
+    FF, RF, FR under their own NgramSet bits, else keeps the single term.  -> [(words tuple, NgramType)]"""
+    out, i, n = [], 0, len(terms)
+    f = [t in frequent for t in terms]
+    while i < n:
+        if i + 2 < n:
+            tri = ((NgramSet.NgramFFF, f[i] and f[i + 1] and f[i + 2], NgramType.NgramFFF),
+                   (NgramSet.NgramRFF, (not f[i]) and f[i + 1] and f[i + 2], NgramType.NgramRFF),
+                   (NgramSet.NgramFFR, f[i] and f[i + 1] and not f[i + 2], NgramType.NgramFFR),
+                   (NgramSet.NgramFRF, f[i] and (not f[i + 1]) and f[i + 2], NgramType.NgramFRF))
+            hit = next((ty for bit, ok, ty in tri if ngram_set & bit and ok), None)
+            if hit is not None:
+                out.append((tuple(terms[i:i + 3]), hit))
+                i += 3
+                continue
+        if i + 1 < n:
+            bi = ((NgramSet.NgramFF, f[i] and f[i + 1], NgramType.NgramFF),
+                  (NgramSet.NgramRF, (not f[i]) and f[i + 1], NgramType.NgramRF),
+                  (NgramSet.NgramFR, f[i] and not f[i + 1], NgramType.NgramFR))
+            hit = next((ty for bit, ok, ty in bi if ngram_set & bit and ok), None)
+            if hit is not None:
+                out.append((tuple(terms[i:i + 2]), hit))
+                i += 2
+                continue
+        out.append(((terms[i],), NgramType.SingleTerm))
+        i += 1
+    return out
+
+
 def _morton_spread(v):
     x = v.astype(np.uint64)
     for sh, m in ((16, 0x0000FFFF0000FFFF), (8, 0x00FF00FF00FF00FF), (4, 0x0F0F0F0F0F0F0F0F), (2, 0x3333333333333333), (1, 0x5555555555555555)):
@@ -378,11 +445,24 @@ class Index:
         if len(getattr(self, "field_names", [])) != len(b):
             self.field_names = [f"field{f}" for f in range(len(b))]      # names of the indexed fields in schema order (Index.search field_filter)
 
-    def add_lexical_level(self, level_id: int, n_docs: int, term_keys, posting_offsets, doc_ids, tfs, doc_len_bytes, positions=None):
+    def set_ngram_config(self, frequent_terms=(), ngram_set: int = 0, similarity: LexicalSimilarity = LexicalSimilarity.Bm25fProximity,
+                         df_rule: int = _lib.NGRAM_DF_FIRST_LEVEL):
+        """An index built with n-gram lists (NGRAM_SEARCH.md), before the first level: the frequent-term set and NgramSet bits of the
+        query rewrite, the LexicalSimilarity, and which level's key-head df bytes an n-gram list keeps (NGRAM_DF_FIRST_LEVEL: the
+        reference's Ram access, NGRAM_DF_LAST_LEVEL: its Mmap access)."""
+        check(lib().ssb_lexical_set_ngram_config(self._h, int(similarity), int(df_rule)))
+        self.frequent_terms = frozenset(frequent_terms)
+        self.ngram_set = int(ngram_set)
+        self.lexical_similarity = LexicalSimilarity(similarity)
+
+    def add_lexical_level(self, level_id: int, n_docs: int, term_keys, posting_offsets, doc_ids, tfs, doc_len_bytes, positions=None,
+                          ngram_tfs=None, ngram_df_bytes=None):
         """One committed 64K-doc level in the neutral layout (arrays: numpy on host or torch on the device).  positions: u16 [sum of tfs], the
         term positions of every posting in posting order (phrase queries), or None.  With several indexed fields (tfs [n_postings, F]) a
         posting holds the sum of its F tfs positions, one run per field in field order (field 0's first), each run ascending and starting
-        again from 0 in every field; a phrase matches inside one field only."""
+        again from 0 in every field; a phrase matches inside one field only.
+        ngram_tfs u16 [n_postings, 3] / ngram_df_bytes u8 [n_terms, 3]: the component tfs and key-head df bytes of the n-gram lists (keys
+        with low bits set) of an index with n-gram lists (ssb_lexical_add_level_ngrams)."""
         if positions is not None:
             n_pos = positions.size if isinstance(positions, np.ndarray) else positions.numel()
             want = int(tfs.astype(np.int64).sum()) if isinstance(tfs, np.ndarray) else int((tfs.long() & 0xFFFF).sum())
@@ -391,7 +471,11 @@ class Index:
         n_terms = int(term_keys.shape[0])
         d = SsbLevelDesc(level_id, n_docs, n_terms, getattr(self, "_n_fields", 1), _addr(term_keys), _addr(posting_offsets), _addr(doc_ids),
                          _addr(tfs), _addr(doc_len_bytes), _addr(positions))
-        check(lib().ssb_lexical_add_level(self._h, C.byref(d)))
+        if ngram_tfs is not None or ngram_df_bytes is not None:
+            ng = SsbLevelNgrams(_addr(ngram_tfs), _addr(ngram_df_bytes))
+            check(lib().ssb_lexical_add_level_ngrams(self._h, C.byref(d), C.byref(ng)))
+        else:
+            check(lib().ssb_lexical_add_level(self._h, C.byref(d)))
 
     def add_synth_level(self, lv):
         """Convenience: a seekstorm_b200.synth.Level (tensors on CPU or on this index's device)."""
@@ -403,14 +487,17 @@ class Index:
             self.add_lexical_level(n["level_id"], n["n_docs"], n["term_keys"], n["posting_offsets"], n["doc_ids"],
                                    n["tfs"], n["doc_len_bytes"], n.get("positions"))
 
-    def load_index_bin(self, data, indexed_field_count: int = 1, key_head_size: int = 20, segment_number_bits: int = 11, decode_positions: bool = False) -> int:
+    def load_index_bin(self, data, indexed_field_count: int = 1, key_head_size: int = 20, segment_number_bits: int = 11, decode_positions: bool = False,
+                       ngrams: bool = False) -> int:
         """Load one shard's index.bin (bytes / mmap / numpy uint8 array, the reference's own format, index.rs:3253-3516) and commit.
+        ngrams: also load its n-gram posting lists (22 / 23-byte key heads; ssb_load_index_bin_ngrams, set_ngram_config first).
         Returns indexed_doc_count."""
         from ._lib import SsbIndexBinParams
         buf = np.frombuffer(data, dtype=np.uint8) if not isinstance(data, np.ndarray) else np.ascontiguousarray(data, dtype=np.uint8)
         prm = SsbIndexBinParams(indexed_field_count, key_head_size, segment_number_bits, 1 if decode_positions else 0)   # positions: phrase queries
         n = C.c_uint64(0)
-        check(lib().ssb_load_index_bin(self._h, buf.ctypes.data, buf.size, C.byref(prm), C.byref(n)))
+        load = lib().ssb_load_index_bin_ngrams if ngrams else lib().ssb_load_index_bin
+        check(load(self._h, buf.ctypes.data, buf.size, C.byref(prm), C.byref(n)))
         self.indexed_doc_count = n.value
         return n.value
 
@@ -1024,8 +1111,11 @@ class Index:
                 raise NotImplementedError("NOT terms next to a phrase are outside the GPU hot path")
         elif phrase:
             qt = QueryType.Intersection
-        ro.query_terms = list(dict.fromkeys(terms))
-        keys = [self.term_key_fn(t) for t in terms]
+        ro.query_terms = list(dict.fromkeys(terms))    # the component terms, also of a phrase rewritten to n-grams (search.rs:3333-3357)
+        if qt == QueryType.Phrase and getattr(self, "ngram_set", 0):
+            keys = [ngram_key(w, ty, self.term_key_fn) for w, ty in ngram_rewrite(terms, self.frequent_terms, self.ngram_set)]
+        else:
+            keys = [self.term_key_fn(t) for t in terms]
         nkeys = [self.term_key_fn(t) for t in dict.fromkeys(not_terms)]
         lex, vec, total = [], [], 0
         want_lex = search_mode.kind in ("Lexical", "Hybrid") and len(keys) > 0
