@@ -293,6 +293,9 @@ int32_t ssb_load_index_bin_ngrams(ssb_index* ix, const void* bytes, uint64_t len
 int32_t ssb_index_bin_inspect_ngrams(const void* bytes, uint64_t len, const ssb_index_bin_params* params, uint64_t out[8]);
 /* vector.bin of one shard (vector.rs:1066-1094; Precision::F32 records of 24 + 4*dims bytes); dims = the index's vector_dims */
 int32_t ssb_load_vector_bin(ssb_index* ix, const void* bytes, uint64_t len, uint64_t* n_vectors_out);
+/* ssb_load_vector_bin that also keeps each record's VectorHeader.field_id / chunk_id (vector.rs:62-73) and adds the levels through
+ * ssb_vector_add_level_fields.  A field id >= 32 -> SSB_E_INVALID; a handle with a communicator -> SSB_E_UNSUPPORTED. */
+int32_t ssb_load_vector_bin_fields(ssb_index* ix, const void* bytes, uint64_t len, uint64_t* n_vectors_out);
 
 /* ---- delete set ---------------------------------------------------------------------------------------- */
 /* shard.delete_hashset (index.rs:1594; delete_document index.rs:5110): deleted docs are neither scored nor counted, in the
@@ -335,6 +338,14 @@ int32_t ssb_vector_add_level(ssb_index* ix, uint32_t level_id, const float* rows
 int32_t ssb_vector_add_level_clustered(ssb_index* ix, uint32_t level_id, const float* rows, uint64_t row_stride_floats,
                                        const uint16_t* local_ids, uint32_t n, uint32_t dims,
                                        const uint32_t* cluster_counts, uint32_t n_clusters);
+/* Multi-vector documents: the level with each row's indexed field (field_ids, u8 [n], the reference's indexed_field_id, < 32 else
+ * SSB_E_INVALID) and chunk id (chunk_ids, u32 [n]); cluster_counts as in _clustered, or NULL for one cluster.  Every vector level of an
+ * index carries field ids or none does (mixing -> SSB_E_STATE).  The field filter of ssb_search_vector_fields / ssb_search_hybrid then
+ * applies to the rows (search_vector_shard, vector.rs:1226-1238, 1411-1412), and ssb_hit_ext.field_id / chunk_id name each hit's best
+ * row (TopK::push, vector.rs:436-470).  A handle with a communicator -> SSB_E_UNSUPPORTED (another rank's best row cannot be resolved). */
+int32_t ssb_vector_add_level_fields(ssb_index* ix, uint32_t level_id, const float* rows, uint64_t row_stride_floats,
+                                    const uint16_t* local_ids, uint32_t n, uint32_t dims, const uint32_t* cluster_counts,
+                                    uint32_t n_clusters, const uint8_t* field_ids, const uint32_t* chunk_ids);
 /* TurboQuantI8 indexes: the index's sign mask `TurboQuant.seed_mask` (dim = next_power_of_two(vector_dims) values of +1 / -1).  The
  * reference draws it once per index from ChaCha8Rng::seed_from_u64(1234) (vector_similarity.rs:1845-1859, index.rs:2215-2216) — a
  * third-party generator (rand_chacha) that this library does not restate: the host hands over the mask it holds.  Before the first level. */
@@ -474,8 +485,17 @@ typedef struct {
 } ssb_vec_query;
 int32_t ssb_search_vector_ex(ssb_index* ix, const ssb_vec_query* q, ssb_hit* hits, uint32_t* n_hits, ssb_hit_ext* ext,
                              uint64_t* observed);
+/* ssb_search_vector_ex with a field filter per query (search_vector_shard, vector.rs:1226-1238, 1411-1412).  field_masks: HOST array
+ * [n_queries] or NULL; bit f = indexed field f is in the query's filter, 0 = no filter (the bits of ssb_lex_batch.field_masks).  A row
+ * whose field is not in a non-zero mask is neither scored nor counted for that query.  A non-zero mask on an index without field ids
+ * -> SSB_E_STATE.  On a field-tagged index ext.field_id / chunk_id are the field and chunk of the doc's best row among those passing the
+ * mask (the earliest in record order on equal scores), here and in ssb_search_vector_ex; observed of a masked query counts the rows in
+ * scope (every row, or the selected clusters' rows) whose field passes. */
+int32_t ssb_search_vector_fields(ssb_index* ix, const ssb_vec_query* q, const uint32_t* field_masks, ssb_hit* hits,
+                                 uint32_t* n_hits, ssb_hit_ext* ext, uint64_t* observed);
 /* SearchMode::Hybrid: both searches with length k, RRF (k=0.6, rank from 0), sort, truncate to k.
- * hits: [n_queries * k]. */
+ * hits: [n_queries * k].  On an index whose vector rows carry field ids, q->field_masks filters the vector half as well
+ * (search.rs:1702-1731); on other indexes it filters the lexical half only. */
 int32_t ssb_search_hybrid(ssb_index* ix, const ssb_lex_batch* q, const float* queries, uint32_t k,
                           ssb_hit* hits, uint32_t* n_hits);
 

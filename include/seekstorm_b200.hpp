@@ -146,6 +146,21 @@ public:
                           const uint16_t* local_ids = nullptr) {
         check(ssb_vector_add_level(h_, level_id, rows, row_stride, local_ids, n, dims));
     }
+    // multi-vector documents: each row's indexed field (< 32) and chunk (VectorHeader.field_id / chunk_id, vector.rs:62-73); every level of
+    // an index carries them or none does.  search()'s field_filter then applies to the vector half as well (vector.rs:1226-1238).
+    void add_vector_level_fields(uint32_t level_id, const float* rows, uint32_t n, uint32_t dims, const uint8_t* field_ids, const uint32_t* chunk_ids,
+                                 uint64_t row_stride = 0, const uint16_t* local_ids = nullptr, const uint32_t* cluster_counts = nullptr,
+                                 uint32_t n_clusters = 0) {
+        check(ssb_vector_add_level_fields(h_, level_id, rows, row_stride, local_ids, n, dims, cluster_counts, n_clusters, field_ids, chunk_ids));
+        if (n) vector_fields_ = true;
+    }
+    // a shard's vector.bin with every record's field / chunk id kept (ssb_load_vector_bin_fields); returns the number of vectors
+    uint64_t load_vector_bin_fields(const void* bytes, uint64_t len) {
+        uint64_t n = 0;
+        check(ssb_load_vector_bin_fields(h_, bytes, len, &n));
+        if (n) vector_fields_ = true;
+        return n;
+    }
     // the shard's facet file (facets_file_mmap): one row of row_bytes per doc id, typed fields at their offsets
     void set_facets(const void* rows, uint64_t first_doc_id, uint64_t n_docs, uint32_t row_bytes, const std::vector<ssb_facet_field>& fields) {
         check(ssb_set_facets(h_, rows, first_doc_id, n_docs, row_bytes, fields.data(), static_cast<uint32_t>(fields.size())));
@@ -286,7 +301,9 @@ public:
             vq.similarity_threshold = search_mode.similarity_threshold ? *search_mode.similarity_threshold : 0.f;
             vq.ann_mode = search_mode.ann_mode.kind; vq.n_probe = search_mode.ann_mode.n_probe; vq.cluster_threshold = search_mode.ann_mode.threshold;
             uint64_t observed = 0;
-            check(ssb_search_vector_ex(h_, &vq, vec.data(), &n, nullptr, &observed));
+            // the field filter reaches the vector rows when they carry field ids (the reference tests every record, vector.rs:1226-1238)
+            const uint32_t* vmask = field_mask && vector_fields_ ? &field_mask : nullptr;
+            check(ssb_search_vector_fields(h_, &vq, vmask, vec.data(), &n, nullptr, &observed));
             vec.resize(n < heap ? n : heap);
             ro.observed_vector_count = static_cast<size_t>(observed);
         }
@@ -388,6 +405,7 @@ private:
     VectorSimilarity sim_;
     uint64_t indexed_doc_count_ = 0;
     std::vector<std::string> field_names_;
+    bool vector_fields_ = false;   // vector rows carry field ids (add_vector_level_fields / load_vector_bin_fields)
 };
 
 }  // namespace ssb

@@ -123,6 +123,7 @@ EXPORTS = [
     "ssb_abi_version", "ssb_last_error", "ssb_create", "ssb_destroy", "ssb_lexical_add_level",
     "ssb_vector_add_level_clustered", "ssb_lexical_set_field_boosts", "ssb_lexical_set_ngram_config", "ssb_lexical_add_level_ngrams", "ssb_lexical_commit", "ssb_lexical_dict_size", "ssb_lexical_dict_export", "ssb_lexical_set_global_df",
     "ssb_load_index_bin", "ssb_load_index_bin_ngrams", "ssb_load_vector_bin", "ssb_index_bin_inspect", "ssb_index_bin_inspect_ngrams", "ssb_set_deleted", "ssb_set_facets", "ssb_set_facet_value_order", "ssb_set_facet_string_sets", "ssb_vector_set_turboquant_mask", "ssb_vector_add_level", "ssb_vector_count", "ssb_vector_reserve", "ssb_set_vector_kernel", "ssb_search_lexical", "ssb_search_lexical_sorted", "ssb_search_lexical_sorted_ex", "ssb_search_lexical_facets", "ssb_search_empty", "ssb_search_empty_facets", "ssb_search_vector", "ssb_search_vector_ex", "ssb_search_hybrid",
+    "ssb_vector_add_level_fields", "ssb_load_vector_bin_fields", "ssb_search_vector_fields",
     "ssb_rrf_fuse", "ssb_comm_unique_id", "ssb_comm_init", "ssb_comm_attach", "ssb_comm_destroy", "ssb_lexical_sync_df",
     "ssb_search_vector_keys", "ssb_search_lexical_keys", "ssb_merge_keys", "ssb_sync",
     "ssb_stream", "ssb_set_stream", "ssb_last_stats",
@@ -181,6 +182,9 @@ def lib():
         "ssb_search_vector": [vp, vp, u32, u32, vp, vp],
         "ssb_search_vector_ex": [vp, C.POINTER(SsbVecQuery), vp, vp, vp, vp],
         "ssb_search_hybrid": [vp, C.POINTER(SsbLexBatch), vp, u32, vp, vp],
+        "ssb_vector_add_level_fields": [vp, u32, vp, u64, vp, u32, u32, vp, u32, vp, vp],
+        "ssb_load_vector_bin_fields": [vp, vp, u64, C.POINTER(u64)],
+        "ssb_search_vector_fields": [vp, C.POINTER(SsbVecQuery), vp, vp, vp, vp, vp],
         "ssb_rrf_fuse": [vp, u32, vp, u32, vp, C.POINTER(u32)],
         "ssb_search_vector_keys": [vp, vp, u32, u32, vp],
         "ssb_search_lexical_keys": [vp, C.POINTER(SsbLexBatch), u32, u32, vp, vp],

@@ -70,6 +70,7 @@ struct SearchCtx {
     DevBuf<float> qpad, qstage, qhi, qlo, q_scale, q_norm; DevBuf<int8_t> q_i8; DevBuf<int> q_aff;
     DevBuf<uint64_t> ceil, scratch, keys_a, keys_b, counts, gather;
     DevBuf<float> ivf_scores; DevBuf<uint32_t> ivf_sel; DevBuf<uint64_t> ivf_obs; std::vector<uint64_t> h_obs;   // IVF probe (vec_ivf.cu)
+    DevBuf<uint32_t> fmask, fsel, best; std::vector<uint32_t> h_best;   // field filter: per-query masks, per (query, cluster) fields; best-row step
     std::vector<uint64_t> h_ceil, h_keys_a, h_keys_b, h_counts;
     ssb_stats stats{};
     cudaEvent_t ev0 = nullptr, ev1 = nullptr; bool ev_used = false, last_lex = false;
@@ -118,6 +119,15 @@ struct ssb_index {
     // IVF cluster tables (vector.rs:1066-1094; f32 indexes): one entry per add call ("level"), clusters numbered across levels
     DevBuf<float> medoids; DevBuf<uint32_t> row_cluster, cl_count, lvl_begin;
     std::vector<uint32_t> h_lvl_begin; uint32_t n_clusters = 0, max_level_clusters = 0;
+    // multi-vector documents (ssb_vector_add_level_fields; VectorHeader.field_id / chunk_id, vector.rs:62-73): every level carries them or
+    // none does.  row_field: the byte the best-row step tests; row_class: cluster * 32 + field, what the scans' IVF test reads under a field
+    // mask (int8 indexes: one cluster); h_field / h_chunk: what the best-row step reports; field_rows / cl_field_rows: rows per field, and
+    // per (cluster, field) on f32 indexes, for observed_vector_count under a mask.  doc_rows (device) lists every doc's rows in record
+    // order, grouped by doc; doc_key / doc_off (host) index it.
+    int tagged = -1;                  // -1: no vector level yet, 0: untagged, 1: field-tagged
+    DevBuf<uint8_t> row_field; DevBuf<uint32_t> row_class; std::vector<uint8_t> h_field; std::vector<uint32_t> h_chunk;
+    uint64_t field_rows[32] = {}; std::vector<uint32_t> cl_field_rows;   // [n_clusters][32]
+    DevBuf<uint32_t> doc_rows; std::vector<uint64_t> doc_pairs /*(doc << 32) | row, sorted*/; std::vector<uint32_t> doc_key, doc_off;
     uint64_t n_rows = 0;
 };
 
@@ -173,7 +183,8 @@ namespace {
 struct IvfQuery { uint32_t mode, n_probe; float thr; };   // AnnMode of one call (thr pre-mapped, vector.rs:388-399)
 
 int32_t vec_keys(ssb_index* ix, SearchCtx& c, const void* queries, bool queries_i8, uint32_t nq, uint32_t k, uint64_t* keys_out_dev /*[nq][32]*/,
-                 const uint64_t* ceil_dev = nullptr /*[>= nq_pad] paging ceilings*/, const IvfQuery* ivf = nullptr /*null = AnnMode::All*/) {
+                 const uint64_t* ceil_dev = nullptr /*[>= nq_pad] paging ceilings*/, const IvfQuery* ivf = nullptr /*null = AnnMode::All*/,
+                 const uint32_t* fmask_host = nullptr /*[nq] field masks of a field-tagged index, or null: no query has one*/) {
     if (ivf && (ix->quant_i8 || !ix->medoids.p)) { set_error("AnnMode other than All needs an f32 vector index"); return SSB_E_UNSUPPORTED; }
     if (ix->dims == 0) { set_error("no vector index configured (vector_dims = 0)"); return SSB_E_STATE; }
     if (k == 0 || k > SSB_K_MAX) { set_error("k must be in 1..%u", SSB_K_MAX); return SSB_E_UNSUPPORTED; }
@@ -263,6 +274,19 @@ int32_t vec_keys(ssb_index* ix, SearchCtx& c, const void* queries, bool queries_
         v.scores = c.ivf_scores.p; v.sel = c.ivf_sel.p; v.observed = c.ivf_obs.p; v.launches = &c.stats.kernel_launches;
         SSB_TRY(vec::launch_ivf_select(v, st));
         a.ivf_sel = c.ivf_sel.p; a.ivf_words = v.words; a.row_cluster = ix->row_cluster.p;
+    }
+    if (fmask_host) {
+        // field filter (vector.rs:1226-1238): folded into the scans' per-candidate IVF test — a row's class is cluster * 32 + field and
+        // the selection holds, per (query, cluster), the fields the query scans.  Like the IVF mask it turns the threshold seed off.
+        const uint32_t n_cl = ix->quant_i8 ? 1u : ix->n_clusters;
+        SSB_TRY(c.fmask.reserve(nq_pad, 0, st));
+        SSB_TRY(c.fsel.reserve((size_t)nq_pad * n_cl, 0, st));
+        SSB_CUDA_TRY(cudaMemsetAsync(c.fmask.p, 0, (size_t)nq_pad * 4, st));   // padding queries: no filter (they collect nothing anyway)
+        SSB_CUDA_TRY(cudaMemcpyAsync(c.fmask.p, fmask_host, (size_t)nq * 4, cudaMemcpyHostToDevice, st));
+        c.stats.h2d_bytes += (uint64_t)nq * 4;
+        SSB_TRY(vec::launch_field_sel(a.ivf_sel, a.ivf_words, c.fmask.p, nq_pad, n_cl, c.fsel.p, st));
+        c.stats.kernel_launches += 1;
+        a.ivf_sel = c.fsel.p; a.ivf_words = n_cl; a.row_cluster = ix->row_class.p;
     }
     if (scan == vec::Scan::I8_128) {
         a.rows_i8 = ix->rows_i8.p; a.queries_i8 = c.q_i8.p; a.dpad8 = ix->dpad8;
@@ -415,7 +439,7 @@ void finish_stats(ssb_index* ix, SearchCtx& c) {
 
 // host-facing vector search: paging beyond 32 results, de-duplication, optional threshold
 int32_t search_vector_host(ssb_index* ix, SearchCtx& c, const void* queries, bool queries_i8, uint32_t nq, uint32_t k, ssb_hit* hits, uint32_t* n_hits,
-                           const IvfQuery* ivf = nullptr) {
+                           const IvfQuery* ivf = nullptr, const uint32_t* fmask_host = nullptr) {
     SSB_TRY(c.keys_a.reserve((size_t)nq * LIST, 0, c.st));
     c.h_keys_a.resize((size_t)nq * LIST);
     PageState<1> ps(c, nq, k, hits, n_hits, ix->dup_docs);
@@ -423,7 +447,7 @@ int32_t search_vector_host(ssb_index* ix, SearchCtx& c, const void* queries, boo
     // keys strictly below the last key of the previous one (keys are a total order on (score desc, doc id asc))
     uint32_t kk = ix->dup_docs ? SSB_K_MAX : (k < SSB_K_MAX ? k : SSB_K_MAX);
     for (uint32_t page = 0; page < 4096; page++) {
-        SSB_TRY(vec_keys(ix, c, queries, queries_i8, nq, kk, c.keys_a.p, page ? c.ceil.p : nullptr, ivf));
+        SSB_TRY(vec_keys(ix, c, queries, queries_i8, nq, kk, c.keys_a.p, page ? c.ceil.p : nullptr, ivf, fmask_host));
         SSB_TRY(shard_merge(ix, c, c.keys_a.p, nq));
         if (ivf && page == 0) {   // observed_vector_count = the vectors of the selected clusters (summed over the shards)
             SSB_TRY(shard_sum_counts(ix, c, c.ivf_obs.p, nq));
@@ -441,6 +465,102 @@ int32_t search_vector_host(ssb_index* ix, SearchCtx& c, const void* queries, boo
         SSB_TRY(ps.upload_ceilings());
     }
     ps.finish();
+    return SSB_OK;
+}
+
+// field masks of a vector search (HOST array [nq], bit f = indexed field f, 0 = no filter; the bits of ssb_lex_batch.field_masks).
+// *use = the array when some query has a mask, else null: an unmasked batch runs exactly the unfiltered path.  A mask on an index
+// whose rows carry no field ids is refused rather than ignored.
+int32_t vec_field_masks(const ssb_index* ix, const uint32_t* masks, uint32_t nq, const char* who, const uint32_t** use) {
+    *use = nullptr;
+    if (!masks) return SSB_OK;
+    if (is_device_ptr(masks)) { set_error("%s: field_masks must be a host array", who); return SSB_E_INVALID; }
+    bool any = false;
+    for (uint32_t q = 0; q < nq; q++) any = any || masks[q] != 0u;
+    if (!any) return SSB_OK;
+    if (ix->tagged != 1) { set_error("%s: a field mask needs vector rows with field ids (ssb_vector_add_level_fields)", who); return SSB_E_STATE; }
+    *use = masks;
+    return SSB_OK;
+}
+
+// vb field_id / chunk_id of every returned hit of a field-tagged index: the doc's best row among those passing the query's mask
+// (launch_best_rows).  Runs after the search, on the queries it left in the context (f32: prepared again, int8: its quantised codes).
+int32_t fill_best_rows(ssb_index* ix, SearchCtx& c, const void* queries, uint32_t nq, uint32_t k, const ssb_hit* hits, const uint32_t* nh,
+                       const uint32_t* fmask_host, ssb_hit_ext* ext) {
+    cudaStream_t st = c.st;
+    std::vector<uint32_t> hq;   // per hit: (query, first CSR entry, row count, 0)
+    std::vector<uint32_t> slot;  // ext index of each hit
+    for (uint32_t q = 0; q < nq; q++)
+        for (uint32_t j = 0; j < nh[q]; j++) {
+            const uint32_t doc = (uint32_t)hits[(size_t)q * k + j].doc_id;
+            const auto it = std::lower_bound(ix->doc_key.begin(), ix->doc_key.end(), doc);
+            if (it == ix->doc_key.end() || *it != doc) continue;
+            const size_t d = (size_t)(it - ix->doc_key.begin());
+            hq.insert(hq.end(), {q, ix->doc_off[d], ix->doc_off[d + 1] - ix->doc_off[d], 0u});
+            slot.push_back(q * k + j);
+        }
+    const uint32_t n = (uint32_t)slot.size();
+    if (n == 0) return SSB_OK;
+    SSB_TRY(c.best.reserve((size_t)n * 5, 0, st));
+    SSB_TRY(c.fmask.reserve(nq, 0, st));
+    if (fmask_host) SSB_CUDA_TRY(cudaMemcpyAsync(c.fmask.p, fmask_host, (size_t)nq * 4, cudaMemcpyHostToDevice, st));
+    else SSB_CUDA_TRY(cudaMemsetAsync(c.fmask.p, 0, (size_t)nq * 4, st));
+    SSB_CUDA_TRY(cudaMemcpyAsync(c.best.p, hq.data(), (size_t)n * 16, cudaMemcpyHostToDevice, st));
+    vec::BestRowArgs b{};
+    b.n_hits = n; b.hits = reinterpret_cast<const uint4*>(c.best.p); b.doc_rows = ix->doc_rows.p; b.best_row = c.best.p + (size_t)n * 4;
+    b.field_mask = c.fmask.p; b.row_field = ix->row_field.p;
+    if (ix->quant_i8) {
+        // the int8 codes (and scales) of the queries are still in the context from the search's last page
+        b.rows_i8 = ix->rows_i8.p; b.queries_i8 = c.q_i8.p; b.dpad8 = ix->dpad8;
+        if (ix->turbo || ix->cfg.vector_similarity != SSB_SIM_COSINE) {
+            b.i8_scaled = ix->cfg.vector_similarity == SSB_SIM_EUCLIDEAN ? (ix->affine ? 3 : 2) : 1;
+            b.row_scale = ix->row_scale.p; b.row_norm = ix->row_norm.p; b.q_scale = c.q_scale.p; b.q_norm = c.q_norm.p;
+            b.row_aff = ix->row_aff.p; b.q_aff = c.q_aff.p;
+        }
+    } else {
+        const void* qsrc = is_device_ptr(queries) ? queries : c.qstage.p;   // host queries were staged by the search
+        SSB_TRY(c.qpad.reserve((size_t)nq * ix->dpad, 0, st));
+        SSB_TRY(vec::launch_prep_queries((const float*)qsrc, nq, ix->dims, ix->dims, c.qpad.p, nq, ix->dpad,
+                                         ix->cfg.vector_similarity == SSB_SIM_COSINE, st));
+        c.stats.kernel_launches += 1;
+        b.rows = ix->rows.p; b.queries = c.qpad.p; b.dpad = ix->dpad; b.euclid = ix->cfg.vector_similarity == SSB_SIM_EUCLIDEAN;
+    }
+    SSB_TRY(vec::launch_best_rows(b, st));
+    c.stats.kernel_launches += 1;
+    c.h_best.resize(n);
+    SSB_CUDA_TRY(cudaMemcpyAsync(c.h_best.data(), b.best_row, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
+    SSB_CUDA_TRY(cudaStreamSynchronize(st));
+    c.stats.h2d_bytes += (uint64_t)n * 16; c.stats.d2h_bytes += (uint64_t)n * 4;
+    for (uint32_t i = 0; i < n; i++) {
+        const uint32_t row = c.h_best[i];
+        if (row == 0xFFFFFFFFu) continue;
+        ext[slot[i]].field_id = ix->h_field[row];
+        ext[slot[i]].chunk_id = ix->h_chunk[row];
+    }
+    return SSB_OK;
+}
+
+// observed_vector_count of a masked query: the rows in scope whose field passes the mask — every row (AnnMode::All) or the rows of the
+// clusters the probe selected (its selection bits are still in the context)
+int32_t masked_observed(ssb_index* ix, SearchCtx& c, uint32_t nq, const uint32_t* fmask_host, bool use_ivf, uint64_t* observed) {
+    std::vector<uint32_t> sel;
+    const uint32_t words = (ix->n_clusters + 31) / 32;
+    if (use_ivf) {
+        sel.resize((size_t)nq * words);
+        SSB_CUDA_TRY(cudaMemcpyAsync(sel.data(), c.ivf_sel.p, sel.size() * 4, cudaMemcpyDeviceToHost, c.st));
+        SSB_CUDA_TRY(cudaStreamSynchronize(c.st));
+    }
+    for (uint32_t q = 0; q < nq; q++) {
+        const uint32_t m = fmask_host[q];
+        if (!m) continue;
+        uint64_t n = 0;
+        if (!use_ivf) { for (uint32_t f = 0; f < 32; f++) if ((m >> f) & 1u) n += ix->field_rows[f]; }
+        else
+            for (uint32_t cl = 0; cl < ix->n_clusters; cl++)
+                if ((sel[(size_t)q * words + cl / 32] >> (cl % 32)) & 1u)
+                    for (uint32_t f = 0; f < 32; f++) if ((m >> f) & 1u) n += ix->cl_field_rows[(size_t)cl * 32 + f];
+        observed[q] = n;
+    }
     return SSB_OK;
 }
 
@@ -590,6 +710,7 @@ int32_t ssb_destroy(ssb_index* ix) {
         ix->facets.release();
         cudaFree(ix->tq_mask); ix->tq_mask = nullptr;
         ix->rows.release(); ix->rows_hi.release(); ix->rows_lo.release(); ix->rows_i8.release(); ix->row_scale.release(); ix->row_norm.release(); ix->row_aff.release(); ix->doc_ids.release();
+        ix->row_field.release(); ix->row_class.release(); ix->doc_rows.release();
         cudaStreamDestroy(ix->load_st);
     }
     delete ix;
@@ -686,7 +807,8 @@ int32_t ssb_vector_reserve(ssb_index* ix, uint64_t n_rows) {
 // one level (= one add call) of the vector index; cluster_counts = the level's IVF cluster table or null (one cluster).  n is only
 // bounded by the loader (a level may hold one record per chunk, i.e. more than 64K).
 static int32_t vector_add_level_impl(ssb_index* ix, uint32_t level_id, const float* rows, uint64_t row_stride, const uint16_t* local_ids,
-                                     uint32_t n, uint32_t dims, const uint32_t* cluster_counts, uint32_t n_clusters) {
+                                     uint32_t n, uint32_t dims, const uint32_t* cluster_counts, uint32_t n_clusters,
+                                     const uint8_t* field_ids = nullptr, const uint32_t* chunk_ids = nullptr) {
     SSB_API_BEGIN
     if (!ix || (n && !rows)) { set_error("ssb_vector_add_level: null argument"); return SSB_E_INVALID; }
     if (ix->dims == 0 || dims != ix->dims) { set_error("dims %u != configured vector_dims %u", dims, ix->dims); return SSB_E_INVALID; }
@@ -700,9 +822,22 @@ static int32_t vector_add_level_impl(ssb_index* ix, uint32_t level_id, const flo
     if (level_id >= 65536) { set_error("level_id must be < 65536 (doc id = level_id << 16 | local)"); return SSB_E_INVALID; }
     if (row_stride == 0) row_stride = dims;
     if (row_stride < dims) { set_error("row stride < dims"); return SSB_E_INVALID; }
+    if ((field_ids == nullptr) != (chunk_ids == nullptr)) { set_error("ssb_vector_add_level_fields: field_ids and chunk_ids go together"); return SSB_E_INVALID; }
     std::unique_lock<std::shared_mutex> g(ix->rw);
     SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
-    if (n == 0) return SSB_OK;
+    if (n == 0) return SSB_OK;   // an empty level (a block whose docs carry no vectors, vector.rs:1056-1073) is neither tagged nor untagged
+    const int tag = field_ids ? 1 : 0;
+    if (ix->tagged >= 0 && ix->tagged != tag) {
+        set_error("vector levels %s field ids, this one %s: every level carries them or none does", ix->tagged ? "carry" : "carry no", tag ? "does" : "does not");
+        return SSB_E_STATE;
+    }
+    std::vector<uint8_t> h_fld; std::vector<uint32_t> h_chk;
+    if (tag) {   // validated before anything is written
+        h_fld.resize(n); h_chk.resize(n);
+        SSB_CUDA_TRY(cudaMemcpy(h_fld.data(), field_ids, n, cudaMemcpyDefault));
+        SSB_CUDA_TRY(cudaMemcpy(h_chk.data(), chunk_ids, (size_t)n * 4, cudaMemcpyDefault));
+        for (uint32_t i = 0; i < n; i++) if (h_fld[i] >= 32) { set_error("field id %u of row %u: indexed field ids must be < 32", h_fld[i], i); return SSB_E_INVALID; }
+    }
     cudaStream_t st = ix->load_st;
     // device-resident inputs may still be in flight on the caller's stream (the load stream is non-blocking): load time is not
     // hot, wait for the device once
@@ -810,6 +945,7 @@ static int32_t vector_add_level_impl(ssb_index* ix, uint32_t level_id, const flo
         lid = tmp.p;
     }
     SSB_TRY(vec::launch_fill_doc_ids(ix->doc_ids.p + ix->n_rows, lid, level_id, n, st));
+    std::vector<uint32_t> row_cl;   // tagged f32 levels: each row's global cluster id
     if (!ix->quant_i8) {
         // IVF tables: clusters are numbered across levels; a cluster's medoid is its first row (vector.rs:1316-1320)
         const uint32_t one = n;
@@ -829,6 +965,11 @@ static int32_t vector_add_level_impl(ssb_index* ix, uint32_t level_id, const flo
         SSB_CUDA_TRY(cudaMemcpyAsync(ix->cl_count.p + ix->n_clusters, cluster_counts, (size_t)n_clusters * 4, cudaMemcpyHostToDevice, st));
         SSB_CUDA_TRY(cudaMemcpyAsync(midx.p, mrow.data(), (size_t)n_clusters * 4, cudaMemcpyHostToDevice, st));
         SSB_TRY(vec::launch_gather_rows(ix->rows.p, midx.p, n_clusters, ix->dpad, ix->medoids.p + (size_t)ix->n_clusters * ix->dpad, st));
+        if (tag) {
+            ix->cl_field_rows.resize((size_t)(ix->n_clusters + n_clusters) * 32, 0u);
+            for (uint32_t i = 0; i < n; i++) ix->cl_field_rows[(size_t)rc[i] * 32 + h_fld[i]]++;
+            row_cl = std::move(rc);
+        }
         std::vector<uint32_t> lb = ix->h_lvl_begin; lb.push_back(ix->n_clusters); lb.push_back(ix->n_clusters + n_clusters);
         SSB_CUDA_TRY(cudaMemcpyAsync(ix->lvl_begin.p, lb.data(), lb.size() * 4, cudaMemcpyHostToDevice, st));
         SSB_CUDA_TRY(cudaStreamSynchronize(st));
@@ -836,7 +977,44 @@ static int32_t vector_add_level_impl(ssb_index* ix, uint32_t level_id, const flo
         ix->n_clusters += n_clusters;
         if (n_clusters > ix->max_level_clusters) ix->max_level_clusters = n_clusters;
     }
+    if (tag) {
+        // row fields for the scans; the doc -> rows table of the best-row step: the level's (doc, row) pairs merged into the sorted list
+        SSB_TRY(ix->row_field.reserve(ix->n_rows + n, ix->n_rows, st));
+        SSB_CUDA_TRY(cudaMemcpyAsync(ix->row_field.p + ix->n_rows, h_fld.data(), n, cudaMemcpyHostToDevice, st));
+        std::vector<uint32_t> cls(n);
+        for (uint32_t i = 0; i < n; i++) cls[i] = (ix->quant_i8 ? 0u : row_cl[i]) * 32u + h_fld[i];
+        SSB_TRY(ix->row_class.reserve(ix->n_rows + n, ix->n_rows, st));
+        SSB_CUDA_TRY(cudaMemcpyAsync(ix->row_class.p + ix->n_rows, cls.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
+        for (uint32_t i = 0; i < n; i++) ix->field_rows[h_fld[i]]++;
+        const size_t old = ix->doc_pairs.size();
+        for (uint32_t i = 0; i < n; i++) {
+            const uint32_t doc = (level_id << 16) | (local_ids ? (uint32_t)h_ids[i] : i);
+            ix->doc_pairs.push_back(((uint64_t)doc << 32) | (ix->n_rows + i));
+        }
+        std::sort(ix->doc_pairs.begin() + old, ix->doc_pairs.end());
+        // levels usually arrive in level order: every new doc sorts after the table's last one, and the level's entries are appended (host
+        // index and device rows).  Otherwise the pairs are merged and the table is rebuilt.
+        const bool append = old == 0 || (uint32_t)(ix->doc_pairs[old] >> 32) > ix->doc_key.back();
+        size_t from = old;
+        if (append) { if (!ix->doc_off.empty()) ix->doc_off.pop_back(); }
+        else {
+            std::inplace_merge(ix->doc_pairs.begin(), ix->doc_pairs.begin() + old, ix->doc_pairs.end());
+            ix->doc_key.clear(); ix->doc_off.clear(); from = 0;
+        }
+        std::vector<uint32_t> rows_of(ix->doc_pairs.size() - from);
+        for (size_t i = from; i < ix->doc_pairs.size(); i++) {
+            const uint32_t doc = (uint32_t)(ix->doc_pairs[i] >> 32);
+            if (ix->doc_key.empty() || ix->doc_key.back() != doc) { ix->doc_key.push_back(doc); ix->doc_off.push_back((uint32_t)i); }
+            rows_of[i - from] = (uint32_t)ix->doc_pairs[i];
+        }
+        ix->doc_off.push_back((uint32_t)ix->doc_pairs.size());
+        SSB_TRY(ix->doc_rows.reserve(ix->doc_pairs.size(), from, st));
+        SSB_CUDA_TRY(cudaMemcpyAsync(ix->doc_rows.p + from, rows_of.data(), rows_of.size() * 4, cudaMemcpyHostToDevice, st));
+        ix->h_field.insert(ix->h_field.end(), h_fld.begin(), h_fld.end());
+        ix->h_chunk.insert(ix->h_chunk.end(), h_chk.begin(), h_chk.end());
+    }
     SSB_CUDA_TRY(cudaStreamSynchronize(st));
+    ix->tagged = tag;
     ix->n_rows += n;
     return SSB_OK;
     SSB_API_END
@@ -855,6 +1033,16 @@ int32_t ssb_vector_add_level_clustered(ssb_index* ix, uint32_t level_id, const f
     if (n > 65536) { set_error("a level holds at most 65536 vectors"); return SSB_E_INVALID; }
     if (n && !cluster_counts) { set_error("ssb_vector_add_level_clustered: null cluster table"); return SSB_E_INVALID; }
     return vector_add_level_impl(ix, level_id, rows, row_stride, local_ids, n, dims, n ? cluster_counts : nullptr, n_clusters);
+}
+
+int32_t ssb_vector_add_level_fields(ssb_index* ix, uint32_t level_id, const float* rows, uint64_t row_stride, const uint16_t* local_ids,
+                                    uint32_t n, uint32_t dims, const uint32_t* cluster_counts, uint32_t n_clusters,
+                                    const uint8_t* field_ids, const uint32_t* chunk_ids) {
+    if (n > 65536) { set_error("a level holds at most 65536 vectors"); return SSB_E_INVALID; }
+    if (n && (!field_ids || !chunk_ids)) { set_error("ssb_vector_add_level_fields: null field_ids / chunk_ids"); return SSB_E_INVALID; }
+    if (ix && ix->comm.active()) { set_error("ssb_vector_add_level_fields: field-tagged rows on a sharded index are not supported"); return SSB_E_UNSUPPORTED; }
+    return vector_add_level_impl(ix, level_id, rows, row_stride, local_ids, n, dims, n ? cluster_counts : nullptr, n_clusters,
+                                 n ? field_ids : nullptr, n ? chunk_ids : nullptr);
 }
 
 int32_t ssb_load_index_bin(ssb_index* ix, const void* bytes, uint64_t len, const ssb_index_bin_params* params, uint64_t* n_docs_out) {
@@ -892,13 +1080,17 @@ int32_t ssb_index_bin_inspect_ngrams(const void* bytes, uint64_t len, const ssb_
     SSB_API_END
 }
 
-int32_t ssb_load_vector_bin(ssb_index* ix, const void* bytes, uint64_t len, uint64_t* n_vectors_out) {
+}  // extern "C"
+
+// keep_fields: VectorHeader.field_id / chunk_id go through the field-tagged add (ssb_load_vector_bin_fields)
+static int32_t load_vector_bin_impl(ssb_index* ix, const void* bytes, uint64_t len, uint64_t* n_vectors_out, bool keep_fields) {
     SSB_API_BEGIN
     if (!ix || !bytes) { set_error("ssb_load_vector_bin: null argument"); return SSB_E_INVALID; }
     if (is_device_ptr(bytes)) { set_error("ssb_load_vector_bin: bytes must be host memory"); return SSB_E_INVALID; }
     if (ix->dims == 0) { set_error("ssb_load_vector_bin: the index has no vector_dims"); return SSB_E_STATE; }
+    if (keep_fields && ix->comm.active()) { set_error("ssb_load_vector_bin_fields: field-tagged rows on a sharded index are not supported"); return SSB_E_UNSUPPORTED; }
     std::vector<VectorLevel> levels;
-    SSB_TRY(parse_vector_bin((const uint8_t*)bytes, len, ix->dims, levels));
+    SSB_TRY(parse_vector_bin((const uint8_t*)bytes, len, ix->dims, levels, keep_fields));
     uint64_t total = 0;
     for (auto& vl : levels) {
         // a level may hold more than 64K records (one per chunk); its cluster table (IVF, vector.rs:1066-1094) rides along.  Empty clusters
@@ -906,12 +1098,23 @@ int32_t ssb_load_vector_bin(ssb_index* ix, const void* bytes, uint64_t len, uint
         bool ok = !vl.cluster_counts.empty() && !ix->quant_i8;
         for (uint32_t c : vl.cluster_counts) ok = ok && c != 0;
         SSB_TRY(vector_add_level_impl(ix, vl.level_id, vl.rows.data(), ix->dims, vl.ids.data(), (uint32_t)vl.ids.size(), ix->dims,
-                                      ok ? vl.cluster_counts.data() : nullptr, ok ? (uint32_t)vl.cluster_counts.size() : 0));
+                                      ok ? vl.cluster_counts.data() : nullptr, ok ? (uint32_t)vl.cluster_counts.size() : 0,
+                                      keep_fields && !vl.ids.empty() ? vl.fields.data() : nullptr, keep_fields && !vl.ids.empty() ? vl.chunks.data() : nullptr));
         total += vl.ids.size();
     }
     if (n_vectors_out) *n_vectors_out = total;
     return SSB_OK;
     SSB_API_END
+}
+
+extern "C" {
+
+int32_t ssb_load_vector_bin(ssb_index* ix, const void* bytes, uint64_t len, uint64_t* n_vectors_out) {
+    return load_vector_bin_impl(ix, bytes, len, n_vectors_out, false);
+}
+
+int32_t ssb_load_vector_bin_fields(ssb_index* ix, const void* bytes, uint64_t len, uint64_t* n_vectors_out) {
+    return load_vector_bin_impl(ix, bytes, len, n_vectors_out, true);
 }
 
 // shard.delete_hashset (index.rs:1594, filled by delete_document index.rs:5110): deleted docs are neither scored nor counted
@@ -1059,7 +1262,10 @@ int32_t ssb_search_vector(ssb_index* ix, const float* queries, uint32_t nq, uint
     SSB_API_END
 }
 
-int32_t ssb_search_vector_ex(ssb_index* ix, const ssb_vec_query* vq, ssb_hit* hits, uint32_t* n_hits, ssb_hit_ext* ext, uint64_t* observed) {
+}  // extern "C"
+
+static int32_t search_vector_ex_impl(ssb_index* ix, const ssb_vec_query* vq, const uint32_t* field_masks, ssb_hit* hits, uint32_t* n_hits,
+                                     ssb_hit_ext* ext, uint64_t* observed) {
     SSB_API_BEGIN
     if (!ix || !vq || (vq->n_queries && (!vq->queries || !hits))) { set_error("ssb_search_vector_ex: null argument"); return SSB_E_INVALID; }
     if (vq->query_format > SSB_QFMT_I8) { set_error("bad query_format"); return SSB_E_INVALID; }
@@ -1067,6 +1273,8 @@ int32_t ssb_search_vector_ex(ssb_index* ix, const ssb_vec_query* vq, ssb_hit* hi
     SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
     const uint32_t nq = vq->n_queries, k = vq->k;
     if (nq == 0) return SSB_OK;
+    const uint32_t* fm = nullptr;
+    SSB_TRY(vec_field_masks(ix, field_masks, nq, "ssb_search_vector_fields", &fm));
     if (k == 0 || k > SSB_K_LIMIT) { set_error("k must be in 1..%u", SSB_K_LIMIT); return SSB_E_UNSUPPORTED; }
     CtxLease l(ix); SSB_TRY(l.acquire());
     std::vector<uint32_t> nh(nq, 0);
@@ -1078,7 +1286,7 @@ int32_t ssb_search_vector_ex(ssb_index* ix, const ssb_vec_query* vq, ssb_hit* hi
         ivf.thr = euclid ? -vq->cluster_threshold : c21 / (1.0f / 16129.0f);
     }
     const bool use_ivf = vq->ann_mode != SSB_ANN_ALL;
-    SSB_TRY(search_vector_host(ix, *l.c, vq->queries, vq->query_format == SSB_QFMT_I8, nq, k, hits, nh.data(), use_ivf ? &ivf : nullptr));
+    SSB_TRY(search_vector_host(ix, *l.c, vq->queries, vq->query_format == SSB_QFMT_I8, nq, k, hits, nh.data(), use_ivf ? &ivf : nullptr, fm));
     finish_stats(ix, *l.c);
     // TopK::new (vector.rs:388-399): threshold pre-map (2t-1)*16129 for Dot/Cosine, -t for Euclidean; TopK::push (:421) rejects
     // score < threshold.  The hits are sorted by score, so dropping the tail is the same filter.
@@ -1092,6 +1300,7 @@ int32_t ssb_search_vector_ex(ssb_index* ix, const ssb_vec_query* vq, ssb_hit* hi
             for (uint32_t j = m; j < n; j++) hits[(size_t)q * k + j] = ssb_hit{0, 0.f, 0};
             n = m;
         }
+        nh[q] = n;
         if (n_hits) n_hits[q] = n;
         if (observed) observed[q] = use_ivf ? l.c->h_obs[q] : ix->n_rows;   // AnnMode::All scores every record (observed_vector_count, vector.rs:420); else: the selected clusters' vectors
         if (ext) for (uint32_t j = 0; j < k; j++) {
@@ -1106,8 +1315,22 @@ int32_t ssb_search_vector_ex(ssb_index* ix, const ssb_vec_query* vq, ssb_hit* hi
             e.source = SSB_SOURCE_VECTOR;
         }
     }
+    if (fm && observed) SSB_TRY(masked_observed(ix, *l.c, nq, fm, use_ivf, observed));
+    // field-tagged rows: which field and chunk of each doc won (after the threshold: only the hits returned)
+    if (ext && ix->tagged == 1) SSB_TRY(fill_best_rows(ix, *l.c, vq->queries, nq, k, hits, nh.data(), fm, ext));
     return SSB_OK;
     SSB_API_END
+}
+
+extern "C" {
+
+int32_t ssb_search_vector_ex(ssb_index* ix, const ssb_vec_query* vq, ssb_hit* hits, uint32_t* n_hits, ssb_hit_ext* ext, uint64_t* observed) {
+    return search_vector_ex_impl(ix, vq, nullptr, hits, n_hits, ext, observed);
+}
+
+int32_t ssb_search_vector_fields(ssb_index* ix, const ssb_vec_query* vq, const uint32_t* field_masks, ssb_hit* hits, uint32_t* n_hits,
+                                 ssb_hit_ext* ext, uint64_t* observed) {
+    return search_vector_ex_impl(ix, vq, field_masks, hits, n_hits, ext, observed);
 }
 
 int32_t ssb_search_lexical_keys(ssb_index* ix, const ssb_lex_batch* q, uint32_t k, uint32_t result_type, uint64_t* keys_out_dev,
@@ -1261,6 +1484,9 @@ int32_t ssb_search_hybrid(ssb_index* ix, const ssb_lex_batch* q, const float* qu
     SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
     const uint32_t nq = q->n_queries;
     if (nq == 0) return SSB_OK;
+    // the lexical field filter applies to the vector half as well (search.rs:1702-1731), on an index whose rows carry field ids
+    const uint32_t* fm = nullptr;
+    if (ix->tagged == 1) SSB_TRY(vec_field_masks(ix, q->field_masks, nq, "ssb_search_hybrid", &fm));
     // the two per-shard searches are independent until the fusion: the lexical one runs on this context's stream, the vector one
     // on a second context's stream, so lex_score and the scan share the GPU instead of running back to back
     CtxLease l(ix); SSB_TRY(l.acquire());
@@ -1277,7 +1503,7 @@ int32_t ssb_search_hybrid(ssb_index* ix, const ssb_lex_batch* q, const float* qu
     SSB_TRY(shard_merge(ix, c, c.keys_a.p, nq));
     SSB_CUDA_TRY(cudaMemcpyAsync(c.h_keys_a.data(), c.keys_a.p, (size_t)nq * LIST * 8, cudaMemcpyDeviceToHost, c.st));
     // multi-chunk documents: fetch the full 32-list so that k distinct docs survive the per-doc de-duplication
-    SSB_TRY(vec_keys(ix, *cv, queries, false, nq, ix->dup_docs ? SSB_K_MAX : k, cv->keys_b.p));
+    SSB_TRY(vec_keys(ix, *cv, queries, false, nq, ix->dup_docs ? SSB_K_MAX : k, cv->keys_b.p, nullptr, nullptr, fm));
     SSB_TRY(shard_merge(ix, *cv, cv->keys_b.p, nq));
     SSB_CUDA_TRY(cudaMemcpyAsync(cv->h_keys_b.data(), cv->keys_b.p, (size_t)nq * LIST * 8, cudaMemcpyDeviceToHost, cv->st));
     SSB_CUDA_TRY(cudaStreamSynchronize(c.st));
@@ -1334,6 +1560,7 @@ int32_t ssb_comm_init(ssb_index* ix, const uint8_t* id128, uint32_t rank, uint32
     SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
     if (ix->comm.comm) { set_error("ssb_comm_init: the index already has a communicator"); return SSB_E_STATE; }
     if (ix->lex->has_ngrams() && world > 1) { set_error("ssb_comm_init: n-gram lists on a sharded index are not supported"); return SSB_E_UNSUPPORTED; }
+    if (ix->tagged == 1 && world > 1) { set_error("ssb_comm_init: field-tagged vector rows on a sharded index are not supported"); return SSB_E_UNSUPPORTED; }
     SSB_TRY(comm_init(ix->comm, id128, rank, world));
     std::lock_guard<std::mutex> g2(ix->pool_mu);
     if (ix->pool.size() > 1) { ix->pool.resize(1); ix->free_ctx.clear(); ix->free_ctx.push_back(ix->pool[0].get()); ix->last_ctx = nullptr; }
@@ -1347,6 +1574,7 @@ int32_t ssb_comm_attach(ssb_index* ix, void* nccl_comm, uint32_t rank, uint32_t 
     std::unique_lock<std::shared_mutex> g(ix->rw);
     if (ix->comm.comm) { set_error("ssb_comm_attach: the index already has a communicator"); return SSB_E_STATE; }
     if (ix->lex->has_ngrams() && world > 1) { set_error("ssb_comm_attach: n-gram lists on a sharded index are not supported"); return SSB_E_UNSUPPORTED; }
+    if (ix->tagged == 1 && world > 1) { set_error("ssb_comm_attach: field-tagged vector rows on a sharded index are not supported"); return SSB_E_UNSUPPORTED; }
     ix->comm.comm = nccl_comm; ix->comm.rank = rank; ix->comm.world = world; ix->comm.owned = false;
     std::lock_guard<std::mutex> g2(ix->pool_mu);
     if (ix->pool.size() > 1) { ix->pool.resize(1); ix->free_ctx.clear(); ix->free_ctx.push_back(ix->pool[0].get()); ix->last_ctx = nullptr; }

@@ -300,10 +300,11 @@ int32_t launch_facet_select(const FacetSet& fs, const FacetReqDev* req, uint32_t
                             ssb_facet_count* out, uint32_t out_stride, uint32_t* n_out, cudaStream_t st);
 
 // loader.cu: the reference's on-disk files -> index
-struct VectorLevel { uint32_t level_id; std::vector<uint16_t> ids; std::vector<float> rows; std::vector<uint32_t> cluster_counts; };
+struct VectorLevel { uint32_t level_id; std::vector<uint16_t> ids; std::vector<float> rows; std::vector<uint32_t> cluster_counts;
+                     std::vector<uint8_t> fields; std::vector<uint32_t> chunks; /* keep_fields only */ };
 int32_t load_index_bin(LexIndex* lex, const uint8_t* bytes, uint64_t len, const ssb_index_bin_params* prm, uint64_t* n_docs_out, bool ngrams = false);
 int32_t inspect_index_bin(const uint8_t* bytes, uint64_t len, const ssb_index_bin_params* prm, uint64_t out[8]);
 int32_t inspect_index_bin_ngrams(const uint8_t* bytes, uint64_t len, const ssb_index_bin_params* prm, uint64_t out[8]);
-int32_t parse_vector_bin(const uint8_t* bytes, uint64_t len, uint32_t dims, std::vector<VectorLevel>& out);
+int32_t parse_vector_bin(const uint8_t* bytes, uint64_t len, uint32_t dims, std::vector<VectorLevel>& out, bool keep_fields = false);
 
 }  // namespace ssb

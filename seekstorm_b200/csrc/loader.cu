@@ -335,7 +335,7 @@ int32_t inspect_index_bin_ngrams(const uint8_t* bytes, uint64_t len, const ssb_i
 }
 
 // vector.bin -> per level (local ids, rows); the caller appends them through the normal add path
-int32_t parse_vector_bin(const uint8_t* bytes, uint64_t len, uint32_t dims, std::vector<VectorLevel>& out) {
+int32_t parse_vector_bin(const uint8_t* bytes, uint64_t len, uint32_t dims, std::vector<VectorLevel>& out, bool keep_fields) {
     Reader r{bytes, len};
     const uint64_t rec = 24 + (uint64_t)dims * 4;
     uint32_t level = 0;
@@ -348,9 +348,15 @@ int32_t parse_vector_bin(const uint8_t* bytes, uint64_t len, uint32_t dims, std:
         if (n > 65536ull * 64) { set_error("load_vector_bin: level %u holds %llu records", level, (unsigned long long)n); return SSB_E_INVALID; }
         if (!r.need(n * rec)) { set_error("load_vector_bin: truncated records (level %u)", level); return SSB_E_INVALID; }
         VectorLevel vl; vl.level_id = level; vl.ids.resize(n); vl.rows.resize(n * dims); vl.cluster_counts = std::move(counts);
+        if (keep_fields) { vl.fields.resize(n); vl.chunks.resize(n); }
         for (uint64_t i = 0; i < n; i++) {
             const uint8_t* h = bytes + r.pos + i * rec;
-            vl.ids[i] = rd16(h);                                   // VectorHeader.doc_id (vector.rs:65-73); field / chunk ids are not kept
+            vl.ids[i] = rd16(h);                                   // VectorHeader.doc_id (vector.rs:65-73); packed: field_id at +2, chunk_id at +6
+            if (keep_fields) {
+                const uint32_t f = rd32(h + 2);
+                if (f >= 32) { set_error("load_vector_bin: field id %u of record %llu (level %u): indexed field ids must be < 32", f, (unsigned long long)i, level); return SSB_E_INVALID; }
+                vl.fields[i] = (uint8_t)f; vl.chunks[i] = rd32(h + 6);
+            }
             memcpy(vl.rows.data() + i * dims, h + 24, (size_t)dims * 4);
         }
         r.pos += n * rec;

@@ -84,7 +84,26 @@ __global__ void gather_rows(const float* __restrict__ src, const uint32_t* __res
     for (uint32_t i = threadIdx.x; i < dpad; i += blockDim.x) dst[(size_t)r * dpad + i] = src[(size_t)idx[r] * dpad + i];
 }
 
+// out[q][c] = fields of cluster c that query q scans: its mask (0 = every field) if the probe selected c, else none
+__global__ void field_sel(const uint32_t* __restrict__ sel, uint32_t sel_words, const uint32_t* __restrict__ fmask, uint32_t n_cl,
+                          uint32_t nq, uint32_t* __restrict__ out) {
+    const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= n_cl) return;
+    for (uint32_t q = blockIdx.y; q < nq; q += gridDim.y) {   // any batch size: the grid's y extent is capped below 65536
+        const uint32_t m = fmask[q] ? fmask[q] : 0xFFFFFFFFu;
+        const bool on = !sel || ((sel[(size_t)q * sel_words + (c >> 5)] >> (c & 31u)) & 1u);
+        out[(size_t)q * n_cl + c] = on ? m : 0u;
+    }
+}
+
 }  // namespace ivf
+
+int32_t launch_field_sel(const uint32_t* sel, uint32_t sel_words, const uint32_t* fmask, uint32_t nq_pad, uint32_t n_cl, uint32_t* out, cudaStream_t st) {
+    if (nq_pad == 0 || n_cl == 0) return SSB_OK;
+    ivf::field_sel<<<dim3((n_cl + 127) / 128, nq_pad < 4096u ? nq_pad : 4096u), 128, 0, st>>>(sel, sel_words, fmask, n_cl, nq_pad, out);
+    SSB_CUDA_TRY(cudaGetLastError());
+    return SSB_OK;
+}
 
 int32_t launch_gather_rows(const float* src, const uint32_t* idx_dev, uint32_t n, uint32_t dpad, float* dst, cudaStream_t st) {
     if (n == 0) return SSB_OK;

@@ -146,7 +146,61 @@ fallback_merge(const uint32_t* __restrict__ fb_state, const uint64_t* __restrict
     }
 }
 
+// one warp per returned (query, doc): the doc's rows in record order, each scored like the scan that produced the hit — f32: the plain
+// f32 dot product of refine_candidates (Euclidean: the negated sum of squared differences); int8: the exact int32 dot product through
+// the scaled epilogue of scan_tc, so that the winning row's score is the hit's score bit for bit
+__global__ void __launch_bounds__(256)
+best_rows(BestRowArgs a) {
+    const uint32_t h = blockIdx.x * 8 + (threadIdx.x >> 5);
+    const int lane = threadIdx.x & 31;
+    if (h >= a.n_hits) return;
+    const uint4 hit = a.hits[h];
+    const uint32_t q = hit.x;
+    const uint32_t m = __ldg(&a.field_mask[q]);
+    uint32_t best = 0xFFFFFFFFu; float best_s = 0.f;
+    for (uint32_t e = hit.y; e < hit.y + hit.z; e++) {
+        const uint32_t row = __ldg(&a.doc_rows[e]);
+        if (m != 0u && ((m >> __ldg(&a.row_field[row])) & 1u) == 0u) continue;
+        float sc;
+        if (a.rows_i8) {
+            const int* rr = reinterpret_cast<const int*>(a.rows_i8 + (size_t)row * a.dpad8);
+            const int* qq = reinterpret_cast<const int*>(a.queries_i8 + (size_t)q * a.dpad8);
+            int di = 0;
+            for (uint32_t i = lane; i < a.dpad8 / 4; i += 32) di = __dp4a(__ldg(&rr[i]), __ldg(&qq[i]), di);
+            for (int o = 16; o; o >>= 1) di += __shfl_xor_sync(FULL, di, o);
+            if (!a.i8_scaled) sc = (float)di;
+            else {
+                if (a.i8_scaled == 3) di = di - a.row_aff[2 * row] * a.q_aff[2 * q + 1] + a.q_aff[2 * q] * a.row_aff[2 * row + 1];
+                const float dotf = __fmul_rn(__fmul_rn((float)di, a.q_scale[q]), a.row_scale[row]);
+                sc = a.i8_scaled >= 2 ? -fmaxf(__fsub_rn(__fadd_rn(a.q_norm[q], a.row_norm[row]), __fmul_rn(2.0f, dotf)), 0.0f) : dotf;
+            }
+        } else {
+            const float* r = a.rows + (size_t)row * a.dpad;
+            const float* qv = a.queries + (size_t)q * a.dpad;
+            float s = 0.f;
+            for (uint32_t i = lane * 4; i < a.dpad; i += 128) {
+                const float4 x = __ldg(reinterpret_cast<const float4*>(r + i)), y = *reinterpret_cast<const float4*>(qv + i);
+                if (a.euclid) {
+                    const float4 d = make_float4(y.x - x.x, y.y - x.y, y.z - x.z, y.w - x.w);
+                    s = dot4(d, d, s);
+                } else s = dot4(x, y, s);
+            }
+            for (int o = 16; o; o >>= 1) s += __shfl_xor_sync(FULL, s, o);
+            sc = a.euclid ? -s : s;
+        }
+        if (sc == sc && (best == 0xFFFFFFFFu || sc > best_s)) { best = row; best_s = sc; }
+    }
+    if (lane == 0) a.best_row[h] = best;
+}
+
 }  // namespace rf
+
+int32_t launch_best_rows(const BestRowArgs& a, cudaStream_t st) {
+    if (a.n_hits == 0) return SSB_OK;
+    rf::best_rows<<<(a.n_hits + 7) / 8, 256, 0, st>>>(a);
+    SSB_CUDA_TRY(cudaGetLastError());
+    return SSB_OK;
+}
 
 size_t refine_scratch_words(int n_sms, uint32_t nq_pad) { return (size_t)nq_pad * (size_t)n_sms * LIST + (nq_pad + 2) / 2 + 1; }
 

@@ -41,7 +41,8 @@ struct ScanArgs {
     const uint32_t* del_slot = nullptr; const uint64_t* del_words = nullptr;   // delete set (null = none): deleted docs never enter a list
     bool sample_groupmax = false;                  // internal (int8): threshold-seeding pass, writes thr_buf instead of lists
     // IVF probe (vec_ivf.cu): selection mask [nq_pad][ivf_words] (bit per (query, cluster)) and each row's cluster id; null = AnnMode::All.
-    // f32 scans only.  Like the delete set it disables the threshold-seeding sample pass (an unselected row must never seed a threshold).
+    // A field mask of a field-tagged index arrives the same way (launch_field_sel: row_cluster = cluster * 32 + field), on the int8 scans
+    // too.  Like the delete set it disables the threshold-seeding sample pass (an unselected row must never seed a threshold).
     const uint32_t* ivf_sel = nullptr; uint32_t ivf_words = 0; const uint32_t* row_cluster = nullptr;
     // filter scan: receives the number of lists per query the scan left unmerged in `scratch` ([nq_pad / NQ][n][NQ][32]) for the refine
     // step to merge (the seeded 256-query pass, one list per query per CTA), or 0 when keys_out holds the merged lists.  Null: always merge.
@@ -93,6 +94,20 @@ struct RefineArgs {
     int n_sms;
     uint64_t* launches;
 };
+// best row of each returned (query, doc) of a field-tagged index (vb field_id / chunk_id, TopK::push vector.rs:436-470): re-score the doc's
+// rows that pass the query's field mask and keep the argmax, the earliest row on equal scores (push replaces only on a strictly better score)
+struct BestRowArgs {
+    uint32_t n_hits;
+    const uint4* hits;                // [n_hits] (query, first CSR entry, row count, -)
+    const uint32_t* doc_rows;         // CSR: the rows of every doc, grouped by doc, ascending (= record order) inside a doc
+    const uint32_t* field_mask; const uint8_t* row_field;   // [nq] masks (0 = none), [n_rows] field ids
+    const float* rows; const float* queries; uint32_t dpad; int euclid;   // f32 index: rows / padded queries (normalised for Cosine)
+    const int8_t* rows_i8 = nullptr; const int8_t* queries_i8 = nullptr; uint32_t dpad8 = 0; int i8_scaled = 0;   // int8 index (ScanArgs)
+    const float* row_scale = nullptr; const float* row_norm = nullptr; const float* q_scale = nullptr; const float* q_norm = nullptr;
+    const int* row_aff = nullptr; const int* q_aff = nullptr;
+    uint32_t* best_row;               // out [n_hits]: the winning row, 0xFFFFFFFF when no row passes
+};
+int32_t launch_best_rows(const BestRowArgs& a, cudaStream_t st);
 // IVF probe: medoid scores + per-(query, level) cluster selection -> sel bits, observed vector counts (vec_ivf.cu)
 struct IvfArgs {
     const float* medoids;             // [n_clusters][dpad] f32 copies of each cluster's first row
@@ -108,6 +123,10 @@ struct IvfArgs {
     uint64_t* launches;
 };
 int32_t launch_ivf_select(const IvfArgs& a, cudaStream_t st);
+// field filter of a field-tagged index, folded into the scans' IVF test: a row's class is cluster * 32 + field (row_cluster of the
+// scans), and out[q][c] holds the fields of cluster c that query q scans — its mask (all 32 bits for mask 0) where the probe selected
+// the cluster (sel = [nq_pad][sel_words] bits, or null = every cluster), else 0.  out: [nq_pad][n_cl]
+int32_t launch_field_sel(const uint32_t* sel, uint32_t sel_words, const uint32_t* fmask, uint32_t nq_pad, uint32_t n_cl, uint32_t* out, cudaStream_t st);
 int32_t launch_gather_rows(const float* src, const uint32_t* idx_dev, uint32_t n, uint32_t dpad, float* dst, cudaStream_t st);
 // re-score the candidates in f32, sort, flag candidate-set overflows; then the exact fallback scan for flagged queries (exits at once when none)
 int32_t launch_refine(const RefineArgs& a, cudaStream_t st);

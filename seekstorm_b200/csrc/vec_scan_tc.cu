@@ -936,7 +936,7 @@ static int32_t launch_tc_n(const ScanArgs& a, cudaStream_t st) {
                                     a.k, a.doc_ids, a.scratch, a.thr_init, a.nq_valid ? a.nq_valid : a.nq_pad, a.ceil_keys, nst,
                                     a.del_slot, a.del_words, a.row_scale, a.row_norm, a.q_scale, a.q_norm,
                                     (const int2*)a.row_aff, (const int2*)a.q_aff,
-                                    PREC == tc::PREC_I8 ? nullptr : a.ivf_sel, a.ivf_words, a.row_cluster,
+                                    a.ivf_sel, a.ivf_words, a.row_cluster,
                                     a.sample_groupmax ? 1u : 0u));
     if (a.ev1) cudaEventRecord(a.ev1, st);
     if (a.sample_groupmax) {   // threshold seeding pass: scratch holds gmax[nq_pad][n_tiles * TROWS / 32]

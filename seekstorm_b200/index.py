@@ -404,6 +404,13 @@ def _hits_array(n):
     return np.zeros(n, dtype=np.dtype([("doc_id", "<u8"), ("score", "<f4"), ("pad", "<u4")]))
 
 
+def vector_field_mask(field_mask: int, n_lexical_fields: int) -> int:
+    """The field filter of the vector search: the reference builds field_filter_set from the indexed lexical fields only
+    (vector.rs:1228-1231), so bits past the lexical fields (or beyond the 32 a mask holds) name no field and are dropped; a mask left
+    empty filters nothing."""
+    return int(field_mask) & ((1 << min(max(int(n_lexical_fields), 0), 32)) - 1)
+
+
 class Index:
     """One shard's GPU-resident mirror: committed lexical levels + vector levels on one H100."""
 
@@ -423,6 +430,7 @@ class Index:
         self.term_key_fn = term_key_fn
         self.indexed_doc_count = 0
         self._keep = []
+        self.vector_fields = False          # vector rows carry field ids (add_vector_level(field_ids=...), load_vector_bin(keep_fields=True))
 
     def close(self):
         if getattr(self, "_h", None) and self._h.value:
@@ -501,11 +509,16 @@ class Index:
         self.indexed_doc_count = n.value
         return n.value
 
-    def load_vector_bin(self, data) -> int:
-        """Load one shard's vector.bin (vector.rs:1066-1094, f32 records).  Returns the number of vectors."""
+    def load_vector_bin(self, data, keep_fields: bool = False) -> int:
+        """Load one shard's vector.bin (vector.rs:1066-1094, f32 records).  Returns the number of vectors.  keep_fields: also keep every
+        record's VectorHeader.field_id / chunk_id (ssb_load_vector_bin_fields): the vector search then applies field filters and
+        reports each hit's best field / chunk."""
         buf = np.frombuffer(data, dtype=np.uint8) if not isinstance(data, np.ndarray) else np.ascontiguousarray(data, dtype=np.uint8)
         n = C.c_uint64(0)
-        check(lib().ssb_load_vector_bin(self._h, buf.ctypes.data, buf.size, C.byref(n)))
+        load = lib().ssb_load_vector_bin_fields if keep_fields else lib().ssb_load_vector_bin
+        check(load(self._h, buf.ctypes.data, buf.size, C.byref(n)))
+        if keep_fields and n.value:
+            self.vector_fields = True
         return n.value
 
     def commit(self, n_docs: int, len_sum_normalized: int):
@@ -772,12 +785,27 @@ class Index:
                 per_field[name] = v
         return merge_facets(per_field, lengths)
 
-    def add_vector_level(self, level_id: int, rows, local_ids=None, cluster_counts=None):
+    def add_vector_level(self, level_id: int, rows, local_ids=None, cluster_counts=None, field_ids=None, chunk_ids=None):
         """rows: [n, dims] f32 (numpy or torch, host or device), n <= 65536.  cluster_counts: the level's IVF cluster table (rows in
-        cluster order, medoid = first row of each cluster; vector.rs:1066-1094) or None = one cluster."""
+        cluster order, medoid = first row of each cluster; vector.rs:1066-1094) or None = one cluster.  field_ids (u8, < 32) / chunk_ids
+        (u32): each row's indexed field and chunk (multi-vector documents, ssb_vector_add_level_fields) — every level of an index carries
+        them or none does."""
         n, dims = int(rows.shape[0]), int(rows.shape[1])
         stride = rows.strides[0] // 4 if isinstance(rows, np.ndarray) else rows.stride(0)
-        if cluster_counts is None:
+        if field_ids is not None or chunk_ids is not None:
+            if field_ids is None or chunk_ids is None:
+                raise ValueError("field_ids and chunk_ids go together")
+            fi = np.ascontiguousarray(field_ids, dtype=np.uint8)
+            ci = np.ascontiguousarray(chunk_ids, dtype=np.uint32)
+            if fi.size != n or ci.size != n:
+                raise ValueError("field_ids / chunk_ids need one entry per row")
+            cc = None if cluster_counts is None else np.ascontiguousarray(cluster_counts, dtype=np.uint32)
+            check(lib().ssb_vector_add_level_fields(self._h, level_id, _addr(rows), stride, _addr(local_ids), n, dims,
+                                                    None if cc is None else cc.ctypes.data, 0 if cc is None else len(cc),
+                                                    fi.ctypes.data, ci.ctypes.data))
+            if n:
+                self.vector_fields = True
+        elif cluster_counts is None:
             check(lib().ssb_vector_add_level(self._h, level_id, _addr(rows), stride, _addr(local_ids), n, dims))
         else:
             cc = np.ascontiguousarray(cluster_counts, dtype=np.uint32)
@@ -973,9 +1001,11 @@ class Index:
         return _hits_array(n)
 
     def search_vector_ex(self, queries, k: int, similarity_threshold=None, int8_queries: bool = False, ann_mode: int = 0, n_probe: int = 0,
-                         cluster_threshold: float = 0.0):
+                         cluster_threshold: float = 0.0, field_masks=None):
         """ssb_search_vector_ex: threshold (vector.rs:388-399), int8 query codes, vb result fields, observed_vector_count.
-        Returns (hits per query, ext structured array [nq, k], observed [nq])."""
+        field_masks: per query a bitmask of indexed fields (0 = no filter; ssb_search_vector_fields) — needs field-tagged rows.
+        Returns (hits per query, ext structured array [nq, k], observed [nq]); on a field-tagged index ext carries each hit's best
+        field_id / chunk_id."""
         from ._lib import SsbHitExt, SsbVecQuery
         nq = int(queries.shape[0])
         if isinstance(queries, np.ndarray):
@@ -986,16 +1016,25 @@ class Index:
         observed = np.zeros(max(nq, 1), dtype=np.uint64)
         vq = SsbVecQuery(_addr(queries), nq, k, 1 if int8_queries else 0, 0 if similarity_threshold is None else 1,
                          0.0 if similarity_threshold is None else float(similarity_threshold), int(ann_mode), int(n_probe), float(cluster_threshold))
-        check(lib().ssb_search_vector_ex(self._h, C.byref(vq), hits.ctypes.data, n_hits.ctypes.data, C.addressof(ext), observed.ctypes.data))
+        if field_masks is None:
+            check(lib().ssb_search_vector_ex(self._h, C.byref(vq), hits.ctypes.data, n_hits.ctypes.data, C.addressof(ext), observed.ctypes.data))
+        else:
+            fm = np.ascontiguousarray(np.asarray(list(field_masks), dtype=np.uint32))
+            if fm.size != nq:
+                raise ValueError("field_masks needs one mask per query")
+            check(lib().ssb_search_vector_fields(self._h, C.byref(vq), fm.ctypes.data, hits.ctypes.data, n_hits.ctypes.data, C.addressof(ext),
+                                                 observed.ctypes.data))
         out = []
         for i in range(nq):
             h = hits[i * k: i * k + int(n_hits[i])]
             out.append([(int(d), float(s)) for d, s in zip(h["doc_id"], h["score"])])
         return out, ext, observed[:nq]
 
-    def search_hybrid_batch(self, queries_keys, query_type: QueryType, queries, k: int):
+    def search_hybrid_batch(self, queries_keys, query_type: QueryType, queries, k: int, field_masks=None):
+        """ssb_search_hybrid.  field_masks: per query a bitmask of indexed fields (0 = none) — the lexical half's field filter, and the
+        vector half's too when the vector rows carry field ids."""
         nq = len(queries_keys)
-        b, keep = self._lex_batch(queries_keys, query_type)
+        b, keep = self._lex_batch(queries_keys, query_type, field_masks=field_masks)
         if isinstance(queries, np.ndarray):
             queries = np.ascontiguousarray(queries, dtype=np.float32)
         hits = _hits_array(max(nq * k, 1))
@@ -1063,6 +1102,11 @@ class Index:
         the result type is Topk (search.rs:1748).
         enable_empty_query with query_string "" and no query_vector (Lexical mode): every live doc through facet_filter, result_sort and
         the paging, the index-wide String facet counts in `facets` (_search_empty).
+        field_filter: names (or indices) of indexed lexical fields (field_names).  It filters the lexical search, and the vector search
+        when the vector rows carry field ids (add_vector_level(field_ids=...), load_vector_bin(keep_fields=True)): a row counts only if its
+        field is in the filter, as the reference builds the filter from the lexical fields alone (vector.rs:1228-1231).  A filter that names
+        no indexed field — an index past the lexical fields, or no lexical fields at all — filters no vector row (vector_field_mask); on a
+        vector index without field ids the vector search is unfiltered.
         Unsupported reference features (facet counts of vector-only queries or of an empty query without enable_empty_query, sorting
         vector / hybrid results, a base on a non-Point facet, uncommitted, rewriting) raise NotImplementedError rather than being silently
         ignored."""
@@ -1138,8 +1182,11 @@ class Index:
             qv = np.asarray(query_vector, dtype=np.float32).reshape(1, -1)
             # similarity_threshold (TopK::new, vector.rs:388-399) and observed_vector_count are handled behind the C-ABI
             am = search_mode.ann_mode or AnnMode.All
+            # field_filter on the vector rows (vector.rs:1226-1238): only on an index whose rows carry field ids
+            vm = vector_field_mask(fmask, len(getattr(self, "field_names", [])))
+            vmask = [vm] if vm and self.vector_fields else None
             res, _, observed = self.search_vector_ex(qv, max(heap, 1), search_mode.similarity_threshold, ann_mode=am.kind, n_probe=am.n_probe,
-                                                     cluster_threshold=am.threshold)
+                                                     cluster_threshold=am.threshold, field_masks=vmask)
             vec = res[0][:heap]
             ro.observed_vector_count = int(observed[0])
         if search_mode.kind == "Lexical":
