@@ -1,5 +1,5 @@
-// api.cu — the extern "C" ABI of libseekstorm_b200.so (include/seekstorm_b200.h): handle, vector index
-// storage, search entry points, hybrid RRF, key decoding.  No torch types; CUDA runtime only.
+// api.cu — the extern "C" ABI of libseekstorm_b200.so (include/seekstorm_b200.h): handle, search-context pool, search entry
+// points with their paging, hybrid RRF, shard merge.  No torch types; CUDA runtime only.
 #include <stdarg.h>
 #include <string.h>
 #include <algorithm>
@@ -14,7 +14,7 @@
 #include "bm25.h"
 #include "comm.h"
 #include "common.cuh"
-#include "vec_scan.h"
+#include "vec_index.h"
 
 namespace ssb {
 
@@ -67,14 +67,11 @@ struct SearchCtx {
     cudaStream_t st = nullptr;       // stream this context launches on (its own, or the caller's after ssb_set_stream)
     cudaStream_t own_st = nullptr;
     LexWorkspace lex;
-    DevBuf<float> qpad, qstage, qhi, qlo, q_scale, q_norm; DevBuf<int8_t> q_i8; DevBuf<int> q_aff;
-    DevBuf<uint64_t> ceil, scratch, keys_a, keys_b, counts, gather;
-    DevBuf<float> ivf_scores; DevBuf<uint32_t> ivf_sel; DevBuf<uint64_t> ivf_obs; std::vector<uint64_t> h_obs;   // IVF probe (vec_ivf.cu)
-    DevBuf<uint32_t> fmask, fsel, best; std::vector<uint32_t> h_best;   // field filter: per-query masks, per (query, cluster) fields; best-row step
+    VecWorkspace vec;
+    DevBuf<uint64_t> ceil, keys_a, keys_b, counts, gather;   // paging ceilings, result pages, counts, shard all-gather
     std::vector<uint64_t> h_ceil, h_keys_a, h_keys_b, h_counts;
     ssb_stats stats{};
     cudaEvent_t ev0 = nullptr, ev1 = nullptr; bool ev_used = false, last_lex = false;
-    const uint32_t* fb_state = nullptr;   // filter scan of the current call: device count of queries that took the exact fallback
     ~SearchCtx() {
         if (own_st) cudaStreamSynchronize(own_st);
         if (ev0) cudaEventDestroy(ev0);
@@ -86,7 +83,7 @@ struct SearchCtx {
 constexpr size_t SSB_MAX_CTX = 16;
 
 struct ssb_index {
-    ssb_config cfg;
+    int device = 0;
     int n_sms = 0;
     cudaStream_t load_st = nullptr;   // load-time stream (add_level / commit)
     // searches hold `rw` shared, index mutation exclusive (mirrors the reference's RwLock around the shard, commit.rs:142)
@@ -96,39 +93,10 @@ struct ssb_index {
     bool ext_stream_set = false; cudaStream_t ext_stream = nullptr;   // ssb_set_stream: every search runs on the caller's stream (one context)
     std::mutex stats_mu; SearchCtx* last_ctx = nullptr; ssb_stats last_stats{};
     LexIndex* lex = nullptr;
+    VecIndex vec;
     DeleteSet del;                    // shard.delete_hashset mirrored on the device (ssb_set_deleted)
     FacetSet facets;                  // the shard's facet file as one key column per facet (ssb_set_facets)
     ShardComm comm;                   // set: this handle is one shard of a `world`-way sharded index (one process per GPU)
-    // vector index
-    uint32_t dims = 0, dpad = 0, dpad8 = 0;
-    bool quant_i8 = false;            // ScalarQuantizationI8 / TurboQuantI8: int8 corpus, exact int32 dot products
-    bool turbo = false;               // TurboQuantI8: rows and queries are sign-flipped, FWHT-rotated and quantised at tq_dim = next_pow2(dims)
-    uint32_t tq_dim = 0; float* tq_mask = nullptr;   // the index's seed mask (+-1), ssb_vector_set_turboquant_mask
-    bool dup_docs = false;            // some doc id occurs on more than one vector row (multi-chunk documents): results are de-duplicated
-    DevBuf<float> rows;
-    DevBuf<uint16_t> rows_hi, rows_lo;   // bf16 planes of `rows` (hi = bf16_rn(x), lo = bf16_rn(x - hi)): what the tensor-core bf16 scan streams
-    DevBuf<int8_t> rows_i8;
-    DevBuf<float> row_scale, row_norm;   // Dot / Euclidean + ScalarQuantizationI8: per-vector scale (and norm), QuantizedVector vector_similarity.rs:1340-1371
-    // Euclidean + ScalarQuantizationI8 over integer-valued 0..255 data: the AFFINE quantiser (new_scale_norm_affine, vector_similarity.rs:1414-1463)
-    bool affine = false; float aff_min = 3.402823466e+38f /* f32::MAX */, aff_max = -3.402823466e+38f /* f32::MIN */;   // shard.min / max_vector_value
-    DevBuf<int> row_aff;                 // int2 per row: (zero_point, dims * zero_point - sum_q)
-    DevBuf<uint32_t> doc_ids;
-    DevBuf<uint16_t> rows_h16;        // filter scan: fp16 plane half_rn(rows * vec_scale)
-    DevBuf<uint32_t> vec_err;         // filter scan: {max_r |a_r*scale - h_r|, max_r |h_r|, scratch} as f32 bits (launch_rows_f16_err)
-    float vec_scale = 0.f;            // power of two; 0 = not chosen yet (first add_level)
-    // IVF cluster tables (vector.rs:1066-1094; f32 indexes): one entry per add call ("level"), clusters numbered across levels
-    DevBuf<float> medoids; DevBuf<uint32_t> row_cluster, cl_count, lvl_begin;
-    std::vector<uint32_t> h_lvl_begin; uint32_t n_clusters = 0, max_level_clusters = 0;
-    // multi-vector documents (ssb_vector_add_level_fields; VectorHeader.field_id / chunk_id, vector.rs:62-73): every level carries them or
-    // none does.  row_field: the byte the best-row step tests; row_class: cluster * 32 + field, what the scans' IVF test reads under a field
-    // mask (int8 indexes: one cluster); h_field / h_chunk: what the best-row step reports; field_rows / cl_field_rows: rows per field, and
-    // per (cluster, field) on f32 indexes, for observed_vector_count under a mask.  doc_rows (device) lists every doc's rows in record
-    // order, grouped by doc; doc_key / doc_off (host) index it.
-    int tagged = -1;                  // -1: no vector level yet, 0: untagged, 1: field-tagged
-    DevBuf<uint8_t> row_field; DevBuf<uint32_t> row_class; std::vector<uint8_t> h_field; std::vector<uint32_t> h_chunk;
-    uint64_t field_rows[32] = {}; std::vector<uint32_t> cl_field_rows;   // [n_clusters][32]
-    DevBuf<uint32_t> doc_rows; std::vector<uint64_t> doc_pairs /*(doc << 32) | row, sorted*/; std::vector<uint32_t> doc_key, doc_off;
-    uint64_t n_rows = 0;
 };
 
 namespace {
@@ -150,7 +118,7 @@ struct CtxLease {
                 if (!n) { set_error("out of host memory"); return SSB_E_NOMEM; }
                 if (cudaStreamCreateWithFlags(&n->own_st, cudaStreamNonBlocking) != cudaSuccess) { cudaGetLastError(); set_error("stream create failed"); return SSB_E_CUDA; }
                 cudaEventCreate(&n->ev0); cudaEventCreate(&n->ev1);
-                n->lex.ev0 = n->ev0; n->lex.ev1 = n->ev1;
+                n->lex.ev0 = n->vec.ev0 = n->ev0; n->lex.ev1 = n->vec.ev1 = n->ev1;
                 c = n.get(); ix->pool.push_back(std::move(n));
                 break;
             }
@@ -158,7 +126,7 @@ struct CtxLease {
             ix->pool_cv.wait(g);
         }
         c->st = ix->ext_stream_set ? ix->ext_stream : c->own_st;
-        c->stats = ssb_stats{}; c->ev_used = false; c->last_lex = false; c->fb_state = nullptr;
+        c->stats = ssb_stats{}; c->ev_used = false; c->last_lex = false; c->vec.fb_state = nullptr;
         return SSB_OK;
     }
     ~CtxLease() {
@@ -175,176 +143,6 @@ struct CtxLease {
     } catch (const std::bad_alloc&) { cudaGetLastError(); set_error("out of memory (host or device)"); return SSB_E_NOMEM; \
     } catch (const std::exception& e) { cudaGetLastError(); set_error("internal error: %s", e.what()); return SSB_E_CUDA;   \
     } catch (...) { cudaGetLastError(); set_error("internal error: unknown exception"); return SSB_E_CUDA; }
-
-}  // namespace
-
-namespace {
-
-struct IvfQuery { uint32_t mode, n_probe; float thr; };   // AnnMode of one call (thr pre-mapped, vector.rs:388-399)
-
-int32_t vec_keys(ssb_index* ix, SearchCtx& c, const void* queries, bool queries_i8, uint32_t nq, uint32_t k, uint64_t* keys_out_dev /*[nq][32]*/,
-                 const uint64_t* ceil_dev = nullptr /*[>= nq_pad] paging ceilings*/, const IvfQuery* ivf = nullptr /*null = AnnMode::All*/,
-                 const uint32_t* fmask_host = nullptr /*[nq] field masks of a field-tagged index, or null: no query has one*/) {
-    if (ivf && (ix->quant_i8 || !ix->medoids.p)) { set_error("AnnMode other than All needs an f32 vector index"); return SSB_E_UNSUPPORTED; }
-    if (ix->dims == 0) { set_error("no vector index configured (vector_dims = 0)"); return SSB_E_STATE; }
-    if (k == 0 || k > SSB_K_MAX) { set_error("k must be in 1..%u", SSB_K_MAX); return SSB_E_UNSUPPORTED; }
-    if (queries_i8 && !ix->quant_i8) { set_error("int8 queries need a ScalarQuantizationI8 index"); return SSB_E_INVALID; }
-    if (nq == 0) return SSB_OK;
-    const vec::Scan scan = vec::plan_scan(ix->cfg.vector_kernel, ix->cfg.vector_similarity, ix->quant_i8, ix->rows_h16.p && ix->vec_err.p, nq, k,
-                                          ceil_dev != nullptr);
-    const bool filter = vec::is_filter(scan);
-    const uint32_t passes = (nq + vec::queries_per_pass(scan) - 1) / vec::queries_per_pass(scan);   // corpus passes of the scan
-    const uint32_t nq_pad = passes * vec::queries_per_pass(scan);
-    cudaStream_t st = c.st;
-    if (scan != vec::Scan::I8_128) SSB_TRY(c.qpad.reserve((size_t)nq_pad * ix->dpad, 0, st));
-    const size_t qbytes = (size_t)nq * ix->dims * (queries_i8 ? 1 : 4);
-    const void* qsrc = queries;
-    if (!is_device_ptr(queries)) {
-        SSB_TRY(c.qstage.reserve(((size_t)nq * ix->dims + 3) / (queries_i8 ? 4 : 1) + 1, 0, st));
-        SSB_CUDA_TRY(cudaMemcpyAsync(c.qstage.p, queries, qbytes, cudaMemcpyHostToDevice, st));
-        c.stats.h2d_bytes += qbytes;
-        qsrc = c.qstage.p;
-    }
-    if (scan == vec::Scan::I8_128) {
-        SSB_TRY(c.q_i8.reserve((size_t)nq_pad * ix->dpad8, 0, st));
-        if (queries_i8 && (ix->turbo || ix->cfg.vector_similarity != SSB_SIM_COSINE)) { set_error("int8 query codes are accepted for Cosine + ScalarQuantizationI8 only (the other quantisers need the query scale)"); return SSB_E_UNSUPPORTED; }
-        if (ix->turbo) {
-            // the query goes through the same TurboQuant as the rows (search.rs:1545-1556, 1592-1602).  Dot / Cosine: the reference's score is
-            // -(dot * query_scale * row_scale) (vector_similarity.rs:161-176): the NEGATED query scale through the scaled epilogue is exactly that
-            SSB_TRY(c.q_scale.reserve(nq_pad, 0, st)); SSB_TRY(c.q_norm.reserve(nq_pad, 0, st));
-            SSB_TRY(vec::launch_quantize_rows_turbo_i8((const float*)qsrc, ix->dims, nq, nq_pad, ix->dims, ix->tq_dim, ix->tq_mask, c.q_i8.p, ix->dpad8, c.q_scale.p,
-                                                       c.q_norm.p, ix->cfg.vector_similarity == SSB_SIM_COSINE, ix->cfg.vector_similarity != SSB_SIM_EUCLIDEAN, st));
-        } else if (ix->affine) {
-            // affine Euclidean: the query is quantised with a COPY of the shard's (min, max) state (search.rs:1514-1530, 1562-1580)
-            SSB_TRY(c.q_scale.reserve(nq_pad, 0, st)); SSB_TRY(c.q_norm.reserve(nq_pad, 0, st)); SSB_TRY(c.q_aff.reserve((size_t)nq_pad * 2, 0, st));
-            SSB_TRY(vec::launch_quantize_rows_affine_i8((const float*)qsrc, ix->dims, nq, nq_pad, ix->dims, nullptr, nullptr, ix->aff_min, ix->aff_max, c.q_i8.p, ix->dpad8,
-                                                        c.q_scale.p, c.q_norm.p, c.q_aff.p, 1, st));
-        } else if (ix->cfg.vector_similarity != SSB_SIM_COSINE) {
-            // Dot / Euclidean: the query goes through the same QuantizedVector::new_scale[_norm] as the rows (search.rs:1499-1530)
-            SSB_TRY(c.q_scale.reserve(nq_pad, 0, st)); SSB_TRY(c.q_norm.reserve(nq_pad, 0, st));
-            SSB_TRY(vec::launch_quantize_rows_scale_i8((const float*)qsrc, ix->dims, nq, nq_pad, ix->dims, c.q_i8.p, ix->dpad8, c.q_scale.p, c.q_norm.p,
-                                                       ix->cfg.vector_similarity == SSB_SIM_EUCLIDEAN, st));
-        } else if (queries_i8) {
-            // the caller already ran normalize + quantize_f32_to_i8 (what the reference's server holds after search.rs:1477-1490): pad only
-            SSB_CUDA_TRY(cudaMemsetAsync(c.q_i8.p, 0, (size_t)nq_pad * ix->dpad8, st));
-            SSB_CUDA_TRY(cudaMemcpy2DAsync(c.q_i8.p, ix->dpad8, qsrc, ix->dims, ix->dims, nq, cudaMemcpyDeviceToDevice, st));
-        } else {
-            // the query is normalised and quantised exactly like the corpus (search.rs:1464-1475, vector_similarity.rs:1226-1232)
-            SSB_TRY(vec::launch_quantize_rows_i8((const float*)qsrc, ix->dims, nq, nq_pad, ix->dims, c.q_i8.p, ix->dpad8, st));
-        }
-    } else if (filter || scan == vec::Scan::Bf16_64 || scan == vec::Scan::Bf16_128 || scan == vec::Scan::Bf16_256) {
-        // one launch: pad + normalise + bf16 hi/lo split (the scan reads only the split parts)
-        SSB_TRY(c.qhi.reserve((size_t)nq_pad * ix->dpad, 0, st));
-        SSB_TRY(c.qlo.reserve((size_t)nq_pad * ix->dpad, 0, st));
-        if (filter) SSB_TRY(c.q_scale.reserve(nq_pad, 0, st));   // per-query margins 2 eps_q
-        SSB_TRY(vec::launch_prep_split_queries_bf16((const float*)qsrc, nq, ix->dims, ix->dims, c.qhi.p, c.qlo.p, nq_pad, ix->dpad,
-                                                    ix->cfg.vector_similarity == SSB_SIM_COSINE, st, (filter || ivf) ? c.qpad.p : nullptr,
-                                                    filter ? c.q_scale.p : nullptr, filter ? ix->vec_err.p : nullptr));
-    } else
-    SSB_TRY(vec::launch_prep_queries((const float*)qsrc, nq, ix->dims, ix->dims, c.qpad.p, nq_pad, ix->dpad,
-                                     ix->cfg.vector_similarity == SSB_SIM_COSINE, st));
-    c.stats.kernel_launches += 1;
-    if (ix->n_rows == 0) { SSB_CUDA_TRY(cudaMemsetAsync(keys_out_dev, 0, (size_t)nq * LIST * 8, st)); return SSB_OK; }
-    size_t sb = vec::is_tensor_core(scan) ? vec::scan_tc_scratch_bytes(ix->n_sms, nq_pad) : vec::scan_scratch_bytes(ix->n_sms, nq_pad);
-    const size_t head_words = sb / 8 + (size_t)nq_pad * LIST + (nq_pad + 1) / 2;
-    SSB_TRY(c.scratch.reserve(head_words + (filter ? vec::refine_scratch_words(ix->n_sms, nq_pad) : 0), 0, st));
-    vec::ScanArgs a{};
-    a.rows = ix->rows.p; a.rows_hi = ix->rows_hi.p; a.rows_lo = ix->rows_lo.p; a.rows_h16 = ix->rows_h16.p; a.doc_ids = ix->doc_ids.p; a.n_rows = ix->n_rows; a.dpad = ix->dpad; a.queries_padded = c.qpad.p;
-    a.nq_pad = nq_pad; a.nq_valid = nq; a.k = k; a.similarity = ix->cfg.vector_similarity; a.n_sms = ix->n_sms;
-    a.scratch = c.scratch.p; a.scratch_bytes = sb;
-    uint64_t* merged = c.scratch.p + sb / 8;   // [nq_pad][32]
-    a.keys_out = merged; a.ev0 = c.ev0; a.ev1 = c.ev1; c.ev_used = true;
-    a.thr_buf = reinterpret_cast<uint32_t*>(merged + (size_t)nq_pad * LIST);
-    a.ceil_keys = ceil_dev;
-    if (ix->del.n) { a.del_slot = ix->del.d_slot; a.del_words = ix->del.d_words; }
-    a.launches = &c.stats.kernel_launches;
-    uint32_t unmerged = 0;
-    if (filter) a.unmerged_lists = &unmerged;
-    if (ivf) {
-        // cluster probe: medoid scores, per-(query, level) selection -> one bit per (query, cluster); the scans test it per candidate
-        vec::IvfArgs v{};
-        v.medoids = ix->medoids.p; v.lvl_begin = ix->lvl_begin.p; v.cl_count = ix->cl_count.p;
-        v.n_clusters = ix->n_clusters; v.n_levels = (uint32_t)ix->h_lvl_begin.size(); v.max_level_clusters = ix->max_level_clusters;
-        v.queries_padded = c.qpad.p; v.nq = nq; v.nq_pad = nq_pad; v.dpad = ix->dpad; v.similarity = ix->cfg.vector_similarity;
-        v.ann_mode = ivf->mode; v.n_probe = ivf->n_probe; v.cluster_threshold = ivf->thr;
-        v.words = (ix->n_clusters + 31) / 32;
-        SSB_TRY(c.ivf_scores.reserve((size_t)nq * ix->n_clusters, 0, st));
-        SSB_TRY(c.ivf_sel.reserve((size_t)nq_pad * v.words, 0, st));
-        SSB_TRY(c.ivf_obs.reserve(nq, 0, st));
-        v.scores = c.ivf_scores.p; v.sel = c.ivf_sel.p; v.observed = c.ivf_obs.p; v.launches = &c.stats.kernel_launches;
-        SSB_TRY(vec::launch_ivf_select(v, st));
-        a.ivf_sel = c.ivf_sel.p; a.ivf_words = v.words; a.row_cluster = ix->row_cluster.p;
-    }
-    if (fmask_host) {
-        // field filter (vector.rs:1226-1238): folded into the scans' per-candidate IVF test — a row's class is cluster * 32 + field and
-        // the selection holds, per (query, cluster), the fields the query scans.  Like the IVF mask it turns the threshold seed off.
-        const uint32_t n_cl = ix->quant_i8 ? 1u : ix->n_clusters;
-        SSB_TRY(c.fmask.reserve(nq_pad, 0, st));
-        SSB_TRY(c.fsel.reserve((size_t)nq_pad * n_cl, 0, st));
-        SSB_CUDA_TRY(cudaMemsetAsync(c.fmask.p, 0, (size_t)nq_pad * 4, st));   // padding queries: no filter (they collect nothing anyway)
-        SSB_CUDA_TRY(cudaMemcpyAsync(c.fmask.p, fmask_host, (size_t)nq * 4, cudaMemcpyHostToDevice, st));
-        c.stats.h2d_bytes += (uint64_t)nq * 4;
-        SSB_TRY(vec::launch_field_sel(a.ivf_sel, a.ivf_words, c.fmask.p, nq_pad, n_cl, c.fsel.p, st));
-        c.stats.kernel_launches += 1;
-        a.ivf_sel = c.fsel.p; a.ivf_words = n_cl; a.row_cluster = ix->row_class.p;
-    }
-    if (scan == vec::Scan::I8_128) {
-        a.rows_i8 = ix->rows_i8.p; a.queries_i8 = c.q_i8.p; a.dpad8 = ix->dpad8;
-        if (ix->turbo || ix->cfg.vector_similarity != SSB_SIM_COSINE) {
-            a.i8_scaled = ix->cfg.vector_similarity == SSB_SIM_EUCLIDEAN ? (ix->affine ? 3 : 2) : 1;
-            a.row_aff = ix->row_aff.p; a.q_aff = c.q_aff.p;
-            a.row_scale = ix->row_scale.p; a.row_norm = ix->row_norm.p; a.q_scale = c.q_scale.p; a.q_norm = c.q_norm.p;
-        }
-    } else if (vec::is_tensor_core(scan)) {
-        SSB_TRY(c.qhi.reserve((size_t)nq_pad * ix->dpad, 0, st));
-        SSB_TRY(c.qlo.reserve((size_t)nq_pad * ix->dpad, 0, st));
-        a.q_hi = c.qhi.p; a.q_lo = c.qlo.p;
-        if (filter) a.q_scale = c.q_scale.p;
-    }
-    SSB_TRY(vec::is_tensor_core(scan) ? vec::launch_scan_tc(a, scan, st) : vec::launch_scan_ffma(a, st));
-    if (filter) {
-        vec::RefineArgs r{};
-        r.rows = ix->rows.p; r.doc_ids = ix->doc_ids.p; r.n_rows = ix->n_rows; r.dpad = ix->dpad; r.queries_padded = c.qpad.p; r.margin = c.q_scale.p;
-        r.keys = merged; r.keys_out = keys_out_dev;   // the refine step writes the caller's buffer directly
-        if (unmerged) { r.lists = a.scratch; r.n_lists = unmerged; r.qt = vec::queries_per_pass(scan); }   // seeded 256-query pass: merged in the refine step
-        r.nq = nq; r.nq_pad = nq_pad; r.k = k;
-        r.fb_lists = c.scratch.p + head_words;
-        r.fb_state = reinterpret_cast<uint32_t*>(r.fb_lists + (size_t)nq_pad * ix->n_sms * LIST);
-        r.del_slot = a.del_slot; r.del_words = a.del_words; r.ivf_sel = a.ivf_sel; r.ivf_words = a.ivf_words; r.row_cluster = a.row_cluster; r.n_sms = ix->n_sms; r.launches = &c.stats.kernel_launches;
-        SSB_TRY(vec::launch_refine(r, st));
-        c.fb_state = r.fb_state;
-    } else {
-        SSB_CUDA_TRY(cudaMemcpyAsync(keys_out_dev, merged, (size_t)nq * LIST * 8, cudaMemcpyDeviceToDevice, st));
-    }
-    const uint64_t pass_bytes = ix->n_rows * ix->dims * (scan == vec::Scan::I8_128 ? 1 : 4);   // algorithmic bytes of one corpus pass
-    c.stats.algorithmic_bytes += passes * pass_bytes;
-    // bytes the scan kernel actually streams per call: the filter scan reads the 2-byte fp16 plane (half the f32 bytes), the refine step
-    // <= 32 f32 rows per query
-    c.stats.scan_bytes_read += filter ? passes * pass_bytes / 2 + (uint64_t)nq * LIST * ix->dims * 4 : passes * pass_bytes;
-    return SSB_OK;
-}
-
-// keys of one query -> hits; `dedup`: keep only the best-scoring row of a doc id (TopK::push, vector.rs:436-470)
-uint32_t decode_list(const uint64_t* keys, uint32_t k, ssb_hit* hits, bool dedup) {
-    uint32_t n = 0;
-    for (uint32_t j = 0; j < LIST && n < k; j++) {
-        const uint64_t key = keys[j];
-        if (!key) break;
-        const uint64_t doc = key_doc(key);
-        if (dedup) { bool seen = false; for (uint32_t i = 0; i < n; i++) seen = seen || hits[i].doc_id == doc; if (seen) continue; }
-        hits[n].doc_id = doc; hits[n].score = key_score(key); hits[n].pad = 0;
-        n++;
-    }
-    return n;
-}
-
-void decode_keys(const uint64_t* keys, uint32_t nq, uint32_t k, ssb_hit* hits, uint32_t* n_hits, bool dedup = false) {
-    for (uint32_t q = 0; q < nq; q++) {
-        const uint32_t n = decode_list(keys + (size_t)q * LIST, k, hits + (size_t)q * k, dedup);
-        for (uint32_t j = n; j < k; j++) { hits[(size_t)q * k + j].doc_id = 0; hits[(size_t)q * k + j].score = 0.f; hits[(size_t)q * k + j].pad = 0; }
-        if (n_hits) n_hits[q] = n;
-    }
-}
 
 // Sharded index: all-gather every rank's [nq][32] key lists and merge them (G*k -> k with the canonical tie rule; the reference
 // concatenates the shard results and sorts, search.rs:1875-1928, 2097-2106).  In place; identical result on every rank.
@@ -426,6 +224,14 @@ struct PageState {
     }
 };
 
+// Field-tagged vector rows and a sharded handle exclude each other (the field filter and the best-row step are not built across
+// shards): refused when such rows are added to a sharded handle (what = "rows") and when a handle holding them is sharded ("vector rows")
+int32_t refuse_tagged_sharded(const char* who, const char* what, bool tagged, bool sharded) {
+    if (!tagged || !sharded) return SSB_OK;
+    set_error("%s: field-tagged %s on a sharded index are not supported", who, what);
+    return SSB_E_UNSUPPORTED;
+}
+
 inline bool hit_better(const ssb_hit& a, const ssb_hit& b) { return a.score > b.score || (a.score == b.score && a.doc_id < b.doc_id); }
 
 void finish_stats(ssb_index* ix, SearchCtx& c) {
@@ -437,131 +243,56 @@ void finish_stats(ssb_index* ix, SearchCtx& c) {
     }
 }
 
-// host-facing vector search: paging beyond 32 results, de-duplication, optional threshold
-int32_t search_vector_host(ssb_index* ix, SearchCtx& c, const void* queries, bool queries_i8, uint32_t nq, uint32_t k, ssb_hit* hits, uint32_t* n_hits,
-                           const IvfQuery* ivf = nullptr, const uint32_t* fmask_host = nullptr) {
-    SSB_TRY(c.keys_a.reserve((size_t)nq * LIST, 0, c.st));
-    c.h_keys_a.resize((size_t)nq * LIST);
-    PageState<1> ps(c, nq, k, hits, n_hits, ix->dup_docs);
-    // the fused kernels keep 32 results per query; longer result lists are produced page by page, each page restricted to
-    // keys strictly below the last key of the previous one (keys are a total order on (score desc, doc id asc))
-    uint32_t kk = ix->dup_docs ? SSB_K_MAX : (k < SSB_K_MAX ? k : SSB_K_MAX);
-    for (uint32_t page = 0; page < 4096; page++) {
-        SSB_TRY(vec_keys(ix, c, queries, queries_i8, nq, kk, c.keys_a.p, page ? c.ceil.p : nullptr, ivf, fmask_host));
-        SSB_TRY(shard_merge(ix, c, c.keys_a.p, nq));
-        if (ivf && page == 0) {   // observed_vector_count = the vectors of the selected clusters (summed over the shards)
-            SSB_TRY(shard_sum_counts(ix, c, c.ivf_obs.p, nq));
-            c.h_obs.resize(nq);
-            SSB_CUDA_TRY(cudaMemcpyAsync(c.h_obs.data(), c.ivf_obs.p, (size_t)nq * 8, cudaMemcpyDeviceToHost, c.st));
-        }
-        SSB_CUDA_TRY(cudaMemcpyAsync(c.h_keys_a.data(), c.keys_a.p, (size_t)nq * LIST * 8, cudaMemcpyDeviceToHost, c.st));
-        uint32_t n_fb = 0;
-        if (c.fb_state) SSB_CUDA_TRY(cudaMemcpyAsync(&n_fb, c.fb_state, 4, cudaMemcpyDeviceToHost, c.st));
-        SSB_CUDA_TRY(cudaStreamSynchronize(c.st));
-        c.stats.filter_fallbacks += n_fb;
-        c.stats.d2h_bytes += (uint64_t)nq * LIST * 8;
-        if (!ps.append(c.h_keys_a.data(), kk)) break;
-        kk = ps.next_page_k();
+// read back the page the last fetch left in c.keys_a ([nq][32] keys of W words); with it, after a vector filter scan, the count of
+// queries that took the exact fallback
+template <int W>
+int32_t read_page(SearchCtx& c, uint32_t nq) {
+    SSB_CUDA_TRY(cudaMemcpyAsync(c.h_keys_a.data(), c.keys_a.p, (size_t)nq * LIST * W * 8, cudaMemcpyDeviceToHost, c.st));
+    uint32_t n_fb = 0;
+    if (c.vec.fb_state) SSB_CUDA_TRY(cudaMemcpyAsync(&n_fb, c.vec.fb_state, 4, cudaMemcpyDeviceToHost, c.st));
+    SSB_CUDA_TRY(cudaStreamSynchronize(c.st));
+    c.stats.filter_fallbacks += n_fb;
+    c.stats.d2h_bytes += (uint64_t)nq * LIST * W * 8;
+    return SSB_OK;
+}
+
+// The pages after the first one of a host-facing search (k > SSB_K_MAX, or de-duplication): the first page, read back with k1 results
+// per query, is appended; then, while a query wants more, fetch(kk) enqueues into c.keys_a the next kk keys per query strictly below
+// the ceilings in c.ceil (the last key of the previous page: keys are a total order).  At most 4096 pages in all.
+template <int W, class Fetch>
+int32_t page_rest(SearchCtx& c, PageState<W>& ps, uint32_t k1, Fetch fetch) {
+    bool more = ps.append(c.h_keys_a.data(), k1);
+    for (uint32_t page = 1; more && page < 4096; page++) {
+        const uint32_t kk = ps.next_page_k();
         SSB_TRY(ps.upload_ceilings());
+        SSB_TRY(fetch(kk));
+        SSB_TRY(read_page<W>(c, ps.nq));
+        more = ps.append(c.h_keys_a.data(), kk);
     }
     ps.finish();
     return SSB_OK;
 }
 
-// field masks of a vector search (HOST array [nq], bit f = indexed field f, 0 = no filter; the bits of ssb_lex_batch.field_masks).
-// *use = the array when some query has a mask, else null: an unmasked batch runs exactly the unfiltered path.  A mask on an index
-// whose rows carry no field ids is refused rather than ignored.
-int32_t vec_field_masks(const ssb_index* ix, const uint32_t* masks, uint32_t nq, const char* who, const uint32_t** use) {
-    *use = nullptr;
-    if (!masks) return SSB_OK;
-    if (is_device_ptr(masks)) { set_error("%s: field_masks must be a host array", who); return SSB_E_INVALID; }
-    bool any = false;
-    for (uint32_t q = 0; q < nq; q++) any = any || masks[q] != 0u;
-    if (!any) return SSB_OK;
-    if (ix->tagged != 1) { set_error("%s: a field mask needs vector rows with field ids (ssb_vector_add_level_fields)", who); return SSB_E_STATE; }
-    *use = masks;
-    return SSB_OK;
-}
-
-// vb field_id / chunk_id of every returned hit of a field-tagged index: the doc's best row among those passing the query's mask
-// (launch_best_rows).  Runs after the search, on the queries it left in the context (f32: prepared again, int8: its quantised codes).
-int32_t fill_best_rows(ssb_index* ix, SearchCtx& c, const void* queries, uint32_t nq, uint32_t k, const ssb_hit* hits, const uint32_t* nh,
-                       const uint32_t* fmask_host, ssb_hit_ext* ext) {
-    cudaStream_t st = c.st;
-    std::vector<uint32_t> hq;   // per hit: (query, first CSR entry, row count, 0)
-    std::vector<uint32_t> slot;  // ext index of each hit
-    for (uint32_t q = 0; q < nq; q++)
-        for (uint32_t j = 0; j < nh[q]; j++) {
-            const uint32_t doc = (uint32_t)hits[(size_t)q * k + j].doc_id;
-            const auto it = std::lower_bound(ix->doc_key.begin(), ix->doc_key.end(), doc);
-            if (it == ix->doc_key.end() || *it != doc) continue;
-            const size_t d = (size_t)(it - ix->doc_key.begin());
-            hq.insert(hq.end(), {q, ix->doc_off[d], ix->doc_off[d + 1] - ix->doc_off[d], 0u});
-            slot.push_back(q * k + j);
-        }
-    const uint32_t n = (uint32_t)slot.size();
-    if (n == 0) return SSB_OK;
-    SSB_TRY(c.best.reserve((size_t)n * 5, 0, st));
-    SSB_TRY(c.fmask.reserve(nq, 0, st));
-    if (fmask_host) SSB_CUDA_TRY(cudaMemcpyAsync(c.fmask.p, fmask_host, (size_t)nq * 4, cudaMemcpyHostToDevice, st));
-    else SSB_CUDA_TRY(cudaMemsetAsync(c.fmask.p, 0, (size_t)nq * 4, st));
-    SSB_CUDA_TRY(cudaMemcpyAsync(c.best.p, hq.data(), (size_t)n * 16, cudaMemcpyHostToDevice, st));
-    vec::BestRowArgs b{};
-    b.n_hits = n; b.hits = reinterpret_cast<const uint4*>(c.best.p); b.doc_rows = ix->doc_rows.p; b.best_row = c.best.p + (size_t)n * 4;
-    b.field_mask = c.fmask.p; b.row_field = ix->row_field.p;
-    if (ix->quant_i8) {
-        // the int8 codes (and scales) of the queries are still in the context from the search's last page
-        b.rows_i8 = ix->rows_i8.p; b.queries_i8 = c.q_i8.p; b.dpad8 = ix->dpad8;
-        if (ix->turbo || ix->cfg.vector_similarity != SSB_SIM_COSINE) {
-            b.i8_scaled = ix->cfg.vector_similarity == SSB_SIM_EUCLIDEAN ? (ix->affine ? 3 : 2) : 1;
-            b.row_scale = ix->row_scale.p; b.row_norm = ix->row_norm.p; b.q_scale = c.q_scale.p; b.q_norm = c.q_norm.p;
-            b.row_aff = ix->row_aff.p; b.q_aff = c.q_aff.p;
-        }
-    } else {
-        const void* qsrc = is_device_ptr(queries) ? queries : c.qstage.p;   // host queries were staged by the search
-        SSB_TRY(c.qpad.reserve((size_t)nq * ix->dpad, 0, st));
-        SSB_TRY(vec::launch_prep_queries((const float*)qsrc, nq, ix->dims, ix->dims, c.qpad.p, nq, ix->dpad,
-                                         ix->cfg.vector_similarity == SSB_SIM_COSINE, st));
-        c.stats.kernel_launches += 1;
-        b.rows = ix->rows.p; b.queries = c.qpad.p; b.dpad = ix->dpad; b.euclid = ix->cfg.vector_similarity == SSB_SIM_EUCLIDEAN;
+// host-facing vector search: paging beyond 32 results, de-duplication, optional threshold
+int32_t search_vector_host(ssb_index* ix, SearchCtx& c, const void* queries, bool queries_i8, uint32_t nq, uint32_t k, ssb_hit* hits, uint32_t* n_hits,
+                           const IvfQuery* ivf = nullptr, const uint32_t* fmask_host = nullptr) {
+    SSB_TRY(c.keys_a.reserve((size_t)nq * LIST, 0, c.st));
+    c.h_keys_a.resize((size_t)nq * LIST);
+    const bool dedup = ix->vec.dup_docs();
+    PageState<1> ps(c, nq, k, hits, n_hits, dedup);
+    const auto fetch = [&](uint32_t kk, const uint64_t* ceil) -> int32_t {
+        SSB_TRY(ix->vec.search_keys(c.vec, c.st, c.stats, &c.ev_used, queries, queries_i8, nq, kk, c.keys_a.p, ceil, ivf, fmask_host));
+        return shard_merge(ix, c, c.keys_a.p, nq);
+    };
+    const uint32_t k1 = dedup ? SSB_K_MAX : (k < SSB_K_MAX ? k : SSB_K_MAX);
+    SSB_TRY(fetch(k1, nullptr));
+    if (ivf) {   // observed_vector_count = the vectors of the selected clusters (summed over the shards)
+        SSB_TRY(shard_sum_counts(ix, c, c.vec.ivf_obs.p, nq));
+        c.vec.h_obs.resize(nq);
+        SSB_CUDA_TRY(cudaMemcpyAsync(c.vec.h_obs.data(), c.vec.ivf_obs.p, (size_t)nq * 8, cudaMemcpyDeviceToHost, c.st));
     }
-    SSB_TRY(vec::launch_best_rows(b, st));
-    c.stats.kernel_launches += 1;
-    c.h_best.resize(n);
-    SSB_CUDA_TRY(cudaMemcpyAsync(c.h_best.data(), b.best_row, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
-    SSB_CUDA_TRY(cudaStreamSynchronize(st));
-    c.stats.h2d_bytes += (uint64_t)n * 16; c.stats.d2h_bytes += (uint64_t)n * 4;
-    for (uint32_t i = 0; i < n; i++) {
-        const uint32_t row = c.h_best[i];
-        if (row == 0xFFFFFFFFu) continue;
-        ext[slot[i]].field_id = ix->h_field[row];
-        ext[slot[i]].chunk_id = ix->h_chunk[row];
-    }
-    return SSB_OK;
-}
-
-// observed_vector_count of a masked query: the rows in scope whose field passes the mask — every row (AnnMode::All) or the rows of the
-// clusters the probe selected (its selection bits are still in the context)
-int32_t masked_observed(ssb_index* ix, SearchCtx& c, uint32_t nq, const uint32_t* fmask_host, bool use_ivf, uint64_t* observed) {
-    std::vector<uint32_t> sel;
-    const uint32_t words = (ix->n_clusters + 31) / 32;
-    if (use_ivf) {
-        sel.resize((size_t)nq * words);
-        SSB_CUDA_TRY(cudaMemcpyAsync(sel.data(), c.ivf_sel.p, sel.size() * 4, cudaMemcpyDeviceToHost, c.st));
-        SSB_CUDA_TRY(cudaStreamSynchronize(c.st));
-    }
-    for (uint32_t q = 0; q < nq; q++) {
-        const uint32_t m = fmask_host[q];
-        if (!m) continue;
-        uint64_t n = 0;
-        if (!use_ivf) { for (uint32_t f = 0; f < 32; f++) if ((m >> f) & 1u) n += ix->field_rows[f]; }
-        else
-            for (uint32_t cl = 0; cl < ix->n_clusters; cl++)
-                if ((sel[(size_t)q * words + cl / 32] >> (cl % 32)) & 1u)
-                    for (uint32_t f = 0; f < 32; f++) if ((m >> f) & 1u) n += ix->cl_field_rows[(size_t)cl * 32 + f];
-        observed[q] = n;
-    }
-    return SSB_OK;
+    SSB_TRY(read_page<1>(c, nq));
+    return page_rest(c, ps, k1, [&](uint32_t kk) { return fetch(kk, c.ceil.p); });
 }
 
 // host-facing lexical search: the first page of <= SSB_K_MAX hits with the counts, then Topk pages below the previous page's last key.
@@ -578,28 +309,19 @@ int32_t search_lexical_host(ssb_index* ix, SearchCtx& c, const ssb_lex_batch* q,
     SSB_TRY(ix->lex->search_keys(c.lex, c.st, q, k1, result_type, c.keys_a.p, c.counts.p, &c.stats.kernel_launches, nullptr, sort));
     if (W == 1) SSB_TRY(shard_merge(ix, c, c.keys_a.p, nq));         // (sorted searches refuse a communicator)
     SSB_TRY(shard_sum_counts(ix, c, c.counts.p, nq));
-    SSB_CUDA_TRY(cudaMemcpyAsync(c.h_keys_a.data(), c.keys_a.p, (size_t)nq * LIST * W * 8, cudaMemcpyDeviceToHost, c.st));
     SSB_CUDA_TRY(cudaMemcpyAsync(c.h_counts.data(), c.counts.p, (size_t)nq * 8, cudaMemcpyDeviceToHost, c.st));
-    SSB_CUDA_TRY(cudaStreamSynchronize(c.st));
-    c.stats.d2h_bytes += (uint64_t)nq * (LIST * W * 8 + 8);
+    c.stats.d2h_bytes += (uint64_t)nq * 8;
+    SSB_TRY(read_page<W>(c, nq));
     c.ev_used = true;
     finish_stats(ix, c);                                        // the first page's scoring kernel is the one reported
     const LexStats ls = LexIndex::read_stats(c.lex, c.st);
     if (want_hits) {
         PageState<W> ps(c, nq, k, hits, n_hits, false, sort && sort->score_asc);
-        bool more = ps.append(c.h_keys_a.data(), k1);
         // pages beyond the first 32 results: Topk search restricted to keys below the previous page's last key
-        while (more) {
-            const uint32_t kk = ps.next_page_k();
-            SSB_TRY(ps.upload_ceilings());
+        SSB_TRY(page_rest(c, ps, k1, [&](uint32_t kk) -> int32_t {
             SSB_TRY(ix->lex->search_keys(c.lex, c.st, q, kk, SSB_RESULT_TOPK, c.keys_a.p, nullptr, &c.stats.kernel_launches, c.ceil.p, sort));
-            if (W == 1) SSB_TRY(shard_merge(ix, c, c.keys_a.p, nq));
-            SSB_CUDA_TRY(cudaMemcpyAsync(c.h_keys_a.data(), c.keys_a.p, (size_t)nq * LIST * W * 8, cudaMemcpyDeviceToHost, c.st));
-            SSB_CUDA_TRY(cudaStreamSynchronize(c.st));
-            c.stats.d2h_bytes += (uint64_t)nq * LIST * W * 8;
-            more = ps.append(c.h_keys_a.data(), kk);
-        }
-        ps.finish();
+            return W == 1 ? shard_merge(ix, c, c.keys_a.p, nq) : SSB_OK;
+        }));
     } else if (n_hits) for (uint32_t i = 0; i < nq; i++) n_hits[i] = 0;
     if (count_total) for (uint32_t i = 0; i < nq; i++) count_total[i] = c.h_counts[i];
     c.stats.postings_visited = ls.postings_visited;
@@ -622,25 +344,16 @@ int32_t search_empty_host(ssb_index* ix, SearchCtx& c, const ssb_lex_batch* q, u
     const uint32_t k1 = want_hits ? (k < SSB_K_MAX ? k : SSB_K_MAX) : 0;
     EmptyStats es{};
     SSB_TRY(ix->lex->search_empty(c.lex, c.st, q, k1, result_type, sort, c.keys_a.p, c.counts.p, nullptr, &es));
-    SSB_CUDA_TRY(cudaMemcpyAsync(c.h_keys_a.data(), c.keys_a.p, (size_t)nq * LIST * 16, cudaMemcpyDeviceToHost, c.st));
     SSB_CUDA_TRY(cudaMemcpyAsync(c.h_counts.data(), c.counts.p, (size_t)nq * 8, cudaMemcpyDeviceToHost, c.st));
-    SSB_CUDA_TRY(cudaStreamSynchronize(c.st));
-    c.stats.d2h_bytes += (uint64_t)nq * (LIST * 16 + 8);
+    c.stats.d2h_bytes += (uint64_t)nq * 8;
+    SSB_TRY(read_page<2>(c, nq));
     c.ev_used = true;
     finish_stats(ix, c);                                        // the first page's scan is the one reported
     if (want_hits) {
         PageState<2> ps(c, nq, k, hits, n_hits, false, false, true);
-        bool more = ps.append(c.h_keys_a.data(), k1);
-        while (more) {
-            const uint32_t kk = ps.next_page_k();
-            SSB_TRY(ps.upload_ceilings());
-            SSB_TRY(ix->lex->search_empty(c.lex, c.st, q, kk, SSB_RESULT_TOPK, sort, c.keys_a.p, nullptr, c.ceil.p, &es));
-            SSB_CUDA_TRY(cudaMemcpyAsync(c.h_keys_a.data(), c.keys_a.p, (size_t)nq * LIST * 16, cudaMemcpyDeviceToHost, c.st));
-            SSB_CUDA_TRY(cudaStreamSynchronize(c.st));
-            c.stats.d2h_bytes += (uint64_t)nq * LIST * 16;
-            more = ps.append(c.h_keys_a.data(), kk);
-        }
-        ps.finish();
+        SSB_TRY(page_rest(c, ps, k1, [&](uint32_t kk) {
+            return ix->lex->search_empty(c.lex, c.st, q, kk, SSB_RESULT_TOPK, sort, c.keys_a.p, nullptr, c.ceil.p, &es);
+        }));
     } else if (n_hits) for (uint32_t i = 0; i < nq; i++) n_hits[i] = 0;
     if (count_total) for (uint32_t i = 0; i < nq; i++) count_total[i] = c.h_counts[i];
     c.stats.kernel_launches += es.launches; c.stats.algorithmic_bytes = es.alg_bytes;
@@ -672,25 +385,15 @@ int32_t ssb_create(const ssb_config* cfg, ssb_index** out) {
     if (prop.major != 9 || prop.minor != 0) { set_error("device %d is sm_%d%d; this library is built for sm_90a (H100) only", cfg->device, prop.major, prop.minor); return SSB_E_UNSUPPORTED; }
     std::unique_ptr<ssb_index> ix(new (std::nothrow) ssb_index());
     if (!ix) { set_error("out of host memory"); return SSB_E_NOMEM; }
-    ix->cfg = *cfg;
-    if (ix->cfg.max_batch == 0) ix->cfg.max_batch = 4096;
+    ix->device = cfg->device;
     ix->n_sms = prop.multiProcessorCount;
     if (cudaStreamCreateWithFlags(&ix->load_st, cudaStreamNonBlocking) != cudaSuccess) { cudaGetLastError(); set_error("stream create failed"); return SSB_E_CUDA; }
-    ix->lex = new (std::nothrow) LexIndex(ix->load_st, ix->n_sms, ix->cfg.max_batch);
+    ix->lex = new (std::nothrow) LexIndex(ix->load_st, ix->n_sms, cfg->max_batch ? cfg->max_batch : 4096);
     if (!ix->lex) { cudaStreamDestroy(ix->load_st); set_error("out of host memory"); return SSB_E_NOMEM; }
     ix->lex->set_deleted(&ix->del);
     ix->lex->set_facets(&ix->facets);
-    ix->dims = cfg->vector_dims;
-    ix->dpad = (cfg->vector_dims + 31) / 32 * 32;
-    ix->dpad8 = (cfg->vector_dims + 127) / 128 * 128;
-    ix->quant_i8 = cfg->vector_quantization == SSB_QUANT_SCALAR_I8 || cfg->vector_quantization == SSB_QUANT_TURBO_I8;
-    ix->turbo = cfg->vector_quantization == SSB_QUANT_TURBO_I8;
-    if (ix->turbo) {
-        // TurboQuant::new: dim = next power of two >= vector_dims (vector_similarity.rs:1836-1859); the codes of a row span tq_dim bytes
-        uint32_t d = 1; while (d < cfg->vector_dims) d <<= 1;
-        ix->tq_dim = d;
-        ix->dpad8 = (d + 127) / 128 * 128;
-    }
+    ix->vec.init(*cfg, ix->n_sms, ix->load_st);
+    ix->vec.set_deleted(&ix->del);
     *out = ix.release();
     return SSB_OK;
     SSB_API_END
@@ -699,7 +402,7 @@ int32_t ssb_create(const ssb_config* cfg, ssb_index** out) {
 int32_t ssb_destroy(ssb_index* ix) {
     SSB_API_BEGIN
     if (!ix) return SSB_OK;
-    cudaSetDevice(ix->cfg.device);
+    cudaSetDevice(ix->device);
     {
         std::unique_lock<std::shared_mutex> g(ix->rw);    // waits for searches in flight
         cudaStreamSynchronize(ix->load_st);
@@ -708,9 +411,6 @@ int32_t ssb_destroy(ssb_index* ix) {
         comm_destroy(ix->comm);
         ix->del.release();
         ix->facets.release();
-        cudaFree(ix->tq_mask); ix->tq_mask = nullptr;
-        ix->rows.release(); ix->rows_hi.release(); ix->rows_lo.release(); ix->rows_i8.release(); ix->row_scale.release(); ix->row_norm.release(); ix->row_aff.release(); ix->doc_ids.release();
-        ix->row_field.release(); ix->row_class.release(); ix->doc_rows.release();
         cudaStreamDestroy(ix->load_st);
     }
     delete ix;
@@ -722,7 +422,7 @@ int32_t ssb_lexical_add_level(ssb_index* ix, const ssb_level_desc* level) {
     SSB_API_BEGIN
     if (!ix) { set_error("null index"); return SSB_E_INVALID; }
     std::unique_lock<std::shared_mutex> g(ix->rw);
-    SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
+    SSB_CUDA_TRY(cudaSetDevice(ix->device));
     if (level && (is_device_ptr(level->doc_ids) || is_device_ptr(level->term_keys))) SSB_CUDA_TRY(cudaDeviceSynchronize());   // inputs produced on another stream
     return ix->lex->add_level_plain(level);
     SSB_API_END
@@ -749,7 +449,7 @@ int32_t ssb_lexical_add_level_ngrams(ssb_index* ix, const ssb_level_desc* level,
     SSB_API_BEGIN
     if (!ix) { set_error("null index"); return SSB_E_INVALID; }
     std::unique_lock<std::shared_mutex> g(ix->rw);
-    SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
+    SSB_CUDA_TRY(cudaSetDevice(ix->device));
     if (ngrams && ix->comm.active()) { set_error("ssb_lexical_add_level_ngrams: n-gram lists on a sharded index are not supported"); return SSB_E_UNSUPPORTED; }
     if (level && (is_device_ptr(level->doc_ids) || is_device_ptr(level->term_keys))) SSB_CUDA_TRY(cudaDeviceSynchronize());   // inputs produced on another stream
     return ix->lex->add_level_ngrams(level, ngrams);
@@ -760,7 +460,7 @@ int32_t ssb_lexical_commit(ssb_index* ix, uint64_t n_docs, uint64_t len_sum) {
     SSB_API_BEGIN
     if (!ix) { set_error("null index"); return SSB_E_INVALID; }
     std::unique_lock<std::shared_mutex> g(ix->rw);
-    SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
+    SSB_CUDA_TRY(cudaSetDevice(ix->device));
     return ix->lex->commit(n_docs, len_sum);
     SSB_API_END
 }
@@ -771,7 +471,7 @@ int32_t ssb_lexical_set_global_df(ssb_index* ix, const uint64_t* keys, const uin
     SSB_API_BEGIN
     if (!ix || (n && (!keys || !dfs))) return SSB_E_INVALID;
     std::unique_lock<std::shared_mutex> g(ix->rw);
-    SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
+    SSB_CUDA_TRY(cudaSetDevice(ix->device));
     return ix->lex->set_global_df(keys, dfs, n);
     SSB_API_END
 }
@@ -781,24 +481,10 @@ int32_t ssb_lexical_set_global_df(ssb_index* ix, const uint64_t* keys, const uin
 int32_t ssb_vector_reserve(ssb_index* ix, uint64_t n_rows) {
     SSB_API_BEGIN
     if (!ix) { set_error("null index"); return SSB_E_INVALID; }
-    if (ix->dims == 0) { set_error("no vector index configured (vector_dims = 0)"); return SSB_E_STATE; }
+    if (ix->vec.dims() == 0) { set_error("no vector index configured (vector_dims = 0)"); return SSB_E_STATE; }
     std::unique_lock<std::shared_mutex> g(ix->rw);
-    SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
-    cudaStream_t st = ix->load_st;
-    if (n_rows <= ix->n_rows) return SSB_OK;
-    SSB_TRY(ix->doc_ids.reserve(n_rows, ix->n_rows, st, true));
-    if (ix->quant_i8) {
-        SSB_TRY(ix->rows_i8.reserve(n_rows * ix->dpad8, ix->n_rows * ix->dpad8, st, true));
-        if (ix->cfg.vector_similarity != SSB_SIM_COSINE) { SSB_TRY(ix->row_scale.reserve(n_rows, ix->n_rows, st, true)); SSB_TRY(ix->row_norm.reserve(n_rows, ix->n_rows, st, true)); }
-    } else {
-        SSB_TRY(ix->rows.reserve(n_rows * ix->dpad, ix->n_rows * ix->dpad, st, true));
-        if (ix->cfg.vector_similarity != SSB_SIM_EUCLIDEAN) {
-            SSB_TRY(ix->rows_hi.reserve(n_rows * ix->dpad, ix->n_rows * ix->dpad, st, true));
-            SSB_TRY(ix->rows_lo.reserve(n_rows * ix->dpad, ix->n_rows * ix->dpad, st, true));
-            SSB_TRY(ix->rows_h16.reserve(n_rows * ix->dpad, ix->n_rows * ix->dpad, st, true));
-        }
-    }
-    return SSB_OK;
+    SSB_CUDA_TRY(cudaSetDevice(ix->device));
+    return ix->vec.reserve(n_rows);
     SSB_API_END
 }
 
@@ -811,212 +497,21 @@ static int32_t vector_add_level_impl(ssb_index* ix, uint32_t level_id, const flo
                                      const uint8_t* field_ids = nullptr, const uint32_t* chunk_ids = nullptr) {
     SSB_API_BEGIN
     if (!ix || (n && !rows)) { set_error("ssb_vector_add_level: null argument"); return SSB_E_INVALID; }
-    if (ix->dims == 0 || dims != ix->dims) { set_error("dims %u != configured vector_dims %u", dims, ix->dims); return SSB_E_INVALID; }
+    if (ix->vec.dims() == 0 || dims != ix->vec.dims()) { set_error("dims %u != configured vector_dims %u", dims, ix->vec.dims()); return SSB_E_INVALID; }
     if (cluster_counts) {
         if (is_device_ptr(cluster_counts)) { set_error("cluster_counts must be host memory"); return SSB_E_INVALID; }
         uint64_t sum = 0;
         for (uint32_t c = 0; c < n_clusters; c++) { if (cluster_counts[c] == 0) { set_error("empty cluster %u", c); return SSB_E_INVALID; } sum += cluster_counts[c]; }
         if (sum != n || (n && n_clusters == 0)) { set_error("cluster table covers %llu of %u rows", (unsigned long long)sum, n); return SSB_E_INVALID; }
-        if (ix->quant_i8 && n_clusters > 1) { set_error("IVF cluster tables need an f32 vector index"); return SSB_E_UNSUPPORTED; }
+        if (ix->vec.quant_i8() && n_clusters > 1) { set_error("IVF cluster tables need an f32 vector index"); return SSB_E_UNSUPPORTED; }
     }
     if (level_id >= 65536) { set_error("level_id must be < 65536 (doc id = level_id << 16 | local)"); return SSB_E_INVALID; }
     if (row_stride == 0) row_stride = dims;
     if (row_stride < dims) { set_error("row stride < dims"); return SSB_E_INVALID; }
     if ((field_ids == nullptr) != (chunk_ids == nullptr)) { set_error("ssb_vector_add_level_fields: field_ids and chunk_ids go together"); return SSB_E_INVALID; }
     std::unique_lock<std::shared_mutex> g(ix->rw);
-    SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
-    if (n == 0) return SSB_OK;   // an empty level (a block whose docs carry no vectors, vector.rs:1056-1073) is neither tagged nor untagged
-    const int tag = field_ids ? 1 : 0;
-    if (ix->tagged >= 0 && ix->tagged != tag) {
-        set_error("vector levels %s field ids, this one %s: every level carries them or none does", ix->tagged ? "carry" : "carry no", tag ? "does" : "does not");
-        return SSB_E_STATE;
-    }
-    std::vector<uint8_t> h_fld; std::vector<uint32_t> h_chk;
-    if (tag) {   // validated before anything is written
-        h_fld.resize(n); h_chk.resize(n);
-        SSB_CUDA_TRY(cudaMemcpy(h_fld.data(), field_ids, n, cudaMemcpyDefault));
-        SSB_CUDA_TRY(cudaMemcpy(h_chk.data(), chunk_ids, (size_t)n * 4, cudaMemcpyDefault));
-        for (uint32_t i = 0; i < n; i++) if (h_fld[i] >= 32) { set_error("field id %u of row %u: indexed field ids must be < 32", h_fld[i], i); return SSB_E_INVALID; }
-    }
-    cudaStream_t st = ix->load_st;
-    // device-resident inputs may still be in flight on the caller's stream (the load stream is non-blocking): load time is not
-    // hot, wait for the device once
-    if (is_device_ptr(rows) || (local_ids && is_device_ptr(local_ids))) SSB_CUDA_TRY(cudaDeviceSynchronize());
-    // multi-chunk documents: several rows may share a local id (one vector per chunk, vector.rs:62-73); the reference's TopK keeps
-    // the best chunk per doc id (vector.rs:436-470) — remember that this index needs the de-duplicating result path
-    std::vector<uint16_t> h_ids;
-    if (local_ids) {
-        h_ids.resize(n);
-        SSB_CUDA_TRY(cudaMemcpy(h_ids.data(), local_ids, (size_t)n * 2, cudaMemcpyDefault));
-        std::vector<bool> seen(65536, false);
-        for (uint32_t i = 0; i < n; i++) { if (seen[h_ids[i]]) ix->dup_docs = true; seen[h_ids[i]] = true; }
-    }
-    SSB_TRY(ix->doc_ids.reserve(ix->n_rows + n, ix->n_rows, st));
-    DevTmp<float> stage;
-    if (ix->quant_i8) {
-        // index-time normalise + quantise (vector.rs:585-640); the f32 rows are only staged
-        SSB_TRY(ix->rows_i8.reserve((ix->n_rows + n) * ix->dpad8, ix->n_rows * ix->dpad8, st));
-        SSB_CUDA_TRY(stage.alloc((size_t)n * dims));
-        SSB_CUDA_TRY(cudaMemcpy2DAsync(stage.p, (size_t)dims * 4, rows, row_stride * 4, (size_t)dims * 4, n, cudaMemcpyDefault, st));
-        if (ix->turbo) {
-            // TurboQuant::quantize_f32_i8 for every similarity (vector.rs:684-695, 729-740), after normalize_f32 for Cosine (:585-596)
-            if (!ix->tq_mask) { set_error("TurboQuantI8: call ssb_vector_set_turboquant_mask before adding vectors"); return SSB_E_STATE; }
-            SSB_TRY(ix->row_scale.reserve(ix->n_rows + n, ix->n_rows, st));
-            SSB_TRY(ix->row_norm.reserve(ix->n_rows + n, ix->n_rows, st));
-            SSB_TRY(vec::launch_quantize_rows_turbo_i8(stage.p, dims, n, n, dims, ix->tq_dim, ix->tq_mask, ix->rows_i8.p + ix->n_rows * ix->dpad8, ix->dpad8,
-                                                       ix->row_scale.p + ix->n_rows, ix->row_norm.p + ix->n_rows,
-                                                       ix->cfg.vector_similarity == SSB_SIM_COSINE, 0, st));
-        } else if (ix->cfg.vector_similarity == SSB_SIM_COSINE)
-            SSB_TRY(vec::launch_quantize_rows_i8(stage.p, dims, n, n, dims, ix->rows_i8.p + ix->n_rows * ix->dpad8, ix->dpad8, st));
-        else {
-            // Dot: QuantizedVector::new_scale; Euclidean: new_scale_norm — the NON-AFFINE variant the reference picks when the first
-            // vector is not all integers in 0..255 (vector.rs:651-660); integer-valued data (affine quantisation) is not built
-            if (ix->cfg.vector_similarity == SSB_SIM_EUCLIDEAN && ix->n_rows == 0) {
-                std::vector<float> first(dims);
-                SSB_CUDA_TRY(cudaMemcpyAsync(first.data(), stage.p, (size_t)dims * 4, cudaMemcpyDeviceToHost, st));
-                SSB_CUDA_TRY(cudaStreamSynchronize(st));
-                bool non_affine = false;
-                for (float x : first) non_affine = non_affine || x != floorf(x) || x < 0.0f || x > 255.0f;
-                ix->affine = !non_affine;      // decided by the FIRST vector of the shard, for its whole life (vector.rs:657-664)
-            }
-            if (ix->affine) {
-                // new_scale_norm_affine: every vector is quantised with the running (min, max) of everything indexed before it — the state is
-                // walked on the host over the level's per-row (min, max) (64K rows), the codes are written by one more kernel
-                DevTmp<float> mm, d_scale; DevTmp<int> d_zp;
-                SSB_CUDA_TRY(mm.alloc((size_t)n * 2)); SSB_CUDA_TRY(d_scale.alloc(n)); SSB_CUDA_TRY(d_zp.alloc(n));
-                SSB_TRY(vec::launch_rows_minmax(stage.p, dims, n, dims, mm.p, st));
-                std::vector<float> h_mm((size_t)n * 2), h_scale(n); std::vector<int> h_zp(n);
-                SSB_CUDA_TRY(cudaMemcpyAsync(h_mm.data(), mm.p, (size_t)n * 8, cudaMemcpyDeviceToHost, st));
-                SSB_CUDA_TRY(cudaStreamSynchronize(st));
-                float smin = ix->aff_min, smax = ix->aff_max;
-                vec::affine_walk_rows(h_mm.data(), n, &smin, &smax, h_scale.data(), h_zp.data());
-                SSB_CUDA_TRY(cudaMemcpyAsync(d_scale.p, h_scale.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
-                SSB_CUDA_TRY(cudaMemcpyAsync(d_zp.p, h_zp.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
-                SSB_TRY(ix->row_scale.reserve(ix->n_rows + n, ix->n_rows, st));
-                SSB_TRY(ix->row_norm.reserve(ix->n_rows + n, ix->n_rows, st));
-                SSB_TRY(ix->row_aff.reserve((ix->n_rows + n) * 2, ix->n_rows * 2, st));
-                SSB_TRY(vec::launch_quantize_rows_affine_i8(stage.p, dims, n, n, dims, d_scale.p, d_zp.p, 0.f, 0.f, ix->rows_i8.p + ix->n_rows * ix->dpad8, ix->dpad8,
-                                                            ix->row_scale.p + ix->n_rows, ix->row_norm.p + ix->n_rows, ix->row_aff.p + ix->n_rows * 2, 0, st));
-                SSB_CUDA_TRY(cudaStreamSynchronize(st));
-                ix->aff_min = smin; ix->aff_max = smax;
-            } else {
-            SSB_TRY(ix->row_scale.reserve(ix->n_rows + n, ix->n_rows, st));
-            SSB_TRY(ix->row_norm.reserve(ix->n_rows + n, ix->n_rows, st));
-            SSB_TRY(vec::launch_quantize_rows_scale_i8(stage.p, dims, n, n, dims, ix->rows_i8.p + ix->n_rows * ix->dpad8, ix->dpad8,
-                                                       ix->row_scale.p + ix->n_rows, ix->row_norm.p + ix->n_rows,
-                                                       ix->cfg.vector_similarity == SSB_SIM_EUCLIDEAN, st));
-            }
-        }
-    } else {
-        SSB_TRY(ix->rows.reserve((ix->n_rows + n) * ix->dpad, ix->n_rows * ix->dpad, st));
-        float* dst = ix->rows.p + ix->n_rows * ix->dpad;
-        SSB_CUDA_TRY(cudaMemcpy2DAsync(dst, (size_t)ix->dpad * 4, rows, row_stride * 4, (size_t)dims * 4, n, cudaMemcpyDefault, st));
-        SSB_TRY(vec::launch_normalize_rows(dst, n, dims, ix->dpad, ix->cfg.vector_similarity == SSB_SIM_COSINE, st));
-        if (ix->cfg.vector_similarity != SSB_SIM_EUCLIDEAN) {
-            // the tensor-core scan reads the corpus as two bf16 planes (same 4 bytes per element as the f32 rows, which stay for
-            // the FP32 scan): split once here instead of per stage in shared memory
-            SSB_TRY(ix->rows_hi.reserve((ix->n_rows + n) * ix->dpad, ix->n_rows * ix->dpad, st));
-            SSB_TRY(ix->rows_lo.reserve((ix->n_rows + n) * ix->dpad, ix->n_rows * ix->dpad, st));
-            SSB_TRY(vec::launch_split_rows_bf16(dst, ix->rows_hi.p + ix->n_rows * ix->dpad, ix->rows_lo.p + ix->n_rows * ix->dpad, (size_t)n * ix->dpad, st));
-            // filter scan: scaled fp16 plane + its index-wide error bounds.  The scale (a power of two, fixed for the life of the index)
-            // puts Cosine's unit rows below 256 and a Dot index's first level into [128, 256): later rows may be 255x larger before fp16
-            // overflows — an overflowing row makes the error bound infinite and every filter query takes the exact fallback.
-            if (!ix->vec_err.p) { SSB_TRY(ix->vec_err.reserve(4, 0, st, true)); SSB_CUDA_TRY(cudaMemsetAsync(ix->vec_err.p, 0, 16, st)); }
-            if (ix->vec_scale == 0.f) {
-                if (ix->cfg.vector_similarity == SSB_SIM_COSINE) ix->vec_scale = 256.f;
-                else {
-                    uint32_t bits = 0;
-                    SSB_TRY(vec::launch_max_abs_f32(dst, (size_t)n * ix->dpad, ix->vec_err.p + 2, st));
-                    SSB_CUDA_TRY(cudaMemcpyAsync(&bits, ix->vec_err.p + 2, 4, cudaMemcpyDeviceToHost, st));
-                    SSB_CUDA_TRY(cudaStreamSynchronize(st));
-                    float mx; memcpy(&mx, &bits, 4);
-                    ix->vec_scale = mx > 0.f ? exp2f((float)(7 - ilogbf(mx))) : 1.f;
-                }
-            }
-            SSB_TRY(ix->rows_h16.reserve((ix->n_rows + n) * ix->dpad, ix->n_rows * ix->dpad, st));
-            SSB_TRY(vec::launch_rows_f16_err(dst, ix->rows_h16.p + ix->n_rows * ix->dpad, n, ix->dpad, ix->vec_scale, ix->vec_err.p, st));
-        }
-    }
-    DevTmp<uint16_t> tmp;
-    const uint16_t* lid = local_ids;
-    if (local_ids && !is_device_ptr(local_ids)) {
-        SSB_CUDA_TRY(tmp.alloc(n));
-        SSB_CUDA_TRY(cudaMemcpyAsync(tmp.p, h_ids.data(), (size_t)n * 2, cudaMemcpyHostToDevice, st));
-        lid = tmp.p;
-    }
-    SSB_TRY(vec::launch_fill_doc_ids(ix->doc_ids.p + ix->n_rows, lid, level_id, n, st));
-    std::vector<uint32_t> row_cl;   // tagged f32 levels: each row's global cluster id
-    if (!ix->quant_i8) {
-        // IVF tables: clusters are numbered across levels; a cluster's medoid is its first row (vector.rs:1316-1320)
-        const uint32_t one = n;
-        if (!cluster_counts) { cluster_counts = &one; n_clusters = 1; }
-        std::vector<uint32_t> rc(n), mrow(n_clusters);
-        uint32_t r = 0;
-        for (uint32_t c = 0; c < n_clusters; c++) {
-            mrow[c] = (uint32_t)ix->n_rows + r;
-            for (uint32_t i = 0; i < cluster_counts[c]; i++) rc[r++] = ix->n_clusters + c;
-        }
-        SSB_TRY(ix->row_cluster.reserve(ix->n_rows + n, ix->n_rows, st));
-        SSB_TRY(ix->cl_count.reserve(ix->n_clusters + n_clusters, ix->n_clusters, st));
-        SSB_TRY(ix->medoids.reserve((size_t)(ix->n_clusters + n_clusters) * ix->dpad, (size_t)ix->n_clusters * ix->dpad, st));
-        SSB_TRY(ix->lvl_begin.reserve(ix->h_lvl_begin.size() + 2, 0, st));
-        DevTmp<uint32_t> midx; SSB_CUDA_TRY(midx.alloc(n_clusters));
-        SSB_CUDA_TRY(cudaMemcpyAsync(ix->row_cluster.p + ix->n_rows, rc.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
-        SSB_CUDA_TRY(cudaMemcpyAsync(ix->cl_count.p + ix->n_clusters, cluster_counts, (size_t)n_clusters * 4, cudaMemcpyHostToDevice, st));
-        SSB_CUDA_TRY(cudaMemcpyAsync(midx.p, mrow.data(), (size_t)n_clusters * 4, cudaMemcpyHostToDevice, st));
-        SSB_TRY(vec::launch_gather_rows(ix->rows.p, midx.p, n_clusters, ix->dpad, ix->medoids.p + (size_t)ix->n_clusters * ix->dpad, st));
-        if (tag) {
-            ix->cl_field_rows.resize((size_t)(ix->n_clusters + n_clusters) * 32, 0u);
-            for (uint32_t i = 0; i < n; i++) ix->cl_field_rows[(size_t)rc[i] * 32 + h_fld[i]]++;
-            row_cl = std::move(rc);
-        }
-        std::vector<uint32_t> lb = ix->h_lvl_begin; lb.push_back(ix->n_clusters); lb.push_back(ix->n_clusters + n_clusters);
-        SSB_CUDA_TRY(cudaMemcpyAsync(ix->lvl_begin.p, lb.data(), lb.size() * 4, cudaMemcpyHostToDevice, st));
-        SSB_CUDA_TRY(cudaStreamSynchronize(st));
-        ix->h_lvl_begin.push_back(ix->n_clusters);
-        ix->n_clusters += n_clusters;
-        if (n_clusters > ix->max_level_clusters) ix->max_level_clusters = n_clusters;
-    }
-    if (tag) {
-        // row fields for the scans; the doc -> rows table of the best-row step: the level's (doc, row) pairs merged into the sorted list
-        SSB_TRY(ix->row_field.reserve(ix->n_rows + n, ix->n_rows, st));
-        SSB_CUDA_TRY(cudaMemcpyAsync(ix->row_field.p + ix->n_rows, h_fld.data(), n, cudaMemcpyHostToDevice, st));
-        std::vector<uint32_t> cls(n);
-        for (uint32_t i = 0; i < n; i++) cls[i] = (ix->quant_i8 ? 0u : row_cl[i]) * 32u + h_fld[i];
-        SSB_TRY(ix->row_class.reserve(ix->n_rows + n, ix->n_rows, st));
-        SSB_CUDA_TRY(cudaMemcpyAsync(ix->row_class.p + ix->n_rows, cls.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
-        for (uint32_t i = 0; i < n; i++) ix->field_rows[h_fld[i]]++;
-        const size_t old = ix->doc_pairs.size();
-        for (uint32_t i = 0; i < n; i++) {
-            const uint32_t doc = (level_id << 16) | (local_ids ? (uint32_t)h_ids[i] : i);
-            ix->doc_pairs.push_back(((uint64_t)doc << 32) | (ix->n_rows + i));
-        }
-        std::sort(ix->doc_pairs.begin() + old, ix->doc_pairs.end());
-        // levels usually arrive in level order: every new doc sorts after the table's last one, and the level's entries are appended (host
-        // index and device rows).  Otherwise the pairs are merged and the table is rebuilt.
-        const bool append = old == 0 || (uint32_t)(ix->doc_pairs[old] >> 32) > ix->doc_key.back();
-        size_t from = old;
-        if (append) { if (!ix->doc_off.empty()) ix->doc_off.pop_back(); }
-        else {
-            std::inplace_merge(ix->doc_pairs.begin(), ix->doc_pairs.begin() + old, ix->doc_pairs.end());
-            ix->doc_key.clear(); ix->doc_off.clear(); from = 0;
-        }
-        std::vector<uint32_t> rows_of(ix->doc_pairs.size() - from);
-        for (size_t i = from; i < ix->doc_pairs.size(); i++) {
-            const uint32_t doc = (uint32_t)(ix->doc_pairs[i] >> 32);
-            if (ix->doc_key.empty() || ix->doc_key.back() != doc) { ix->doc_key.push_back(doc); ix->doc_off.push_back((uint32_t)i); }
-            rows_of[i - from] = (uint32_t)ix->doc_pairs[i];
-        }
-        ix->doc_off.push_back((uint32_t)ix->doc_pairs.size());
-        SSB_TRY(ix->doc_rows.reserve(ix->doc_pairs.size(), from, st));
-        SSB_CUDA_TRY(cudaMemcpyAsync(ix->doc_rows.p + from, rows_of.data(), rows_of.size() * 4, cudaMemcpyHostToDevice, st));
-        ix->h_field.insert(ix->h_field.end(), h_fld.begin(), h_fld.end());
-        ix->h_chunk.insert(ix->h_chunk.end(), h_chk.begin(), h_chk.end());
-    }
-    SSB_CUDA_TRY(cudaStreamSynchronize(st));
-    ix->tagged = tag;
-    ix->n_rows += n;
-    return SSB_OK;
+    SSB_CUDA_TRY(cudaSetDevice(ix->device));
+    return ix->vec.add_level(level_id, rows, row_stride, local_ids, n, cluster_counts, n_clusters, field_ids, chunk_ids);
     SSB_API_END
 }
 
@@ -1040,7 +535,7 @@ int32_t ssb_vector_add_level_fields(ssb_index* ix, uint32_t level_id, const floa
                                     const uint8_t* field_ids, const uint32_t* chunk_ids) {
     if (n > 65536) { set_error("a level holds at most 65536 vectors"); return SSB_E_INVALID; }
     if (n && (!field_ids || !chunk_ids)) { set_error("ssb_vector_add_level_fields: null field_ids / chunk_ids"); return SSB_E_INVALID; }
-    if (ix && ix->comm.active()) { set_error("ssb_vector_add_level_fields: field-tagged rows on a sharded index are not supported"); return SSB_E_UNSUPPORTED; }
+    if (ix) SSB_TRY(refuse_tagged_sharded("ssb_vector_add_level_fields", "rows", true, ix->comm.active()));
     return vector_add_level_impl(ix, level_id, rows, row_stride, local_ids, n, dims, n ? cluster_counts : nullptr, n_clusters,
                                  n ? field_ids : nullptr, n ? chunk_ids : nullptr);
 }
@@ -1050,7 +545,7 @@ int32_t ssb_load_index_bin(ssb_index* ix, const void* bytes, uint64_t len, const
     if (!ix || !bytes || !params) { set_error("ssb_load_index_bin: null argument"); return SSB_E_INVALID; }
     if (is_device_ptr(bytes)) { set_error("ssb_load_index_bin: bytes must be host memory"); return SSB_E_INVALID; }
     std::unique_lock<std::shared_mutex> g(ix->rw);
-    SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
+    SSB_CUDA_TRY(cudaSetDevice(ix->device));
     return load_index_bin(ix->lex, (const uint8_t*)bytes, len, params, n_docs_out);
     SSB_API_END
 }
@@ -1067,7 +562,7 @@ int32_t ssb_load_index_bin_ngrams(ssb_index* ix, const void* bytes, uint64_t len
     if (!ix || !bytes || !params) { set_error("ssb_load_index_bin_ngrams: null argument"); return SSB_E_INVALID; }
     if (is_device_ptr(bytes)) { set_error("ssb_load_index_bin_ngrams: bytes must be host memory"); return SSB_E_INVALID; }
     std::unique_lock<std::shared_mutex> g(ix->rw);
-    SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
+    SSB_CUDA_TRY(cudaSetDevice(ix->device));
     if (ix->comm.active()) { set_error("ssb_load_index_bin_ngrams: n-gram lists on a sharded index are not supported"); return SSB_E_UNSUPPORTED; }
     return load_index_bin(ix->lex, (const uint8_t*)bytes, len, params, n_docs_out, true);
     SSB_API_END
@@ -1087,17 +582,18 @@ static int32_t load_vector_bin_impl(ssb_index* ix, const void* bytes, uint64_t l
     SSB_API_BEGIN
     if (!ix || !bytes) { set_error("ssb_load_vector_bin: null argument"); return SSB_E_INVALID; }
     if (is_device_ptr(bytes)) { set_error("ssb_load_vector_bin: bytes must be host memory"); return SSB_E_INVALID; }
-    if (ix->dims == 0) { set_error("ssb_load_vector_bin: the index has no vector_dims"); return SSB_E_STATE; }
-    if (keep_fields && ix->comm.active()) { set_error("ssb_load_vector_bin_fields: field-tagged rows on a sharded index are not supported"); return SSB_E_UNSUPPORTED; }
+    const uint32_t dims = ix->vec.dims();
+    if (dims == 0) { set_error("ssb_load_vector_bin: the index has no vector_dims"); return SSB_E_STATE; }
+    SSB_TRY(refuse_tagged_sharded("ssb_load_vector_bin_fields", "rows", keep_fields, ix->comm.active()));
     std::vector<VectorLevel> levels;
-    SSB_TRY(parse_vector_bin((const uint8_t*)bytes, len, ix->dims, levels, keep_fields));
+    SSB_TRY(parse_vector_bin((const uint8_t*)bytes, len, dims, levels, keep_fields));
     uint64_t total = 0;
     for (auto& vl : levels) {
         // a level may hold more than 64K records (one per chunk); its cluster table (IVF, vector.rs:1066-1094) rides along.  Empty clusters
         // cannot be probed (their medoid would be another cluster's record): such a table is dropped, the level becomes one cluster.
-        bool ok = !vl.cluster_counts.empty() && !ix->quant_i8;
+        bool ok = !vl.cluster_counts.empty() && !ix->vec.quant_i8();
         for (uint32_t c : vl.cluster_counts) ok = ok && c != 0;
-        SSB_TRY(vector_add_level_impl(ix, vl.level_id, vl.rows.data(), ix->dims, vl.ids.data(), (uint32_t)vl.ids.size(), ix->dims,
+        SSB_TRY(vector_add_level_impl(ix, vl.level_id, vl.rows.data(), dims, vl.ids.data(), (uint32_t)vl.ids.size(), dims,
                                       ok ? vl.cluster_counts.data() : nullptr, ok ? (uint32_t)vl.cluster_counts.size() : 0,
                                       keep_fields && !vl.ids.empty() ? vl.fields.data() : nullptr, keep_fields && !vl.ids.empty() ? vl.chunks.data() : nullptr));
         total += vl.ids.size();
@@ -1124,7 +620,7 @@ int32_t ssb_set_deleted(ssb_index* ix, const uint64_t* doc_ids, uint64_t n) {
     if (!ix || (n && !doc_ids)) { set_error("ssb_set_deleted: null argument"); return SSB_E_INVALID; }
     if (n >= (1ull << 31)) { set_error("ssb_set_deleted: too many doc ids"); return SSB_E_UNSUPPORTED; }
     std::unique_lock<std::shared_mutex> g(ix->rw);
-    SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
+    SSB_CUDA_TRY(cudaSetDevice(ix->device));
     std::vector<uint32_t> docs(n);
     for (uint64_t i = 0; i < n; i++) {
         if (doc_ids[i] >> 32) { set_error("ssb_set_deleted: doc id %llu out of range", (unsigned long long)doc_ids[i]); return SSB_E_INVALID; }
@@ -1158,7 +654,7 @@ int32_t ssb_set_facets(ssb_index* ix, const void* rows, uint64_t first_doc_id, u
     SSB_API_BEGIN
     if (!ix) { set_error("ssb_set_facets: null index"); return SSB_E_INVALID; }
     std::unique_lock<std::shared_mutex> g(ix->rw);
-    SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
+    SSB_CUDA_TRY(cudaSetDevice(ix->device));
     SSB_CUDA_TRY(cudaDeviceSynchronize());        // searches may run on a caller-owned stream (ssb_set_stream): nothing may still read the old columns
     return ix->facets.set_columns(rows, first_doc_id, n_docs, row_bytes, fields, n_fields, ix->load_st);
     SSB_API_END
@@ -1168,7 +664,7 @@ int32_t ssb_set_facet_value_order(ssb_index* ix, uint32_t facet, const uint32_t*
     SSB_API_BEGIN
     if (!ix || (n_ids && !rank_of_id)) { set_error("ssb_set_facet_value_order: null argument"); return SSB_E_INVALID; }
     std::unique_lock<std::shared_mutex> g(ix->rw);
-    SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
+    SSB_CUDA_TRY(cudaSetDevice(ix->device));
     FacetSet& fs = ix->facets;
     if (!fs.n_facets) { set_error("ssb_set_facet_value_order: no facets (ssb_set_facets)"); return SSB_E_STATE; }
     if (facet >= fs.n_facets) { set_error("ssb_set_facet_value_order: facet %u of %u", facet, fs.n_facets); return SSB_E_INVALID; }
@@ -1187,7 +683,7 @@ int32_t ssb_set_facet_string_sets(ssb_index* ix, uint32_t facet, const uint64_t*
     SSB_API_BEGIN
     if (!ix || !set_offsets) { set_error("ssb_set_facet_string_sets: null argument"); return SSB_E_INVALID; }
     std::unique_lock<std::shared_mutex> g(ix->rw);
-    SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
+    SSB_CUDA_TRY(cudaSetDevice(ix->device));
     FacetSet& fs = ix->facets;
     if (!fs.n_facets) { set_error("ssb_set_facet_string_sets: no facets (ssb_set_facets)"); return SSB_E_STATE; }
     if (facet >= fs.n_facets) { set_error("ssb_set_facet_string_sets: facet %u of %u", facet, fs.n_facets); return SSB_E_INVALID; }
@@ -1207,22 +703,12 @@ int32_t ssb_set_facet_string_sets(ssb_index* ix, uint32_t facet, const uint64_t*
     SSB_API_END
 }
 
-// TurboQuant.seed_mask (vector_similarity.rs:1845-1859): the reference draws the +-1 mask once per index from ChaCha8Rng::seed_from_u64(1234)
-// (index.rs:2215-2216) — a third-party generator this library does not restate; the host hands over the mask it holds.
 int32_t ssb_vector_set_turboquant_mask(ssb_index* ix, const float* seed_mask, uint32_t dim) {
     SSB_API_BEGIN
     if (!ix || !seed_mask) { set_error("ssb_vector_set_turboquant_mask: null argument"); return SSB_E_INVALID; }
     std::unique_lock<std::shared_mutex> g(ix->rw);
-    if (!ix->turbo) { set_error("ssb_vector_set_turboquant_mask: the index was not created with SSB_QUANT_TURBO_I8"); return SSB_E_STATE; }
-    if (ix->n_rows) { set_error("ssb_vector_set_turboquant_mask: call it before the first vector level"); return SSB_E_STATE; }
-    if (dim != ix->tq_dim) { set_error("ssb_vector_set_turboquant_mask: dim %u, expected next_power_of_two(vector_dims) = %u", dim, ix->tq_dim); return SSB_E_INVALID; }
-    std::vector<float> m(dim);
-    SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
-    SSB_CUDA_TRY(cudaMemcpy(m.data(), seed_mask, (size_t)dim * 4, cudaMemcpyDefault));
-    for (float x : m) if (x != 1.0f && x != -1.0f) { set_error("ssb_vector_set_turboquant_mask: the mask must hold +1 / -1"); return SSB_E_INVALID; }
-    if (!ix->tq_mask) SSB_CUDA_TRY(cudaMalloc(&ix->tq_mask, (size_t)dim * 4));
-    SSB_CUDA_TRY(cudaMemcpy(ix->tq_mask, m.data(), (size_t)dim * 4, cudaMemcpyHostToDevice));
-    return SSB_OK;
+    SSB_CUDA_TRY(cudaSetDevice(ix->device));
+    return ix->vec.set_turboquant_mask(seed_mask, dim);
     SSB_API_END
 }
 
@@ -1230,20 +716,20 @@ int32_t ssb_set_vector_kernel(ssb_index* ix, uint32_t kernel) {
     SSB_API_BEGIN
     if (!ix || kernel > SSB_VEC_KERNEL_TCGEN05_FILTER_N256_PAIR) { set_error("bad vector kernel"); return SSB_E_INVALID; }
     std::unique_lock<std::shared_mutex> g(ix->rw);
-    ix->cfg.vector_kernel = kernel;
+    ix->vec.set_kernel(kernel);
     return SSB_OK;
     SSB_API_END
 }
 
-int32_t ssb_vector_count(const ssb_index* ix, uint64_t* n) { if (!ix || !n) return SSB_E_INVALID; *n = ix->n_rows; return SSB_OK; }
+int32_t ssb_vector_count(const ssb_index* ix, uint64_t* n) { if (!ix || !n) return SSB_E_INVALID; *n = ix->vec.n_rows(); return SSB_OK; }
 
 int32_t ssb_search_vector_keys(ssb_index* ix, const float* queries, uint32_t nq, uint32_t k, uint64_t* keys_out_dev) {
     SSB_API_BEGIN
     if (!ix || (nq && (!queries || !keys_out_dev))) { set_error("ssb_search_vector_keys: null argument"); return SSB_E_INVALID; }
     std::shared_lock<std::shared_mutex> g(ix->rw);
-    SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
+    SSB_CUDA_TRY(cudaSetDevice(ix->device));
     CtxLease l(ix); SSB_TRY(l.acquire());
-    SSB_TRY(vec_keys(ix, *l.c, queries, false, nq, k, keys_out_dev));
+    SSB_TRY(ix->vec.search_keys(l.c->vec, l.c->st, l.c->stats, &l.c->ev_used, queries, false, nq, k, keys_out_dev));
     return shard_merge(ix, *l.c, keys_out_dev, nq);
     SSB_API_END
 }
@@ -1252,7 +738,7 @@ int32_t ssb_search_vector(ssb_index* ix, const float* queries, uint32_t nq, uint
     SSB_API_BEGIN
     if (!ix || (nq && (!queries || !hits))) { set_error("ssb_search_vector: null argument"); return SSB_E_INVALID; }
     std::shared_lock<std::shared_mutex> g(ix->rw);
-    SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
+    SSB_CUDA_TRY(cudaSetDevice(ix->device));
     if (nq == 0) return SSB_OK;
     if (k == 0 || k > SSB_K_LIMIT) { set_error("k must be in 1..%u", SSB_K_LIMIT); return SSB_E_UNSUPPORTED; }
     CtxLease l(ix); SSB_TRY(l.acquire());
@@ -1270,15 +756,15 @@ static int32_t search_vector_ex_impl(ssb_index* ix, const ssb_vec_query* vq, con
     if (!ix || !vq || (vq->n_queries && (!vq->queries || !hits))) { set_error("ssb_search_vector_ex: null argument"); return SSB_E_INVALID; }
     if (vq->query_format > SSB_QFMT_I8) { set_error("bad query_format"); return SSB_E_INVALID; }
     std::shared_lock<std::shared_mutex> g(ix->rw);
-    SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
+    SSB_CUDA_TRY(cudaSetDevice(ix->device));
     const uint32_t nq = vq->n_queries, k = vq->k;
     if (nq == 0) return SSB_OK;
     const uint32_t* fm = nullptr;
-    SSB_TRY(vec_field_masks(ix, field_masks, nq, "ssb_search_vector_fields", &fm));
+    SSB_TRY(ix->vec.field_masks(field_masks, nq, "ssb_search_vector_fields", &fm));
     if (k == 0 || k > SSB_K_LIMIT) { set_error("k must be in 1..%u", SSB_K_LIMIT); return SSB_E_UNSUPPORTED; }
     CtxLease l(ix); SSB_TRY(l.acquire());
     std::vector<uint32_t> nh(nq, 0);
-    const bool euclid = ix->cfg.vector_similarity == SSB_SIM_EUCLIDEAN;
+    const bool euclid = ix->vec.euclid();
     if (vq->ann_mode > SSB_ANN_NPROBE_SIMILARITY_THRESHOLD) { set_error("bad ann_mode"); return SSB_E_INVALID; }
     IvfQuery ivf{vq->ann_mode, vq->n_probe, 0.f};
     {   // the cluster threshold goes through the same pre-map as the result threshold (TopK::new, vector.rs:388-399)
@@ -1302,7 +788,7 @@ static int32_t search_vector_ex_impl(ssb_index* ix, const ssb_vec_query* vq, con
         }
         nh[q] = n;
         if (n_hits) n_hits[q] = n;
-        if (observed) observed[q] = use_ivf ? l.c->h_obs[q] : ix->n_rows;   // AnnMode::All scores every record (observed_vector_count, vector.rs:420); else: the selected clusters' vectors
+        if (observed) observed[q] = use_ivf ? l.c->vec.h_obs[q] : ix->vec.n_rows();   // AnnMode::All scores every record (observed_vector_count, vector.rs:420); else: the selected clusters' vectors
         if (ext) for (uint32_t j = 0; j < k; j++) {
             ssb_hit_ext& e = ext[(size_t)q * k + j];
             memset(&e, 0, sizeof(e));
@@ -1315,9 +801,9 @@ static int32_t search_vector_ex_impl(ssb_index* ix, const ssb_vec_query* vq, con
             e.source = SSB_SOURCE_VECTOR;
         }
     }
-    if (fm && observed) SSB_TRY(masked_observed(ix, *l.c, nq, fm, use_ivf, observed));
+    if (fm && observed) SSB_TRY(ix->vec.masked_observed(l.c->vec, l.c->st, nq, fm, use_ivf, observed));
     // field-tagged rows: which field and chunk of each doc won (after the threshold: only the hits returned)
-    if (ext && ix->tagged == 1) SSB_TRY(fill_best_rows(ix, *l.c, vq->queries, nq, k, hits, nh.data(), fm, ext));
+    if (ext && ix->vec.tagged()) SSB_TRY(ix->vec.best_rows(l.c->vec, l.c->st, l.c->stats, vq->queries, nq, k, hits, nh.data(), fm, ext));
     return SSB_OK;
     SSB_API_END
 }
@@ -1338,7 +824,7 @@ int32_t ssb_search_lexical_keys(ssb_index* ix, const ssb_lex_batch* q, uint32_t 
     SSB_API_BEGIN
     if (!ix || !q) { set_error("ssb_search_lexical_keys: null argument"); return SSB_E_INVALID; }
     std::shared_lock<std::shared_mutex> g(ix->rw);
-    SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
+    SSB_CUDA_TRY(cudaSetDevice(ix->device));
     CtxLease l(ix); SSB_TRY(l.acquire());
     l.c->ev_used = true; l.c->last_lex = true;
     SSB_TRY(ix->lex->search_keys(l.c->lex, l.c->st, q, k, result_type, keys_out_dev, count_dev, &l.c->stats.kernel_launches));
@@ -1352,7 +838,7 @@ int32_t ssb_search_lexical(ssb_index* ix, const ssb_lex_batch* q, uint32_t k, ui
     SSB_API_BEGIN
     if (!ix || !q || (q->n_queries && k && result_type != SSB_RESULT_COUNT && !hits)) { set_error("ssb_search_lexical: null argument"); return SSB_E_INVALID; }
     std::shared_lock<std::shared_mutex> g(ix->rw);
-    SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
+    SSB_CUDA_TRY(cudaSetDevice(ix->device));
     if (q->n_queries == 0) return SSB_OK;
     if (k > SSB_K_LIMIT) { set_error("k=%u exceeds SSB_K_LIMIT=%u", k, SSB_K_LIMIT); return SSB_E_UNSUPPORTED; }
     CtxLease l(ix); SSB_TRY(l.acquire());
@@ -1373,7 +859,7 @@ int32_t ssb_search_lexical_sorted_ex(ssb_index* ix, const ssb_lex_batch* q, cons
     if (result_type == SSB_RESULT_COUNT || k == 0) return ssb_search_lexical(ix, q, k, result_type, hits, n_hits, count_total);
     if (!ix || !q || (q->n_queries && !hits)) { set_error("ssb_search_lexical_sorted: null argument"); return SSB_E_INVALID; }
     std::shared_lock<std::shared_mutex> g(ix->rw);
-    SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
+    SSB_CUDA_TRY(cudaSetDevice(ix->device));
     SortDev sd{}; bool sorted = false;
     SSB_TRY(ix->lex->prepare_sort(sort, n_sort, bases != nullptr, &sd, &sorted));
     if (sorted && ix->comm.active()) { set_error("ssb_search_lexical_sorted: sorted search across shards is not built"); return SSB_E_UNSUPPORTED; }
@@ -1392,7 +878,7 @@ int32_t ssb_search_lexical_facets(ssb_index* ix, const ssb_lex_batch* q, const s
     SSB_API_BEGIN
     if (!ix || !q) { set_error("ssb_search_lexical_facets: null argument"); return SSB_E_INVALID; }
     std::shared_lock<std::shared_mutex> g(ix->rw);
-    SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
+    SSB_CUDA_TRY(cudaSetDevice(ix->device));
     if (ix->comm.active()) { set_error("ssb_search_lexical_facets: facet counts across shards are not built"); return SSB_E_UNSUPPORTED; }
     CtxLease l(ix); SSB_TRY(l.acquire());
     SearchCtx& c = *l.c;
@@ -1408,7 +894,7 @@ int32_t ssb_search_empty(ssb_index* ix, const ssb_lex_batch* q, const ssb_sort_c
     if (!ix || !q || (n_sort && !sort) || (q->n_queries && k && result_type != SSB_RESULT_COUNT && !hits)) { set_error("ssb_search_empty: null argument"); return SSB_E_INVALID; }
     if (result_type > SSB_RESULT_TOPKCOUNT) { set_error("ssb_search_empty: bad result_type"); return SSB_E_INVALID; }
     std::shared_lock<std::shared_mutex> g(ix->rw);
-    SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
+    SSB_CUDA_TRY(cudaSetDevice(ix->device));
     if (ix->comm.active()) { set_error("ssb_search_empty: the empty query across shards is not built"); return SSB_E_UNSUPPORTED; }
     if (k > SSB_K_LIMIT) { set_error("k=%u exceeds SSB_K_LIMIT=%u", k, SSB_K_LIMIT); return SSB_E_UNSUPPORTED; }
     if (n_sort > SSB_MAX_SORT_CRITERIA) { set_error("ssb_search_empty: more than %u criteria", SSB_MAX_SORT_CRITERIA); return SSB_E_UNSUPPORTED; }
@@ -1442,7 +928,7 @@ int32_t ssb_search_empty_facets(ssb_index* ix, const ssb_facet_request* req, uin
     SSB_API_BEGIN
     if (!ix) { set_error("ssb_search_empty_facets: null argument"); return SSB_E_INVALID; }
     std::shared_lock<std::shared_mutex> g(ix->rw);
-    SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
+    SSB_CUDA_TRY(cudaSetDevice(ix->device));
     if (ix->comm.active()) { set_error("ssb_search_empty_facets: facet counts across shards are not built"); return SSB_E_UNSUPPORTED; }
     CtxLease l(ix); SSB_TRY(l.acquire());
     SearchCtx& c = *l.c;
@@ -1481,12 +967,12 @@ int32_t ssb_search_hybrid(ssb_index* ix, const ssb_lex_batch* q, const float* qu
     if (!ix || !q || !queries || !hits) { set_error("ssb_search_hybrid: null argument"); return SSB_E_INVALID; }
     if (k == 0 || k > SSB_K_MAX) { set_error("k must be in 1..%u", SSB_K_MAX); return SSB_E_UNSUPPORTED; }
     std::shared_lock<std::shared_mutex> g(ix->rw);
-    SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
+    SSB_CUDA_TRY(cudaSetDevice(ix->device));
     const uint32_t nq = q->n_queries;
     if (nq == 0) return SSB_OK;
     // the lexical field filter applies to the vector half as well (search.rs:1702-1731), on an index whose rows carry field ids
     const uint32_t* fm = nullptr;
-    if (ix->tagged == 1) SSB_TRY(vec_field_masks(ix, q->field_masks, nq, "ssb_search_hybrid", &fm));
+    if (ix->vec.tagged()) SSB_TRY(ix->vec.field_masks(q->field_masks, nq, "ssb_search_hybrid", &fm));
     // the two per-shard searches are independent until the fusion: the lexical one runs on this context's stream, the vector one
     // on a second context's stream, so lex_score and the scan share the GPU instead of running back to back
     CtxLease l(ix); SSB_TRY(l.acquire());
@@ -1503,7 +989,8 @@ int32_t ssb_search_hybrid(ssb_index* ix, const ssb_lex_batch* q, const float* qu
     SSB_TRY(shard_merge(ix, c, c.keys_a.p, nq));
     SSB_CUDA_TRY(cudaMemcpyAsync(c.h_keys_a.data(), c.keys_a.p, (size_t)nq * LIST * 8, cudaMemcpyDeviceToHost, c.st));
     // multi-chunk documents: fetch the full 32-list so that k distinct docs survive the per-doc de-duplication
-    SSB_TRY(vec_keys(ix, *cv, queries, false, nq, ix->dup_docs ? SSB_K_MAX : k, cv->keys_b.p, nullptr, nullptr, fm));
+    SSB_TRY(ix->vec.search_keys(cv->vec, cv->st, cv->stats, &cv->ev_used, queries, false, nq, ix->vec.dup_docs() ? SSB_K_MAX : k, cv->keys_b.p,
+                                nullptr, nullptr, fm));
     SSB_TRY(shard_merge(ix, *cv, cv->keys_b.p, nq));
     SSB_CUDA_TRY(cudaMemcpyAsync(cv->h_keys_b.data(), cv->keys_b.p, (size_t)nq * LIST * 8, cudaMemcpyDeviceToHost, cv->st));
     SSB_CUDA_TRY(cudaStreamSynchronize(c.st));
@@ -1511,12 +998,12 @@ int32_t ssb_search_hybrid(ssb_index* ix, const ssb_lex_batch* q, const float* qu
     c.stats.kernel_launches += cv != &c ? cv->stats.kernel_launches : 0;
     c.stats.h2d_bytes += cv != &c ? cv->stats.h2d_bytes : 0;
     c.stats.d2h_bytes += (uint64_t)nq * LIST * 16;
-    std::vector<ssb_hit> a(k), b(k), f(2 * (size_t)k);
+    std::vector<ssb_hit> a((size_t)nq * k), b((size_t)nq * k), f(2 * (size_t)k);
+    PageState<1> pa(c, nq, k, a.data(), nullptr), pb(c, nq, k, b.data(), nullptr, ix->vec.dup_docs());
+    pa.append(c.h_keys_a.data(), LIST); pb.append(cv->h_keys_b.data(), LIST);
     for (uint32_t i = 0; i < nq; i++) {
         uint32_t nf = 0;
-        const uint32_t na = decode_list(c.h_keys_a.data() + (size_t)i * LIST, k, a.data(), false);
-        const uint32_t nb = decode_list(cv->h_keys_b.data() + (size_t)i * LIST, k, b.data(), ix->dup_docs);
-        ssb_rrf_fuse(a.data(), na, b.data(), nb, f.data(), &nf);
+        ssb_rrf_fuse(a.data() + (size_t)i * k, pa.cnt[i], b.data() + (size_t)i * k, pb.cnt[i], f.data(), &nf);
         uint32_t n = nf < k ? nf : k;     // search.rs:2117-2119 truncate(length)
         for (uint32_t j = 0; j < k; j++) hits[(size_t)i * k + j] = j < n ? f[j] : ssb_hit{0, 0.f, 0};
         if (n_hits) n_hits[i] = n;
@@ -1530,7 +1017,7 @@ int32_t ssb_merge_keys(ssb_index* ix, const uint64_t* keys_dev, uint32_t n_lists
     if (!ix || !keys_dev || !hits) { set_error("ssb_merge_keys: null argument"); return SSB_E_INVALID; }
     if (k == 0 || k > SSB_K_MAX) { set_error("k must be in 1..%u", SSB_K_MAX); return SSB_E_UNSUPPORTED; }
     std::shared_lock<std::shared_mutex> g(ix->rw);
-    SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
+    SSB_CUDA_TRY(cudaSetDevice(ix->device));
     if (nq == 0) return SSB_OK;
     CtxLease l(ix); SSB_TRY(l.acquire());
     SearchCtx& c = *l.c;
@@ -1540,7 +1027,9 @@ int32_t ssb_merge_keys(ssb_index* ix, const uint64_t* keys_dev, uint32_t n_lists
     c.h_keys_b.resize((size_t)nq * LIST);
     SSB_CUDA_TRY(cudaMemcpyAsync(c.h_keys_b.data(), c.keys_b.p, (size_t)nq * LIST * 8, cudaMemcpyDeviceToHost, c.st));
     SSB_CUDA_TRY(cudaStreamSynchronize(c.st));
-    decode_keys(c.h_keys_b.data(), nq, k, hits, n_hits, ix->dup_docs);
+    PageState<1> ps(c, nq, k, hits, n_hits, ix->vec.dup_docs());
+    ps.append(c.h_keys_b.data(), LIST);
+    ps.finish();
     return SSB_OK;
     SSB_API_END
 }
@@ -1557,10 +1046,10 @@ int32_t ssb_comm_init(ssb_index* ix, const uint8_t* id128, uint32_t rank, uint32
     SSB_API_BEGIN
     if (!ix || !id128) { set_error("ssb_comm_init: null argument"); return SSB_E_INVALID; }
     std::unique_lock<std::shared_mutex> g(ix->rw);
-    SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
+    SSB_CUDA_TRY(cudaSetDevice(ix->device));
     if (ix->comm.comm) { set_error("ssb_comm_init: the index already has a communicator"); return SSB_E_STATE; }
     if (ix->lex->has_ngrams() && world > 1) { set_error("ssb_comm_init: n-gram lists on a sharded index are not supported"); return SSB_E_UNSUPPORTED; }
-    if (ix->tagged == 1 && world > 1) { set_error("ssb_comm_init: field-tagged vector rows on a sharded index are not supported"); return SSB_E_UNSUPPORTED; }
+    SSB_TRY(refuse_tagged_sharded("ssb_comm_init", "vector rows", ix->vec.tagged(), world > 1));
     SSB_TRY(comm_init(ix->comm, id128, rank, world));
     std::lock_guard<std::mutex> g2(ix->pool_mu);
     if (ix->pool.size() > 1) { ix->pool.resize(1); ix->free_ctx.clear(); ix->free_ctx.push_back(ix->pool[0].get()); ix->last_ctx = nullptr; }
@@ -1574,7 +1063,7 @@ int32_t ssb_comm_attach(ssb_index* ix, void* nccl_comm, uint32_t rank, uint32_t 
     std::unique_lock<std::shared_mutex> g(ix->rw);
     if (ix->comm.comm) { set_error("ssb_comm_attach: the index already has a communicator"); return SSB_E_STATE; }
     if (ix->lex->has_ngrams() && world > 1) { set_error("ssb_comm_attach: n-gram lists on a sharded index are not supported"); return SSB_E_UNSUPPORTED; }
-    if (ix->tagged == 1 && world > 1) { set_error("ssb_comm_attach: field-tagged vector rows on a sharded index are not supported"); return SSB_E_UNSUPPORTED; }
+    SSB_TRY(refuse_tagged_sharded("ssb_comm_attach", "vector rows", ix->vec.tagged(), world > 1));
     ix->comm.comm = nccl_comm; ix->comm.rank = rank; ix->comm.world = world; ix->comm.owned = false;
     std::lock_guard<std::mutex> g2(ix->pool_mu);
     if (ix->pool.size() > 1) { ix->pool.resize(1); ix->free_ctx.clear(); ix->free_ctx.push_back(ix->pool[0].get()); ix->last_ctx = nullptr; }
@@ -1586,7 +1075,7 @@ int32_t ssb_comm_destroy(ssb_index* ix) {
     SSB_API_BEGIN
     if (!ix) return SSB_E_INVALID;
     std::unique_lock<std::shared_mutex> g(ix->rw);
-    SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
+    SSB_CUDA_TRY(cudaSetDevice(ix->device));
     comm_destroy(ix->comm);
     return SSB_OK;
     SSB_API_END
@@ -1598,7 +1087,7 @@ int32_t ssb_lexical_sync_df(ssb_index* ix) {
     SSB_API_BEGIN
     if (!ix) return SSB_E_INVALID;
     std::unique_lock<std::shared_mutex> g(ix->rw);
-    SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
+    SSB_CUDA_TRY(cudaSetDevice(ix->device));
     if (!ix->comm.active()) return SSB_OK;
     if (ix->lex->has_ngrams()) { set_error("ssb_lexical_sync_df: n-gram lists on a sharded index are not supported"); return SSB_E_UNSUPPORTED; }
     if (!ix->lex->committed()) { set_error("ssb_lexical_sync_df before ssb_lexical_commit"); return SSB_E_STATE; }
@@ -1642,7 +1131,7 @@ int32_t ssb_lexical_sync_df(ssb_index* ix) {
 int32_t ssb_sync(ssb_index* ix) {
     SSB_API_BEGIN
     if (!ix) return SSB_E_INVALID;
-    SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
+    SSB_CUDA_TRY(cudaSetDevice(ix->device));
     std::vector<cudaStream_t> sts;
     {
         std::lock_guard<std::mutex> g(ix->pool_mu);
@@ -1664,7 +1153,7 @@ int32_t ssb_set_stream(ssb_index* ix, void* stream) {
     SSB_API_BEGIN
     if (!ix) return SSB_E_INVALID;
     std::unique_lock<std::shared_mutex> g(ix->rw);       // no search in flight
-    SSB_CUDA_TRY(cudaSetDevice(ix->cfg.device));
+    SSB_CUDA_TRY(cudaSetDevice(ix->device));
     {
         std::lock_guard<std::mutex> g2(ix->pool_mu);
         for (auto& c : ix->pool) SSB_CUDA_TRY(cudaStreamSynchronize(ix->ext_stream_set ? ix->ext_stream : c->own_st));
@@ -1686,7 +1175,7 @@ int32_t ssb_last_stats(const ssb_index* cix, ssb_stats* out) {
     SearchCtx* c = nullptr;
     { std::lock_guard<std::mutex> g(ix->stats_mu); *out = ix->last_stats; c = ix->last_ctx; }
     if (c && c->ev_used && out->dominant_kernel_ns == 0) {   // asynchronous *_keys call: wait for its kernel's events now
-        cudaSetDevice(ix->cfg.device);
+        cudaSetDevice(ix->device);
         float ms = 0.f;
         if (cudaEventSynchronize(c->ev1) == cudaSuccess && cudaEventElapsedTime(&ms, c->ev0, c->ev1) == cudaSuccess)
             out->dominant_kernel_ns = (uint64_t)((double)ms * 1e6);
