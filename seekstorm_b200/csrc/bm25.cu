@@ -1058,7 +1058,7 @@ __device__ __forceinline__ uint32_t count_intersection(const LexView& v, const L
             for (uint32_t c = 0; c < np; c++) a &= __ldg(&v.bm_words[(size_t)rec.t[meta_cperm(meta, c)].bmi * 1024 + wi]);
             acc += (uint32_t)__popcll(a);
         }
-        st_words += np * 32u;
+        st_words += np * 1024u;                                         // warp-uniform: every list's 1024 words, counted once (lane 0 reports)
         return acc;
     }
     const uint32_t sb = meta_cperm(meta, np - 2u);
@@ -1131,7 +1131,7 @@ __device__ __forceinline__ uint32_t count_union(const LexView& v, const LvRec& r
                 b4[i0 + 32u * u] = n[u];
             }
         }
-        st_words += 32u; nw++;
+        st_words += 1024u; nw++;                                         // warp-uniform: the list's 1024 words (lane 0 reports)
     }
     if (nw == 0) for (uint32_t i = lane; i < 512u; i += 32u) b4[i] = make_uint4(0u, 0u, 0u, 0u);
     __syncwarp();
@@ -1706,7 +1706,7 @@ __global__ void __launch_bounds__(FACET_WARPS * 32) lex_facets(LexView v, const 
                 if (tc == 0) continue;
                 if (tb != NONE) {
                     for (uint32_t i = lane; i < 1024u; i += 32u) bm64[i] |= __ldg(&v.bm_words[(size_t)tb * 1024 + i]);
-                    st_words += 32;
+                    st_words += 1024u;                                         // the list's 1024 words, once per warp (lane 0 reports)
                 } else {
                     for_each_posting(v, to, tc, lane, [&](uint32_t d, bool valid) { if (valid) atomicOr(&bm[d >> 5], 1u << (d & 31u)); });
                     st_post += tc;
@@ -1728,7 +1728,7 @@ __global__ void __launch_bounds__(FACET_WARPS * 32) lex_facets(LexView v, const 
                     for (uint32_t t = 0; t < n; t++) a &= __ldg(&v.bm_words[(size_t)__shfl_sync(FULL, bmi, t) * 1024 + i]);
                     bm64[i] = a;
                 }
-                st_words += 32u * n;
+                st_words += 1024u * n;
             } else {
                 for (uint32_t i = lane; i < 2048u; i += 32u) bm[i] = 0u;
                 __syncwarp();
@@ -1750,7 +1750,7 @@ __global__ void __launch_bounds__(FACET_WARPS * 32) lex_facets(LexView v, const 
             uint32_t e;
             if (!find_entry(v, pl->tn[i], lv, e)) continue;
             const uint32_t tc = __ldg(&v.e_count[e]), tb = __ldg(&v.e_bitmap[e]); const uint64_t to = __ldg(&v.e_off[e]);
-            if (tb != NONE) { for (uint32_t w = lane; w < 1024u; w += 32u) bm64[w] &= ~__ldg(&v.bm_words[(size_t)tb * 1024 + w]); st_words += 32; }
+            if (tb != NONE) { for (uint32_t w = lane; w < 1024u; w += 32u) bm64[w] &= ~__ldg(&v.bm_words[(size_t)tb * 1024 + w]); st_words += 1024u; }
             else { for_each_posting(v, to, tc, lane, [&](uint32_t d, bool valid) { if (valid) atomicAnd(&bm[d >> 5], ~(1u << (d & 31u))); }); st_post += tc; }
             __syncwarp();
         }
